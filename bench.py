@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- frame-pair alignments/sec @640x480x5-level (BASELINE.json metric) on N B200s.
+"""bench.py -- frame-pair alignments/sec @640x480x5-level (BASELINE.json metric) on N H100s.
 
 A "step" = one pass of the hot path (DenseTracker::match, all levels, all iterations, 6x6 solves)
 over one batch of synthetic frame pairs.  Workload at every N: 512 independent 640x480 pairs PER GPU
@@ -21,6 +21,9 @@ over one batch of synthetic frame pairs.  Workload at every N: 512 independent 6
            is absent) = the oracle's scalar FAITHFUL restatement.
   --impl reference: the same CPU implementation from host images (pyramid build + match), all host threads.
   --config 5: BASELINE.json configs[4] (1280x960, 6 levels, mu = 0.05, 32 pairs per GPU = 256 over 8 GPUs).
+  --dump-outputs DIR: after the timed steps, the results of the last resident step (what a caller of
+           dvo_b200_match_batch receives for the whole batch) as DIR/<name>.npy in float64, so that two builds
+           can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -46,6 +49,7 @@ ALGO_BYTES_PER_PIXEL_ITERATION = 40.0                         # SURVEY.md 8(d)
 LEVEL_PIXELS = [(W >> l) * (H >> l) for l in range(LEVELS)]
 METRIC = "frame-pair alignments/sec @640x480x5-level"
 DEFAULT_BATCH = 512
+H100_HBM_GBS = 3350.0                                         # NVIDIA H100 SXM data sheet: the roofline's denominator
 
 
 def select_workload(config: int):
@@ -92,11 +96,39 @@ def parse_args():
     ap.add_argument("--cpu-sample", type=int, default=0, help="pairs in the CPU baseline sample (0 = auto)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-consecutive", action="store_true", help="skip the consecutive-frames e2e leg")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the results of the last timed step as DIR/<name>.npy (float64)")
+    args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
+    return args
+
+
+def dump_outputs(directory, results):
+    """The fields of dvo_b200_result for every pair of the batch, in pair order: transformation [n,4,4],
+    information [n,6,6], log_likelihood / num_levels / num_iterations_total [n], and every per-level statistic
+    as levels_<field> [n, levels] (levels coarse to fine as the result lists them, NaN past num_levels)."""
+    from dvo_slam_b200.engine import LevelStats, MAX_LEVELS
+    os.makedirs(directory, exist_ok=True)
+    n = len(results)
+    arrays = {"transformation": np.array([r.transformation[:] for r in results], dtype=np.float64).reshape(n, 4, 4),
+              "information": np.array([r.information[:] for r in results], dtype=np.float64).reshape(n, 6, 6),
+              "log_likelihood": np.array([r.log_likelihood for r in results], dtype=np.float64),
+              "num_levels": np.array([r.num_levels for r in results], dtype=np.float64),
+              "num_iterations_total": np.array([r.num_iterations_total for r in results], dtype=np.float64)}
+    nlev = max([r.num_levels for r in results] + [1])
+    for field, _ in LevelStats._fields_:
+        a = np.full((n, nlev), np.nan, dtype=np.float64)
+        for i, r in enumerate(results):
+            for l in range(min(r.num_levels, MAX_LEVELS)):
+                a[i, l] = float(getattr(r.levels[l], field))
+        arrays["levels_" + field] = a
+    for name, a in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), a)
 
 
 # ---------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
     """Polls nvidia-smi every 200 ms while the timed region runs."""
@@ -368,7 +400,7 @@ def run_ours(args, rank, local_rank, world):
             # build kernel
             pyr = engines[1].pyramid_raw_batch((hG.data_ptr(), hD.data_ptr(), 2 * B, H, W), 1.0 / 5000.0, K, LEVELS)
             # hand the batch over only when its pyramids are complete: the tracker's persistent launch needs every SM at once, and
-            # a loader that runs further ahead interleaves its build kernels with that launch (measured: 28.6 vs 24.0 ms per step)
+            # a loader that runs further ahead interleaves its build kernels with that launch
             engines[1].synchronize()
             q.put(pyr)
 
@@ -430,24 +462,10 @@ def run_ours(args, rank, local_rank, world):
             peaks = json.load(f)
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     achieved = algo_bytes / (stage_ms * 1e-3) / 1e9 if stage_ms > 0 else 0.0
-    # DRAM traffic of the dominant launch from the committed `ncu --set full` capture of THIS build (profiles/,
-    # regenerated by scripts/gpu_ncu.sh + scripts/make_traffic_json.py, which stamps the hash of the CUDA sources);
-    # a capture of another build is reported as stale and not used
-    traffic, traffic_note = None, None
-    if W == 640 and B == 512:
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_traffic.json")) as f:
-                tj = json.load(f)
-            if tj.get("source_stamp") == source_stamp():
-                traffic, traffic_note = tj["dram_bytes_per_step"] / tj["launches_per_step"], tj["note"]
-            else:
-                traffic_note = "stale: profiles/r02_traffic.json was captured from sources %s, this build is %s" % (tj.get("source_stamp"), source_stamp())
-        except Exception as e:
-            traffic_note = f"no capture: {e}"
-    else:
-        traffic_note = "capture exists for the default workload only"
+    # measured DRAM traffic of the level kernel needs a hardware-counter capture, which this benchmark does not take
+    traffic, traffic_note = None, "not measured"
 
     # ---- e2e: host buffers in, host results out, every step ----
     run_e2e(max(2, min(args.warmup, 4)))
@@ -555,6 +573,9 @@ def run_ours(args, rank, local_rank, world):
                "sample": f"first {len(hp)} pairs of the batch, match() on prebuilt pyramids, {cores} threads; {cpu_kind_text(kind, variant)}",
                "value_1core": n1 / t1}
 
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, tensor_to_results(last["gathered"]) if world > 1 else last["res"])
+
     if rank == 0:
         line = {"metric": METRIC, "value": value, "unit": "alignments/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
@@ -581,7 +602,7 @@ def run_ours(args, rank, local_rank, world):
                              "algorithmic_bytes_per_launch": algo_bytes / stage_launches if stage_launches else None,
                              "kernel_ms_per_launch": stage_ms / stage_launches if stage_launches else None,
                              "launches_per_step": stage_launches,
-                             "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 GB/s (of fallback)",
+                             "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, 3350 GB/s (not reached)",
                              "kernel_share_of_step": stage_ms / ms_per_step if ms_per_step else None,
                              "pair_step_ms_per_step": prof["pair_step"]["ms"] / args.steps},
                 "e2e_consecutive_frames": e2e_seq,

@@ -1,6 +1,6 @@
-// f32x2.cuh -- packed fp32 pairs for sm_100a (FFMA2 / FMUL2 / FADD2 issue one instruction for two
-// IEEE round-to-nearest fp32 operations; a pk(s, s) operand is folded by ptxas into the scalar
-// broadcast form "R.F32", so blending a float2 image sample with scalar weights needs no shuffles).
+// f32x2.cuh -- fp32 pairs {lo, hi} kept in one 64-bit register pair.  sm_90 has no packed fp32
+// arithmetic, so every pair operation is two scalar IEEE fp32 instructions with the rounding mode
+// spelled out (ptxas keeps the halves in adjacent registers: packing and unpacking cost nothing).
 // Every operation here is a single correctly rounded fp32 op per lane: results are bit-identical
 // to the scalar __fmaf_rn / __fmul_rn / __fadd_rn sequence the oracle's MIRROR mode restates.
 #pragma once
@@ -15,42 +15,16 @@ __device__ __forceinline__ f2 pk(float lo, float hi) {
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
   return r;
 }
-__device__ __forceinline__ float lo(f2 v) {
-  float a, b;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
-  return a;
-}
-__device__ __forceinline__ float hi(f2 v) {
-  float a, b;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
-  return b;
-}
+__device__ __forceinline__ float lo(f2 v) { return __uint_as_float((unsigned)v); }
+__device__ __forceinline__ float hi(f2 v) { return __uint_as_float((unsigned)(v >> 32)); }
 __device__ __forceinline__ f2 bc(float s) { return pk(s, s); }
 __device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
-  f2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  return pk(__fmaf_rn(lo(a), lo(b), lo(c)), __fmaf_rn(hi(a), hi(b), hi(c)));
 }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) {
-  f2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f2 add2(f2 a, f2 b) {
-  f2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f2 sub2(f2 a, f2 b) {
-  f2 d;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f2 add2_rz(f2 a, f2 b) {
-  f2 d;
-  asm("add.rz.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return pk(__fmul_rn(lo(a), lo(b)), __fmul_rn(hi(a), hi(b))); }
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return pk(__fadd_rn(lo(a), lo(b)), __fadd_rn(hi(a), hi(b))); }
+__device__ __forceinline__ f2 sub2(f2 a, f2 b) { return pk(__fsub_rn(lo(a), lo(b)), __fsub_rn(hi(a), hi(b))); }
+__device__ __forceinline__ f2 add2_rz(f2 a, f2 b) { return pk(__fadd_rz(lo(a), lo(b)), __fadd_rz(hi(a), hi(b))); }
 __device__ __forceinline__ f2 ldg_f2(const float2* p) {
   float2 v = __ldg(p);
   return pk(v.x, v.y);

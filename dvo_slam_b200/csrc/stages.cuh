@@ -35,7 +35,7 @@
 // the factor 0.5 is a power of two and is folded into the constants that multiply the blended gradient,
 // so every rounding step equals the one the precomputed gradient planes would give.
 //
-// All arithmetic that decides validity is explicit round-to-nearest fp32 in a fixed order (packed f32x2
+// All arithmetic that decides validity is explicit round-to-nearest fp32 in a fixed order (f32x2 pairs
 // where two channels share an operation), mirrored bit for bit by the oracle's MIRROR mode; the per-thread
 // accumulation along a row uses whatever contraction the compiler picks.
 #pragma once
@@ -60,7 +60,7 @@ constexpr int kWinCols = DVO_WIN_COLS;                    // window capacity: kT
 constexpr int kWinRows = DVO_WIN_ROWS;                    //                  kTileH + 17 rows
 constexpr int kStages = DVO_STAGES;
 
-// ---- mbarrier / bulk-copy primitives (PTX ISA 8.6, sm_100a) -----------------------------------------
+// ---- mbarrier / bulk-copy primitives (PTX ISA 8.6, sm_90a) ------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(unsigned long long* bar, unsigned count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -75,7 +75,7 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long* bar, u
                : "memory");
 }
 // try_wait may suspend the thread in hardware until the phase completes or a time limit passes; the explicit limit (ns)
-// keeps the polling loop around it from spinning (measured: 7 % of all issued instructions were this loop).
+// keeps the polling loop around it from spinning (0 = no hint, the default).
 #ifndef DVO_TRYWAIT_HINT_NS
 #define DVO_TRYWAIT_HINT_NS 0
 #endif
@@ -833,7 +833,7 @@ constexpr int kNormalValues = 28;   // log-likelihood sum, 21 upper-triangular A
 
 // Accumulators of stage B for one thread.  A is kept as pairs of adjacent columns of one row
 // (A[r][2c], A[r][2c+1]); rows 1, 3 and 5 carry one redundant lower-triangle entry so that every
-// update is a packed FMA of a broadcast row factor with a column pair.
+// update is one fma2 of a broadcast row factor with a column pair.
 struct StageBAcc;
 __device__ __forceinline__ void stage_b_values(const StageBAcc& acc, float out[]);
 struct StageBAcc {

@@ -458,7 +458,7 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
   const Segment& S = a.seg[si];
   // Squads of the second segment of a fused launch form in ORDER OF ARRIVAL: the CTAs leave the first segment at very
   // different times (1 or 2 coarse pairs each, 3..40 iterations per level), and a squad made of neighbouring block indices
-  // would wait for its slowest member (measured: 24 % of the fine segment's CTA time).
+  // would wait for its slowest member.
   int cta_index = blockIdx.x;
   if (fused && si >= 1) {
     if (threadIdx.x == 0) lt.s_flag[1] = atomicAdd(S.arrivals, 1);
@@ -1018,7 +1018,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   const bool fuse = ngroups == 2 && groups[0].g == 1 && !getenv("DVO_B200_NO_FUSE");
   // Fused launch: the fine group is cut into up to three slices of the pair index with squads of g, 2g and 4g CTAs.  Pairs
   // come off a queue, so with one squad size the launch ends with most squads idle while a few finish pairs that need two
-  // or three times the mean number of iterations (measured at batch 512: 16 % of the CTA time).  The last pairs of the
+  // or three times the mean number of iterations.  The last pairs of the
   // batch, which also leave the coarse segment last, therefore go to wider squads that finish a pair in a half / a quarter
   // of the time; the slice a pair belongs to is fixed by its index, so results do not depend on timing.
   GroupPlan segs[kMaxSeg];

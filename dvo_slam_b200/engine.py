@@ -98,7 +98,7 @@ def load_library():
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise RuntimeError(f"{LIB_PATH} is missing: run `python __graft_entry__.py` (nvcc, sm_100a). "
+        raise RuntimeError(f"{LIB_PATH} is missing: run `python __graft_entry__.py` (nvcc, sm_90a). "
                            "There is no CPU fallback for the engine.")
     L = C.CDLL(LIB_PATH)
     vp, fp, dp, i32, i64 = C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_double), C.c_int32, C.c_int64

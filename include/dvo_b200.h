@@ -1,5 +1,5 @@
 /*
- * dvo_b200.h -- C ABI of the B200-native dense RGB-D alignment engine.
+ * dvo_b200.h -- C ABI of the CUDA-native (H100, sm_90a) dense RGB-D alignment engine.
  *
  * This is the drop-in boundary for ONE hot path of tum-vision/dvo_slam: dvo::DenseTracker::match()
  * (dvo_core/src/dense_tracking.cpp:123-376) and the image model it consumes

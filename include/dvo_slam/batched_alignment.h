@@ -1,5 +1,5 @@
 // dvo_slam/batched_alignment.h -- the two places dvo_slam fans independent DenseTracker::match() calls out,
-// restated as ONE batched call on the B200 engine (SURVEY.md 8f row N1):
+// restated as ONE batched call on the CUDA engine (SURVEY.md 8f row N1):
 //
 //   * LocalTracker::update (dvo_slam/src/local_tracker.cpp:155-184): the new frame is aligned against the
 //     keyframe and against the previous frame with tbb::parallel_invoke -- two alignments sharing `current`;

@@ -1,6 +1,6 @@
 // dvo_slam/tracking_result_evaluation.h -- the keyframe-selection scores dvo_slam computes from DenseTracker
 // results (reference interface: dvo_slam/include/dvo_slam/tracking_result_evaluation.h:31-80, behaviour:
-// dvo_slam/src/tracking_result_evaluation.cpp:26-62).  They read only Result fields the B200 engine fills
+// dvo_slam/src/tracking_result_evaluation.cpp:26-62).  They read only Result fields the CUDA engine fills
 // (Information, LogLikelihood, the last iteration's ValidConstraints), so they sit on the adapter unchanged:
 // same class names, constructors and virtuals; header-only here.
 #ifndef DVO_SLAM_TRACKING_RESULT_EVALUATION_H_

@@ -2,7 +2,7 @@
  * dvo_oracle.cpp -- CPU ORACLE (test infrastructure only; see dvo_oracle.h header).
  * PARITY UNPINNED against the reference (no reference tests / goldens exist, reference not
  * buildable here).  Restatement of tum-vision/dvo_slam dvo_core; citations are relative to
- * /root/reference.
+ * the root of a dvo_slam checkout at d25b65bf.
  *
  * Build: see oracle/Makefile (-O2 -msse3 -mfma -ffp-contract=off -frounding-math; NO -ffast-math).
  *  -ffp-contract=off : the reference's mul/add order is kept unfused (its 2012 targets had no

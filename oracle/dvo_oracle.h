@@ -171,7 +171,7 @@ void orc_ldlt_solve6(const double A[36], const double b[6], double x[6]);
 /* SurfacePyramid::convertRawDepthImageSse (surface_pyramid.cpp:45-105): u16 -> f32*scale, 0 -> NaN */
 void orc_convert_raw_depth(const uint16_t* in, float* out, int64_t count, float scale);
 /* cv::cvtColor(rgb, grey, CV_BGR2GRAY) on CV_8UC3 followed by convertTo(CV_32F) (call site benchmark_slam.cpp:58-68).
- * OpenCV (2.4.x, the version dvo_slam's rosbuild manifests pull in) is not vendored in /root/reference; its published
+ * OpenCV (2.4.x, the version dvo_slam's rosbuild manifests pull in) is not vendored in the reference checkout; its published
  * 8-bit algorithm is fixed point: grey = (B*1868 + G*9617 + R*4899 + (1 << 13)) >> 14.  Known answers:
  * pure blue/green/red 255 -> 29/150/76, white -> 255. */
 void orc_bgr_to_grey(const uint8_t* bgr, float* out, int64_t count);

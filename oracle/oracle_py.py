@@ -2,7 +2,8 @@
 
 May be imported by tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
 legs; never by the product package dvo_slam_b200/.  The reference ships no goldens; the FAITHFUL mode is pinned,
-bit for bit, against the reference's own SSE translation units compiled into oracle/_ref (tests/test_reference_pin.py).
+bit for bit, against what the reference's own SSE translation units (oracle/_ref) compute on the golden cases
+(tests/golden/reference_pin.npz, tests/test_reference_pin.py).
 """
 from __future__ import annotations
 
@@ -263,9 +264,9 @@ def ref_available(variant: str = "") -> bool:
 
 
 def ref_lib(variant: str = ""):
-    """libdvo_ref.so = /root/reference/dvo_core/src/{dense_tracking_impl,core/math_sse,core/intrinsic_matrix}.cpp compiled
-    unmodified + ref_driver.cpp (-O2; variant "_O3" = the reference's own optimisation level).  Built by `make -C oracle ref`
-    where /root/reference exists; the built files travel."""
+    """libdvo_ref.so = dvo_core/src/{dense_tracking_impl,core/math_sse,core/intrinsic_matrix}.cpp of a dvo_slam checkout compiled
+    unmodified + ref_driver.cpp (-O2; variant "_O3" = the reference's own optimisation level).  Built by __graft_entry__.build()
+    when DVO_REFERENCE names that checkout (oracle/Makefile target `ref`)."""
     if variant not in _ref:
         L = C.CDLL(os.path.join(_REF_DIR, f"libdvo_ref{variant}.so"))
         fp, dp = C.POINTER(C.c_float), C.POINTER(C.c_double)

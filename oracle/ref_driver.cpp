@@ -1,6 +1,6 @@
 // ref_driver.cpp -- TEST INFRASTRUCTURE.  Drives the REFERENCE'S OWN compiled functions (oracle/_ref/, built by
-// `make -C oracle ref` from /root/reference/dvo_core/src/{dense_tracking_impl,core/math_sse,core/intrinsic_matrix}.cpp,
-// unmodified, against the container shims in oracle/ref_shim/) through one Gauss-Newton linearisation exactly as
+// `make -C oracle ref REF=<dvo_slam checkout>/dvo_core` from src/{dense_tracking_impl,core/math_sse,core/intrinsic_matrix}.cpp,
+// unmodified, against the header-only shims in oracle/ref_shim/) through one Gauss-Newton linearisation exactly as
 // DenseTracker::match() strings them together (dense_tracking.cpp:212-220, 271-343), so that the oracle's FAITHFUL
 // mode can be checked bit for bit against reference-produced numbers (tests/test_reference_pin.py).
 //

@@ -1,5 +1,5 @@
 // shim_eigen.h -- TEST INFRASTRUCTURE.  The smallest stand-in for the parts of Eigen 3 that the reference's SSE
-// translation units touch, so that /root/reference/dvo_core/src/{dense_tracking_impl,core/math_sse,core/intrinsic_matrix}.cpp
+// translation units touch, so that dvo_core/src/{dense_tracking_impl,core/math_sse,core/intrinsic_matrix}.cpp
 // compile UNMODIFIED into oracle/_ref/ (Eigen itself is not in this image).  Those files use Eigen as a container
 // (data(), operator(), fixed-size storage, column-major like Eigen's default) and for a handful of 2x2 / 3x4 expressions;
 // the arithmetic that matters is their own SSE intrinsics.  Fixed-size products are plain loops in index order

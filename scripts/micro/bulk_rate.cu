@@ -1,6 +1,6 @@
 // Micro-benchmark: throughput of cp.async.bulk global->shared per SM as a function of the copy size.
 // Two CTAs per SM, one issuing warp each, double-buffered: every "tile" is `ncopies` copies of `bytes` bytes whose sources lie
-// `pitch` bytes apart (image rows), completion on an mbarrier.  nvcc -arch=sm_100a -O3 -o bulk_rate bulk_rate.cu
+// `pitch` bytes apart (image rows), completion on an mbarrier.  nvcc -arch=sm_90a -O3 -o bulk_rate bulk_rate.cu
 #include <cstdio>
 #include <cstdlib>
 #include <cuda_runtime.h>

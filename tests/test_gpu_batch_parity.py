@@ -11,7 +11,7 @@ another order) agree on every termination for only ~70 % of pairs and on every i
 (scripts/oracle_controlflow.py).  The meaningful statement is therefore relative: the CUDA path is no farther from the
 reference's numerics than that independent IEEE restatement is.  The test measures both distances on the same 512 pairs and
 asserts GPU-vs-FAITHFUL agreement >= MIRROR-vs-FAITHFUL agreement - 5 percentage points, plus absolute floors; the
-distributions of |dt|, |dr|, Information and LogLikelihood error are printed and written to gpurun_out/."""
+distributions of |dt|, |dr|, Information and LogLikelihood error are printed (pytest -s shows them)."""
 import json
 import os
 from concurrent.futures import ThreadPoolExecutor
@@ -53,9 +53,9 @@ def test_batch_512_against_reference_numerics(engine, oracle):
 
     # Every floating-point sum above an image row is taken in an order fixed by the level's geometry (rows of a strip in
     # order, strips in order, fp64), never by how strips are spread over CTAs: the fused 512-pair launch -- one CTA per pair
-    # on the coarse levels, slices with squads of 3, 6 and 12 CTAs on level 0 -- returns bit for bit what the same call
-    # returns again, what the batch in reverse order returns (other slices), and what SINGLE alignments (one launch per
-    # level, squads of up to 69 CTAs) return.  The oracle comparison below therefore also speaks for the single-pair path
+    # on the coarse levels, slices with squads of 3, 6 and 12 CTAs on level 0 (on an H100, 132 SMs x 2 CTAs: pairs
+    # 0-392, 393-471, 472-511) -- returns bit for bit what the same call returns again, what the batch in reverse order
+    # returns (other slices), and what SINGLE alignments (one launch per level, squads of up to 69 CTAs) return.  The oracle comparison below therefore also speaks for the single-pair path
     # and vice versa (tests/test_gpu_parity.py compares that path with the oracle record by record).
     again = engine.match_batch(refs, curs, cfg)
     rev = engine.match_batch(refs[::-1], curs[::-1], cfg)[::-1]
@@ -63,7 +63,7 @@ def test_batch_512_against_reference_numerics(engine, oracle):
         for i in range(B):
             assert np.array_equal(res[i].transformation, other[i].transformation) and np.array_equal(res[i].information, other[i].information), i
             assert res[i].log_likelihood == other[i].log_likelihood and res[i].levels == other[i].levels, i
-    for i in (0, 1, 200, 380, 381, 425, 468, 469, 500, 511):       # both sides of the slice boundaries 381 | 88 | 43
+    for i in (0, 1, 200, 392, 393, 430, 471, 472, 500, 511):       # both sides of the slice boundaries 393 | 79 | 40
         single = engine.match(refs[i], curs[i], cfg)
         assert np.array_equal(res[i].transformation, single.transformation) and np.array_equal(res[i].information, single.information), i
         assert res[i].log_likelihood == single.log_likelihood and res[i].levels == single.levels, i
@@ -119,9 +119,6 @@ def test_batch_512_against_reference_numerics(engine, oracle):
         "vs_faithful": {k: {m: dist(v) for m, v in d.items()} for k, d in err.items()},
     }
     print("\nbatch-512 parity vs FAITHFUL:", json.dumps(summary))
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open(os.path.join("gpurun_out", "batch512_parity.json"), "w") as f:
-        json.dump(summary, f, indent=1)
     # the CUDA path is as close to the reference's numerics as an independent IEEE restatement of the same algorithm:
     # control flow ...
     for m in ("term", "it1", "both"):

@@ -1,187 +1,131 @@
-"""Pins the oracle against the REFERENCE'S OWN OBJECT CODE.
+"""Pins the oracle against the ORIGINAL PROJECT'S OWN OBJECT CODE.
 
-oracle/_ref/libdvo_ref.so is /root/reference/dvo_core/src/{dense_tracking_impl,core/math_sse,core/intrinsic_matrix}.cpp compiled
-unmodified (oracle/Makefile target `ref`; Eigen / OpenCV / Boost containers from oracle/ref_shim/).  oracle/ref_driver.cpp
-strings computeResidualsSse, computeWeightsSse, computeScaleSse, computeCompleteDataLogLikelihood and
-OptimizedSelfAdjointMatrix6x6f::rankUpdate together exactly as DenseTracker::match() does for one Gauss-Newton linearisation
-(dense_tracking.cpp:212-220, 271-343).  The oracle's FAITHFUL mode must reproduce every number BIT FOR BIT: selected and
-valid point counts, which points are valid, all six residual-record channels, the Student-t weights' effect on the scale
-(precision), the log-likelihood, A and b.
-
-The built library travels to the GPU box; where it is absent (a checkout without /root/reference) the tests skip."""
+tests/golden/reference_pin.npz holds what dvo_core/src/{dense_tracking_impl,core/math_sse,core/intrinsic_matrix}.cpp of
+dvo_slam compute on the golden pairs, compiled unmodified (oracle/Makefile target `ref`; Eigen / OpenCV / Boost containers
+from oracle/ref_shim/) and driven by oracle/ref_driver.cpp, which strings computeResidualsSse, computeWeightsSse,
+computeScaleSse, computeCompleteDataLogLikelihood and OptimizedSelfAdjointMatrix6x6f::rankUpdate together exactly as
+DenseTracker::match() does for one Gauss-Newton linearisation (dense_tracking.cpp:212-220, 271-343).  The oracle's FAITHFUL
+mode must reproduce every number BIT FOR BIT: selected and valid point counts, which points are valid, all six
+residual-record channels, the Student-t weights' effect on the scale (precision), the log-likelihood, A and b.
+tests/golden/make_reference_pin.py regenerates the file from a build of that object code."""
 import numpy as np
 import pytest
 
-from helpers import GOLDEN_LEVELS, GOLDEN_SEEDS, golden_images, load_golden
+from helpers import (GOLDEN_LEVELS, GOLDEN_SEEDS, digest, golden_images, load_golden, load_reference_pin, match_cases,
+                     o3_sample_index, odd_point_margin)
 
 
-def _need_ref(oracle, variant=""):
-    if not oracle.ref_available(variant):
-        pytest.skip("oracle/_ref/libdvo_ref%s.so not built (needs /root/reference: make -C oracle ref)" % variant)
-
-
-def _dense(r, h, w):
-    """scatter the reference's compacted records {point (4), i, z, idx, idy, zdx, zdy, -, -} into seven h*w planes"""
-    d = np.full((7, h * w), np.nan, np.float32)
-    d[0:6, r["index"]] = r["records"][:, 4:10].T
-    d[6, r["index"]] = r["records"][:, 2]
-    return d
+@pytest.fixture(scope="module")
+def pin():
+    return load_reference_pin()
 
 
 def _cases(oracle):
-    for seed in GOLDEN_SEEDS:
+    for si, seed in enumerate(GOLDEN_SEEDS):
         g = load_golden(seed)
         im = golden_images(g, oracle)
         oref = oracle.Pyramid(im["I_ref"], im["Z_ref"], g["K"], GOLDEN_LEVELS)
         ocur = oracle.Pyramid(im["I_cur"], im["Z_cur"], g["K"], GOLDEN_LEVELS)
         for lvl in range(GOLDEN_LEVELS):
-            yield g, oref, ocur, lvl
+            yield si, seed, g, oref, ocur, lvl
 
 
-def test_faithful_oracle_equals_reference_object_code_bit_for_bit(oracle):
-    _need_ref(oracle)
+def test_faithful_oracle_equals_reference_object_code_bit_for_bit(oracle, pin):
     fa = oracle.mode("faithful")
     checked = 0
-    for g, oref, ocur, lvl in _cases(oracle):
-        w, h, K = oref.level_info(lvl)
+    for si, seed, g, oref, ocur, lvl in _cases(oracle):
         S, _ = oracle.select(oref, lvl, 0.0, 0.0, fa)
         n_img, img = oracle.residual_image(oref, ocur, lvl, g["kat_T"], fa)
         img = img.reshape(7, -1)
         for uw in (False, True):
-            r = oracle.ref_linearize(oref.planes(lvl), ocur.planes(lvl), K, g["kat_T"], uw, g["kat_prev_precision"])
+            k = (si, lvl, int(uw))
             o = oracle.linearize(oref, ocur, lvl, g["kat_T"], fa, uw, g["kat_prev_precision"])
-            assert r["n_selected"] == S                                   # PointSelection::select
-            assert r["n"] == o["n"] == n_img                              # valid constraints (bounds, NaN and occlusion tests)
-            d = _dense(r, h, w)
-            assert np.array_equal(np.isnan(d), np.isnan(img))             # the same points are valid
-            m = ~np.isnan(d)
-            assert np.array_equal(d[m], img[m])                           # computeResidualsSse: every channel, every point
-            assert np.array_equal(r["precision"], o["precision"])         # computeWeightsSse + computeScaleSse + inverse()
-            assert r["ll"] == o["ll"]                                     # computeCompleteDataLogLikelihood
-            assert np.array_equal(r["A"].astype(np.float64), o["A"])      # rankUpdate(2x6, 2x2) + toEigen, fp32 serial
-            assert np.array_equal(r["b"].astype(np.float64), o["b"])
-            checked += int(m.sum())
+            assert pin["lin_counts"][k][0] == S                                # PointSelection::select
+            assert pin["lin_counts"][k][1] == o["n"] == n_img                  # valid constraints (bounds, NaN and occlusion tests)
+            # computeResidualsSse: the same points are valid, every channel of every point equal
+            assert digest(img) == pin["lin_records"][k]
+            assert np.array_equal(pin["lin_P"][k], o["precision"])             # computeWeightsSse + computeScaleSse + inverse()
+            assert pin["lin_ll"][k] == o["ll"]                                 # computeCompleteDataLogLikelihood
+            assert np.array_equal(pin["lin_A"][k].astype(np.float64), o["A"])  # rankUpdate(2x6, 2x2) + toEigen, fp32 serial
+            assert np.array_equal(pin["lin_b"][k].astype(np.float64), o["b"])
+            checked += int((~np.isnan(img)).sum())
     assert checked > 500000
 
 
-def test_nondefault_thresholds_and_identity_pose(oracle):
+def test_nondefault_thresholds_and_identity_pose(oracle, pin):
     """selection thresholds (Config::Intensity/DepthDerivativeThreshold) and a second transform"""
-    _need_ref(oracle)
     fa = oracle.mode("faithful")
     g = load_golden(12)
     im = golden_images(g, oracle)
     oref = oracle.Pyramid(im["I_ref"], im["Z_ref"], g["K"], GOLDEN_LEVELS)
     ocur = oracle.Pyramid(im["I_cur"], im["Z_cur"], g["K"], GOLDEN_LEVELS)
-    w, h, K = oref.level_info(1)
-    for T, ti, td in ((np.eye(4), 0.0, 0.0), (g["kat_T"], 4.0, 0.02)):
-        r = oracle.ref_linearize(oref.planes(1), ocur.planes(1), K, T, True, g["kat_prev_precision"], ti, td)
+    for c, (T, ti, td) in enumerate(((np.eye(4), 0.0, 0.0), (g["kat_T"], 4.0, 0.02))):
         o = oracle.linearize(oref, ocur, 1, T, fa, True, g["kat_prev_precision"], ti, td)
         S, _ = oracle.select(oref, 1, ti, td, fa)
-        assert r["n_selected"] == S and r["n"] == o["n"]
-        assert np.array_equal(r["precision"], o["precision"]) and r["ll"] == o["ll"]
-        assert np.array_equal(r["A"].astype(np.float64), o["A"]) and np.array_equal(r["b"].astype(np.float64), o["b"])
+        assert pin["thr_counts"][c][0] == S and pin["thr_counts"][c][1] == o["n"]
+        assert np.array_equal(pin["thr_P"][c], o["precision"]) and pin["thr_ll"][c] == o["ll"]
+        assert np.array_equal(pin["thr_A"][c].astype(np.float64), o["A"]) and np.array_equal(pin["thr_b"][c].astype(np.float64), o["b"])
 
 
-def test_reference_built_at_its_own_O3_stays_within_the_stated_spread(oracle):
+def test_reference_built_at_its_own_O3_stays_within_the_stated_spread(oracle, pin):
     """At -O3 (dvo_core/CMakeLists.txt:36-40) GCC 13 schedules floating-point work across the MXCSR switch of
-    dense_tracking_impl.cpp:165-167: the reference's own numbers then differ from the program-order build.  The same points
-    stay valid; records move by < 5e-3 absolute (measured 2.7e-3), precision / A / b by < 5e-4 relative (measured 1.7e-4) -- the noise floor any comparison
-    with 'the reference' has, and two orders of magnitude below the pose tolerance."""
-    _need_ref(oracle, "_O3")
+    dense_tracking_impl.cpp:165-167: the original project's own numbers then differ from the program-order build.  The same
+    points stay valid; records move by < 5e-3 absolute (measured 2.7e-3), precision / A / b by < 5e-4 relative (measured
+    1.7e-4) -- the noise floor any comparison with 'the reference' has, and two orders of magnitude below the pose
+    tolerance.  The records of the -O3 build are stored at a fixed seeded sample of the valid points."""
     fa = oracle.mode("faithful")
-    for g, oref, ocur, lvl in _cases(oracle):
-        w, h, K = oref.level_info(lvl)
-        r = oracle.ref_linearize(oref.planes(lvl), ocur.planes(lvl), K, g["kat_T"], True, g["kat_prev_precision"], variant="_O3")
+    for si, seed, g, oref, ocur, lvl in _cases(oracle):
+        k = (si, lvl)
         o = oracle.linearize(oref, ocur, lvl, g["kat_T"], fa, True, g["kat_prev_precision"])
         n_img, img = oracle.residual_image(oref, ocur, lvl, g["kat_T"], fa)
-        d = _dense(r, h, w)
-        assert r["n"] == o["n"] and np.array_equal(np.isnan(d), np.isnan(img.reshape(7, -1)))
-        m = ~np.isnan(d)
-        assert np.abs(d[m] - img.reshape(7, -1)[m]).max() < 5e-3
-        assert np.allclose(r["precision"], o["precision"], rtol=5e-4)
-        assert np.abs(r["A"] - o["A"]).max() <= 5e-4 * np.abs(o["A"]).max()
-        assert np.abs(r["b"] - o["b"]).max() <= 5e-4 * np.abs(o["b"]).max()
+        img = img.reshape(7, -1)
+        assert pin["o3_n"][k] == o["n"] and digest(np.isnan(img)) == pin["o3_valid"][k]
+        assert np.abs(pin["o3_sample"][k] - img[:, o3_sample_index(img, seed, lvl)]).max() < 5e-3
+        assert np.allclose(pin["o3_P"][k], o["precision"], rtol=5e-4)
+        assert np.abs(pin["o3_A"][k] - o["A"]).max() <= 5e-4 * np.abs(o["A"]).max()
+        assert np.abs(pin["o3_b"][k] - o["b"]).max() <= 5e-4 * np.abs(o["b"]).max()
 
 
-def test_whole_alignment_through_reference_object_code_equals_faithful_oracle(oracle):
-    """DenseTracker::match() end to end: oracle/ref_driver.cpp runs the coarse-to-fine loop (dense_tracking.cpp:131-376) with
-    every per-point pass executed by the reference's own object code; the oracle's FAITHFUL match must take the same control
-    flow on every level and return the same Result (the poses agree to the rounding of the 4x4 bookkeeping, Information and
-    LogLikelihood exactly)."""
-    _need_ref(oracle)
-    from dvo_slam_b200 import synth
+def test_whole_alignment_through_reference_object_code_equals_faithful_oracle(oracle, pin):
+    """DenseTracker::match() end to end: oracle/ref_driver.cpp ran the coarse-to-fine loop (dense_tracking.cpp:131-376) with
+    every per-point pass executed by the original project's own object code; the oracle's FAITHFUL match must take the same
+    control flow on every level and return the same Result (the poses agree to the rounding of the 4x4 bookkeeping,
+    Information and LogLikelihood exactly)."""
     fa = oracle.mode("faithful")
-    cases = []
-    for seed in GOLDEN_SEEDS:
-        g = load_golden(seed)
-        im = golden_images(g, oracle)
-        cases.append((im["I_ref"], im["Z_ref"], im["I_cur"], im["Z_cur"], g["K"], GOLDEN_LEVELS,
-                      dict(first_level=2, last_level=0, max_iterations_per_level=50, precision=1e-4), None))
-    for seed, extra in ((3, {}), (5, dict(mu=0.05, use_initial_estimate=1))):     # 640x480, 5 levels (BASELINE configs[0])
-        p = synth.make_pair(seed)
-        a = {k: p[k].numpy() for k in ("I_ref", "Z_ref", "I_cur", "Z_cur")}
-        cfg = dict(first_level=4, last_level=0, max_iterations_per_level=50, precision=1e-4)
-        cfg.update(extra)
-        T0 = synth.se3_exp(p["xi"] * 0.8) if extra else None
-        cases.append((a["I_ref"], a["Z_ref"], a["I_cur"], a["Z_cur"], p["intrinsics"], 5, cfg, T0))
-    for Ir, Zr, Ic, Zc, K, levels, cfg, T0 in cases:
+    for c, (Ir, Zr, Ic, Zc, K, levels, cfg, T0) in enumerate(match_cases(oracle)):
         oref, ocur = oracle.Pyramid(Ir, Zr, K, levels), oracle.Pyramid(Ic, Zc, K, levels)
-        ocfg = oracle.config(**cfg)
-        o = oracle.match(oref, ocur, ocfg, fa, T_init=T0)
-        r = oracle.ref_match(oracle.RefPyramid(oref), oracle.RefPyramid(ocur), ocfg, T_init=T0)
-        assert [l["termination"] for l in r["levels"]] == [l["termination"] for l in o["levels"]]
-        assert [l["num_iterations"] for l in r["levels"]] == [l["num_iterations"] for l in o["levels"]]
-        assert [l["valid_pixels"] for l in r["levels"]] == [l["valid_pixels"] for l in o["levels"]]
-        assert np.abs(r["T"] - o["T"]).max() < 1e-12
-        assert np.array_equal(r["information"], o["information"])
-        assert r["log_likelihood"] == o["log_likelihood"]
+        o = oracle.match(oref, ocur, oracle.config(**cfg), fa, T_init=T0)
+        want = pin["match_levels"][c][:len(o["levels"])]
+        assert (pin["match_levels"][c][len(o["levels"]):] == -1).all()
+        assert want[:, 0].tolist() == [l["termination"] for l in o["levels"]]
+        assert want[:, 1].tolist() == [l["num_iterations"] for l in o["levels"]]
+        assert want[:, 2].tolist() == [l["valid_pixels"] for l in o["levels"]]
+        assert np.abs(pin["match_T"][c] - o["T"]).max() < 1e-12
+        assert np.array_equal(pin["match_information"][c], o["information"])
+        assert pin["match_ll"][c] == o["log_likelihood"]
 
 
-def test_intensity_error_image_walk_equals_reference_valid_flag_stream(oracle):
+def test_intensity_error_image_walk_equals_reference_valid_flag_stream(oracle, pin):
     """DenseTracker::computeIntensityErrorImage (dense_tracking.cpp:378-444): the oracle's raster walk against the same
-    walk fed by the reference's OWN computeResidualsAndValidFlagsSse (flags and residuals from the Debug instantiation of
-    the SSE loop) -- bit for bit, including the odd last selected point, which the SSE loop never visits and which
-    therefore stays 0 although its warp is valid."""
-    _need_ref(oracle)
+    walk fed by the original project's OWN computeResidualsAndValidFlagsSse (flags and residuals from the Debug
+    instantiation of the SSE loop) -- bit for bit, including the odd last selected point, which the SSE loop never visits
+    and which therefore stays 0 although its warp is valid."""
     fa = oracle.mode("faithful")
-    for seed in GOLDEN_SEEDS:
-        g = load_golden(seed)
-        im = golden_images(g, oracle)
-        oref = oracle.Pyramid(im["I_ref"], im["Z_ref"], g["K"], GOLDEN_LEVELS)
-        ocur = oracle.Pyramid(im["I_cur"], im["Z_cur"], g["K"], GOLDEN_LEVELS)
-        rref, rcur = oracle.RefPyramid(oref), oracle.RefPyramid(ocur)
-        for lvl in range(GOLDEN_LEVELS):
-            for ti, td in ((0.0, 0.0), (2.0, 0.02)):
-                n_o, img_o = oracle.intensity_error_image(oref, ocur, lvl, g["kat_T"], fa, ti, td)
-                n_r, img_r = oracle.ref_intensity_error_image(rref, rcur, lvl, g["kat_T"], ti, td)
-                assert n_o == n_r and n_o > 0
-                assert np.array_equal(img_o, img_r)
-                # semantics, stated independently: |e.i| where the residual stage has a valid residual, 0 elsewhere
-                n_img, planes = oracle.residual_image(oref, ocur, lvl, g["kat_T"], fa, ti, td)
-                want = np.where(np.isnan(planes[0]), 0.0, np.abs(planes[0])).astype(np.float32)
-                assert n_img == n_o and np.array_equal(img_o, want)
-    # The odd-point drop made visible: reference = a frame with its bottom/right margin made invalid, current = the same
-    # frame unmasked, identity transform -> every selected point maps onto itself and is valid, so the only selected pixel
-    # the image may leave at 0 is the odd last one (which EXACT numerics, without the drop, would fill).
-    g = load_golden(GOLDEN_SEEDS[0])
-    im = golden_images(g, oracle)
-    saw_odd = False
-    for margin in range(4, 40):
-        Z = im["Z_ref"].copy()
-        Z[-margin:, :] = np.nan
-        Z[:, -margin:] = np.nan
-        oref = oracle.Pyramid(im["I_ref"], Z, g["K"], 1)
-        ocur = oracle.Pyramid(im["I_ref"], im["Z_ref"], g["K"], 1)
-        S, mask = oracle.select(oref, 0, 0.0, 0.0, None)
-        last = np.flatnonzero(mask.reshape(-1))[-1]
-        _, planes_exact = oracle.residual_image(oref, ocur, 0, np.eye(4), oracle.mode("exact"))
-        if S % 2 == 0 or np.isnan(planes_exact[0].reshape(-1)[last]):   # need: odd count, last point valid by itself
-            continue
-        rref, rcur = oracle.RefPyramid(oref), oracle.RefPyramid(ocur)
-        n_o, img_o = oracle.intensity_error_image(oref, ocur, 0, np.eye(4), fa)
-        n_r, img_r = oracle.ref_intensity_error_image(rref, rcur, 0, np.eye(4))
-        assert np.array_equal(img_o, img_r) and n_o == n_r <= S - 1
-        assert img_o.reshape(-1)[last] == 0.0                      # the point itself is fine and still 0 in the reference's image
-        saw_odd = True
-        break
-    assert saw_odd, "no margin gave an odd selection count with a valid last point"
+    for si, seed, g, oref, ocur, lvl in _cases(oracle):
+        for t, (ti, td) in enumerate(((0.0, 0.0), (2.0, 0.02))):
+            n_o, img_o = oracle.intensity_error_image(oref, ocur, lvl, g["kat_T"], fa, ti, td)
+            assert n_o == pin["iei_n"][si, lvl, t] and n_o > 0
+            assert digest(img_o) == pin["iei_img"][si, lvl, t]
+            # semantics, stated independently: |e.i| where the residual stage has a valid residual, 0 elsewhere
+            n_img, planes = oracle.residual_image(oref, ocur, lvl, g["kat_T"], fa, ti, td)
+            want = np.where(np.isnan(planes[0]), 0.0, np.abs(planes[0])).astype(np.float32)
+            assert n_img == n_o and np.array_equal(img_o, want)
+    # the odd-point drop made visible (helpers.odd_point_margin): the only selected pixel the image may leave at 0 is the odd
+    # last one, which EXACT numerics, without the drop, would fill
+    margin, im, oref, ocur = odd_point_margin(oracle)
+    assert margin == pin["odd"][0]
+    S, mask = oracle.select(oref, 0, 0.0, 0.0, None)
+    last = np.flatnonzero(mask.reshape(-1))[-1]
+    n_o, img_o = oracle.intensity_error_image(oref, ocur, 0, np.eye(4), fa)
+    assert digest(img_o) == pin["odd_img"] and n_o == pin["odd"][1] <= S - 1
+    assert img_o.reshape(-1)[last] == 0.0                      # the point itself is fine and still 0 in the reference's image
