@@ -1,22 +1,20 @@
-// f32x2.cuh -- fp32 pairs {lo, hi} kept in one 64-bit register pair.  sm_90 has no packed fp32
-// arithmetic, so every pair operation is two scalar IEEE fp32 instructions with the rounding mode
-// spelled out (ptxas keeps the halves in adjacent registers: packing and unpacking cost nothing).
-// Every operation here is a single correctly rounded fp32 op per lane: results are bit-identical
-// to the scalar __fmaf_rn / __fmul_rn / __fadd_rn sequence the oracle's MIRROR mode restates.
+// f32x2.cuh -- fp32 pairs {lo, hi}.  sm_90 has no packed fp32 arithmetic, so a pair is a plain two-float struct
+// (ptxas places its halves in any two registers) and every pair operation is two scalar IEEE fp32 instructions
+// with the rounding mode spelled out.  The pair helpers stay because the kernel is written as the operation
+// sequence the oracle's MIRROR mode restates, two channels at a time: every helper is one correctly rounded fp32
+// op per lane, bit-identical to the scalar __fmaf_rn / __fmul_rn / __fadd_rn sequence MIRROR spells out.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace dvo_b200 {
 
-typedef unsigned long long f2;  // {lo, hi} fp32 pair in an aligned 64-bit register pair
+struct f2 {  // {lo, hi} fp32 pair
+  float x, y;
+};
 
-__device__ __forceinline__ f2 pk(float lo, float hi) {
-  f2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ float lo(f2 v) { return __uint_as_float((unsigned)v); }
-__device__ __forceinline__ float hi(f2 v) { return __uint_as_float((unsigned)(v >> 32)); }
+__device__ __forceinline__ f2 pk(float lo, float hi) { return f2{lo, hi}; }
+__device__ __forceinline__ float lo(f2 v) { return v.x; }
+__device__ __forceinline__ float hi(f2 v) { return v.y; }
 __device__ __forceinline__ f2 bc(float s) { return pk(s, s); }
 __device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
   return pk(__fmaf_rn(lo(a), lo(b), lo(c)), __fmaf_rn(hi(a), hi(b), hi(c)));

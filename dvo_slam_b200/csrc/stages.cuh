@@ -157,7 +157,7 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
 template <int kOff>
 __device__ __forceinline__ f2 lds_f2(unsigned addr) {
   f2 v;
-  asm volatile("ld.shared.b64 %0, [%1+%2];" : "=l"(v) : "r"(addr), "n"(kOff));
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2+%3];" : "=f"(v.x), "=f"(v.y) : "r"(addr), "n"(kOff));
   return v;
 }
 __device__ __forceinline__ float lds_f32(unsigned addr) {
@@ -167,7 +167,7 @@ __device__ __forceinline__ float lds_f32(unsigned addr) {
 }
 __device__ __forceinline__ f2 lds_f2_at(unsigned addr) {
   f2 v;
-  asm volatile("ld.shared.b64 %0, [%1];" : "=l"(v) : "r"(addr));
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
   return v;
 }
 
@@ -401,7 +401,7 @@ __device__ __forceinline__ PixelProjection project_pixel(float tx, float ty, flo
   f2 uv = mul2(XY, bc(rcp_rn(p.Zt)));
   const float u = lo(uv), v = hi(uv);
   p.inb = u >= 0.f && u <= c.ubx && v >= 0.f && v <= c.uby;   // NaN compares false
-  uv = p.inb ? uv : 0ull;
+  uv = p.inb ? uv : bc(0.f);
   // truncation without conversions: for 0 <= t < 2^23, RZ(t + 2^23) carries floor(t) in its mantissa
   const f2 t = add2_rz(uv, bc(8388608.0f));
   p.f = sub2(uv, sub2(t, bc(8388608.0f)));
@@ -673,7 +673,7 @@ struct ScaleState {
 };
 
 __device__ __forceinline__ void scale_state_init(ScaleState& s) {
-  s.acc0 = s.acc1 = s.acc2 = 0ull;
+  s.acc0 = s.acc1 = s.acc2 = bc(0.f);
   s.pw = s.po0 = s.po1 = s.po2 = 0.f; s.wfirst = 0.f; s.psign = 0; s.cnt = 0; s.pend = false;
 }
 
@@ -831,36 +831,37 @@ struct StageBConsts {
 
 constexpr int kNormalValues = 28;   // log-likelihood sum, 21 upper-triangular A (row-major), 6 b
 
-// Accumulators of stage B for one thread.  A is kept as pairs of adjacent columns of one row
-// (A[r][2c], A[r][2c+1]); rows 1, 3 and 5 carry one redundant lower-triangle entry so that every
-// update is one fma2 of a broadcast row factor with a column pair.
-struct StageBAcc;
-__device__ __forceinline__ void stage_b_values(const StageBAcc& acc, float out[]);
+// Accumulators of stage B for one thread: the 21 entries of the upper triangle of A (row-major: A[r][c], c >= r, is
+// A[tri(r, c)]) and the 6 of b, one register each.
+constexpr int kTriValues = 21;
+__host__ __device__ constexpr int tri(int r, int c) { return r * 6 - r * (r - 1) / 2 + (c - r); }
 struct StageBAcc {
-  f2 r0[3], r1[3], r2[2], r3[2], r4, r5;   // 12 pairs
-  f2 b[3];
+  float A[kTriValues];
+  float b[6];
   float llsum;     // sum of log2(1 + 0.2 r^T P r) over this thread's kept points
 };
 
 __device__ __forceinline__ void stage_b_init(StageBAcc& a) {
 #pragma unroll
-  for (int i = 0; i < 3; ++i) { a.r0[i] = 0; a.r1[i] = 0; a.b[i] = 0; }
-  a.r2[0] = a.r2[1] = a.r3[0] = a.r3[1] = a.r4 = a.r5 = 0;
+  for (int i = 0; i < kTriValues; ++i) a.A[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < 6; ++i) a.b[i] = 0.f;
   a.llsum = 0.f;
 }
 
-// A += u v^T (upper triangle, column pairs) and b += u * s for one 6-vector given as three pairs V,
-// with u = V * wd.
+// A += u v^T (upper triangle) and b += u * s for one 6-vector v given as three pairs V, with u = v * wd.
 __device__ __forceinline__ void stage_b_rank1(StageBAcc& acc, const f2 V[3], float wd, float s) {
-  const f2 U0 = mul2(V[0], bc(wd)), U1 = mul2(V[1], bc(wd)), U2 = mul2(V[2], bc(wd));
-  const float u0 = lo(U0), u1 = hi(U0), u2 = lo(U1), u3 = hi(U1), u4 = lo(U2), u5 = hi(U2);
-  acc.r0[0] = fma2(bc(u0), V[0], acc.r0[0]); acc.r0[1] = fma2(bc(u0), V[1], acc.r0[1]); acc.r0[2] = fma2(bc(u0), V[2], acc.r0[2]);
-  acc.r1[0] = fma2(bc(u1), V[0], acc.r1[0]); acc.r1[1] = fma2(bc(u1), V[1], acc.r1[1]); acc.r1[2] = fma2(bc(u1), V[2], acc.r1[2]);
-  acc.r2[0] = fma2(bc(u2), V[1], acc.r2[0]); acc.r2[1] = fma2(bc(u2), V[2], acc.r2[1]);
-  acc.r3[0] = fma2(bc(u3), V[1], acc.r3[0]); acc.r3[1] = fma2(bc(u3), V[2], acc.r3[1]);
-  acc.r4 = fma2(bc(u4), V[2], acc.r4);
-  acc.r5 = fma2(bc(u5), V[2], acc.r5);
-  acc.b[0] = fma2(U0, bc(s), acc.b[0]); acc.b[1] = fma2(U1, bc(s), acc.b[1]); acc.b[2] = fma2(U2, bc(s), acc.b[2]);
+  const float v[6] = {lo(V[0]), hi(V[0]), lo(V[1]), hi(V[1]), lo(V[2]), hi(V[2])};
+  float u[6];
+#pragma unroll
+  for (int r = 0; r < 6; ++r) u[r] = __fmul_rn(v[r], wd);
+#pragma unroll
+  for (int r = 0; r < 6; ++r) {
+#pragma unroll
+    for (int c = r; c < 6; ++c) acc.A[tri(r, c)] = __fmaf_rn(u[r], v[c], acc.A[tri(r, c)]);
+  }
+#pragma unroll
+  for (int r = 0; r < 6; ++r) acc.b[r] = __fmaf_rn(u[r], s, acc.b[r]);
 }
 
 // One valid point: log-likelihood term and normal equations with W = w * P_k.
@@ -896,23 +897,41 @@ __device__ __forceinline__ void stage_b_pixel(StageBAcc& acc, const StageBConsts
   stage_b_rank1(acc, V1, wgt * c.wd1, -ez);
 }
 
+// Value k of the row's normal equations (k a compile-time index once unrolled): 0 = log-likelihood sum (the log2 terms
+// scaled by ln 2 once), 1..21 = A upper triangle (row-major), 22..27 = b, 28..31 = zero padding of the exchange.
+__device__ __forceinline__ float stage_b_value(const StageBAcc& acc, int k) {
+  return k == 0 ? acc.llsum * 0.69314718055994531f : k <= kTriValues ? acc.A[k - 1] : k < kNormalValues ? acc.b[k - 1 - kTriValues] : 0.f;
+}
+
+// One step of the halving exchange of flush_row_partial: a[0 .. 2 kHalf) -> a[0 .. kHalf), partner lane ^ kHalf.
+// A template, so that every index is a compile-time constant and the partial sums stay in registers.
+template <int kHalf>
+__device__ __forceinline__ void halving_step(float (&a)[16], int lane) {
+  const bool up = (lane & kHalf) != 0;
+#pragma unroll
+  for (int j = 0; j < kHalf; ++j) {
+    const float mine = up ? a[kHalf + j] : a[j];
+    const float send = up ? a[j] : a[kHalf + j];
+    a[j] = mine + __shfl_xor_sync(kFullMask, send, kHalf);
+  }
+}
+
 // Sum the kNormalValues accumulators of a row over the 32 lanes of its warp in a fixed order (halving exchange: partner
 // lane ^ 16, ^ 8, ... ^ 1; 31 shuffles instead of 5 x 28) and store the row's totals: lane l ends up with value l.
+// The first exchange reads the accumulators directly; the later ones halve the 16 partial sums in place.
 __device__ __forceinline__ void flush_row_partial(const StageBAcc& acc, int lane, float* row_out) {
-  float a[32];
-  stage_b_values(acc, a);
+  float a[16];
+  const bool up = (lane & 16) != 0;
 #pragma unroll
-  for (int i = kNormalValues; i < 32; ++i) a[i] = 0.f;
-#pragma unroll
-  for (int half = 16; half >= 1; half >>= 1) {
-    const bool up = (lane & half) != 0;
-#pragma unroll
-    for (int j = 0; j < half; ++j) {
-      const float mine = up ? a[half + j] : a[j];
-      const float send = up ? a[j] : a[half + j];
-      a[j] = mine + __shfl_xor_sync(kFullMask, send, half);
-    }
+  for (int j = 0; j < 16; ++j) {
+    const float mine = up ? stage_b_value(acc, 16 + j) : stage_b_value(acc, j);
+    const float send = up ? stage_b_value(acc, j) : stage_b_value(acc, 16 + j);
+    a[j] = mine + __shfl_xor_sync(kFullMask, send, 16);
   }
+  halving_step<8>(a, lane);
+  halving_step<4>(a, lane);
+  halving_step<2>(a, lane);
+  halving_step<1>(a, lane);
   if (lane < kNormalValues) row_out[lane] = a[0];
 }
 
@@ -1004,29 +1023,16 @@ __device__ __forceinline__ void stage_b_run(TilePipe& tp, const PairLevel& pl, c
           const float wall = student_weight(c, ei, ez);
           const float wgt = valid ? wall : 0.f;
           // (tx too: past a partial band it comes from shared memory no copy has written)
-          stage_b_pixel(acc, cb, wgt, keep, ei, ez, valid ? G : 0ull, valid ? H : 0ull, valid ? z : 1.0f, valid ? tx : 0.f, ty);
+          stage_b_pixel(acc, cb, wgt, keep, ei, ez, valid ? G : bc(0.f), valid ? H : bc(0.f), valid ? z : 1.0f, valid ? tx : 0.f, ty);
         }
       } else if (kDump && row_ok) {
-        for (int xl = lane; xl < bw; xl += 32) dump_record(dump, (size_t)y * gw + x0 + xl, false, 0ull, 0ull, 0ull, 0.f);
+        for (int xl = lane; xl < bw; xl += 32) dump_record(dump, (size_t)y * gw + x0 + xl, false, bc(0.f), bc(0.f), bc(0.f), 0.f);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive_s(tp_s + (unsigned)offsetof(TilePipe, empty) + bufi * 8u);
     }
     if (row_ok) flush_row_partial(acc, lane, row_partial + (size_t)y * kNormalValues);
   }
-}
-
-// flush the product of the pending log-likelihood terms and unpack: out[0] = ll sum,
-// out[1..21] = A upper triangle (row-major), out[22..27] = b
-__device__ __forceinline__ void stage_b_values(const StageBAcc& acc, float out[]) {
-  out[0] = acc.llsum * 0.69314718055994531f;
-  out[1] = lo(acc.r0[0]); out[2] = hi(acc.r0[0]); out[3] = lo(acc.r0[1]); out[4] = hi(acc.r0[1]); out[5] = lo(acc.r0[2]); out[6] = hi(acc.r0[2]);
-  out[7] = hi(acc.r1[0]); out[8] = lo(acc.r1[1]); out[9] = hi(acc.r1[1]); out[10] = lo(acc.r1[2]); out[11] = hi(acc.r1[2]);
-  out[12] = lo(acc.r2[0]); out[13] = hi(acc.r2[0]); out[14] = lo(acc.r2[1]); out[15] = hi(acc.r2[1]);
-  out[16] = hi(acc.r3[0]); out[17] = lo(acc.r3[1]); out[18] = hi(acc.r3[1]);
-  out[19] = lo(acc.r4); out[20] = hi(acc.r4);
-  out[21] = hi(acc.r5);
-  out[22] = lo(acc.b[0]); out[23] = hi(acc.b[0]); out[24] = lo(acc.b[1]); out[25] = hi(acc.b[1]); out[26] = lo(acc.b[2]); out[27] = hi(acc.b[2]);
 }
 
 __device__ __forceinline__ void load_stage_b_consts(const PairState& st, StageBConsts& c) {

@@ -790,7 +790,9 @@ struct GroupPlan {
 int level_squad_size(int nstrips, int nbands, int grid, int npairs) {
   const char* env = getenv("DVO_B200_STRIPS_PER_CTA");     // developer override (experiments)
   const int forced_spc = env ? atoi(env) : 0;
-  const double overhead_tiles = 20.0;   // per stage: squad barrier + serial step + pipeline fill, in tile-times (fitted: g = 2..5 within 1 % at batch 512, g >= 6 and g = 1 slower)
+  // per stage: squad barrier + serial step + pipeline fill, in tile-times.  Fitted on an H100 at batch 512 (DESIGN §6): level 0
+  // with g = 2 is 1.3 % faster than g = 3, g = 1 and g >= 4 are slower; the model picks g = 2 there for 43 .. 100.
+  const double overhead_tiles = 45.0;
   int best_g = 1;
   double best_cost = -1.0;
   for (int spc = 1; spc <= nstrips; ++spc) {
