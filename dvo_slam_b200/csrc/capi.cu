@@ -372,7 +372,7 @@ int dvo_b200_profile_read(dvo_b200_ctx* ctx, double ms_out[8], int64_t launches_
                       "wait-empty %.1f%% of its stage time\n", 100.0 * (double)v[9] / (double)(v[8] + 1), 100.0 * (double)v[11] / (double)(v[10] + 1),
               100.0 * (double)v[12] / (double)(v[14] + v[15] + 1), 100.0 * (double)v[13] / (double)(v[14] + v[15] + 1));
       const unsigned long long* u = h + 128 + 8 * l;
-      if (u[0]) fprintf(stderr, "[dvo_b200 timing]   tiles %llu (inexact %.2f%%, skipped %.2f%%), stage-B rounds of inexact tiles %.2f%%; CTA lifetime of the last launch-set: "
+      if (u[0]) fprintf(stderr, "[dvo_b200 timing]   tiles %llu (inexact %.2f%%, skipped %.2f%%), stage-B rounds in the generic loop %.2f%%; CTA lifetime of the last launch-set: "
                                 "max %.3f ms, min %.3f ms\n", u[0], 100.0 * (double)u[1] / (double)u[0], 100.0 * (double)u[2] / (double)u[0],
                         100.0 * (double)u[4] / (double)(u[3] + 1), (double)u[5] * 1e-6, (double)u[6] * 1e-6);
       const unsigned long long* e = h + 192 + 8 * l;   // e[7]: critical ns; e[0..5]: sub-phases

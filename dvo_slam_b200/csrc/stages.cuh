@@ -459,10 +459,12 @@ __device__ __forceinline__ float depth_sigma(float z) {
 }
 
 // Stage A pixel: (e.i, e.z) and validity from the four taps of (I, Z').
+// kExact: the caller knows the window is exact, so neither the hit test nor the gather path is compiled in.
+template <bool kExact>
 __device__ __forceinline__ bool residual_pixel(const PixelProjection& p, const WinView& wv, float Ir, float z, const StageConsts& c,
                                                float& ei, float& ez) {
   bool hit = true, any_miss = false;
-  if (!wv.exact) {   // warp-uniform
+  if (!kExact && !wv.exact) {   // warp-uniform
     hit = (unsigned)(p.u0 - wv.ulo) < (unsigned)wv.ucount && (unsigned)(p.v0 - wv.vlo) < (unsigned)wv.vcount;
     any_miss = __any_sync(kFullMask, p.inb && !hit);
   }
@@ -484,11 +486,12 @@ __device__ __forceinline__ bool residual_pixel(const PixelProjection& p, const W
 }
 
 // Stage B pixel: the full record from twelve taps of (I, Z): centre 2x2, the columns left and right of it and the
-// rows above and below it.
+// rows above and below it.  kExact as for residual_pixel.
+template <bool kExact>
 __device__ __forceinline__ bool record_pixel(const PixelProjection& p, const WinView& wv, float Ir, float z, f2 gref,
                                              const StageConsts& c, f2& E, f2& G, f2& H) {
   bool hit = true, any_miss = false;
-  if (!wv.exact) {   // warp-uniform
+  if (!kExact && !wv.exact) {   // warp-uniform
     hit = (unsigned)(p.u0 - wv.ulo) < (unsigned)wv.ucount && (unsigned)(p.v0 - wv.vlo) < (unsigned)wv.vcount;
     any_miss = __any_sync(kFullMask, p.inb && !hit);
   }
@@ -653,8 +656,8 @@ __device__ __forceinline__ SegT<double> combine_strip_exports_warp(const double*
 
 // Student-t weight of computeWeightsSse (dense_tracking_impl.cpp:657-707): w = 7 / (5 + r^T P r), nu = 5;
 // w = 1 on the first iteration of a level (dense_tracking.cpp:286-289).
-__device__ __forceinline__ float student_weight(const StageConsts& c, float ei, float ez) {
-  if (c.first_iteration) return 1.0f;
+__device__ __forceinline__ float student_weight(const StageConsts& c, bool first_iteration, float ei, float ez) {
+  if (first_iteration) return 1.0f;
   const f2 q = fma2(bc(ez), c.Pb, mul2(bc(ei), c.Pa));        // (ei P00 + ez P10, ei P01 + ez P11)
   const float d = fmaf(lo(q), ei, hi(q) * ez);
   return 7.0f * rcp_fast(5.0f + d);
@@ -752,6 +755,44 @@ __device__ __forceinline__ WinView make_view(unsigned bufs, const int4& d0, cons
   wv.w = w; wv.h = h; wv.pitch = pitch;
   return wv;
 }
+
+// The pixel rounds of one tile row come in two loops, chosen per tile (warp-uniform) from the tile descriptor:
+//   kExact = true : the window is exact and the tile covers a full band of kTileW columns, which is almost every tile.  The
+//                   loop has no hit test, no vote, no gather code and no band mask, and reads only base / safe (and w, in
+//                   stage B) of the view; the first-iteration case of the Student-t weight is kFirst, fixed outside the loop.
+//   kExact = false: every other tile -- inexact windows, corners behind the camera, partial bands (kFirst is unused; the
+//                   weight reads c.first_iteration).
+// Both loops call the same pixel functions in the same order, so they compute the same bits.
+
+// Stage A rounds of one tile row: two rounds per trip, whose projection / tap / blend chains are independent and interleave.
+template <bool kExact, bool kFirst>
+__device__ __forceinline__ void stage_a_rounds(const WinView& wv, int bw, unsigned refa, unsigned txa, float ty, const StageConsts& c,
+                                               ScaleState& ss, int lane, unsigned lt_mask) {
+  static_assert(kTileW % 64 == 0, "the exact loop takes whole pairs of rounds");
+  const int nr = kExact ? kTileW / 32 : (bw + 31) >> 5;
+  const int xlim = bw - lane;        // lane's column r*32+lane is inside the band iff r*32 < xlim
+  const bool first = kExact ? kFirst : c.first_iteration != 0;
+#pragma unroll 1
+  for (int r = 0; r < nr; r += 2, refa += 512, txa += 256) {
+    const bool second = kExact || r + 1 < nr;                       // warp-uniform
+    const f2 rz0 = lds_f2_at(refa);
+    const f2 rz1 = second ? lds_f2_at(refa + 256) : pk(0.f, __int_as_float(0x7fc00000));
+    const float tx0 = lds_f32(txa), tx1 = second ? lds_f32(txa + 128) : 0.f;
+    float z0 = hi(rz0), z1 = hi(rz1);
+    if (!kExact && bw < kTileW) {   // past a partial band: not this band's pixels
+      z0 = (r * 32 < xlim) ? z0 : __int_as_float(0x7fc00000);
+      z1 = (r * 32 + 32 < xlim) ? z1 : __int_as_float(0x7fc00000);
+    }
+    const PixelProjection p0 = project_pixel(tx0, ty, z0, c);
+    const PixelProjection p1 = project_pixel(tx1, ty, z1, c);
+    float ei0, ez0, ei1, ez1;
+    const bool v0 = residual_pixel<kExact>(p0, wv, lo(rz0), z0, c, ei0, ez0);
+    const bool v1 = residual_pixel<kExact>(p1, wv, lo(rz1), z1, c, ei1, ez1);
+    const float w0 = student_weight(c, first, ei0, ez0), w1 = student_weight(c, first, ei1, ez1);
+    scale_round32(ss, lane, lt_mask, v0, w0, ei0, ez0);
+    scale_round32(ss, lane, lt_mask, v1, w1, ei1, ez1);
+  }
+}
 // Stage A over this CTA's strips: warp q walks image row strip*kTileH + q band by band, carries the pairwise
 // scale state across the bands (they are consecutive pixels of the row) and writes one segment summary per row
 // to row_exports[y * kSegExportFloats].  Warp kConsumerWarps is the producer: it stages the same tiles, kStages ahead.
@@ -790,30 +831,12 @@ __device__ __forceinline__ void stage_a_run(TilePipe& tp, const PairLevel& pl, c
       if (row_ok && !d0.x) {
         const int4 d1 = lds_i4(tp_s + (unsigned)offsetof(TilePipe, desc) + bufi * 32u + 16u);
         const WinView wv = make_view(bufs, d0, d1, pl.c0, gw, gh, gpitch);
-        const int nr = (bw + 31) >> 5;
-        unsigned refa = bufs + my_ref;
-        unsigned txa = bufs + my_tx;
-        const int xlim = bw - lane;        // lane's column r*32+lane is inside the band iff r*32 < xlim
-        // two rounds per trip: their projection / tap / blend chains are independent and interleave
-#pragma unroll 1
-        for (int r = 0; r < nr; r += 2, refa += 512, txa += 256) {
-          const bool second = r + 1 < nr;                       // warp-uniform
-          const f2 rz0 = lds_f2_at(refa);
-          const f2 rz1 = second ? lds_f2_at(refa + 256) : pk(0.f, __int_as_float(0x7fc00000));
-          const float tx0 = lds_f32(txa), tx1 = second ? lds_f32(txa + 128) : 0.f;
-          float z0 = hi(rz0), z1 = hi(rz1);
-          if (bw < kTileW) {   // past a partial band: not this band's pixels
-            z0 = (r * 32 < xlim) ? z0 : __int_as_float(0x7fc00000);
-            z1 = (r * 32 + 32 < xlim) ? z1 : __int_as_float(0x7fc00000);
-          }
-          const PixelProjection p0 = project_pixel(tx0, ty, z0, c);
-          const PixelProjection p1 = project_pixel(tx1, ty, z1, c);
-          float ei0, ez0, ei1, ez1;
-          const bool v0 = residual_pixel(p0, wv, lo(rz0), z0, c, ei0, ez0);
-          const bool v1 = residual_pixel(p1, wv, lo(rz1), z1, c, ei1, ez1);
-          const float w0 = student_weight(c, ei0, ez0), w1 = student_weight(c, ei1, ez1);
-          scale_round32(ss, lane, lt_mask, v0, w0, ei0, ez0);
-          scale_round32(ss, lane, lt_mask, v1, w1, ei1, ez1);
+        const unsigned refa = bufs + my_ref, txa = bufs + my_tx;
+        if (wv.exact && bw == kTileW) {   // warp-uniform
+          if (c.first_iteration) stage_a_rounds<true, true>(wv, bw, refa, txa, ty, c, ss, lane, lt_mask);
+          else stage_a_rounds<true, false>(wv, bw, refa, txa, ty, c, ss, lane, lt_mask);
+        } else {
+          stage_a_rounds<false, false>(wv, bw, refa, txa, ty, c, ss, lane, lt_mask);
         }
       }
       __syncwarp();
@@ -950,6 +973,43 @@ __device__ __noinline__ void dump_record(const RecordDump& dump, size_t i, bool 
   p[6 * n] = valid ? z : nanv;
 }
 
+// Stage B rounds of one tile row (kExact, kFirst: see stage_a_rounds).  The exact loop also leaves out the rank count of the
+// dropped log-likelihood tail: strips that reach past n_keep (cta_has_tail, at most a few per level) take the generic loop.
+// pix: dump index of the lane's pixel in round 0.
+template <bool kExact, bool kFirst, bool kDump>
+__device__ __forceinline__ void stage_b_rounds(const WinView& wv, int bw, unsigned refa, unsigned txa, float ty, const StageConsts& c,
+                                               const StageBConsts& cb, StageBAcc& acc, bool cta_has_tail, int& rank, int keep_rank,
+                                               const RecordDump& dump, size_t pix, int lane, unsigned lt_mask, PipeTiming& tm) {
+  const int nr = kExact ? kTileW / 32 : (bw + 31) >> 5;
+  const int xlim = bw - lane;
+  const bool first = kExact ? kFirst : c.first_iteration != 0;
+#pragma unroll 1
+  for (int r = 0; r < nr; ++r, refa += 256, txa += 128) {
+    const f2 rz = lds_f2_at(refa);
+    const f2 gr = lds_f2<sizeof(float2) * kRecP1>(refa);              // the gradient rows of the record
+    const float tx = lds_f32(txa);
+    float z = hi(rz);
+    if (!kExact && bw < kTileW) z = (r * 32 < xlim) ? z : __int_as_float(0x7fc00000);
+    const PixelProjection p = project_pixel(tx, ty, z, c);
+    f2 E, G, H;
+    const bool valid = record_pixel<kExact>(p, wv, lo(rz), z, gr, c, E, G, H);
+    DVO_ADD(tm, rounds, 1); DVO_ADD(tm, slow_rounds, kExact ? 0 : 1);
+    bool keep = valid;
+    if (!kExact && cta_has_tail) {   // warp-uniform
+      const unsigned m = __ballot_sync(kFullMask, valid);
+      keep = valid && (rank + __popc(m & lt_mask)) < keep_rank;
+      rank += __popc(m);
+    }
+    if (kDump && r * 32 < xlim) dump_record(dump, pix + r * 32, valid, E, G, H, z);
+    // rejected points: zero weight and finite stand-ins (their own values may be NaN)
+    const float ei = valid ? lo(E) : 0.f, ez = valid ? hi(E) : 0.f;
+    const float wall = student_weight(c, first, ei, ez);
+    const float wgt = valid ? wall : 0.f;
+    // (tx too: past a partial band it comes from shared memory no copy has written)
+    stage_b_pixel(acc, cb, wgt, keep, ei, ez, valid ? G : bc(0.f), valid ? H : bc(0.f), valid ? z : 1.0f, valid ? tx : 0.f, ty);
+  }
+}
+
 // Stage B over this CTA's strips.  row_base[y]: number of valid points before row y inside this CTA (only read
 // when this CTA holds the tail of the point list); points with rank >= n_keep are the dropped tail of
 // computeCompleteDataLogLikelihood (dense_tracking_impl.cpp:413-422).
@@ -996,34 +1056,15 @@ __device__ __forceinline__ void stage_b_run(TilePipe& tp, const PairLevel& pl, c
       if (row_ok && !d0.x) {
         const int4 d1 = lds_i4(tp_s + (unsigned)offsetof(TilePipe, desc) + bufi * 32u + 16u);
         const WinView wv = make_view(bufs, d0, d1, pl.c3, gw, gh, gpitch);
-        const int nr = (bw + 31) >> 5;
-        unsigned refa = bufs + my_ref;
-        unsigned txa = bufs + my_tx;
-        const int xlim = bw - lane;
-#pragma unroll 1
-        for (int r = 0; r < nr; ++r, refa += 256, txa += 128) {
-          const f2 rz = lds_f2_at(refa);
-          const f2 gr = lds_f2<sizeof(float2) * kRecP1>(refa);              // the gradient rows of the record
-          const float tx = lds_f32(txa);
-          float z = hi(rz);
-          if (bw < kTileW) z = (r * 32 < xlim) ? z : __int_as_float(0x7fc00000);
-          const PixelProjection p = project_pixel(tx, ty, z, c);
-          f2 E, G, H;
-          const bool valid = record_pixel(p, wv, lo(rz), z, gr, c, E, G, H);
-          DVO_ADD(tm, rounds, 1); DVO_ADD(tm, slow_rounds, wv.exact ? 0 : 1);
-          bool keep = valid;
-          if (cta_has_tail) {   // warp-uniform
-            const unsigned m = __ballot_sync(kFullMask, valid);
-            keep = valid && (rank + __popc(m & lt_mask)) < keep_rank;
-            rank += __popc(m);
-          }
-          if (kDump && r * 32 < xlim) dump_record(dump, (size_t)y * gw + x0 + r * 32 + lane, valid, E, G, H, z);
-          // rejected points: zero weight and finite stand-ins (their own values may be NaN)
-          const float ei = valid ? lo(E) : 0.f, ez = valid ? hi(E) : 0.f;
-          const float wall = student_weight(c, ei, ez);
-          const float wgt = valid ? wall : 0.f;
-          // (tx too: past a partial band it comes from shared memory no copy has written)
-          stage_b_pixel(acc, cb, wgt, keep, ei, ez, valid ? G : bc(0.f), valid ? H : bc(0.f), valid ? z : 1.0f, valid ? tx : 0.f, ty);
+        const unsigned refa = bufs + my_ref, txa = bufs + my_tx;
+        const size_t pix = (size_t)y * gw + x0 + lane;
+        if (wv.exact && bw == kTileW && !cta_has_tail) {   // warp-uniform
+          if (c.first_iteration)
+            stage_b_rounds<true, true, kDump>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank, dump, pix, lane, lt_mask, tm);
+          else
+            stage_b_rounds<true, false, kDump>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank, dump, pix, lane, lt_mask, tm);
+        } else {
+          stage_b_rounds<false, false, kDump>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank, dump, pix, lane, lt_mask, tm);
         }
       } else if (kDump && row_ok) {
         for (int xl = lane; xl < bw; xl += 32) dump_record(dump, (size_t)y * gw + x0 + xl, false, bc(0.f), bc(0.f), bc(0.f), 0.f);

@@ -371,7 +371,7 @@ struct Segment {
   int cyclic;             // 1: CTA r of a squad takes strips r, r + g, ...; 0: contiguous ranges of strips_per_cta strips
   int pair_begin;         // segments >= 1 of a fused launch own the pairs [pair_begin, pair_begin + npairs_seg)
   int npairs_seg;         // pairs handed out by this segment's queue
-  unsigned long long* dbg2;  // optional (timing build): {tiles, inexact tiles, skipped tiles, rounds, rounds of inexact tiles, max / min CTA lifetime}
+  unsigned long long* dbg2;  // optional (timing build): {tiles, inexact tiles, skipped tiles, rounds, stage-B rounds in the generic loop, max / min CTA lifetime}
   unsigned long long* dbg;   // optional: ns spent per CTA in {stage A, stage B, wait A, wait B, mid, end, queue, total}
   int nlev;               // pyramid levels of the segment (coarse to fine)
   int g, nsquads;
