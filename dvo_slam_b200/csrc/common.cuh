@@ -113,7 +113,8 @@ namespace dvo_b200 {
 
 // ---- per-pair device state ---------------------------------------------------------------------
 struct PairLevel {              // what one alignment reads at the current level (uploaded per level)
-  const float2* r0; const float2* r1;  // reference tile records of the level (r1: unused, kept for layout)
+  const float2* r0;                    // reference tile records of the level
+  const float2* rp0;                   // the reference's own P0 = (I, Z') plane (corrected estimator: depth of the odd last point)
   const uint32_t* rmask;               // reference selection mask
   const int* rsel;                     // {S, last selected pixel}
   const float* rtmpl;                  // tx[w], ty[h]
@@ -181,6 +182,7 @@ struct Workspace {              // per-ctx scratch of the level kernel
 struct dvo_b200_ctx {
   int device = 0;
   int num_sms = 0, ctas_per_sm = 0;   // persistent-kernel grid geometry (queried once)
+  int estimator = DVO_B200_ESTIMATOR_REFERENCE;   // dvo_b200_estimator of every later alignment / test hook on this context
   unsigned long long* d_dbg = nullptr;   // DVO_B200_TIMING=1: per-level phase timers of the persistent kernel (64 slots)
   cudaStream_t stream = nullptr;
   bool own_stream = false;

@@ -120,6 +120,8 @@ __global__ void k_stage_words(const uint4* __restrict__ src, uint4* __restrict__
 
 // one warp per pair: combine the strip summaries of the level in order -> covariance -> P_k (dense_tracking.cpp:276-295).
 // e: the level's nstrips strip summaries; strip_base: nstrips + 1 exclusive prefixes of their valid counts (output).
+// kCorrected: the summaries hold the plain sum of w r r^T (no pairing, no odd tail term) and every point is kept.
+template <bool kCorrected>
 __device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double* e, int* strip_base, int nstrips, int* active,
                                            const LevelLaunch& lp, dvo_b200_iteration_stats* ilog, int max_log, SegCombineSmem& sm) {
   const int lane = threadIdx.x & 31;
@@ -127,7 +129,7 @@ __device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double
   if (lane == 0) {
     long long n = all.n;
     st.n = n;
-    st.n_keep = (n / 50) * 50;
+    st.n_keep = kCorrected ? n : (n / 50) * 50;
     LevelSummary& ls = st.levels[lp.level_index];
     ls.num_iterations += 1;   // level_stats.Iterations.push_back (dense_tracking.cpp:249)
     ls.last_n = n;
@@ -153,7 +155,7 @@ __device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double
     } else {
       // tail term for odd n, normaliser 1/(n-3) (dense_tracking_impl.cpp:596), symmetric 2x2
       double c[3];
-      bool tail = ((n - 1) & 1) == 0;
+      const bool tail = !kCorrected && ((n - 1) & 1) == 0;
       double s = 1.0 / (double)(n - 3);
       for (int k = 0; k < 3; ++k) c[k] = (all.S0[k] + (tail ? all.wl * all.ol[k] : 0.0)) * s;
       float C0 = (float)c[0], C1 = (float)c[1], C3 = (float)c[2];
@@ -435,6 +437,8 @@ __device__ __forceinline__ void squad_wait(SquadState* sq, unsigned episode, int
   __syncthreads();
 }
 
+// kCorrected: the corrected estimator (dvo_b200_estimator), one instance per value, chosen per launch.
+template <bool kCorrected>
 __global__ void __launch_bounds__(kCtaThreads, 2)
 k_level_persistent(const __grid_constant__ PersistentArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -555,7 +559,7 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
         StageConsts c;
         load_stage_consts(st, pl, lp.w, lp.h, false, c);
         const long long ts0 = DVO_CLOCK(tm);
-        stage_a_run(tp, pl, geo, c, row_exports, tile_count, a.error_flag, tm);
+        stage_a_run<kCorrected>(tp, pl, geo, c, row_exports, tile_count, a.error_flag, tm);
         DVO_ADD(tm, rounds_a, DVO_CLOCK(tm) - ts0);
       }
       __syncthreads();
@@ -569,7 +573,7 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
       if (squad_arrive(sq, episode, S.g, lt.s_flag)) {
         DVO_TOCK(2);
         if (warp == 0) {
-          pair_mid_warp(st, pair, strip_exports, strip_base, lp.nstrips, nullptr, lp, a.ilog, a.max_log, lt.comb);
+          pair_mid_warp<kCorrected>(st, pair, strip_exports, strip_base, lp.nstrips, nullptr, lp, a.ilog, a.max_log, lt.comb);
           if (lane == 0) squad_release(sq, episode);
         }
         __syncthreads();
@@ -592,8 +596,8 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
         RecordDump dump;
         dump.planes = a.dump; dump.n = lp.n;
         const long long ts0 = DVO_CLOCK(tm);
-        if (a.dump) stage_b_run<true>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
-        else stage_b_run<false>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
+        if (a.dump) stage_b_run<true, kCorrected>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
+        else stage_b_run<false, kCorrected>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
         DVO_ADD(tm, rounds_b, DVO_CLOCK(tm) - ts0);
       }
       __syncthreads();
@@ -762,9 +766,14 @@ int ensure_geometry(dvo_b200_ctx* ctx) {
   if (ctx->num_sms != 0) return 0;
   cudaDeviceProp prop;
   DVO_CUDA(ctx, cudaGetDeviceProperties(&prop, ctx->device));
-  DVO_CUDA(ctx, cudaFuncSetAttribute(k_level_persistent, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLevelSmemBytes));
-  int per_sm = 0;
-  DVO_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_level_persistent, kCtaThreads, kLevelSmemBytes));
+  // one grid for both estimator instances: the smaller of their occupancies (both are bounded to 128 registers, so equal)
+  int per_sm = 1 << 30;
+  for (auto kern : {k_level_persistent<false>, k_level_persistent<true>}) {
+    DVO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLevelSmemBytes));
+    int k_per_sm = 0;
+    DVO_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k_per_sm, kern, kCtaThreads, kLevelSmemBytes));
+    per_sm = std::min(per_sm, k_per_sm);
+  }
   if (per_sm < 1) return set_error(ctx, DVO_B200_ERR_CUDA, "persistent kernel does not fit on an SM");
   ctx->ctas_per_sm = per_sm;
   ctx->num_sms = prop.multiProcessorCount;
@@ -881,7 +890,7 @@ void fill_pair_levels(PairLevel* h, int n, dvo_b200_pyramid* const* refs, dvo_b2
     const LevelInfo& cl = c->L[level];
     PairLevel& q = h[i];
     const size_t plane = (size_t)rl.pitch * rl.h;
-    q.r0 = r->planes + rl.rec_off; q.r1 = q.r0;
+    q.r0 = r->planes + rl.rec_off; q.rp0 = r->planes + rl.plane_off;
     q.rmask = r->sel_mask + rl.mask_off;
     q.rsel = r->sel_info + 2 * level;
     q.rtmpl = r->tmpl + rl.tmpl_off;
@@ -985,7 +994,9 @@ int launch_segments(dvo_b200_ctx* ctx, int nseg, const LevelLaunch (*lps)[kMaxLe
     ProfScope prof(ctx, 0);
     ProfScope prof_level(ctx, 8 + std::min(group_index, 7));
     void* args[] = {&pa};
-    DVO_CUDA(ctx, cudaLaunchCooperativeKernel((const void*)k_level_persistent, dim3(ctx->num_sms * ctx->ctas_per_sm),
+    const void* kern = ctx->estimator == DVO_B200_ESTIMATOR_CORRECTED ? (const void*)k_level_persistent<true>
+                                                                      : (const void*)k_level_persistent<false>;
+    DVO_CUDA(ctx, cudaLaunchCooperativeKernel(kern, dim3(ctx->num_sms * ctx->ctas_per_sm),
                                               dim3(kCtaThreads), args, kLevelSmemBytes, st));
     ctx->launches++;
   }

@@ -29,7 +29,11 @@ ABI_SYMBOLS = [
     "dvo_b200_profile_read", "dvo_b200_pyramid_device", "dvo_b200_sharded_create", "dvo_b200_sharded_destroy",
     "dvo_b200_sharded_num_shards", "dvo_b200_sharded_ctx", "dvo_b200_sharded_last_error", "dvo_b200_shard_range",
     "dvo_b200_sharded_pyramid_create_batch", "dvo_b200_sharded_pyramid_create_raw_batch", "dvo_b200_match_batch_sharded",
+    "dvo_b200_set_estimator", "dvo_b200_get_estimator",
 ]
+
+# dvo_b200_estimator
+ESTIMATORS = {"reference": 0, "corrected": 1}
 
 
 class Config(C.Structure):
@@ -147,6 +151,8 @@ def load_library():
     L.dvo_b200_residual_image.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, fp, C.POINTER(i64)]
     L.dvo_b200_intensity_error_image.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, fp, C.POINTER(i64)]
     L.dvo_b200_linearize.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, i32, fp, C.POINTER(i64), fp, fp, dp, dp]
+    L.dvo_b200_set_estimator.argtypes = [vp, i32]
+    L.dvo_b200_get_estimator.argtypes = [vp]
     L.dvo_b200_profile_enable.argtypes = [vp, i32]
     L.dvo_b200_profile_read.argtypes = [vp, dp, C.POINTER(i64), i32]
     _lib = L
@@ -197,10 +203,14 @@ class Pyramid:
 
 
 class Engine:
-    """One dvo_b200_ctx (one CUDA stream on one device)."""
+    """One dvo_b200_ctx (one CUDA stream on one device).  estimator: "reference" (dvo::DenseTracker::match()'s numbers) or
+    "corrected" (the same algorithm without the reference's scale-pairing, log-likelihood-tail and odd-point quirks; see
+    dvo_b200_estimator in include/dvo_b200.h).  It applies to every later call on the engine."""
 
-    def __init__(self, device: int = 0, stream: int | None = None):
+    def __init__(self, device: int = 0, stream: int | None = None, estimator: str = "reference"):
         self.lib = load_library()
+        if estimator not in ESTIMATORS:
+            raise ValueError(f"unknown estimator {estimator!r}: one of {sorted(ESTIMATORS)}")
         ctx = C.c_void_p()
         rc = self.lib.dvo_b200_create(device, C.c_void_p(stream) if stream else None, C.byref(ctx))
         if rc != 0:
@@ -208,6 +218,18 @@ class Engine:
                                "(the engine has no CPU fallback)")
         self.ctx = ctx
         self.device = device
+        self.set_estimator(estimator)
+
+    def set_estimator(self, estimator: str):
+        if estimator not in ESTIMATORS:
+            raise ValueError(f"unknown estimator {estimator!r}: one of {sorted(ESTIMATORS)}")
+        self._check(self.lib.dvo_b200_set_estimator(self.ctx, ESTIMATORS[estimator]))
+
+    @property
+    def estimator(self) -> str:
+        e = self.lib.dvo_b200_get_estimator(self.ctx)
+        self._check(min(e, 0))
+        return {v: k for k, v in ESTIMATORS.items()}[e]
 
     def close(self):
         if getattr(self, "ctx", None):
@@ -424,6 +446,14 @@ class ShardedEngine:
     def _check(self, rc):
         if rc != 0:
             raise RuntimeError(f"dvo_b200 sharded status {rc}: {self.lib.dvo_b200_sharded_last_error(self.h).decode()}")
+
+    def set_estimator(self, estimator: str):
+        """the estimator of every shard's context (see Engine)"""
+        if estimator not in ESTIMATORS:
+            raise ValueError(f"unknown estimator {estimator!r}: one of {sorted(ESTIMATORS)}")
+        for k in range(len(self.devices)):
+            ctx = self.lib.dvo_b200_sharded_ctx(self.h, k)
+            self._check(self.lib.dvo_b200_set_estimator(ctx, ESTIMATORS[estimator]))
 
     def shard_range(self, total, shard):
         b, e = C.c_int64(), C.c_int64()

@@ -151,9 +151,17 @@ const DenseTracker::Config& DenseTracker::getDefaultConfig() {
   return c;
 }
 
-DenseTracker::DenseTracker(const Config& config) : ctx_(0), collect_iterations_(false), reference_selection_(selection_predicate_) { configure(config); }
-DenseTracker::DenseTracker(const DenseTracker& other) : ctx_(0), collect_iterations_(other.collect_iterations_), reference_selection_(selection_predicate_) {
+DenseTracker::DenseTracker(const Config& config)
+    : ctx_(0), collect_iterations_(false), corrected_estimator_(false), reference_selection_(selection_predicate_) { configure(config); }
+DenseTracker::DenseTracker(const DenseTracker& other)
+    : ctx_(0), collect_iterations_(other.collect_iterations_), corrected_estimator_(other.corrected_estimator_),
+      reference_selection_(selection_predicate_) {
   configure(other.configuration());
+}
+
+void DenseTracker::useCorrectedEstimator(bool on) {
+  corrected_estimator_ = on;
+  if (ctx_) dvo_b200_set_estimator(ctx_, on ? DVO_B200_ESTIMATOR_CORRECTED : DVO_B200_ESTIMATOR_REFERENCE);
 }
 DenseTracker::~DenseTracker() {
   if (ctx_) dvo_b200_destroy(ctx_);
@@ -171,6 +179,7 @@ dvo_b200_ctx* DenseTracker::context() {
     const char* dev = std::getenv("DVO_B200_DEVICE");
     int rc = dvo_b200_create(dev ? std::atoi(dev) : 0, 0, &ctx_);
     if (rc != 0) throw std::runtime_error("dvo_b200_create failed: no usable CUDA device (the engine has no CPU fallback)");
+    if (corrected_estimator_) dvo_b200_set_estimator(ctx_, DVO_B200_ESTIMATOR_CORRECTED);
   }
   return ctx_;
 }

@@ -106,12 +106,16 @@ class DenseTracker {
 
   // per-iteration statistics are copied back only when requested (they are optional in the C ABI)
   void collectIterationStatistics(bool on) { collect_iterations_ = on; }
+  // Extension: the corrected estimator of dvo_b200_estimator (exact scale sum, log-likelihood over all points, the odd last
+  // point kept) for every later match of this tracker.  Off by default (the reference's numbers); kept across configure().
+  void useCorrectedEstimator(bool on);
 
  private:
   dvo_b200_ctx* context();
   Config cfg;
   dvo_b200_ctx* ctx_;
   bool collect_iterations_;
+  bool corrected_estimator_;
   core::ValidPointAndGradientThresholdPredicate selection_predicate_;
   core::PointSelection reference_selection_;
 };

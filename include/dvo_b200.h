@@ -93,6 +93,21 @@ typedef struct dvo_b200_result {
   dvo_b200_level_stats levels[DVO_B200_MAX_LEVELS];
 } dvo_b200_result;
 
+/* The estimator of the alignments on a context (dvo_b200_set_estimator).
+ * REFERENCE (default): what dvo::DenseTracker::match() computes, including three structural quirks of its SSE code:
+ *   the scale estimate adds w2 r1 r1^T instead of w2 r2 r2^T for every pair of points (dense_tracking_impl.cpp:614-615),
+ *   the log-likelihood drops the last n mod 50 terms (dense_tracking_impl.cpp:413-422), and the last point of an odd
+ *   selection is never visited (dense_tracking_impl.cpp:169).
+ * CORRECTED: the same algorithm without those three: scale = sum_i w_i r_i r_i^T / (n - 3), the log-likelihood over all
+ *   n points, and the odd last point is a constraint like any other.  Everything else is unchanged (Student-t weights with
+ *   nu = 5 and P_{k-1}, the 1/(n-3) normaliser, the float log-likelihood, Jacobians at the untransformed point, the accept
+ *   test, LDL^T, SE(3) update, termination; LevelStats.valid_pixels is still the selection count S).  Results differ from
+ *   the reference's: this is for callers that want the estimator of the DVO papers, not a libdvo_core replacement. */
+typedef enum dvo_b200_estimator {
+  DVO_B200_ESTIMATOR_REFERENCE = 0,
+  DVO_B200_ESTIMATOR_CORRECTED = 1
+} dvo_b200_estimator;
+
 typedef struct dvo_b200_ctx dvo_b200_ctx;          /* one per host thread / CUDA stream */
 typedef struct dvo_b200_pyramid dvo_b200_pyramid;  /* device mirror of dvo::core::RgbdImagePyramid */
 
@@ -109,6 +124,14 @@ void dvo_b200_config_default(dvo_b200_config* cfg);   /* DenseTracker::getDefaul
 int64_t dvo_b200_kernel_launches(dvo_b200_ctx* ctx);
 int64_t dvo_b200_h2d_bytes(dvo_b200_ctx* ctx);
 int64_t dvo_b200_d2h_bytes(dvo_b200_ctx* ctx);
+/* Estimator of every later call on ctx: match, match_batch[_device], and the test hooks residual_image, linearize and
+ * intensity_error_image, which run the same kernel (in CORRECTED mode the odd last point appears in their outputs).  A
+ * sharded caller sets it on each dvo_b200_sharded_ctx(s, i).  Pyramids are not touched: contexts with different
+ * estimators may align against the same pyramids at the same time.  An unknown value or a NULL ctx ->
+ * DVO_B200_ERR_INVALID_ARGUMENT (the setting is unchanged). */
+int dvo_b200_set_estimator(dvo_b200_ctx* ctx, int32_t estimator);
+/* the ctx's dvo_b200_estimator, or DVO_B200_ERR_INVALID_ARGUMENT for a NULL ctx */
+int dvo_b200_get_estimator(const dvo_b200_ctx* ctx);
 
 /* ---- image pyramid (replaces RgbdCameraPyramid::create + RgbdImagePyramid::build +
  *      RgbdImage::buildAccelerationStructure, rgbd_image.cpp:156-172,283-296,534-543) ---------- */
@@ -214,7 +237,8 @@ int dvo_b200_residual_image(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b
                             int64_t* count);
 /* DenseTracker::computeIntensityErrorImage (dense_tracking.cpp:378-444): image = h*w floats on the host,
  * |intensity residual| at every selected reference pixel whose warped residual is valid, 0 elsewhere (the odd
- * last selected point included: the reference's SSE residual loop never visits it).  T as above; the selection
+ * last selected point included: the reference's SSE residual loop never visits it; with DVO_B200_ESTIMATOR_CORRECTED it
+ * is a constraint like any other and appears here and in dvo_b200_residual_image).  T as above; the selection
  * thresholds come from cfg.  *count (optional) = residuals written. */
 int dvo_b200_intensity_error_image(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,
                                    dvo_b200_pyramid* current, int32_t level, const double* T, float* image,
