@@ -139,7 +139,9 @@ __device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double
       st.initial = st.initial_old; st.estimate = st.estimate_old;
       st.termination = DVO_B200_TERM_TOO_FEW_CONSTRAINTS;
       st.phase_ok = 0;
+      // the reference's entry is value-initialised apart from ValidConstraints: log-likelihoods and precision are 0
       st.nll_cur = 0; st.prior_cur = 0;
+      for (int i = 0; i < 4; ++i) st.precision[i] = 0.f;
       log_iteration(ilog, max_log, pair, st, st.iteration, lp.level_id, false);
       // post-loop checks of dense_tracking.cpp:359-363 still apply
       double m = 0; bool nanx = false;
@@ -149,6 +151,8 @@ __device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double
       ls.termination = st.termination;
       ls.has_inc = ls.num_iterations >= 2;   // HasIterationWithIncrement (dense_tracking_config.cpp:138-143)
       if (st.termination != DVO_B200_TERM_TOO_FEW_CONSTRAINTS) ls.has_inc = ls.num_iterations >= 1;
+      // LastIterationWithIncrement is Iterations.back() for every termination but LogLikelihoodDecreased: this entry
+      if (ls.has_inc) { ls.last_inc_n = n; ls.last_inc_nll = 0.0; }
       st.have_done = (st.termination == DVO_B200_TERM_TOO_FEW_CONSTRAINTS) ? -1 : st.have_done;
       st.level_active = 0;
       if (active) atomicSub(active, 1);

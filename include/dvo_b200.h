@@ -79,6 +79,9 @@ typedef struct dvo_b200_level_stats {
   int32_t num_iterations;               /* Iterations.size() */
   int32_t has_iteration_with_increment; /* LevelStats::HasIterationWithIncrement (dense_tracking_config.cpp:138-143) */
   int64_t last_valid_constraints;       /* Iterations.back().ValidConstraints */
+  /* LastIterationWithIncrement() (dense_tracking_config.cpp:145-155) is Iterations[size-2] after LogLikelihoodDecreased and
+   * Iterations.back() after every other termination, TooFewConstraints included: then it is the entry with n < 6
+   * constraints, whose log-likelihood is 0.  Both fields are -1 / NaN while has_iteration_with_increment is 0. */
   int64_t last_increment_valid_constraints; /* LastIterationWithIncrement().ValidConstraints, -1 if none */
   double last_increment_log_likelihood; /* LastIterationWithIncrement().TDistributionLogLikelihood, NaN if none */
 } dvo_b200_level_stats;

@@ -41,6 +41,35 @@ def nan_equal(a, b):
     return np.array_equal(np.isnan(a), np.isnan(b)) and np.array_equal(a[~np.isnan(a)], b[~np.isnan(b)])
 
 
+# TerminationCriteria (dense_tracking.h:62-78), as dvo_b200_termination and the oracle number them
+TERM_ITERATIONS_EXCEEDED, TERM_INCREMENT_TOO_SMALL, TERM_LOG_LIKELIHOOD_DECREASED, TERM_TOO_FEW_CONSTRAINTS = 0, 1, 2, 3
+
+
+def split_levels(result):
+    """a match result's iteration log (dicts with "n", "nll", ...) cut into one list per level, in level order"""
+    its, out, k = result["iterations"] if isinstance(result, dict) else result.iterations, [], 0
+    for l in (result["levels"] if isinstance(result, dict) else result.levels):
+        out.append(its[k:k + l["num_iterations"]])
+        k += l["num_iterations"]
+    assert k == len(its)
+    return out
+
+
+def level_fields(iterations, termination):
+    """LevelStats::HasIterationWithIncrement / LastIterationWithIncrement (dense_tracking_config.cpp:138-155) over one
+    level's iteration log, as the fields of dvo_b200_level_stats: the picked iteration is Iterations[size-2] after
+    LogLikelihoodDecreased and Iterations.back() after every other termination, TooFewConstraints included."""
+    need = 2 if termination in (TERM_LOG_LIKELIHOOD_DECREASED, TERM_TOO_FEW_CONSTRAINTS) else 1
+    has = len(iterations) >= need
+    out = {"has_iteration_with_increment": has, "last_valid_constraints": iterations[-1]["n"] if iterations else 0,
+           "last_increment_valid_constraints": -1, "last_increment_log_likelihood": float("nan")}
+    if has:
+        e = iterations[-2] if termination == TERM_LOG_LIKELIHOOD_DECREASED else iterations[-1]
+        out["last_increment_valid_constraints"] = e["n"]
+        out["last_increment_log_likelihood"] = e["nll"]
+    return out
+
+
 # ---- the pin against the original project's object code (tests/test_reference_pin.py, tests/golden/make_reference_pin.py) ----
 O3_SAMPLE = 128     # valid points per (pair, level) at which the -O3 build's records are stored
 
