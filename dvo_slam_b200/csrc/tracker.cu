@@ -142,6 +142,10 @@ __device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double
       // the reference's entry is value-initialised apart from ValidConstraints: log-likelihoods and precision are 0
       st.nll_cur = 0; st.prior_cur = 0;
       for (int i = 0; i < 4; ++i) st.precision[i] = 0.f;
+      // and no normal equations: what the linearisation hook reports for this iteration (the end step never runs)
+      st.ll = 0.f;
+      for (int i = 0; i < 36; ++i) st.A[i] = 0.0;
+      for (int i = 0; i < 6; ++i) st.b[i] = 0.0;
       log_iteration(ilog, max_log, pair, st, st.iteration, lp.level_id, false);
       // post-loop checks of dense_tracking.cpp:359-363 still apply
       double m = 0; bool nanx = false;
@@ -588,7 +592,11 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
       }
       __syncthreads();
       ++episode;
-      if (!__ldcg(&st.level_active) || *reinterpret_cast<volatile int*>(a.error_flag)) break;   // too few constraints
+      // too few constraints: the level ends here.  The residual-image hook still gets this iteration's records, so with a
+      // dump the CTA runs stage B once more for the dump alone (its sums are discarded).
+      const bool failed = *reinterpret_cast<volatile int*>(a.error_flag) != 0;
+      const bool level_ends = failed || !__ldcg(&st.level_active);
+      if (level_ends && (!a.dump || failed)) break;
 
       // ---- stage B ----
       {
@@ -605,6 +613,7 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
         DVO_ADD(tm, rounds_b, DVO_CLOCK(tm) - ts0);
       }
       __syncthreads();
+      if (level_ends) break;
       // the rows of each of this CTA's strips, in order, in fp64: one thread per (strip, value)
       for (int it = threadIdx.x; it < geo.nmine * kNormalValues; it += kCtaThreads) {
         const int j = it / kNormalValues, i = it - j * kNormalValues;
