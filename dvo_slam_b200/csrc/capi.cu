@@ -81,8 +81,10 @@ int dvo_b200_create(int device, void* stream, dvo_b200_ctx** out) {
     return DVO_B200_ERR_CUDA;   // no CPU fallback: without a CUDA device there is no engine
   }
   if (cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return DVO_B200_ERR_CUDA; }
+  static std::atomic<uint64_t> next_uid{1};
   dvo_b200_ctx* ctx = new dvo_b200_ctx;
   ctx->device = device;
+  ctx->uid = next_uid.fetch_add(1, std::memory_order_relaxed);
   ctx->pool = std::make_shared<SlabPool>();
   ctx->pool->device = device;
   if (stream) { ctx->stream = (cudaStream_t)stream; ctx->own_stream = false; }
@@ -231,9 +233,11 @@ int dvo_b200_pyramid_retain(dvo_b200_pyramid* p) {
 int dvo_b200_pyramid_release(dvo_b200_pyramid* p) {
   if (!p) return DVO_B200_ERR_INVALID_ARGUMENT;
   if (p->refcount.fetch_sub(1, std::memory_order_acq_rel) == 1) {
-    // No synchronisation: the slab returns to the owning ctx's pool and is only ever rewritten by
-    // work enqueued later on that ctx's stream (stream order protects queued readers).  A second
-    // ctx that uses this pyramid holds a reference until its (blocking) match call has returned.
+    // No synchronisation: the pyramid may be released as soon as the calls that used it have returned, on any context,
+    // with their work still queued (dvo_b200_match_batch_device returns before its kernels run).  The slab returns to
+    // the owning ctx's pool and is only rewritten by a later build on that ctx's stream, which is ordered after the
+    // owner's own queued readers by the stream and after other contexts' queued readers by the events those calls
+    // left on the slab (Slab::foreign_uses).  If the owner is gone, the slab is freed once those events complete.
     pyramid_free(p);
   }
   return 0;
@@ -253,7 +257,7 @@ int dvo_b200_pyramid_level_info(const dvo_b200_pyramid* p, int32_t level, int32_
 int dvo_b200_pyramid_download(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p, int32_t level, float* planes6) {
   if (!p || !planes6 || level < 0 || level >= p->levels)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_download: invalid argument");
-  cudaSetDevice(ctx ? ctx->device : (p->slab && p->slab->pool ? p->slab->pool->device : 0));
+  DeviceScope dev(ctx ? ctx->device : p->device);   // the caller's current device is left as it was
   const LevelInfo& L = p->L[level];
   size_t N = L.n;
   const size_t plane = (size_t)L.pitch * L.h;      // float2 elements per plane, rows padded to the pitch
@@ -286,6 +290,7 @@ int dvo_b200_pyramid_select(dvo_b200_ctx* ctx, dvo_b200_pyramid* p, int32_t leve
   if (!ctx || !p || level < 0 || level >= p->levels)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_select: invalid argument");
   cudaSetDevice(ctx->device);
+  wait_for_pyramid(ctx, p);   // the build may still be running, on another context's stream
   int rc = pyramid_reselect(ctx, p, intensity_threshold, depth_threshold);
   if (rc) return rc;
   const LevelInfo& L = p->L[level];

@@ -85,8 +85,23 @@ struct Slab {                  // one cudaMalloc shared by a batch of pyramids
   void* base = nullptr;
   size_t bytes = 0;
   int refs = 0;
-  cudaEvent_t ready = nullptr;   // recorded on the creating stream after the build kernels
+  cudaEvent_t ready = nullptr;   // recorded on the creating stream after the build kernels (and after a re-selection)
+  // Work of OTHER contexts that may still read the slab: per consuming context (dvo_b200_ctx::uid), one event recorded
+  // on its stream after its latest call that read the slab.  Guarded by pool->mu.  A pyramid may be released as soon as
+  // such a call has returned, so the owner's next build into this slab (acquire_slab) waits for these events first.
+  std::vector<std::pair<uint64_t, cudaEvent_t>> foreign_uses;
   std::shared_ptr<SlabPool> pool;
+};
+
+// Sets the calling thread's current device for a scope and restores the previous one: for the calls that need no context
+// (download with a NULL context, the last release of a pyramid) and so must not change the caller's device.
+struct DeviceScope {
+  int prev = -1;
+  explicit DeviceScope(int device) {
+    if (cudaGetDevice(&prev) != cudaSuccess) { cudaGetLastError(); prev = -1; }
+    if (prev != device) cudaSetDevice(device);
+  }
+  ~DeviceScope() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
 }  // namespace dvo_b200
@@ -181,6 +196,7 @@ struct Workspace {              // per-ctx scratch of the level kernel
 
 struct dvo_b200_ctx {
   int device = 0;
+  uint64_t uid = 0;                   // unique over the process lifetime (a context's address may be reused after destroy)
   int num_sms = 0, ctas_per_sm = 0;   // persistent-kernel grid geometry (queried once)
   int estimator = DVO_B200_ESTIMATOR_REFERENCE;   // dvo_b200_estimator of every later alignment / test hook on this context
   unsigned long long* d_dbg = nullptr;   // DVO_B200_TIMING=1: per-level phase timers of the persistent kernel (64 slots)
@@ -229,6 +245,8 @@ int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float*
 int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const void* d_Z, int raw, float zscale, int w, int h,
                               float fx, float fy, float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out);
 int pyramid_reselect(dvo_b200_ctx* ctx, dvo_b200_pyramid* p, float ti, float td);
+void wait_for_pyramid(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p);   // order ctx's stream after the pyramid's build / re-selection
+int note_foreign_use(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p);    // after enqueueing work that reads p (see Slab::foreign_uses)
 void pyramid_free(dvo_b200_pyramid* p);
 void pool_close(dvo_b200_ctx* ctx);
 int ensure_stage(dvo_b200_ctx* ctx, size_t dev_bytes, size_t host_bytes);

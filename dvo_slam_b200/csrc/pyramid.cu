@@ -269,6 +269,10 @@ int ensure_stage(dvo_b200_ctx* ctx, size_t dev_bytes, size_t host_bytes) {
 }
 
 static void destroy_slab(Slab* s) {
+  for (auto& u : s->foreign_uses) {   // another context's queued work may still read the slab
+    cudaEventSynchronize(u.second);
+    cudaEventDestroy(u.second);
+  }
   cudaFree(s->base);
   if (s->ready) cudaEventDestroy(s->ready);
   delete s;
@@ -282,6 +286,8 @@ static Slab* acquire_slab(dvo_b200_ctx* ctx, size_t bytes) {
     Slab* s = it->second;
     pool.free.erase(it);
     s->refs = 0;
+    // the build that follows rewrites the slab on this stream: after every other context's work that read it
+    for (auto& u : s->foreign_uses) cudaStreamWaitEvent(ctx->stream, u.second, 0);
     return s;
   }
   void* p = nullptr;
@@ -305,9 +311,30 @@ void pyramid_free(dvo_b200_pyramid* p) {
   std::shared_ptr<SlabPool> pool = s->pool;    // keeps the pool alive while its mutex is held
   std::lock_guard<std::mutex> lock(pool->mu);
   if (--s->refs == 0) {
-    if (pool->closed) { cudaSetDevice(pool->device); destroy_slab(s); }
+    if (pool->closed) { DeviceScope dev(pool->device); destroy_slab(s); }
     else pool->free.insert({s->bytes, s});
   }
+}
+
+void wait_for_pyramid(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p) {
+  // Also for the context's own pyramids: the event may have been re-recorded by another context's re-selection, and
+  // waiting on an event last recorded on this very stream costs nothing.
+  if (p->slab && p->slab->ready) cudaStreamWaitEvent(ctx->stream, p->slab->ready, 0);
+}
+
+int note_foreign_use(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p) {
+  Slab* s = p->slab;
+  if (!s || s->pool == ctx->pool) return 0;   // the owner's own work is ordered before its later builds by its stream
+  std::lock_guard<std::mutex> lock(s->pool->mu);
+  cudaEvent_t e = nullptr;
+  for (auto& u : s->foreign_uses)
+    if (u.first == ctx->uid) e = u.second;
+  if (!e) {
+    DVO_CUDA(ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    s->foreign_uses.push_back({ctx->uid, e});
+  }
+  DVO_CUDA(ctx, cudaEventRecord(e, ctx->stream));
+  return 0;
 }
 
 // The context goes away: free what is pooled, and have slabs still referenced by live pyramids freed on release.

@@ -875,6 +875,16 @@ int plan_groups(const dvo_b200_pyramid* ref, int first, int last, int grid, int 
   return ngroups;
 }
 
+// One pyramid of each distinct slab among the batch's pyramids (a batch built in one call shares one slab), in slab order.
+std::vector<const dvo_b200_pyramid*> distinct_slabs(int n, dvo_b200_pyramid* const* refs, dvo_b200_pyramid* const* curs) {
+  std::vector<const dvo_b200_pyramid*> v;
+  v.reserve(2 * (size_t)n);
+  for (int i = 0; i < n; ++i) { v.push_back(refs[i]); v.push_back(curs[i]); }
+  std::sort(v.begin(), v.end(), [](const dvo_b200_pyramid* a, const dvo_b200_pyramid* b) { return std::less<Slab*>()(a->slab, b->slab); });
+  v.erase(std::unique(v.begin(), v.end(), [](const dvo_b200_pyramid* a, const dvo_b200_pyramid* b) { return a->slab == b->slab; }), v.end());
+  return v;
+}
+
 int check_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                 dvo_b200_pyramid* const* curs) {
   if (!cfg || n <= 0 || !refs || !curs) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match: null argument");
@@ -883,15 +893,21 @@ int check_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_p
   if (cfg->max_iterations_per_level < 0) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match: max iterations < 0");
   for (int i = 0; i < n; ++i) {
     if (!refs[i] || !curs[i]) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match: null pyramid");
-    // a pyramid built on another ctx's stream: order this stream after its build
-    for (const dvo_b200_pyramid* p : {refs[i], curs[i]})
-      if (p->slab && p->slab->pool != ctx->pool && p->slab->ready) cudaStreamWaitEvent(ctx->stream, p->slab->ready, 0);
     if (refs[i]->levels <= cfg->first_level || curs[i]->levels <= cfg->first_level)
       return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match: pyramid has fewer levels than FirstLevel+1");
     if (refs[i]->L[0].w != refs[0]->L[0].w || refs[i]->L[0].h != refs[0]->L[0].h ||
         curs[i]->L[0].w != refs[0]->L[0].w || curs[i]->L[0].h != refs[0]->L[0].h)
       return set_error(ctx, DVO_B200_ERR_SHAPE_MISMATCH, "match: all pyramids of a batch must share width/height");
   }
+  // order this stream after the builds (possibly on another ctx's stream, possibly still running) of every pyramid
+  for (const dvo_b200_pyramid* p : distinct_slabs(n, refs, curs)) wait_for_pyramid(ctx, p);
+  return 0;
+}
+
+// After enqueueing a call's work on the batch: remember it on every slab of another context (Slab::foreign_uses).
+int note_foreign_uses(dvo_b200_ctx* ctx, int n, dvo_b200_pyramid* const* refs, dvo_b200_pyramid* const* curs) {
+  for (const dvo_b200_pyramid* p : distinct_slabs(n, refs, curs))
+    if (int rc = note_foreign_use(ctx, p)) return rc;
   return 0;
 }
 
@@ -1169,6 +1185,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
     ctx->launches++;
   }
   DVO_CUDA(ctx, cudaGetLastError());
+  if ((rc = note_foreign_uses(ctx, n, refs, curs))) return rc;   // the caller may release the pyramids once this returns
   ctx->pending_level_flags = nlaunch;   // checked at the next synchronisation point (device-results variant)
   if (h_results) {
     size_t bytes = sizeof(dvo_b200_result) * n;
@@ -1263,6 +1280,7 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
   if ((rc = launch_segments(ctx, 1, lps, &plan, &hm, d_pls, nullptr, 1, 0, planes7 ? ws.d_dump : nullptr, 1, 0, &flag))) return rc;
   DVO_CUDA(ctx, cudaMemcpyAsync(&ws.h_active[0], flag, sizeof(int), cudaMemcpyDeviceToHost, st));
   DVO_CUDA(ctx, cudaGetLastError());
+  if ((rc = note_foreign_uses(ctx, 1, refs, curs))) return rc;
   PairState* hs = nullptr;
   if ((rc = ensure_stage(ctx, 0, sizeof(PairState) + 64))) return rc;
   hs = (PairState*)ctx->h_stage;

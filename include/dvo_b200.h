@@ -167,6 +167,10 @@ int dvo_b200_pyramid_create_bgr_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_
                                       float oy, int32_t levels, dvo_b200_pyramid** out /* n handles */);
 int dvo_b200_pyramid_device(const dvo_b200_pyramid* p);   /* CUDA ordinal the pyramid lives on (-1: null handle) */
 int dvo_b200_pyramid_retain(dvo_b200_pyramid* p);   /* boost::shared_ptr semantics of RgbdImagePyramidPtr */
+/* Any context may use a pyramid, also while its build is still queued on the building context's stream: every call
+ * waits for the build on the device.  A pyramid may be released from any host thread as soon as the calls that used it
+ * have returned, on any context, including dvo_b200_match_batch_device with its work still queued: its memory is only
+ * rebuilt after that work.  Does not change the calling thread's current device. */
 int dvo_b200_pyramid_release(dvo_b200_pyramid* p);
 int dvo_b200_pyramid_num_levels(const dvo_b200_pyramid* p);
 int dvo_b200_pyramid_level_info(const dvo_b200_pyramid* p, int32_t level, int32_t* width, int32_t* height, float K[4]);
@@ -174,7 +178,7 @@ int dvo_b200_pyramid_level_info(const dvo_b200_pyramid* p, int32_t level, int32_
  * Z is the tracker's masked depth: NaN wherever the reference would reject the pixel as a bilinear
  * tap or as a reference point (any of I,Z,Ix,Iy,Zx,Zy NaN).  Synchronises.  ctx may be NULL: pyramids are shared objects
  * that can outlive the context that built them (boost::shared_ptr<RgbdImagePyramid>); the read then waits for the
- * pyramid's own build to finish and uses no context at all. */
+ * pyramid's own build to finish and uses no context at all.  Does not change the calling thread's current device. */
 int dvo_b200_pyramid_download(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p, int32_t level, float* planes6);
 /* PointSelection::select result (point_selection.cpp:89-152) for the given thresholds: number of
  * selected points S and (optional) h*w byte mask.  Synchronises. */
