@@ -64,6 +64,58 @@ __global__ void k_convert_bgr(const uint8_t* __restrict__ bgr, uint8_t* __restri
 }
 
 }  // namespace
+
+// Uploads n frames of one dvo_b200_input_format (and their reference masks, if any) into the context's device staging
+// area and builds their pyramids.  The frames stay in their file representation there: the pyramid kernels convert in
+// their loads (no float32 copy of a raw frame is written); BGR is reduced to 8-bit grey first, as cv::cvtColor leaves it.
+// Masks add one byte per pixel after the frames.
+static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image, const void* depth, float depth_scale,
+                         const uint8_t* masks, int width, int height, float fx, float fy, float ox, float oy, int levels,
+                         dvo_b200_pyramid** out) {
+  cudaSetDevice(ctx->device);
+  const size_t npx = (size_t)width * height * n;
+  size_t frames = 0, grey_off = 0, bgr_off = 0;   // bytes of the staged frames; offsets of the grey and BGR images
+  if (format == DVO_B200_INPUT_FLOAT32) {
+    frames = 2 * npx * sizeof(float);
+  } else {
+    grey_off = (npx * 2 + 255) / 256 * 256;
+    bgr_off = grey_off + (npx + 255) / 256 * 256;
+    frames = (format == DVO_B200_INPUT_BGR8_DEPTH16 ? bgr_off + npx * 3 : grey_off + npx) + 64;
+  }
+  const size_t mask_off = (frames + 255) / 256 * 256;
+  int rc = ensure_stage(ctx, masks ? mask_off + npx : frames, 0);
+  if (rc) return rc;
+  char* stage = (char*)ctx->d_stage;
+  const uint8_t* dM = nullptr;
+  if (masks) {
+    DVO_CUDA(ctx, cudaMemcpyAsync(stage + mask_off, masks, npx, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->h2d_bytes += npx;
+    dM = (const uint8_t*)(stage + mask_off);
+  }
+  if (format == DVO_B200_INPUT_FLOAT32) {
+    float* dI = (float*)stage;
+    float* dZ = dI + npx;
+    DVO_CUDA(ctx, cudaMemcpyAsync(dI, image, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    DVO_CUDA(ctx, cudaMemcpyAsync(dZ, depth, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    ctx->h2d_bytes += 2 * npx * sizeof(float);
+    return pyramid_build_batch_input(ctx, n, dI, dZ, 0, 0.f, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM);
+  }
+  uint16_t* dR = (uint16_t*)stage;
+  uint8_t* dG = (uint8_t*)(stage + grey_off);
+  DVO_CUDA(ctx, cudaMemcpyAsync(dR, depth, npx * 2, cudaMemcpyHostToDevice, ctx->stream));
+  if (format == DVO_B200_INPUT_GREY8_DEPTH16) {
+    DVO_CUDA(ctx, cudaMemcpyAsync(dG, image, npx, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->h2d_bytes += npx * 3;
+  } else {
+    uint8_t* dC = (uint8_t*)(stage + bgr_off);
+    DVO_CUDA(ctx, cudaMemcpyAsync(dC, image, npx * 3, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->h2d_bytes += npx * 5;
+    k_convert_bgr<<<(unsigned)((npx + 255) / 256), 256, 0, ctx->stream>>>(dC, dG, (int)npx);   // 8-bit grey, as cv::cvtColor leaves it
+    ctx->launches++;
+  }
+  return pyramid_build_batch_input(ctx, n, dG, dR, 1, depth_scale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM);
+}
+
 }  // namespace dvo_b200
 
 using namespace dvo_b200;
@@ -158,16 +210,7 @@ int dvo_b200_pyramid_create_batch(dvo_b200_ctx* ctx, int32_t n, const float* int
                                   dvo_b200_pyramid** out) {
   if (!ctx || !intensity || !depth || !out || n <= 0 || width <= 0 || height <= 0)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create: null/invalid argument");
-  cudaSetDevice(ctx->device);
-  size_t img = (size_t)width * height * sizeof(float);
-  int rc = ensure_stage(ctx, 2 * img * n, 0);
-  if (rc) return rc;
-  float* dI = (float*)ctx->d_stage;
-  float* dZ = dI + (size_t)n * width * height;
-  DVO_CUDA(ctx, cudaMemcpyAsync(dI, intensity, img * n, cudaMemcpyHostToDevice, ctx->stream));
-  DVO_CUDA(ctx, cudaMemcpyAsync(dZ, depth, img * n, cudaMemcpyHostToDevice, ctx->stream));
-  ctx->h2d_bytes += 2 * img * n;
-  return pyramid_build_batch(ctx, n, dI, dZ, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out);
+  return create_staged(ctx, n, DVO_B200_INPUT_FLOAT32, intensity, depth, 0.f, nullptr, width, height, fx, fy, ox, oy, levels, out);
 }
 
 int dvo_b200_pyramid_create(dvo_b200_ctx* ctx, const float* intensity, const float* depth, int32_t width, int32_t height,
@@ -180,19 +223,8 @@ int dvo_b200_pyramid_create_raw_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_
                                       float oy, int32_t levels, dvo_b200_pyramid** out) {
   if (!ctx || !grey || !raw_depth || !out || n <= 0 || width <= 0 || height <= 0)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_raw: null/invalid argument");
-  cudaSetDevice(ctx->device);
-  // the frames stay in their file representation (3 bytes per pixel) in the device staging area; the pyramid kernels
-  // convert in their loads (no float32 copy of the frame is written, no conversion kernel)
-  size_t npx = (size_t)width * height * n;
-  const size_t grey_off = (npx * 2 + 255) / 256 * 256;
-  int rc = ensure_stage(ctx, grey_off + npx + 64, 0);
-  if (rc) return rc;
-  uint16_t* dR = (uint16_t*)ctx->d_stage;
-  uint8_t* dG = (uint8_t*)((char*)ctx->d_stage + grey_off);
-  DVO_CUDA(ctx, cudaMemcpyAsync(dR, raw_depth, npx * 2, cudaMemcpyHostToDevice, ctx->stream));
-  DVO_CUDA(ctx, cudaMemcpyAsync(dG, grey, npx, cudaMemcpyHostToDevice, ctx->stream));
-  ctx->h2d_bytes += npx * 3;
-  return pyramid_build_batch_input(ctx, n, dG, dR, 1, depth_scale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out);
+  return create_staged(ctx, n, DVO_B200_INPUT_GREY8_DEPTH16, grey, raw_depth, depth_scale, nullptr, width, height, fx, fy, ox, oy,
+                       levels, out);
 }
 
 int dvo_b200_pyramid_create_bgr_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_t* bgr, const uint16_t* raw_depth,
@@ -200,20 +232,18 @@ int dvo_b200_pyramid_create_bgr_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_
                                       float oy, int32_t levels, dvo_b200_pyramid** out) {
   if (!ctx || !bgr || !raw_depth || !out || n <= 0 || width <= 0 || height <= 0)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_bgr: null/invalid argument");
-  cudaSetDevice(ctx->device);
-  size_t npx = (size_t)width * height * n;
-  const size_t grey_off = (npx * 2 + 255) / 256 * 256, bgr_off = grey_off + (npx + 255) / 256 * 256;
-  int rc = ensure_stage(ctx, bgr_off + npx * 3 + 64, 0);
-  if (rc) return rc;
-  uint16_t* dR = (uint16_t*)ctx->d_stage;
-  uint8_t* dG = (uint8_t*)((char*)ctx->d_stage + grey_off);
-  uint8_t* dC = (uint8_t*)((char*)ctx->d_stage + bgr_off);
-  DVO_CUDA(ctx, cudaMemcpyAsync(dR, raw_depth, npx * 2, cudaMemcpyHostToDevice, ctx->stream));
-  DVO_CUDA(ctx, cudaMemcpyAsync(dC, bgr, npx * 3, cudaMemcpyHostToDevice, ctx->stream));
-  ctx->h2d_bytes += npx * 5;
-  k_convert_bgr<<<(unsigned)((npx + 255) / 256), 256, 0, ctx->stream>>>(dC, dG, (int)npx);   // 8-bit grey, as cv::cvtColor leaves it
-  ctx->launches++;
-  return pyramid_build_batch_input(ctx, n, dG, dR, 1, depth_scale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out);
+  return create_staged(ctx, n, DVO_B200_INPUT_BGR8_DEPTH16, bgr, raw_depth, depth_scale, nullptr, width, height, fx, fy, ox, oy,
+                       levels, out);
+}
+
+int dvo_b200_pyramid_create_masked_batch(dvo_b200_ctx* ctx, int32_t n, int32_t format, const void* image, const void* depth,
+                                         float depth_scale, const uint8_t* masks, int32_t width, int32_t height, float fx,
+                                         float fy, float ox, float oy, int32_t levels, dvo_b200_pyramid** out) {
+  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked: null/invalid argument");
+  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked: unknown input format " + std::to_string(format));
+  return create_staged(ctx, n, format, image, depth, depth_scale, masks, width, height, fx, fy, ox, oy, levels, out);
 }
 
 int dvo_b200_pyramid_create_raw(dvo_b200_ctx* ctx, const uint8_t* grey, const uint16_t* raw_depth, float depth_scale,

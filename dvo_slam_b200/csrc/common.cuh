@@ -118,7 +118,8 @@ struct dvo_b200_pyramid {
   uint32_t* sel_mask = nullptr;  // device: selection bitmasks of all levels (default thresholds)
   int* sel_info = nullptr;       // device: per level {S, last selected linear pixel index}
   float* tmpl = nullptr;         // device: per level tx[w], ty[h] point-cloud template (rgbd_image.cpp:197-198)
-  float2* tile_range = nullptr;  // device: per level, per tile {min, max} of the non-NaN Z' (min > max: none)
+  float2* tile_range = nullptr;  // device: per level, per tile {min, max} of the non-NaN Z' (min > max: none); of usable pixels only if masked
+  uint32_t* usable = nullptr;    // device: per level usable bits of the reference mask, layout of sel_mask (NULL: built without a mask)
   float sel_ti = 0.f, sel_td = 0.f;  // thresholds the masks were built with
   std::mutex sel_mu;                 // guards sel_ti / sel_td and the enqueueing of a re-selection
   uint64_t id = 0;
@@ -243,7 +244,8 @@ struct ProfScope {
 int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float* d_Z, int w, int h, float fx, float fy,
                         float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out);
 int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const void* d_Z, int raw, float zscale, int w, int h,
-                              float fx, float fy, float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out);
+                              float fx, float fy, float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out,
+                              const uint8_t* d_masks);   // d_masks: n*h*w device bytes, nonzero = usable reference pixel; or NULL
 int pyramid_reselect(dvo_b200_ctx* ctx, dvo_b200_pyramid* p, float ti, float td);
 void wait_for_pyramid(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p);   // order ctx's stream after the pyramid's build / re-selection
 int note_foreign_use(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p);    // after enqueueing work that reads p (see Slab::foreign_uses)

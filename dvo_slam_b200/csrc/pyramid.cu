@@ -76,18 +76,49 @@ __global__ void k_pyr_intensity_down(const void* __restrict__ I0, size_t in_stri
   D[(size_t)y * dp + x] = make_float2(s * 0.25f, 0.f);
 }
 
+__device__ __forceinline__ bool bit_set(const uint32_t* __restrict__ words, size_t i) { return (__ldg(words + (i >> 5)) >> (i & 31)) & 1u; }
+
+// Usable bits of one level of a pyramid built with a reference mask, in the word layout of the selection masks (bit i of
+// word k = linear pixel 32k+i).  Level 0: the caller's h*w bytes, nonzero = usable.  Level l: a pixel is usable iff the
+// four pixels of its 2x2 block in level l-1 are -- the chain of the 2x2 intensity mean -- so iff every level-0 pixel of
+// its footprint [x 2^l, (x+1) 2^l) x [y 2^l, (y+1) 2^l) is.  Runs before k_pyr_finish of the same level.
+template <bool kLevel0>
+__global__ void __launch_bounds__(256)
+k_usable(const uint8_t* __restrict__ mask0, uint32_t* __restrict__ usable, size_t words_per_image, size_t src_off, int sw,
+         size_t dst_off, int w, int h) {
+  const int img = blockIdx.y;
+  const int n = w * h;
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  uint32_t* U = usable + img * words_per_image;
+  bool u = false;
+  if (idx < n) {
+    if (kLevel0) {
+      u = __ldg(mask0 + (size_t)img * n + idx) != 0;
+    } else {
+      const int y = idx / w, x = idx - y * w;
+      const size_t j = (size_t)(2 * y) * sw + 2 * x;   // top-left pixel of the block in level l-1
+      const uint32_t* S = U + src_off;
+      u = bit_set(S, j) && bit_set(S, j + 1) && bit_set(S, j + sw) && bit_set(S, j + sw + 1);
+    }
+  }
+  const unsigned m = __ballot_sync(0xffffffffu, u);
+  if ((threadIdx.x & 31) == 0 && idx < ((n + 31) / 32) * 32) U[dst_off + (idx >> 5)] = m;
+}
+
 // gradients (clamped central differences), masked and true depth, default selection mask and reference plane
 // (I, Zsel: depth where the pixel is selected, NaN elsewhere) for one level.
 // Depth of level l is the pure subsample chain of level 0 (rgbd_image.cpp:127-139): Z_l(y,x) = Z_0(y<<l, x<<l).
 // Level 0 reads its intensity straight from the input image I0 (no intermediate copy); the other levels read the
 // intensity that k_pyr_intensity_down left in P0.x.  The selection count / last selected index are derived from
 // the masks afterwards (k_sel_info): no atomics here.  Threads walk the linear pixel index y*w+x (the order of the
-// selection mask); the planes are addressed with the row pitch.
-template <bool kLevel0, bool kRaw>
+// selection mask); the planes are addressed with the row pitch.  kMasked: the selection also requires the pixel's usable
+// bit (k_usable); only the reference role changes, P0 / P2 are written as without a mask.
+template <bool kLevel0, bool kRaw, bool kMasked>
 __global__ void __launch_bounds__(256)
 k_pyr_finish(const void* __restrict__ I0, const void* __restrict__ Z0, float zscale, int w0, int n0, float2* __restrict__ planes,
              size_t planes_per_image, size_t plane_off, size_t rec_off, int nbands, int w, int h, int pitch, int level,
-             uint32_t* __restrict__ masks, size_t mask_words_per_image, size_t mask_off, float ti, float td) {
+             uint32_t* __restrict__ masks, size_t mask_words_per_image, size_t mask_off, float ti, float td,
+             const uint32_t* __restrict__ usable) {
   const int img = blockIdx.y;
   const int n = w * h;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -122,6 +153,7 @@ k_pyr_finish(const void* __restrict__ I0, const void* __restrict__ Z0, float zsc
     const size_t o = (size_t)y * pitch + x;
     // ValidPointAndGradientThresholdPredicate::isPointOk (point_selection.h:63-66)
     sel = !bad && (fabsf(ix) > ti || fabsf(iy) > ti || fabsf(zx) > td || fabsf(zy) > td);
+    if (kMasked) sel = sel && bit_set(usable + img * mask_words_per_image + mask_off, idx);
     const float nanv = __int_as_float(0x7fc00000);
     const size_t rc = rec_cell(x, y, nbands);
     P0[o] = make_float2(I, zm);
@@ -158,9 +190,12 @@ __global__ void k_rec_fill(float2* __restrict__ planes, size_t planes_per_image,
 
 // {min, max} of the non-NaN Z' of every tile of kTileW x kTileH pixels (one warp per tile).  The level kernel
 // projects the tile's corner rays at both depths to bound the window of the current image its taps fall into.
+// kMasked: only usable pixels count.  Every selected point, for any thresholds and the corrected estimator's odd point
+// included, is usable with a non-NaN Z', so the range still covers them; a tile without usable depth is skipped.
+template <bool kMasked>
 __global__ void k_tile_range(const float2* __restrict__ planes, size_t planes_per_image, size_t plane_off, int w, int h,
                              int pitch, int nbands, int ntiles, float2* __restrict__ ranges, size_t ranges_per_image,
-                             size_t range_off) {
+                             size_t range_off, const uint32_t* __restrict__ usable, size_t usable_per_image, size_t usable_off) {
   const int img = blockIdx.y;
   const int tile = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (tile >= ntiles) return;
@@ -172,6 +207,7 @@ __global__ void k_tile_range(const float2* __restrict__ planes, size_t planes_pe
   for (int y = y0; y < y1; ++y)
     for (int x = x0 + lane; x < x1; x += 32) {
       const float z = P0[(size_t)y * pitch + x].y;
+      if (kMasked && !bit_set(usable + img * usable_per_image + usable_off, (size_t)y * w + x)) continue;
       if (z == z) { lo = fminf(lo, z); hi = fmaxf(hi, z); }
     }
 #pragma unroll
@@ -218,9 +254,11 @@ __global__ void k_drop_odd_last(float2* __restrict__ planes, size_t planes_per_i
   }
 }
 
-// recompute the selection mask and the reference plane of one level for non-default thresholds
+// recompute the selection mask and the reference plane of one level for non-default thresholds (kMasked: usable = the
+// level's usable bits, which the selection keeps honouring)
+template <bool kMasked>
 __global__ void k_reselect(const float2* __restrict__ P0, float2* __restrict__ rec, int nbands, int w, int h, int pitch,
-                           uint32_t* __restrict__ mask, float ti, float td) {
+                           uint32_t* __restrict__ mask, float ti, float td, const uint32_t* __restrict__ usable) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const int n = w * h;
   bool sel = false;
@@ -234,6 +272,7 @@ __global__ void k_reselect(const float2* __restrict__ P0, float2* __restrict__ r
     const float zx = (P2[(size_t)y * pitch + xn].y - P2[(size_t)y * pitch + xp].y) * 0.5f;
     const float zy = (P2[(size_t)yn * pitch + x].y - P2[(size_t)yp * pitch + x].y) * 0.5f;
     sel = !is_nan(a.y) && (fabsf(b.x) > ti || fabsf(b.y) > ti || fabsf(zx) > td || fabsf(zy) > td);
+    if (kMasked) sel = sel && bit_set(usable, idx);
     rec[rc] = make_float2(a.x, sel ? a.y : __int_as_float(0x7fc00000));
   }
   unsigned m = __ballot_sync(0xffffffffu, sel);
@@ -251,6 +290,12 @@ __global__ void k_template(float* __restrict__ tmpl, size_t tmpl_per_image, size
 }
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+
+template <bool kLevel0, bool kRaw, typename... Args>
+void launch_finish(bool masked, dim3 g, cudaStream_t st, Args... a) {
+  if (masked) k_pyr_finish<kLevel0, kRaw, true><<<g, 256, 0, st>>>(a...);
+  else k_pyr_finish<kLevel0, kRaw, false><<<g, 256, 0, st>>>(a...);
+}
 
 }  // namespace
 
@@ -348,12 +393,15 @@ void pool_close(dvo_b200_ctx* ctx) {
 
 int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float* d_Z, int w, int h, float fx, float fy,
                         float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out) {
-  return pyramid_build_batch_input(ctx, n, d_I, d_Z, 0, 0.f, w, h, fx, fy, ox, oy, levels, ti, td, out);
+  return pyramid_build_batch_input(ctx, n, d_I, d_Z, 0, 0.f, w, h, fx, fy, ox, oy, levels, ti, td, out, nullptr);
 }
 
 // d_I / d_Z: raw == 0: float32 intensity / float32 depth; raw == 1: 8-bit grey / 16-bit raw depth (depth = raw * zscale, 0 -> NaN)
+// d_masks: n consecutive h*w byte reference masks (nonzero = usable) or NULL.  Without masks the slab holds no usable bits
+// and the build runs exactly the kernels it ran before masks existed.
 int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const void* d_Z, int raw, float zscale, int w, int h,
-                              float fx, float fy, float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out) {
+                              float fx, float fy, float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out,
+                              const uint8_t* d_masks) {
   if (n <= 0 || levels < 1 || levels > kMaxLevels || w < 32 || h < 2)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid: bad geometry");
   LevelInfo L[kMaxLevels];
@@ -390,7 +438,9 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
   size_t bytes_tmpl = (size_t)n * tmpl_floats * sizeof(float);
   size_t bytes_sel = align_up((size_t)n * sel_ints * sizeof(int), 256);
   size_t bytes_range = (size_t)n * range_f2 * sizeof(float2);
-  size_t total = bytes_planes + bytes_masks + bytes_tmpl + bytes_sel + bytes_range;
+  const bool masked = d_masks != nullptr;
+  size_t bytes_usable = masked ? bytes_masks : 0;   // usable bits: the layout of the selection masks
+  size_t total = bytes_planes + bytes_masks + bytes_tmpl + bytes_sel + bytes_range + bytes_usable;
   Slab* slab = acquire_slab(ctx, total);
   if (!slab) return set_error(ctx, DVO_B200_ERR_OUT_OF_MEMORY, "pyramid: cudaMalloc failed");
   char* base = (char*)slab->base;
@@ -399,10 +449,11 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
   float* tmpl = (float*)(base + bytes_planes + bytes_masks);
   int* sel = (int*)(base + bytes_planes + bytes_masks + bytes_tmpl);
   float2* ranges = (float2*)(base + bytes_planes + bytes_masks + bytes_tmpl + bytes_sel);
+  uint32_t* usable = masked ? (uint32_t*)(base + bytes_planes + bytes_masks + bytes_tmpl + bytes_sel + bytes_range) : nullptr;
 
   cudaStream_t st = ctx->stream;
   {
-    ProfScope prof(ctx, 3, 6 * levels - 1);
+    ProfScope prof(ctx, 3, (masked ? 7 : 6) * levels - 1);
     const int T = 256;
     for (int l = 0; l < levels; ++l) {
       const LevelInfo& q = L[l];
@@ -420,18 +471,28 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
     for (int l = 0; l < levels; ++l) {
       const LevelInfo& q = L[l];
       dim3 g((q.words * 32 + T - 1) / T, n);
-      if (l == 0 && raw) k_pyr_finish<true, true><<<g, T, 0, st>>>(d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td);
-      else if (l == 0) k_pyr_finish<true, false><<<g, T, 0, st>>>(d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td);
-      else if (raw) k_pyr_finish<false, true><<<g, T, 0, st>>>(d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td);
-      else k_pyr_finish<false, false><<<g, T, 0, st>>>(d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td);
+      if (masked) {
+        if (l == 0) k_usable<true><<<g, T, 0, st>>>(d_masks, usable, mask_words, 0, 0, q.mask_off, q.w, q.h);
+        else k_usable<false><<<g, T, 0, st>>>(nullptr, usable, mask_words, L[l - 1].mask_off, L[l - 1].w, q.mask_off, q.w, q.h);
+        ctx->launches += 1;
+      }
+      if (l == 0 && raw) launch_finish<true, true>(masked, g, st, d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
+      else if (l == 0) launch_finish<true, false>(masked, g, st, d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
+      else if (raw) launch_finish<false, true>(masked, g, st, d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
+      else launch_finish<false, false>(masked, g, st, d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
       k_sel_info<<<n, 32, 0, st>>>(masks, mask_words, q.mask_off, q.words, sel, sel_ints, l);
       k_drop_odd_last<<<(n + 127) / 128, 128, 0, st>>>(planes, plane_f2, q.rec_off, q.nbands, q.w, sel, sel_ints, l, n);
       const int ntiles = q.nbands * q.nstrips;
       k_rec_fill<<<dim3((ntiles * kTileW + T - 1) / T, n), T, 0, st>>>(planes, plane_f2, q.rec_off, q.nbands, ntiles, q.w, q.h,
                                                                               tmpl, tmpl_floats, q.tmpl_off);
       ctx->launches += 1;
-      k_tile_range<<<dim3((ntiles + 7) / 8, n), 256, 0, st>>>(planes, plane_f2, q.plane_off, q.w, q.h, q.pitch, q.nbands, ntiles,
-                                                              ranges, range_f2, q.range_off);
+      const dim3 gr((ntiles + 7) / 8, n);
+      if (masked)
+        k_tile_range<true><<<gr, 256, 0, st>>>(planes, plane_f2, q.plane_off, q.w, q.h, q.pitch, q.nbands, ntiles, ranges, range_f2,
+                                               q.range_off, usable, mask_words, q.mask_off);
+      else
+        k_tile_range<false><<<gr, 256, 0, st>>>(planes, plane_f2, q.plane_off, q.w, q.h, q.pitch, q.nbands, ntiles, ranges, range_f2,
+                                                q.range_off, nullptr, 0, 0);
       ctx->launches += 4;
     }
   }
@@ -448,6 +509,7 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
     p->sel_info = sel + (size_t)i * sel_ints;
     p->tmpl = tmpl + (size_t)i * tmpl_floats;
     p->tile_range = ranges + (size_t)i * range_f2;
+    p->usable = masked ? usable + (size_t)i * mask_words : nullptr;
     p->sel_ti = ti; p->sel_td = td;
     p->id = ctx->next_pyramid_id++;
     out[i] = p;
@@ -470,8 +532,13 @@ int pyramid_reselect(dvo_b200_ctx* ctx, dvo_b200_pyramid* p, float ti, float td)
   for (int l = 0; l < p->levels; ++l) {
     const LevelInfo& q = p->L[l];
     const int T = 256;
-    k_reselect<<<(q.words * 32 + T - 1) / T, T, 0, st>>>(p->planes + q.plane_off, p->planes + q.rec_off, q.nbands, q.w, q.h, q.pitch,
-                                                         p->sel_mask + q.mask_off, ti, td);
+    const int blocks = (q.words * 32 + T - 1) / T;
+    if (p->usable)
+      k_reselect<true><<<blocks, T, 0, st>>>(p->planes + q.plane_off, p->planes + q.rec_off, q.nbands, q.w, q.h, q.pitch,
+                                             p->sel_mask + q.mask_off, ti, td, p->usable + q.mask_off);
+    else
+      k_reselect<false><<<blocks, T, 0, st>>>(p->planes + q.plane_off, p->planes + q.rec_off, q.nbands, q.w, q.h, q.pitch,
+                                              p->sel_mask + q.mask_off, ti, td, nullptr);
     k_sel_info<<<1, 32, 0, st>>>(p->sel_mask, 0, q.mask_off, q.words, p->sel_info, 0, l);
     k_drop_odd_last<<<1, 32, 0, st>>>(p->planes, 0, q.rec_off, q.nbands, q.w, p->sel_info, 0, l, 1);
     ctx->launches += 3;

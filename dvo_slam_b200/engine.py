@@ -29,11 +29,14 @@ ABI_SYMBOLS = [
     "dvo_b200_profile_read", "dvo_b200_pyramid_device", "dvo_b200_sharded_create", "dvo_b200_sharded_destroy",
     "dvo_b200_sharded_num_shards", "dvo_b200_sharded_ctx", "dvo_b200_sharded_last_error", "dvo_b200_shard_range",
     "dvo_b200_sharded_pyramid_create_batch", "dvo_b200_sharded_pyramid_create_raw_batch", "dvo_b200_match_batch_sharded",
-    "dvo_b200_set_estimator", "dvo_b200_get_estimator",
+    "dvo_b200_set_estimator", "dvo_b200_get_estimator", "dvo_b200_pyramid_create_masked_batch",
 ]
 
 # dvo_b200_estimator
 ESTIMATORS = {"reference": 0, "corrected": 1}
+
+# dvo_b200_input_format (dvo_b200_pyramid_create_masked_batch)
+INPUT_FORMATS = {"float32": 0, "grey8_depth16": 1, "bgr8_depth16": 2}
 
 
 class Config(C.Structure):
@@ -124,6 +127,8 @@ def load_library():
     L.dvo_b200_pyramid_create_raw.argtypes = [vp, vp, vp, C.c_float, i32, i32, C.c_float, C.c_float, C.c_float, C.c_float, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_create_raw_batch.argtypes = [vp, i32, vp, vp, C.c_float, i32, i32, C.c_float, C.c_float, C.c_float, C.c_float, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_create_bgr_batch.argtypes = [vp, i32, vp, vp, C.c_float, i32, i32, C.c_float, C.c_float, C.c_float, C.c_float, i32, C.POINTER(vp)]
+    L.dvo_b200_pyramid_create_masked_batch.argtypes = [vp, i32, i32, vp, vp, C.c_float, vp, i32, i32, C.c_float, C.c_float, C.c_float,
+                                                       C.c_float, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_device.argtypes = [vp]
     L.dvo_b200_sharded_create.argtypes = [i32, C.POINTER(i32), C.POINTER(vp)]
     L.dvo_b200_sharded_destroy.argtypes = [vp]
@@ -263,19 +268,53 @@ class Engine:
         return self.lib.dvo_b200_d2h_bytes(self.ctx)
 
     # ---- pyramids ----
-    def pyramid(self, intensity, depth, intrinsics, levels: int) -> Pyramid:
+    # mask= / masks=: reference masks (dvo_b200_pyramid_create_masked_batch): None, an array of n*h*w values (nonzero = usable
+    # reference pixel; shape [h, w] or [n, h, w]) or, for the host-pointer forms, a host pointer (int) to n*h*w bytes.
+    def _create_masked(self, n, fmt, pI, pZ, depth_scale, masks, w, h, intrinsics, levels) -> list[Pyramid]:
+        keep = None
+        if isinstance(masks, int):
+            pM = masks
+        else:
+            keep = np.asarray(masks)
+            keep = np.ascontiguousarray(keep if keep.dtype == np.uint8 else (keep != 0).astype(np.uint8))
+            assert keep.size == n * h * w, f"masks: {keep.shape} for {n} images of {h}x{w}"
+            pM = keep.ctypes.data
+        fx, fy, ox, oy = intrinsics
+        out = (C.c_void_p * n)()
+        self._check(self.lib.dvo_b200_pyramid_create_masked_batch(self.ctx, n, INPUT_FORMATS[fmt], pI, pZ, depth_scale, pM, w, h,
+                                                                  fx, fy, ox, oy, levels, out))
+        if keep is not None and keep is not masks:
+            self.synchronize()   # the converted copy dies with this call
+        return [Pyramid(self, out[i]) for i in range(n)]
+
+    def pyramid(self, intensity, depth, intrinsics, levels: int, mask=None) -> Pyramid:
         I = np.ascontiguousarray(intensity, dtype=np.float32)
         Z = np.ascontiguousarray(depth, dtype=np.float32)
         assert I.ndim == 2 and I.shape == Z.shape
         h, w = I.shape
+        if mask is not None:
+            p = self._create_masked(1, "float32", I.ctypes.data, Z.ctypes.data, 0.0, mask, w, h, intrinsics, levels)[0]
+            self.synchronize()
+            return p
         fx, fy, ox, oy = intrinsics
         out = C.c_void_p()
         self._check(self.lib.dvo_b200_pyramid_create(self.ctx, I.ctypes.data, Z.ctypes.data, w, h, fx, fy, ox, oy, levels, C.byref(out)))
         self.synchronize()  # numpy temporaries may die
         return Pyramid(self, out.value)
 
-    def pyramid_batch(self, intensity, depth, intrinsics, levels: int, host_ptrs=None) -> list[Pyramid]:
+    def pyramid_batch(self, intensity, depth, intrinsics, levels: int, host_ptrs=None, masks=None) -> list[Pyramid]:
         """intensity/depth: [n,h,w] float32 arrays, or (ptr_I, ptr_Z, n, h, w) raw host pointers via host_ptrs."""
+        if masks is not None:
+            if host_ptrs is not None:
+                pI, pZ, n, h, w = host_ptrs
+                return self._create_masked(n, "float32", pI, pZ, 0.0, masks, w, h, intrinsics, levels)
+            I = np.ascontiguousarray(intensity, dtype=np.float32)
+            Z = np.ascontiguousarray(depth, dtype=np.float32)
+            assert I.ndim == 3 and I.shape == Z.shape
+            n, h, w = I.shape
+            out = self._create_masked(n, "float32", I.ctypes.data, Z.ctypes.data, 0.0, masks, w, h, intrinsics, levels)
+            self.synchronize()
+            return out
         if host_ptrs is not None:
             pI, pZ, n, h, w = host_ptrs
         else:
@@ -291,28 +330,36 @@ class Engine:
             self.synchronize()
         return [Pyramid(self, out[i]) for i in range(n)]
 
-    def pyramid_raw_batch(self, host_ptrs, depth_scale, intrinsics, levels: int) -> list[Pyramid]:
+    def pyramid_raw_batch(self, host_ptrs, depth_scale, intrinsics, levels: int, masks=None) -> list[Pyramid]:
         """host_ptrs = (ptr_grey_u8, ptr_depth_u16, n, h, w): n consecutive raw images in (pinned) host memory."""
         pG, pD, n, h, w = host_ptrs
+        if masks is not None:
+            return self._create_masked(n, "grey8_depth16", pG, pD, depth_scale, masks, w, h, intrinsics, levels)
         fx, fy, ox, oy = intrinsics
         out = (C.c_void_p * n)()
         self._check(self.lib.dvo_b200_pyramid_create_raw_batch(self.ctx, n, pG, pD, depth_scale, w, h, fx, fy, ox, oy, levels, out))
         return [Pyramid(self, out[i]) for i in range(n)]
 
-    def pyramid_bgr_batch(self, host_ptrs, depth_scale, intrinsics, levels: int) -> list[Pyramid]:
+    def pyramid_bgr_batch(self, host_ptrs, depth_scale, intrinsics, levels: int, masks=None) -> list[Pyramid]:
         """host_ptrs = (ptr_bgr_u8x3, ptr_depth_u16, n, h, w): n consecutive interleaved-BGR images and raw depth images
         in (pinned) host memory; grey conversion (OpenCV BGR2GRAY) and depth scaling run on the device."""
         pC, pD, n, h, w = host_ptrs
+        if masks is not None:
+            return self._create_masked(n, "bgr8_depth16", pC, pD, depth_scale, masks, w, h, intrinsics, levels)
         fx, fy, ox, oy = intrinsics
         out = (C.c_void_p * n)()
         self._check(self.lib.dvo_b200_pyramid_create_bgr_batch(self.ctx, n, pC, pD, depth_scale, w, h, fx, fy, ox, oy, levels, out))
         return [Pyramid(self, out[i]) for i in range(n)]
 
-    def pyramid_raw(self, grey_u8, depth_u16, depth_scale, intrinsics, levels: int) -> Pyramid:
+    def pyramid_raw(self, grey_u8, depth_u16, depth_scale, intrinsics, levels: int, mask=None) -> Pyramid:
         G = np.ascontiguousarray(grey_u8, dtype=np.uint8)
         D = np.ascontiguousarray(depth_u16, dtype=np.uint16)
         assert G.ndim == 2 and G.shape == D.shape
         h, w = G.shape
+        if mask is not None:
+            p = self._create_masked(1, "grey8_depth16", G.ctypes.data, D.ctypes.data, depth_scale, mask, w, h, intrinsics, levels)[0]
+            self.synchronize()
+            return p
         fx, fy, ox, oy = intrinsics
         out = C.c_void_p()
         self._check(self.lib.dvo_b200_pyramid_create_raw(self.ctx, G.ctypes.data, D.ctypes.data, depth_scale, w, h, fx, fy, ox, oy,

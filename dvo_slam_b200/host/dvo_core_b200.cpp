@@ -54,6 +54,22 @@ void RgbdImagePyramid::build(const size_t num_levels) {
 }
 double RgbdImagePyramid::timestamp() const { return !levels_.empty() ? levels_[0]->timestamp : 0.0; }
 
+bool RgbdImagePyramid::setReferenceMask(const cv::Mat& mask) {
+  std::lock_guard<std::mutex> lock(mutex_);
+  const RgbdImage& l0 = *levels_[0];
+  if (device_ || mask.type() != CV_8UC1 || mask.rows != l0.intensity.rows || mask.cols != l0.intensity.cols) return false;
+  mask_ = mask.clone();
+  return true;
+}
+
+// the reference mask as n*h*w contiguous bytes (a cv::Mat need not be continuous), or empty without one
+static void append_mask(const cv::Mat& mask, int w, int h, std::vector<uint8_t>& out) {
+  const size_t base = out.size();
+  out.resize(base + size_t(w) * h, 1);   // no mask: all usable, the same bits as an unmasked pyramid
+  if (mask.empty()) return;
+  for (int y = 0; y < h; ++y) std::memcpy(&out[base + size_t(y) * w], mask.ptr<uint8_t>(y), size_t(w));
+}
+
 dvo_b200_pyramid* RgbdImagePyramid::device(dvo_b200_ctx* ctx, size_t levels) {
   std::lock_guard<std::mutex> lock(mutex_);
   if (levels < requested_levels_) levels = requested_levels_;
@@ -63,9 +79,12 @@ dvo_b200_pyramid* RgbdImagePyramid::device(dvo_b200_ctx* ctx, size_t levels) {
   if (l0.intensity.type() != CV_32FC1 || l0.depth.type() != CV_32FC1)
     throw std::runtime_error("RgbdImagePyramid: intensity and depth must be CV_32FC1 (benchmark_slam.cpp:60-77)");
   const IntrinsicMatrix& k = camera_.level(0).intrinsics();
-  int rc = dvo_b200_pyramid_create(ctx, l0.intensity.ptr<float>(), l0.depth.ptr<float>(), l0.intensity.cols, l0.intensity.rows,
-                                   k.fx(), k.fy(), k.ox(), k.oy(), int(levels), &device_);
-  if (rc != 0) throw std::runtime_error(std::string("dvo_b200_pyramid_create: ") + dvo_b200_last_error(ctx));
+  std::vector<uint8_t> mask;
+  if (!mask_.empty()) append_mask(mask_, l0.intensity.cols, l0.intensity.rows, mask);
+  int rc = dvo_b200_pyramid_create_masked_batch(ctx, 1, DVO_B200_INPUT_FLOAT32, l0.intensity.ptr<float>(), l0.depth.ptr<float>(), 0.f,
+                                                mask.empty() ? nullptr : mask.data(), l0.intensity.cols, l0.intensity.rows,
+                                                k.fx(), k.fy(), k.ox(), k.oy(), int(levels), &device_);
+  if (rc != 0) throw std::runtime_error(std::string("dvo_b200_pyramid_create_masked_batch: ") + dvo_b200_last_error(ctx));
   dvo_b200_synchronize(ctx);   // the host cv::Mat may be released by the caller
   device_ctx_ = ctx;
   device_levels_ = levels;
@@ -94,16 +113,22 @@ void RgbdImagePyramid::deviceBatch(dvo_b200_ctx* ctx, const std::vector<RgbdImag
     size_t lv = levels;
     for (size_t i = 0; i < n; ++i) lv = std::max(lv, todo[i]->requested_levels_);
     std::vector<float> I(n * npx), Z(n * npx);
+    bool any_mask = false;
     for (size_t i = 0; i < n; ++i) {
       for (int y = 0; y < h; ++y) {   // row by row: a cv::Mat need not be continuous
         std::memcpy(&I[i * npx + size_t(y) * w], todo[i]->levels_[0]->intensity.ptr<float>(y), sizeof(float) * w);
         std::memcpy(&Z[i * npx + size_t(y) * w], todo[i]->levels_[0]->depth.ptr<float>(y), sizeof(float) * w);
       }
+      any_mask = any_mask || !todo[i]->mask_.empty();
     }
+    std::vector<uint8_t> masks;   // one upload for the batch: the pyramids without a mask get an all-usable one
+    if (any_mask)
+      for (size_t i = 0; i < n; ++i) append_mask(todo[i]->mask_, w, h, masks);
     const IntrinsicMatrix& k = todo[0]->camera_.level(0).intrinsics();
     std::vector<dvo_b200_pyramid*> handles(n);
-    int rc = dvo_b200_pyramid_create_batch(ctx, int(n), I.data(), Z.data(), w, h, k.fx(), k.fy(), k.ox(), k.oy(), int(lv), handles.data());
-    if (rc != 0) throw std::runtime_error(std::string("dvo_b200_pyramid_create_batch: ") + dvo_b200_last_error(ctx));
+    int rc = dvo_b200_pyramid_create_masked_batch(ctx, int(n), DVO_B200_INPUT_FLOAT32, I.data(), Z.data(), 0.f, any_mask ? masks.data() : nullptr,
+                                                  w, h, k.fx(), k.fy(), k.ox(), k.oy(), int(lv), handles.data());
+    if (rc != 0) throw std::runtime_error(std::string("dvo_b200_pyramid_create_masked_batch: ") + dvo_b200_last_error(ctx));
     dvo_b200_synchronize(ctx);   // one synchronisation for the whole upload: the staging vectors go out of scope
     for (size_t i = 0; i < n; ++i) {
       std::lock_guard<std::mutex> lock(todo[i]->mutex_);

@@ -169,3 +169,35 @@ def make_sequence(seed: int, n_frames: int, cfg: SceneConfig | None = None, devi
         frames.append(_render(cfg, T_cam, tex, box, rng, device))
         poses.append(np.linalg.inv(T_cam))
     return frames, poses
+
+
+def make_moving_object_pair(seed: int, cfg: SceneConfig | None = None, patch=(150, 120), corner=(250, 200), shift=(24, 10),
+                            z_obj: float = 0.9, margin: int = 8):
+    """make_pair plus an object that moves on its own: a textured fronto-parallel patch (patch = (w, h) pixels at depth
+    ~z_obj, the size of a person at ~1 m) pasted at corner = (x, y) in the reference frame and at corner + shift in the
+    current frame, whatever the camera did.  Returns make_pair's dict (float32 numpy images, T_true of the camera) plus
+    "mask": the uint8 reference mask that excludes the patch and a margin of `margin` pixels around it (0 = excluded),
+    as a dilated segmentation mask would."""
+    p = make_pair(seed, cfg)
+    out = dict(p)
+    for k in ("I_ref", "Z_ref", "I_cur", "Z_cur"):
+        out[k] = p[k].cpu().numpy().copy()
+    rng = np.random.default_rng(1000 + seed)
+    pw, ph = patch
+    yy, xx = np.mgrid[0:ph, 0:pw]
+    tex = np.zeros((ph, pw))
+    for _ in range(12):
+        kx, ky = rng.uniform(-0.25, 0.25, 2)
+        tex += rng.uniform(0.3, 1.0) * np.sin(kx * xx + ky * yy + rng.uniform(0, 2 * math.pi))
+    tex = np.round(np.clip(127.5 + 40.0 * tex, 0, 255)).astype(np.float32)
+    zt = (np.float32(z_obj) + np.float32(0.0002) * np.round(xx / 8.0)).astype(np.float32)
+    x0, y0 = corner
+    x1, y1 = x0 + shift[0], y0 + shift[1]
+    out["I_ref"][y0:y0 + ph, x0:x0 + pw] = tex
+    out["Z_ref"][y0:y0 + ph, x0:x0 + pw] = zt
+    out["I_cur"][y1:y1 + ph, x1:x1 + pw] = tex
+    out["Z_cur"][y1:y1 + ph, x1:x1 + pw] = zt
+    mask = np.ones(out["I_ref"].shape, np.uint8)
+    mask[max(y0 - margin, 0):y0 + ph + margin, max(x0 - margin, 0):x0 + pw + margin] = 0
+    out["mask"] = mask
+    return out

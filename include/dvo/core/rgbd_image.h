@@ -81,9 +81,15 @@ class RgbdImagePyramid {   // rgbd_image.h:242-262
   // list -- a keyframe in several proposals -- are uploaded once); out[i] = device mirror of pyramids[i]
   static void deviceBatch(dvo_b200_ctx* ctx, const std::vector<RgbdImagePyramid*>& pyramids, size_t levels,
                           std::vector<dvo_b200_pyramid*>& out);
+  // --- extension: a reference mask, CV_8U of the base size, nonzero = usable, 0 = excluded.  Excluded pixels never become
+  // constraints while this pyramid is the reference of an alignment, at any level (a coarse pixel is usable iff its whole
+  // footprint is; dvo_b200_pyramid_create_masked_batch).  The mask is copied.  Returns false and changes nothing once the
+  // device mirror exists (after the first match) or if the size or type is wrong. ---
+  bool setReferenceMask(const cv::Mat& mask);
  private:
   RgbdCameraPyramid& camera_;
   std::vector<RgbdImagePtr> levels_;
+  cv::Mat mask_;   // setReferenceMask; empty: no mask
   dvo_b200_pyramid* device_;
   dvo_b200_ctx* device_ctx_;
   size_t device_levels_, requested_levels_;

@@ -165,6 +165,33 @@ int dvo_b200_pyramid_create_raw_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_
 int dvo_b200_pyramid_create_bgr_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_t* bgr, const uint16_t* raw_depth,
                                       float depth_scale, int32_t width, int32_t height, float fx, float fy, float ox,
                                       float oy, int32_t levels, dvo_b200_pyramid** out /* n handles */);
+/* Input forms of dvo_b200_pyramid_create_masked_batch */
+typedef enum dvo_b200_input_format {
+  DVO_B200_INPUT_FLOAT32 = 0,        /* float intensity + float depth in metres (NaN = invalid), as dvo_b200_pyramid_create_batch */
+  DVO_B200_INPUT_GREY8_DEPTH16 = 1,  /* 8-bit grey + 16-bit raw depth, as dvo_b200_pyramid_create_raw_batch */
+  DVO_B200_INPUT_BGR8_DEPTH16 = 2    /* 8-bit interleaved BGR + 16-bit raw depth, as dvo_b200_pyramid_create_bgr_batch */
+} dvo_b200_input_format;
+/* The create calls above with a REFERENCE MASK per image: pixels the caller knows to be wrong (dynamic objects, the robot's
+ * own body, specular or over-exposed areas, a vignetted border) never become constraints when the pyramid is the reference
+ * of an alignment.  format: a dvo_b200_input_format (anything else -> DVO_B200_ERR_INVALID_ARGUMENT, nothing is created);
+ * image / depth as in the call that format names; depth_scale is ignored for FLOAT32.  Host pointers are staged and may be
+ * pageable or pinned, as in the other create calls.
+ *   masks: n*height*width bytes, image i at i*height*width, row-major; nonzero = usable, 0 = excluded (an OpenCV CV_8U
+ *     mask).  NULL: no mask, the pyramids are those of the call the format names, bit for bit.  An all-nonzero mask gives
+ *     the same bits as no mask in every plane, selection and result.
+ *   Coarser levels: a pixel of level l is usable iff every level-0 pixel of its footprint [x 2^l, (x+1) 2^l) x
+ *     [y 2^l, (y+1) 2^l) is usable (an AND over each 2x2 block, level by level, the chain of the 2x2 intensity mean; the
+ *     depth subsample point lies inside the footprint).
+ *   Selection: at every level and for any thresholds, a pixel is selected iff isPointOk(ti, td) holds AND it is usable.
+ *     Everything that follows from the selection follows the mask: LevelStats.valid_pixels (S), the odd last point
+ *     (dropped by the reference estimator, re-admitted by the corrected one), dvo_b200_pyramid_select, the residual and
+ *     intensity error images.  max_valid_pixels does not change.
+ *   Reference role only: the mask does not change the pyramid as the CURRENT image of an alignment (its pixels stay valid
+ *     bilinear taps) nor dvo_b200_pyramid_download.
+ *   Fixed at creation: a pyramid's mask never changes, so sharing it across contexts and threads needs no new rule. */
+int dvo_b200_pyramid_create_masked_batch(dvo_b200_ctx* ctx, int32_t n, int32_t format, const void* image, const void* depth,
+                                         float depth_scale, const uint8_t* masks, int32_t width, int32_t height, float fx,
+                                         float fy, float ox, float oy, int32_t levels, dvo_b200_pyramid** out /* n handles */);
 int dvo_b200_pyramid_device(const dvo_b200_pyramid* p);   /* CUDA ordinal the pyramid lives on (-1: null handle) */
 int dvo_b200_pyramid_retain(dvo_b200_pyramid* p);   /* boost::shared_ptr semantics of RgbdImagePyramidPtr */
 /* Any context may use a pyramid, also while its build is still queued on the building context's stream: every call
