@@ -53,17 +53,18 @@ def test_batch_512_against_reference_numerics(engine, oracle):
 
     # Every floating-point sum above an image row is taken in an order fixed by the level's geometry (rows of a strip in
     # order, strips in order, fp64), never by how strips are spread over CTAs: the fused 512-pair launch -- one CTA per pair
-    # on the coarse levels, slices with squads of 3, 6 and 12 CTAs on level 0 (on an H100, 132 SMs x 2 CTAs: pairs
-    # 0-392, 393-471, 472-511) -- returns bit for bit what the same call returns again, what the batch in reverse order
-    # returns (other slices), and what SINGLE alignments (one launch per level, squads of up to 69 CTAs) return.  The oracle comparison below therefore also speaks for the single-pair path
-    # and vice versa (tests/test_gpu_parity.py compares that path with the oracle record by record).
+    # on the coarse levels, slices with squads of 2, 4 and 8 CTAs on level 0 (on an H100, 132 SMs x 2 CTAs: pairs
+    # 0-333, 334-452, 453-511) -- returns bit for bit what the same call returns again, what the batch in reverse order
+    # returns (other slices), and what SINGLE alignments (one launch per level, squads of up to 69 CTAs) return.  The oracle
+    # comparison below therefore also speaks for the single-pair path and vice versa (tests/test_gpu_parity.py compares that
+    # path with the oracle record by record; tests/test_gpu_launch_plans.py checks every plan shape against single alignments).
     again = engine.match_batch(refs, curs, cfg)
     rev = engine.match_batch(refs[::-1], curs[::-1], cfg)[::-1]
     for other in (again, rev):
         for i in range(B):
             assert np.array_equal(res[i].transformation, other[i].transformation) and np.array_equal(res[i].information, other[i].information), i
             assert res[i].log_likelihood == other[i].log_likelihood and res[i].levels == other[i].levels, i
-    for i in (0, 1, 200, 392, 393, 430, 471, 472, 500, 511):       # both sides of the slice boundaries 393 | 79 | 40
+    for i in (0, 1, 200, 333, 334, 430, 452, 453, 500, 511):       # both sides of the slice boundaries 334 | 119 | 59
         single = engine.match(refs[i], curs[i], cfg)
         assert np.array_equal(res[i].transformation, single.transformation) and np.array_equal(res[i].information, single.information), i
         assert res[i].log_likelihood == single.log_likelihood and res[i].levels == single.levels, i
