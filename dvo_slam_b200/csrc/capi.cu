@@ -70,8 +70,8 @@ __global__ void k_convert_bgr(const uint8_t* __restrict__ bgr, uint8_t* __restri
 // their loads (no float32 copy of a raw frame is written); BGR is reduced to 8-bit grey first, as cv::cvtColor leaves it.
 // Masks add one byte per pixel after the frames.
 static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image, const void* depth, float depth_scale,
-                         const uint8_t* masks, int width, int height, float fx, float fy, float ox, float oy, int levels,
-                         dvo_b200_pyramid** out) {
+                         const uint8_t* masks, int mask_roles, int width, int height, float fx, float fy, float ox, float oy,
+                         int levels, dvo_b200_pyramid** out) {
   cudaSetDevice(ctx->device);
   const size_t npx = (size_t)width * height * n;
   size_t frames = 0, grey_off = 0, bgr_off = 0;   // bytes of the staged frames; offsets of the grey and BGR images
@@ -98,7 +98,7 @@ static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image
     DVO_CUDA(ctx, cudaMemcpyAsync(dI, image, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     DVO_CUDA(ctx, cudaMemcpyAsync(dZ, depth, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     ctx->h2d_bytes += 2 * npx * sizeof(float);
-    return pyramid_build_batch_input(ctx, n, dI, dZ, 0, 0.f, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM);
+    return pyramid_build_batch_input(ctx, n, dI, dZ, 0, 0.f, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM, mask_roles);
   }
   uint16_t* dR = (uint16_t*)stage;
   uint8_t* dG = (uint8_t*)(stage + grey_off);
@@ -113,7 +113,7 @@ static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image
     k_convert_bgr<<<(unsigned)((npx + 255) / 256), 256, 0, ctx->stream>>>(dC, dG, (int)npx);   // 8-bit grey, as cv::cvtColor leaves it
     ctx->launches++;
   }
-  return pyramid_build_batch_input(ctx, n, dG, dR, 1, depth_scale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM);
+  return pyramid_build_batch_input(ctx, n, dG, dR, 1, depth_scale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM, mask_roles);
 }
 
 }  // namespace dvo_b200
@@ -162,7 +162,7 @@ int dvo_b200_destroy(dvo_b200_ctx* ctx) {
   Workspace& ws = ctx->ws;
   cudaFree(ws.d_pair_level); cudaFree(ws.d_state); cudaFree(ws.d_row_exports); cudaFree(ws.d_row_base);
   cudaFree(ws.d_strip_exports); cudaFree(ws.d_strip_base); cudaFree(ws.d_row_partial); cudaFree(ws.d_strip_partial); cudaFree(ws.d_dump); cudaFree(ws.d_tinit);
-  cudaFree(ws.d_iter_log); cudaFree(ws.d_squads);
+  cudaFree(ws.d_iter_log); cudaFree(ws.d_squads); cudaFree(ws.d_csat);
   if (ws.h_active) cudaFreeHost(ws.h_active);
   pool_close(ctx);
   cudaFree(ctx->d_stage);
@@ -210,7 +210,7 @@ int dvo_b200_pyramid_create_batch(dvo_b200_ctx* ctx, int32_t n, const float* int
                                   dvo_b200_pyramid** out) {
   if (!ctx || !intensity || !depth || !out || n <= 0 || width <= 0 || height <= 0)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create: null/invalid argument");
-  return create_staged(ctx, n, DVO_B200_INPUT_FLOAT32, intensity, depth, 0.f, nullptr, width, height, fx, fy, ox, oy, levels, out);
+  return create_staged(ctx, n, DVO_B200_INPUT_FLOAT32, intensity, depth, 0.f, nullptr, 0, width, height, fx, fy, ox, oy, levels, out);
 }
 
 int dvo_b200_pyramid_create(dvo_b200_ctx* ctx, const float* intensity, const float* depth, int32_t width, int32_t height,
@@ -223,7 +223,7 @@ int dvo_b200_pyramid_create_raw_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_
                                       float oy, int32_t levels, dvo_b200_pyramid** out) {
   if (!ctx || !grey || !raw_depth || !out || n <= 0 || width <= 0 || height <= 0)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_raw: null/invalid argument");
-  return create_staged(ctx, n, DVO_B200_INPUT_GREY8_DEPTH16, grey, raw_depth, depth_scale, nullptr, width, height, fx, fy, ox, oy,
+  return create_staged(ctx, n, DVO_B200_INPUT_GREY8_DEPTH16, grey, raw_depth, depth_scale, nullptr, 0, width, height, fx, fy, ox, oy,
                        levels, out);
 }
 
@@ -232,7 +232,7 @@ int dvo_b200_pyramid_create_bgr_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_
                                       float oy, int32_t levels, dvo_b200_pyramid** out) {
   if (!ctx || !bgr || !raw_depth || !out || n <= 0 || width <= 0 || height <= 0)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_bgr: null/invalid argument");
-  return create_staged(ctx, n, DVO_B200_INPUT_BGR8_DEPTH16, bgr, raw_depth, depth_scale, nullptr, width, height, fx, fy, ox, oy,
+  return create_staged(ctx, n, DVO_B200_INPUT_BGR8_DEPTH16, bgr, raw_depth, depth_scale, nullptr, 0, width, height, fx, fy, ox, oy,
                        levels, out);
 }
 
@@ -243,8 +243,24 @@ int dvo_b200_pyramid_create_masked_batch(dvo_b200_ctx* ctx, int32_t n, int32_t f
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked: null/invalid argument");
   if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked: unknown input format " + std::to_string(format));
-  return create_staged(ctx, n, format, image, depth, depth_scale, masks, width, height, fx, fy, ox, oy, levels, out);
+  return create_staged(ctx, n, format, image, depth, depth_scale, masks, DVO_B200_MASK_ROLE_REFERENCE, width, height, fx, fy, ox,
+                       oy, levels, out);
 }
+
+int dvo_b200_pyramid_create_masked_batch_roles(dvo_b200_ctx* ctx, int32_t n, int32_t format, const void* image,
+                                               const void* depth, float depth_scale, const uint8_t* masks, int32_t roles,
+                                               int32_t width, int32_t height, float fx, float fy, float ox, float oy,
+                                               int32_t levels, dvo_b200_pyramid** out) {
+  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked_roles: null/invalid argument");
+  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked_roles: unknown input format " + std::to_string(format));
+  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked_roles: unsupported role set " + std::to_string(roles));
+  return create_staged(ctx, n, format, image, depth, depth_scale, masks, roles, width, height, fx, fy, ox, oy, levels, out);
+}
+
+int dvo_b200_pyramid_mask_roles(const dvo_b200_pyramid* p) { return p ? p->mask_roles : DVO_B200_ERR_INVALID_ARGUMENT; }
 
 int dvo_b200_pyramid_create_raw(dvo_b200_ctx* ctx, const uint8_t* grey, const uint16_t* raw_depth, float depth_scale,
                                 int32_t width, int32_t height, float fx, float fy, float ox, float oy, int32_t levels,
@@ -420,6 +436,8 @@ int dvo_b200_profile_read(dvo_b200_ctx* ctx, double ms_out[8], int64_t launches_
       if (u[0]) fprintf(stderr, "[dvo_b200 timing]   tiles %llu (inexact %.2f%%, skipped %.2f%%), stage-B rounds in the generic loop %.2f%%; CTA lifetime of the last launch-set: "
                                 "max %.3f ms, min %.3f ms\n", u[0], 100.0 * (double)u[1] / (double)u[0], 100.0 * (double)u[2] / (double)u[0],
                         100.0 * (double)u[4] / (double)(u[3] + 1), (double)u[5] * 1e-6, (double)u[6] * 1e-6);
+      if (u[7]) fprintf(stderr, "[dvo_b200 timing]   cmask tiles %llu (%.2f%% of all tiles): stage-B tiles that test the current image's mask "
+                                "per tap\n", u[7], 100.0 * (double)u[7] / (double)(u[0] + 1));
       const unsigned long long* e = h + 192 + 8 * l;   // e[7]: critical ns; e[0..5]: sub-phases
       if (e[7]) {
         double tot = 0;

@@ -46,7 +46,15 @@ struct LevelInfo {
   size_t mask_off;             // uint32 offset inside sel_mask
   size_t tmpl_off;             // float offset of tx[w] then ty[h] inside tmpl
   size_t range_off;            // float2 offset of the per-tile depth range {zmin, zmax} inside tile_range
+  size_t sat_off;              // int offset of the unusable-pixel summary inside cur_sat (BOTH pyramids only)
 };
+
+// Unusable-pixel summary of one level of a pyramid whose mask also acts in the CURRENT role: a summed-area table of the
+// unusable pixel counts over kSatBlock x kSatBlock blocks, (ceil(w/8) + 1) x (ceil(h/8) + 1) ints, row 0 and column 0 zero.
+// Whether a rectangle of the level holds an unusable pixel is then four loads (a conservative answer at block granularity).
+constexpr int kSatBlock = 8;
+__host__ __device__ __forceinline__ int sat_cols(int w) { return (w + kSatBlock - 1) / kSatBlock + 1; }
+__host__ __device__ __forceinline__ int sat_rows(int h) { return (h + kSatBlock - 1) / kSatBlock + 1; }
 
 // tile geometry of the level kernel (tracker.cu) and of the per-tile depth ranges (pyramid.cu)
 constexpr int kTileW = 128;    // reference pixels per tile row: 4 warp rounds
@@ -120,6 +128,8 @@ struct dvo_b200_pyramid {
   float* tmpl = nullptr;         // device: per level tx[w], ty[h] point-cloud template (rgbd_image.cpp:197-198)
   float2* tile_range = nullptr;  // device: per level, per tile {min, max} of the non-NaN Z' (min > max: none); of usable pixels only if masked
   uint32_t* usable = nullptr;    // device: per level usable bits of the reference mask, layout of sel_mask (NULL: built without a mask)
+  int* cur_sat = nullptr;        // device: per level unusable-pixel summary (see kSatBlock); only if the mask acts in the current role
+  int mask_roles = 0;            // 0: no mask; DVO_B200_MASK_ROLE_REFERENCE, optionally | DVO_B200_MASK_ROLE_CURRENT
   float sel_ti = 0.f, sel_td = 0.f;  // thresholds the masks were built with
   std::mutex sel_mu;                 // guards sel_ti / sel_td and the enqueueing of a re-selection
   uint64_t id = 0;
@@ -138,6 +148,12 @@ struct PairLevel {              // what one alignment reads at the current level
   const float2* c0; const float2* c3;  // current P0 (I, Z') and P2 (I, Z)
   float cfx, cfy, cox, coy;            // current-image intrinsics (dense_tracking.cpp:212)
   long long max_valid_pixels;          // PointSelection::getMaximumNumberOfPoints
+};
+// What a pair reads at the current level in the level kernel instance with current-role masks (tracker.cu, kCurMask).  The
+// summary pointer travels in an array of its own (Workspace::d_csat, same index as the descriptors): PairLevel is copied
+// to the stack of the level kernel, and a bigger PairLevel would change the stack frame of the default instances.
+struct CurPairLevel : PairLevel {
+  const int* csat;                     // unusable-pixel summary of the current image's level (NULL: no mask in the current role)
 };
 
 struct LevelSummary {           // device mirror of dvo_b200_level_stats
@@ -177,6 +193,7 @@ struct PairState {
 
 struct Workspace {              // per-ctx scratch of the level kernel
   PairLevel* d_pair_level = nullptr;
+  const int** d_csat = nullptr;      // per descriptor of d_pair_level: CurPairLevel::csat (only written for kCurMask launches)
   PairState* d_state = nullptr;
   float* d_row_exports = nullptr;    // per squad: one scale summary per image row (kSegExportFloats)
   int* d_row_base = nullptr;         // per squad, per row: valid points before the row inside its CTA
@@ -190,7 +207,7 @@ struct Workspace {              // per-ctx scratch of the level kernel
   int* h_active = nullptr;           // pinned: per level, the kernel's error flag
   char* d_squads = nullptr;          // persistent kernel: SquadState[nsquads] + {queue head, error flag}
   size_t cap_pairs = 0, cap_row_exports = 0, cap_row_base = 0, cap_strip_exports = 0, cap_strip_base = 0, cap_row_partial = 0, cap_strip_partial = 0,
-         cap_squads = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0;
+         cap_squads = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0;
 };
 
 }  // namespace dvo_b200
@@ -245,7 +262,8 @@ int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float*
                         float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out);
 int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const void* d_Z, int raw, float zscale, int w, int h,
                               float fx, float fy, float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out,
-                              const uint8_t* d_masks);   // d_masks: n*h*w device bytes, nonzero = usable reference pixel; or NULL
+                              const uint8_t* d_masks, int mask_roles);   // d_masks: n*h*w device bytes, nonzero = usable; or NULL
+                                                                         // mask_roles: DVO_B200_MASK_ROLE_* bits (ignored without masks)
 int pyramid_reselect(dvo_b200_ctx* ctx, dvo_b200_pyramid* p, float ti, float td);
 void wait_for_pyramid(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p);   // order ctx's stream after the pyramid's build / re-selection
 int note_foreign_use(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p);    // after enqueueing work that reads p (see Slab::foreign_uses)

@@ -218,6 +218,54 @@ __global__ void k_tile_range(const float2* __restrict__ planes, size_t planes_pe
   if (lane == 0) ranges[img * ranges_per_image + range_off + tile] = make_float2(lo, hi);
 }
 
+// Masks that also act in the CURRENT role, one level, after k_pyr_finish: one thread per kSatBlock x kSatBlock block writes
+// Z' = NaN into P0 at the block's unusable pixels -- the residual stage then rejects any point with an unusable bilinear
+// tap through its NaN test on the blended Z', as for a NaN depth -- and stores the block's unusable count into the
+// summary (cell (by + 1, bx + 1), summed up by k_cur_sat).  P2 keeps the true (I, Z), so the gradients of usable taps
+// next to an excluded region are those of the unmasked build.  Nothing else reads Z' at an unusable pixel: the selection,
+// the tile depth ranges and the odd last point only look at usable pixels, and the next level's intensity reads P0.x.
+__global__ void __launch_bounds__(256)
+k_cur_mask(float2* __restrict__ planes, size_t planes_per_image, size_t plane_off, int w, int h, int pitch,
+           const uint32_t* __restrict__ usable, size_t usable_per_image, size_t usable_off, int* __restrict__ sat,
+           size_t sat_per_image, size_t sat_off) {
+  const int img = blockIdx.y;
+  const int cols = sat_cols(w) - 1, rows = sat_rows(h) - 1;
+  const int blk = blockIdx.x * blockDim.x + threadIdx.x;
+  if (blk >= cols * rows) return;
+  const int by = blk / cols, bx = blk - by * cols;
+  float2* P0 = planes + img * planes_per_image + plane_off;
+  const uint32_t* U = usable + img * usable_per_image + usable_off;
+  const int x0 = bx * kSatBlock, y0 = by * kSatBlock;
+  const int x1 = min(x0 + kSatBlock, w), y1 = min(y0 + kSatBlock, h);
+  int cnt = 0;
+  for (int y = y0; y < y1; ++y)
+    for (int x = x0; x < x1; ++x)
+      if (!bit_set(U, (size_t)y * w + x)) {
+        ++cnt;
+        P0[(size_t)y * pitch + x].y = __int_as_float(0x7fc00000);
+      }
+  sat[img * sat_per_image + sat_off + (size_t)(by + 1) * (cols + 1) + bx + 1] = cnt;
+}
+
+// The summed-area table of one level from the block counts k_cur_mask stored: one CTA per image.
+__global__ void __launch_bounds__(256)
+k_cur_sat(int* __restrict__ sat, size_t sat_per_image, size_t sat_off, int w, int h) {
+  int* S = sat + blockIdx.x * sat_per_image + sat_off;
+  const int W = sat_cols(w), H = sat_rows(h);
+  for (int i = threadIdx.x; i < W; i += blockDim.x) S[i] = 0;
+  for (int j = threadIdx.x; j < H; j += blockDim.x) S[(size_t)j * W] = 0;
+  __syncthreads();
+  for (int j = 1 + threadIdx.x; j < H; j += blockDim.x) {   // rows
+    int acc = 0;
+    for (int i = 1; i < W; ++i) { acc += S[(size_t)j * W + i]; S[(size_t)j * W + i] = acc; }
+  }
+  __syncthreads();
+  for (int i = 1 + threadIdx.x; i < W; i += blockDim.x) {   // columns
+    int acc = 0;
+    for (int j = 1; j < H; ++j) { acc += S[(size_t)j * W + i]; S[(size_t)j * W + i] = acc; }
+  }
+}
+
 // {S, last selected linear index} of one (image, level) from its selection mask: one warp each
 __global__ void k_sel_info(const uint32_t* __restrict__ masks, size_t mask_words_per_image, size_t mask_off, int words,
                            int* __restrict__ sel_info, int sel_info_per_image, int level) {
@@ -393,19 +441,21 @@ void pool_close(dvo_b200_ctx* ctx) {
 
 int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float* d_Z, int w, int h, float fx, float fy,
                         float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out) {
-  return pyramid_build_batch_input(ctx, n, d_I, d_Z, 0, 0.f, w, h, fx, fy, ox, oy, levels, ti, td, out, nullptr);
+  return pyramid_build_batch_input(ctx, n, d_I, d_Z, 0, 0.f, w, h, fx, fy, ox, oy, levels, ti, td, out, nullptr, 0);
 }
 
 // d_I / d_Z: raw == 0: float32 intensity / float32 depth; raw == 1: 8-bit grey / 16-bit raw depth (depth = raw * zscale, 0 -> NaN)
 // d_masks: n consecutive h*w byte reference masks (nonzero = usable) or NULL.  Without masks the slab holds no usable bits
-// and the build runs exactly the kernels it ran before masks existed.
+// and the build runs exactly the kernels it ran before masks existed.  mask_roles with DVO_B200_MASK_ROLE_CURRENT: the
+// masks also act in the current role (k_cur_mask, k_cur_sat after the other kernels of each level); otherwise the build is
+// the reference-mask build, kernel for kernel.
 int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const void* d_Z, int raw, float zscale, int w, int h,
                               float fx, float fy, float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out,
-                              const uint8_t* d_masks) {
+                              const uint8_t* d_masks, int mask_roles) {
   if (n <= 0 || levels < 1 || levels > kMaxLevels || w < 32 || h < 2)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid: bad geometry");
   LevelInfo L[kMaxLevels];
-  size_t plane_f2 = 0, mask_words = 0, tmpl_floats = 0, range_f2 = 0;
+  size_t plane_f2 = 0, mask_words = 0, tmpl_floats = 0, range_f2 = 0, sat_ints = 0;
   for (int l = 0; l < levels; ++l) {
     LevelInfo& q = L[l];
     if (l == 0) { q.w = w; q.h = h; q.fx = fx; q.fy = fy; q.ox = ox; q.oy = oy; }
@@ -427,11 +477,13 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
     q.mask_off = mask_words; mask_words += q.words;
     q.tmpl_off = tmpl_floats; tmpl_floats += (size_t)((q.w + q.h + 3) & ~3);   // every level's tx[] starts 16-byte aligned (bulk copies)
     q.range_off = range_f2; range_f2 += (size_t)q.nbands * q.nstrips;
+    q.sat_off = sat_ints; sat_ints += (size_t)sat_cols(q.w) * sat_rows(q.h);
   }
   plane_f2 = align_up(plane_f2, 32);          // keep every image 256-byte aligned
   mask_words = align_up(mask_words, 64);
   tmpl_floats = align_up(tmpl_floats + kTileW, 64);   // lanes past a partial band read (and discard) up to kTileW floats beyond tx[w]
   range_f2 = align_up(range_f2, 32);
+  sat_ints = align_up(sat_ints, 64);
   const int sel_ints = 2 * kMaxLevels;
   size_t bytes_planes = (size_t)n * plane_f2 * sizeof(float2);
   size_t bytes_masks = (size_t)n * mask_words * sizeof(uint32_t);
@@ -440,7 +492,9 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
   size_t bytes_range = (size_t)n * range_f2 * sizeof(float2);
   const bool masked = d_masks != nullptr;
   size_t bytes_usable = masked ? bytes_masks : 0;   // usable bits: the layout of the selection masks
-  size_t total = bytes_planes + bytes_masks + bytes_tmpl + bytes_sel + bytes_range + bytes_usable;
+  const bool cur_masked = masked && (mask_roles & DVO_B200_MASK_ROLE_CURRENT) != 0;
+  size_t bytes_sat = cur_masked ? (size_t)n * sat_ints * sizeof(int) : 0;   // unusable-pixel summaries, after the usable bits
+  size_t total = bytes_planes + bytes_masks + bytes_tmpl + bytes_sel + bytes_range + bytes_usable + bytes_sat;
   Slab* slab = acquire_slab(ctx, total);
   if (!slab) return set_error(ctx, DVO_B200_ERR_OUT_OF_MEMORY, "pyramid: cudaMalloc failed");
   char* base = (char*)slab->base;
@@ -450,10 +504,11 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
   int* sel = (int*)(base + bytes_planes + bytes_masks + bytes_tmpl);
   float2* ranges = (float2*)(base + bytes_planes + bytes_masks + bytes_tmpl + bytes_sel);
   uint32_t* usable = masked ? (uint32_t*)(base + bytes_planes + bytes_masks + bytes_tmpl + bytes_sel + bytes_range) : nullptr;
+  int* sat = cur_masked ? (int*)(base + bytes_planes + bytes_masks + bytes_tmpl + bytes_sel + bytes_range + bytes_usable) : nullptr;
 
   cudaStream_t st = ctx->stream;
   {
-    ProfScope prof(ctx, 3, (masked ? 7 : 6) * levels - 1);
+    ProfScope prof(ctx, 3, (cur_masked ? 9 : masked ? 7 : 6) * levels - 1);
     const int T = 256;
     for (int l = 0; l < levels; ++l) {
       const LevelInfo& q = L[l];
@@ -494,6 +549,13 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
         k_tile_range<false><<<gr, 256, 0, st>>>(planes, plane_f2, q.plane_off, q.w, q.h, q.pitch, q.nbands, ntiles, ranges, range_f2,
                                                 q.range_off, nullptr, 0, 0);
       ctx->launches += 4;
+      if (cur_masked) {
+        const int nblk = (sat_cols(q.w) - 1) * (sat_rows(q.h) - 1);
+        k_cur_mask<<<dim3((nblk + T - 1) / T, n), T, 0, st>>>(planes, plane_f2, q.plane_off, q.w, q.h, q.pitch, usable, mask_words,
+                                                                q.mask_off, sat, sat_ints, q.sat_off);
+        k_cur_sat<<<n, T, 0, st>>>(sat, sat_ints, q.sat_off, q.w, q.h);
+        ctx->launches += 2;
+      }
     }
   }
   DVO_CUDA(ctx, cudaGetLastError());
@@ -510,6 +572,8 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
     p->tmpl = tmpl + (size_t)i * tmpl_floats;
     p->tile_range = ranges + (size_t)i * range_f2;
     p->usable = masked ? usable + (size_t)i * mask_words : nullptr;
+    p->cur_sat = cur_masked ? sat + (size_t)i * sat_ints : nullptr;
+    p->mask_roles = !masked ? 0 : cur_masked ? (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT) : DVO_B200_MASK_ROLE_REFERENCE;
     p->sel_ti = ti; p->sel_td = td;
     p->id = ctx->next_pyramid_id++;
     out[i] = p;

@@ -187,7 +187,8 @@ struct __align__(16) TileDesc {   // written by the producer before it arms the 
   int ulo, ucount;         // a tap (u0, v0) is served by the window iff (unsigned)(u0 - ulo) < ucount
   int vlo, vcount;         //                                       and (unsigned)(v0 - vlo) < vcount
   int exact;               // 1: the window holds the whole bounding box of the tile's taps -- no in-bounds tap can miss it
-  int pad_;
+  int cmask;               // stage B of a kCurMask kernel: 1 if a tap of the tile may be unusable in the current image (the
+                           // consumers then test every valid point's four taps); 0 otherwise and in every other kernel
 };
 struct __align__(128) StageBuf {
   // the reference tile record (common.cuh), filled by ONE bulk copy: stage A takes the first two members, stage B all three
@@ -210,7 +211,7 @@ static_assert(sizeof(TileDesc) == 32 && offsetof(TilePipe, desc) % 16 == 0, "Til
 #ifdef DVO_PIPE_TIMING
 struct PipeTiming {
   unsigned long long wait_full_a = 0, wait_full_b = 0, wait_empty = 0, produce = 0, rounds_a = 0, rounds_b = 0;
-  unsigned long long tiles = 0, tiles_inexact = 0, tiles_skipped = 0, slow_rounds = 0, rounds = 0;
+  unsigned long long tiles = 0, tiles_inexact = 0, tiles_skipped = 0, tiles_cmask = 0, slow_rounds = 0, rounds = 0;
   bool on = false;
 };
 #define DVO_CLOCK(tm) ((tm).on ? clock64() : 0)
@@ -269,7 +270,11 @@ __device__ __forceinline__ void load_stage_consts(const PairState& st, const Pai
 // that describe a window travel from the tile's lane group to the whole warp by shuffle.  (One tile per trip made
 // the producer the slowest warp of the CTA in stage A: ~600 instructions and two dependent global loads per tile
 // against ~500 instructions per consumer warp.)
-template <bool kStageB>
+// kCurMask (stage B only): pl is a CurPairLevel; the current image may have a mask in the current role (csat != NULL).  A tile whose exact
+// window touches an unusable block of the summary loses `exact` and gets `cmask`; so does every unskipped tile without an
+// exact window when the level has any unusable pixel (its taps may come from anywhere).  A clean exact window needs no
+// test: every tap lies inside it.  Stage A needs none of this: its taps read Z' = NaN at unusable pixels.
+template <bool kStageB, bool kCurMask = false>
 __device__ __noinline__ void produce_tiles(TilePipe& tp, const PairLevel& pl, const LevelGeom& g, const StageConsts& c, unsigned tbase,
                                            int ntiles, int* error_flag, PipeTiming& tm) {
   const int lane = threadIdx.x & 31, sub = lane >> 3;
@@ -278,7 +283,7 @@ __device__ __noinline__ void produce_tiles(TilePipe& tp, const PairLevel& pl, co
   for (int i0 = 0; i0 < ntiles; i0 += 4) {
     const long long tp0 = DVO_CLOCK(tm);
     // ---- windows of tiles i0 .. i0+3: corner rays x {zmin, zmax} (lane & 7 selects the corner, lane >> 3 the tile) ----
-    unsigned wordA, wordD;   // skip | exact << 1 | ncols << 2 | nrows << 10;  bx0 | (row_lo + 1) << 16
+    unsigned wordA, wordD;   // skip | exact << 1 | ncols << 2 | nrows << 10 | cmask << 31;  bx0 | (row_lo + 1) << 16
     {
       const int ii = min(i0 + sub, ntiles - 1);
       const int sd = ii / g.nbands;
@@ -324,7 +329,22 @@ __device__ __noinline__ void produce_tiles(TilePipe& tp, const PairLevel& pl, co
         if (ncols < 4 || nrows < 4) { ncols = 0; nrows = 0; bx0 = 0; row_lo = 0; }
         else exact = whole ? 1 : 0;
       }
-      wordA = (unsigned)skip | ((unsigned)exact << 1) | ((unsigned)ncols << 2) | ((unsigned)nrows << 10);
+      int cmask = 0;
+      const int* csat = nullptr;
+      if constexpr (kStageB && kCurMask) csat = static_cast<const CurPairLevel&>(pl).csat;
+      if (kStageB && kCurMask && csat != nullptr && !skip) {
+        const int sw = sat_cols(g.w);
+        if (exact) {   // the window's pixels inside the image: columns [bx0, bx0 + ncols - 1], rows [row_lo, row_lo + nrows - 1]
+          const int cx0 = bx0 >> 3, cx1 = (min(bx0 + ncols - 1, g.w - 1) >> 3) + 1;
+          const int cy0 = max(row_lo, 0) >> 3, cy1 = (min(row_lo + nrows - 1, g.h - 1) >> 3) + 1;
+          const int dirty = __ldg(csat + cy1 * sw + cx1) - __ldg(csat + cy0 * sw + cx1) - __ldg(csat + cy1 * sw + cx0) +
+                            __ldg(csat + cy0 * sw + cx0);
+          if (dirty) { exact = 0; cmask = 1; }
+        } else {       // taps from anywhere: any unusable pixel of the level
+          cmask = __ldg(csat + (sat_rows(g.h) - 1) * sw + sw - 1) != 0 ? 1 : 0;
+        }
+      }
+      wordA = (unsigned)skip | ((unsigned)exact << 1) | ((unsigned)ncols << 2) | ((unsigned)nrows << 10) | ((unsigned)cmask << 31);
       wordD = (unsigned)bx0 | ((unsigned)(row_lo + 1) << 16);
     }
     DVO_ADD(tm, produce, DVO_CLOCK(tm) - tp0);
@@ -337,10 +357,10 @@ __device__ __noinline__ void produce_tiles(TilePipe& tp, const PairLevel& pl, co
       const unsigned wa = __shfl_sync(kFullMask, wordA, k * 8), wd = __shfl_sync(kFullMask, wordD, k * 8);
       const int s = s_issue, b = b_issue;
       if (++b_issue == g.nbands) { b_issue = 0; s_issue += g.strip_step; }
-      const int skip = (int)(wa & 1u), ncols = (int)((wa >> 2) & 0xffu), nrows = (int)(wa >> 10);
+      const int skip = (int)(wa & 1u), ncols = (int)((wa >> 2) & 0xffu), nrows = (int)((kCurMask ? wa & 0x7fffffffu : wa) >> 10);
       const int win_bx0 = (int)(wd & 0xffffu), win_row_lo = (int)(wd >> 16) - 1;
       TileDesc d;
-      d.skip = skip; d.exact = (int)((wa >> 1) & 1u); d.pad_ = 0;
+      d.skip = skip; d.exact = (int)((wa >> 1) & 1u); d.cmask = kCurMask ? (int)(wa >> 31) : 0;
       d.origin = 0; d.ulo = 0; d.ucount = 0; d.vlo = 0; d.vcount = 0;
       if (ncols) {
         d.origin = (win_row_lo * kWinCols + win_bx0) * 8;
@@ -359,6 +379,7 @@ __device__ __noinline__ void produce_tiles(TilePipe& tp, const PairLevel& pl, co
       mbar_wait(&tp.empty[bufi], ((t / kStages) & 1u) ^ 1u, error_flag);
       DVO_ADD(tm, wait_empty, DVO_CLOCK(tm) - tp1);
       DVO_ADD(tm, tiles, 1); DVO_ADD(tm, tiles_inexact, (!d.skip && !d.exact) ? 1 : 0); DVO_ADD(tm, tiles_skipped, d.skip ? 1 : 0);
+      DVO_ADD(tm, tiles_cmask, d.cmask ? 1 : 0);
       if (lane == 0) {
         tp.desc[bufi] = d;
         if (total) mbar_arrive_expect_tx(&tp.full[bufi], total);
@@ -812,7 +833,7 @@ __device__ __forceinline__ void scale_state_export(ScaleState& st, int lane, flo
 __device__ __forceinline__ WinView make_view(unsigned bufs, const int4& d0, const int4& d1, const float2* plane, int w, int h, int pitch) {
   WinView wv;
   const unsigned w0 = bufs + (unsigned)offsetof(StageBuf, win);
-  wv.base = pin(w0 - (unsigned)d0.y);                       // TileDesc: {skip, origin, ulo, ucount}, {vlo, vcount, exact, pad}
+  wv.base = pin(w0 - (unsigned)d0.y);                       // TileDesc: {skip, origin, ulo, ucount}, {vlo, vcount, exact, cmask}
   wv.safe = pin(w0 + (unsigned)((kWinCols + 1) * 8));
   wv.plane = plane;
   wv.exact = d1.z != 0;
@@ -1054,11 +1075,13 @@ __device__ __noinline__ void dump_record(const RecordDump& dump, size_t i, bool 
 // dropped log-likelihood tail: strips that reach past n_keep (cta_has_tail, at most a few per level) take the generic loop.
 // pix: dump index of the lane's pixel in round 0.  kCorrected: no tail (every valid point is kept); the generic loop
 // re-admits the odd last point at tile column odd_col (-1: none), as stage_a_rounds does.
-template <bool kCorrected, bool kExact, bool kFirst, bool kDump>
+// kCurMask, generic loop, cmask (warp-uniform): a valid point also needs four usable taps -- four non-NaN Z' in the current
+// image's P0 (cur0), the very test stage A makes on its blended Z' -- so both stages keep the same points.
+template <bool kCorrected, bool kExact, bool kFirst, bool kDump, bool kCurMask = false>
 __device__ __forceinline__ void stage_b_rounds(const WinView& wv, int bw, unsigned refa, unsigned txa, float ty, const StageConsts& c,
                                                const StageBConsts& cb, StageBAcc& acc, bool cta_has_tail, int& rank, int keep_rank,
                                                const RecordDump& dump, size_t pix, int lane, unsigned lt_mask, int odd_col, float odd_z,
-                                               PipeTiming& tm) {
+                                               PipeTiming& tm, bool cmask = false, const float2* cur0 = nullptr) {
   const int nr = kExact ? kTileW / 32 : (bw + 31) >> 5;
   const int xlim = bw - lane;
   const bool first = kExact ? kFirst : c.first_iteration != 0;
@@ -1072,7 +1095,12 @@ __device__ __forceinline__ void stage_b_rounds(const WinView& wv, int bw, unsign
     if (kCorrected && !kExact) z = (r * 32 + lane == odd_col) ? odd_z : z;
     const PixelProjection p = project_pixel(tx, ty, z, c);
     f2 E, G, H;
-    const bool valid = record_pixel<kExact>(p, wv, lo(rz), z, gr, c, E, G, H);
+    bool valid = record_pixel<kExact>(p, wv, lo(rz), z, gr, c, E, G, H);
+    if (kCurMask && !kExact && cmask && valid) {   // valid: the taps lie inside the image
+      const float2* t = cur0 + (size_t)p.v0 * wv.pitch + p.u0;   // u0 may be odd: four 8-byte loads
+      const float z00 = __ldg(t).y, z10 = __ldg(t + 1).y, z01 = __ldg(t + wv.pitch).y, z11 = __ldg(t + wv.pitch + 1).y;
+      valid = z00 == z00 && z10 == z10 && z01 == z01 && z11 == z11;
+    }
     DVO_ADD(tm, rounds, 1); DVO_ADD(tm, slow_rounds, kExact ? 0 : 1);
     bool keep = valid;
     if (!kCorrected && !kExact && cta_has_tail) {   // warp-uniform
@@ -1094,7 +1122,8 @@ __device__ __forceinline__ void stage_b_rounds(const WinView& wv, int bw, unsign
 // when this CTA holds the tail of the point list); points with rank >= n_keep are the dropped tail of
 // computeCompleteDataLogLikelihood (dense_tracking_impl.cpp:413-422).  kCorrected: the log-likelihood keeps every point, so
 // no strip has a tail and ranks are never counted; the tile row that holds the odd last point takes the generic loop.
-template <bool kDump, bool kCorrected>
+// kCurMask: tiles with the cmask bit take the generic loop with the per-tap mask test (produce_tiles clears their `exact`).
+template <bool kDump, bool kCorrected, bool kCurMask = false>
 __device__ __forceinline__ void stage_b_run(TilePipe& tp, const PairLevel& pl, const LevelGeom& g, const StageConsts& c,
                                             const StageBConsts& cb, const int* row_base, const int* strip_base, long long n_keep,
                                             const RecordDump& dump, float* row_partial, unsigned& tile_count, int* error_flag,
@@ -1105,7 +1134,7 @@ __device__ __forceinline__ void stage_b_run(TilePipe& tp, const PairLevel& pl, c
   const unsigned tbase = tile_count;
   tile_count += ntiles;
   if (q == kConsumerWarps) {   // the producer warp
-    produce_tiles<true>(tp, pl, g, c, tbase, ntiles, error_flag, tm);
+    produce_tiles<true, kCurMask>(tp, pl, g, c, tbase, ntiles, error_flag, tm);
     return;
   }
   int i = 0;
@@ -1155,8 +1184,9 @@ __device__ __forceinline__ void stage_b_run(TilePipe& tp, const PairLevel& pl, c
             stage_b_rounds<kCorrected, true, false, kDump>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank, dump, pix, lane,
                                                            lt_mask, -1, 0.f, tm);
         } else {
-          stage_b_rounds<kCorrected, false, false, kDump>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank, dump, pix, lane,
-                                                          lt_mask, odd_tile ? odd.x - x0 : -1, odd.z, tm);
+          stage_b_rounds<kCorrected, false, false, kDump, kCurMask>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank, dump,
+                                                                    pix, lane, lt_mask, odd_tile ? odd.x - x0 : -1, odd.z, tm,
+                                                                    kCurMask && d1.w != 0, pl.c0);
         }
       } else if (kDump && row_ok) {
         for (int xl = lane; xl < bw; xl += 32) dump_record(dump, (size_t)y * gw + x0 + xl, false, bc(0.f), bc(0.f), bc(0.f), 0.f);

@@ -400,6 +400,23 @@ struct PersistentArgs {
   int npairs;
   int nseg;               // 1, or >= 2 = fused launch: coarse segment + slices of the fine levels
   Segment seg[kMaxSeg];
+  const PairLevel* pls0;  // kCurMask: csat[i] belongs to the descriptor pls0[i]
+  const int* const* csat;
+};
+
+// The descriptor of one pair at one level of a segment: a PairLevel, or with kCurMask a CurPairLevel.
+template <bool kCurMask> struct LevelOf {
+  using type = PairLevel;
+  static __device__ __forceinline__ PairLevel load(const PersistentArgs& a, const Segment& S, size_t i) { return S.pls[i]; }
+};
+template <> struct LevelOf<true> {
+  using type = CurPairLevel;
+  static __device__ __forceinline__ CurPairLevel load(const PersistentArgs& a, const Segment& S, size_t i) {
+    CurPairLevel q;
+    static_cast<PairLevel&>(q) = S.pls[i];
+    q.csat = a.csat[(size_t)(S.pls - a.pls0) + i];
+    return q;
+  }
 };
 
 __device__ __forceinline__ unsigned long long global_ns() {
@@ -446,7 +463,10 @@ __device__ __forceinline__ void squad_wait(SquadState* sq, unsigned episode, int
 }
 
 // kCorrected: the corrected estimator (dvo_b200_estimator), one instance per value, chosen per launch.
-template <bool kCorrected>
+// kCurMask: some pair's current image has a mask in the current role (PairLevel::csat); stage B then tests the taps of the
+// tiles whose window touches an unusable pixel (produce_tiles, stage_b_rounds).  Without it the instance is the one that
+// existed before current-role masks.
+template <bool kCorrected, bool kCurMask = false>
 __global__ void __launch_bounds__(kCtaThreads, 2)
 k_level_persistent(const __grid_constant__ PersistentArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -536,7 +556,7 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
     // ---- the squad walks its pair through the levels of this launch, coarse to fine ----
     for (int li = 0; li < S.nlev; ++li) {
     const LevelLaunch& lp = S.lp[li];
-    const PairLevel pl = S.pls[(size_t)li * a.npairs + pair];
+    const typename LevelOf<kCurMask>::type pl = LevelOf<kCurMask>::load(a, S, (size_t)li * a.npairs + pair);
     LevelGeom geo;
     geo.w = lp.w; geo.h = lp.h; geo.n = lp.n; geo.pitch = lp.pitch; geo.nbands = lp.nbands; geo.nstrips = lp.nstrips;
     if (S.cyclic) {   // CTA r takes strips r, r + g, r + 2g, ...: every CTA of the squad samples the whole image
@@ -608,8 +628,8 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
         RecordDump dump;
         dump.planes = a.dump; dump.n = lp.n;
         const long long ts0 = DVO_CLOCK(tm);
-        if (a.dump) stage_b_run<true, kCorrected>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
-        else stage_b_run<false, kCorrected>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
+        if (a.dump) stage_b_run<true, kCorrected, kCurMask>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
+        else stage_b_run<false, kCorrected, kCurMask>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
         DVO_ADD(tm, rounds_b, DVO_CLOCK(tm) - ts0);
       }
       __syncthreads();
@@ -663,7 +683,7 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
     if (warp == 0) { atomicAdd(S.dbg + 8, tm.rounds_a); atomicAdd(S.dbg + 9, tm.wait_full_a); atomicAdd(S.dbg + 10, tm.rounds_b); atomicAdd(S.dbg + 11, tm.wait_full_b); }
     else { atomicAdd(S.dbg + 12, tm.produce); atomicAdd(S.dbg + 13, tm.wait_empty); atomicAdd(S.dbg + 14, tm.rounds_a); atomicAdd(S.dbg + 15, tm.rounds_b); }
     if (warp == 0) { atomicAdd(S.dbg2 + 3, tm.rounds); atomicAdd(S.dbg2 + 4, tm.slow_rounds); }
-    else { atomicAdd(S.dbg2 + 0, tm.tiles); atomicAdd(S.dbg2 + 1, tm.tiles_inexact); atomicAdd(S.dbg2 + 2, tm.tiles_skipped); }
+    else { atomicAdd(S.dbg2 + 0, tm.tiles); atomicAdd(S.dbg2 + 1, tm.tiles_inexact); atomicAdd(S.dbg2 + 2, tm.tiles_skipped); atomicAdd(S.dbg2 + 7, tm.tiles_cmask); }
   }
   if (timing) { atomicMax(S.dbg2 + 5, t_acc[7]); atomicMin(S.dbg2 + 6, t_acc[7]); }
 #endif
@@ -779,9 +799,10 @@ int ensure_geometry(dvo_b200_ctx* ctx) {
   if (ctx->num_sms != 0) return 0;
   cudaDeviceProp prop;
   DVO_CUDA(ctx, cudaGetDeviceProperties(&prop, ctx->device));
-  // one grid for both estimator instances: the smaller of their occupancies (both are bounded to 128 registers, so equal)
+  // one grid for every instance: the smaller of their occupancies (all are bounded to 128 registers, so equal)
   int per_sm = 1 << 30;
-  for (auto kern : {k_level_persistent<false>, k_level_persistent<true>}) {
+  for (auto kern : {k_level_persistent<false, false>, k_level_persistent<true, false>, k_level_persistent<false, true>,
+                    k_level_persistent<true, true>}) {
     DVO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLevelSmemBytes));
     int k_per_sm = 0;
     DVO_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k_per_sm, kern, kCtaThreads, kLevelSmemBytes));
@@ -930,6 +951,17 @@ void fill_pair_levels(PairLevel* h, int n, dvo_b200_pyramid* const* refs, dvo_b2
     q.max_valid_pixels = (long long)(size_t)((double)r->L[0].n * pow(0.25, (double)level));
   }
 }
+// CurPairLevel::csat of the same pairs (kCurMask launches)
+void fill_pair_csat(const int** h, int n, dvo_b200_pyramid* const* curs, int level) {
+  for (int i = 0; i < n; ++i) h[i] = curs[i]->cur_sat ? curs[i]->cur_sat + curs[i]->L[level].sat_off : nullptr;
+}
+
+// The level kernel instance with the current-role mask test: iff some pair's current pyramid has a mask in that role.
+bool any_current_mask(int n, dvo_b200_pyramid* const* curs) {
+  for (int i = 0; i < n; ++i)
+    if (curs[i]->cur_sat) return true;
+  return false;
+}
 
 LevelLaunch make_level_launch(const LevelInfo& L, const dvo_b200_config* cfg, int li, int level) {
   LevelLaunch lp;
@@ -975,7 +1007,7 @@ void add_launch_need(ScratchNeed& need, int nseg, const int* hmax, const GroupPl
 // zeroed first.  lps / d_pls: per segment.  `flag_out` receives the device address of the launch's error flag.
 int launch_segments(dvo_b200_ctx* ctx, int nseg, const LevelLaunch (*lps)[kMaxLevels], const GroupPlan* plans, const int* hmax,
                     const PairLevel* const* d_pls, const double* d_Tinit, int npairs, int max_log, float* dump, int skip_begin,
-                    int group_index, int** flag_out) {
+                    int group_index, bool cur_mask, int** flag_out) {
   Workspace& ws = ctx->ws;
   cudaStream_t st = ctx->stream;
   size_t nsq = 0;
@@ -992,6 +1024,7 @@ int launch_segments(dvo_b200_ctx* ctx, int nseg, const LevelLaunch (*lps)[kMaxLe
   pa.T_init = d_Tinit; pa.skip_begin = skip_begin;
   pa.dump = dump;
   pa.npairs = npairs; pa.nseg = nseg;
+  pa.pls0 = ws.d_pair_level; pa.csat = ws.d_csat;
   ScratchNeed off;
   size_t sq_off = 0;
   for (int s = 0; s < nseg; ++s) {
@@ -1023,8 +1056,9 @@ int launch_segments(dvo_b200_ctx* ctx, int nseg, const LevelLaunch (*lps)[kMaxLe
     ProfScope prof(ctx, 0);
     ProfScope prof_level(ctx, 8 + std::min(group_index, 7));
     void* args[] = {&pa};
-    const void* kern = ctx->estimator == DVO_B200_ESTIMATOR_CORRECTED ? (const void*)k_level_persistent<true>
-                                                                      : (const void*)k_level_persistent<false>;
+    const bool corrected = ctx->estimator == DVO_B200_ESTIMATOR_CORRECTED;
+    const void* kern = cur_mask ? (corrected ? (const void*)k_level_persistent<true, true> : (const void*)k_level_persistent<false, true>)
+                                : (corrected ? (const void*)k_level_persistent<true, false> : (const void*)k_level_persistent<false, false>);
     DVO_CUDA(ctx, cudaLaunchCooperativeKernel(kern, dim3(ctx->num_sms * ctx->ctas_per_sm),
                                               dim3(kCtaThreads), args, kLevelSmemBytes, st));
     ctx->launches++;
@@ -1119,13 +1153,19 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   const size_t desc_bytes = (sizeof(PairLevel) * (size_t)n * nlev + 15) / 16 * 16;
   const bool have_init = cfg->use_initial_estimate && T_init;
   const size_t init_bytes = have_init ? sizeof(double) * 16 * (size_t)n : 0;
-  if ((rc = ensure_stage(ctx, 0, desc_bytes + init_bytes))) return rc;
+  const bool cur_mask = any_current_mask(n, curs);
+  const size_t csat_bytes = cur_mask ? (sizeof(const int*) * (size_t)n * nlev + 15) / 16 * 16 : 0;
+  if ((rc = ensure_stage(ctx, 0, desc_bytes + init_bytes + csat_bytes))) return rc;
+  if (cur_mask && (rc = grow(ctx, ws.d_csat, ws.cap_csat, csat_bytes / sizeof(const int*)))) return rc;
   if ((rc = grow(ctx, ws.d_tinit, ws.cap_tinit, (size_t)16 * n))) return rc;
   DVO_CUDA(ctx, cudaStreamSynchronize(st));   // previous use of the pinned stage has drained
   PairLevel* h_desc = (PairLevel*)ctx->h_stage;
   for (int level = first, li = 0; level >= last; --level, ++li) fill_pair_levels(h_desc + (size_t)li * n, n, refs, curs, level);
   if (have_init) std::memcpy((char*)ctx->h_stage + desc_bytes, T_init, init_bytes);
-  ctx->h2d_bytes += desc_bytes + init_bytes;
+  const int** h_csat = (const int**)((char*)ctx->h_stage + desc_bytes + init_bytes);
+  if (cur_mask)
+    for (int level = first, li = 0; level >= last; --level, ++li) fill_pair_csat(h_csat + (size_t)li * n, n, curs, level);
+  ctx->h2d_bytes += desc_bytes + init_bytes + csat_bytes;
   {
     ProfScope prof(ctx, 2);
     const size_t n16 = desc_bytes / 16;
@@ -1134,6 +1174,11 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
     if (have_init) {
       const size_t m16 = init_bytes / 16;
       k_stage_words<<<(unsigned)((m16 + 255) / 256), 256, 0, st>>>((const uint4*)((char*)ctx->h_stage + desc_bytes), (uint4*)ws.d_tinit, m16);
+      ctx->launches++;
+    }
+    if (cur_mask) {
+      const size_t c16 = csat_bytes / 16;
+      k_stage_words<<<(unsigned)((c16 + 255) / 256), 256, 0, st>>>((const uint4*)h_csat, (uint4*)ws.d_csat, c16);
       ctx->launches++;
     }
   }
@@ -1160,14 +1205,15 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
       seg_pls[sgi] = d_pls[gi];
     }
     int* flag = nullptr;
-    if ((rc = launch_segments(ctx, nseg, seg_lps, segs, seg_hmax, seg_pls, have_init ? ws.d_tinit : nullptr, n, max_log, nullptr, 0, 0, &flag)))
+    if ((rc = launch_segments(ctx, nseg, seg_lps, segs, seg_hmax, seg_pls, have_init ? ws.d_tinit : nullptr, n, max_log, nullptr, 0, 0,
+                              cur_mask, &flag)))
       return rc;
     DVO_CUDA(ctx, cudaMemcpyAsync(&ws.h_active[level_flag_slot(0)], flag, sizeof(int), cudaMemcpyDeviceToHost, st));
   } else {
     for (int gi = 0; gi < nlaunch; ++gi) {
       int* flag = nullptr;
       if ((rc = launch_segments(ctx, 1, lps + gi, groups + gi, hmaxs + gi, d_pls + gi, have_init ? ws.d_tinit : nullptr, n, max_log,
-                                nullptr, 0, gi, &flag)))
+                                nullptr, 0, gi, cur_mask, &flag)))
         return rc;
       DVO_CUDA(ctx, cudaMemcpyAsync(&ws.h_active[level_flag_slot(gi)], flag, sizeof(int), cudaMemcpyDeviceToHost, st));
     }
@@ -1258,9 +1304,16 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
   lp.max_iterations = use_weights ? 2 : 1;    // k_set_state starts at iteration 1 / 0: exactly one iteration runs
   lp.first_level = 1; lp.use_initial_estimate = 0; lp.precision = 0.0; lp.mu = 0.0;
   if ((rc = ensure_stage(ctx, 1024, sizeof(PairLevel) + 1024))) return rc;
+  const bool cur_mask = any_current_mask(1, curs);
+  if (cur_mask && (rc = grow(ctx, ws.d_csat, ws.cap_csat, 2))) return rc;
   DVO_CUDA(ctx, cudaStreamSynchronize(st));
   fill_pair_levels((PairLevel*)ctx->h_stage, 1, refs, curs, level);
   DVO_CUDA(ctx, cudaMemcpyAsync(ws.d_pair_level, ctx->h_stage, sizeof(PairLevel), cudaMemcpyHostToDevice, st));
+  if (cur_mask) {
+    const int** h_csat = (const int**)((char*)ctx->h_stage + 512);
+    fill_pair_csat(h_csat, 1, curs, level);
+    DVO_CUDA(ctx, cudaMemcpyAsync(ws.d_csat, h_csat, sizeof(const int*), cudaMemcpyHostToDevice, st));
+  }
   DVO_CUDA(ctx, cudaStreamSynchronize(st));
   std::memcpy(ctx->h_stage, T, sizeof(double) * 16);
   float pp[4] = {0, 0, 0, 0};
@@ -1277,7 +1330,8 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
   lps[0][0] = lp;
   const int hm = L.h;
   const PairLevel* d_pls[1] = {ws.d_pair_level};
-  if ((rc = launch_segments(ctx, 1, lps, &plan, &hm, d_pls, nullptr, 1, 0, planes7 ? ws.d_dump : nullptr, 1, 0, &flag))) return rc;
+  if ((rc = launch_segments(ctx, 1, lps, &plan, &hm, d_pls, nullptr, 1, 0, planes7 ? ws.d_dump : nullptr, 1, 0, cur_mask, &flag)))
+    return rc;
   DVO_CUDA(ctx, cudaMemcpyAsync(&ws.h_active[0], flag, sizeof(int), cudaMemcpyDeviceToHost, st));
   DVO_CUDA(ctx, cudaGetLastError());
   if ((rc = note_foreign_uses(ctx, 1, refs, curs))) return rc;

@@ -30,6 +30,7 @@ ABI_SYMBOLS = [
     "dvo_b200_sharded_num_shards", "dvo_b200_sharded_ctx", "dvo_b200_sharded_last_error", "dvo_b200_shard_range",
     "dvo_b200_sharded_pyramid_create_batch", "dvo_b200_sharded_pyramid_create_raw_batch", "dvo_b200_match_batch_sharded",
     "dvo_b200_set_estimator", "dvo_b200_get_estimator", "dvo_b200_pyramid_create_masked_batch",
+    "dvo_b200_pyramid_create_masked_batch_roles", "dvo_b200_pyramid_mask_roles",
 ]
 
 # dvo_b200_estimator
@@ -37,6 +38,9 @@ ESTIMATORS = {"reference": 0, "corrected": 1}
 
 # dvo_b200_input_format (dvo_b200_pyramid_create_masked_batch)
 INPUT_FORMATS = {"float32": 0, "grey8_depth16": 1, "bgr8_depth16": 2}
+
+# role sets of a mask (DVO_B200_MASK_ROLE_*): "reference" = the selection only, "both" = also the current image's taps
+MASK_ROLES = {"reference": 1, "both": 3}
 
 
 class Config(C.Structure):
@@ -129,6 +133,9 @@ def load_library():
     L.dvo_b200_pyramid_create_bgr_batch.argtypes = [vp, i32, vp, vp, C.c_float, i32, i32, C.c_float, C.c_float, C.c_float, C.c_float, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_create_masked_batch.argtypes = [vp, i32, i32, vp, vp, C.c_float, vp, i32, i32, C.c_float, C.c_float, C.c_float,
                                                        C.c_float, i32, C.POINTER(vp)]
+    L.dvo_b200_pyramid_create_masked_batch_roles.argtypes = [vp, i32, i32, vp, vp, C.c_float, vp, i32, i32, i32, C.c_float, C.c_float,
+                                                             C.c_float, C.c_float, i32, C.POINTER(vp)]
+    L.dvo_b200_pyramid_mask_roles.argtypes = [vp]
     L.dvo_b200_pyramid_device.argtypes = [vp]
     L.dvo_b200_sharded_create.argtypes = [i32, C.POINTER(i32), C.POINTER(vp)]
     L.dvo_b200_sharded_destroy.argtypes = [vp]
@@ -179,6 +186,13 @@ class Pyramid:
         K = (C.c_float * 4)()
         self.engine._check(load_library().dvo_b200_pyramid_level_info(self.handle, level, C.byref(w), C.byref(h), K))
         return w.value, h.value, tuple(K)
+
+    @property
+    def mask_roles(self) -> str | None:
+        """None (no mask), "reference" or "both" (see Engine.pyramid)"""
+        r = load_library().dvo_b200_pyramid_mask_roles(self.handle)
+        self.engine._check(min(r, 0))
+        return {0: None, 1: "reference", 3: "both"}[r]
 
     def download(self, level: int) -> np.ndarray:
         w, h, _ = self.level_info(level)
@@ -270,7 +284,11 @@ class Engine:
     # ---- pyramids ----
     # mask= / masks=: reference masks (dvo_b200_pyramid_create_masked_batch): None, an array of n*h*w values (nonzero = usable
     # reference pixel; shape [h, w] or [n, h, w]) or, for the host-pointer forms, a host pointer (int) to n*h*w bytes.
-    def _create_masked(self, n, fmt, pI, pZ, depth_scale, masks, w, h, intrinsics, levels) -> list[Pyramid]:
+    # mask_roles="reference" (default): the mask keeps its pixels out of the point selection; "both": also out of the
+    # bilinear taps when the pyramid is the current image of an alignment (dvo_b200_pyramid_create_masked_batch_roles).
+    def _create_masked(self, n, fmt, pI, pZ, depth_scale, masks, w, h, intrinsics, levels, mask_roles="reference") -> list[Pyramid]:
+        if mask_roles not in MASK_ROLES:
+            raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
         keep = None
         if isinstance(masks, int):
             pM = masks
@@ -281,19 +299,19 @@ class Engine:
             pM = keep.ctypes.data
         fx, fy, ox, oy = intrinsics
         out = (C.c_void_p * n)()
-        self._check(self.lib.dvo_b200_pyramid_create_masked_batch(self.ctx, n, INPUT_FORMATS[fmt], pI, pZ, depth_scale, pM, w, h,
-                                                                  fx, fy, ox, oy, levels, out))
+        self._check(self.lib.dvo_b200_pyramid_create_masked_batch_roles(self.ctx, n, INPUT_FORMATS[fmt], pI, pZ, depth_scale, pM,
+                                                                        MASK_ROLES[mask_roles], w, h, fx, fy, ox, oy, levels, out))
         if keep is not None and keep is not masks:
             self.synchronize()   # the converted copy dies with this call
         return [Pyramid(self, out[i]) for i in range(n)]
 
-    def pyramid(self, intensity, depth, intrinsics, levels: int, mask=None) -> Pyramid:
+    def pyramid(self, intensity, depth, intrinsics, levels: int, mask=None, mask_roles="reference") -> Pyramid:
         I = np.ascontiguousarray(intensity, dtype=np.float32)
         Z = np.ascontiguousarray(depth, dtype=np.float32)
         assert I.ndim == 2 and I.shape == Z.shape
         h, w = I.shape
         if mask is not None:
-            p = self._create_masked(1, "float32", I.ctypes.data, Z.ctypes.data, 0.0, mask, w, h, intrinsics, levels)[0]
+            p = self._create_masked(1, "float32", I.ctypes.data, Z.ctypes.data, 0.0, mask, w, h, intrinsics, levels, mask_roles)[0]
             self.synchronize()
             return p
         fx, fy, ox, oy = intrinsics
@@ -302,17 +320,17 @@ class Engine:
         self.synchronize()  # numpy temporaries may die
         return Pyramid(self, out.value)
 
-    def pyramid_batch(self, intensity, depth, intrinsics, levels: int, host_ptrs=None, masks=None) -> list[Pyramid]:
+    def pyramid_batch(self, intensity, depth, intrinsics, levels: int, host_ptrs=None, masks=None, mask_roles="reference") -> list[Pyramid]:
         """intensity/depth: [n,h,w] float32 arrays, or (ptr_I, ptr_Z, n, h, w) raw host pointers via host_ptrs."""
         if masks is not None:
             if host_ptrs is not None:
                 pI, pZ, n, h, w = host_ptrs
-                return self._create_masked(n, "float32", pI, pZ, 0.0, masks, w, h, intrinsics, levels)
+                return self._create_masked(n, "float32", pI, pZ, 0.0, masks, w, h, intrinsics, levels, mask_roles)
             I = np.ascontiguousarray(intensity, dtype=np.float32)
             Z = np.ascontiguousarray(depth, dtype=np.float32)
             assert I.ndim == 3 and I.shape == Z.shape
             n, h, w = I.shape
-            out = self._create_masked(n, "float32", I.ctypes.data, Z.ctypes.data, 0.0, masks, w, h, intrinsics, levels)
+            out = self._create_masked(n, "float32", I.ctypes.data, Z.ctypes.data, 0.0, masks, w, h, intrinsics, levels, mask_roles)
             self.synchronize()
             return out
         if host_ptrs is not None:
@@ -330,34 +348,35 @@ class Engine:
             self.synchronize()
         return [Pyramid(self, out[i]) for i in range(n)]
 
-    def pyramid_raw_batch(self, host_ptrs, depth_scale, intrinsics, levels: int, masks=None) -> list[Pyramid]:
+    def pyramid_raw_batch(self, host_ptrs, depth_scale, intrinsics, levels: int, masks=None, mask_roles="reference") -> list[Pyramid]:
         """host_ptrs = (ptr_grey_u8, ptr_depth_u16, n, h, w): n consecutive raw images in (pinned) host memory."""
         pG, pD, n, h, w = host_ptrs
         if masks is not None:
-            return self._create_masked(n, "grey8_depth16", pG, pD, depth_scale, masks, w, h, intrinsics, levels)
+            return self._create_masked(n, "grey8_depth16", pG, pD, depth_scale, masks, w, h, intrinsics, levels, mask_roles)
         fx, fy, ox, oy = intrinsics
         out = (C.c_void_p * n)()
         self._check(self.lib.dvo_b200_pyramid_create_raw_batch(self.ctx, n, pG, pD, depth_scale, w, h, fx, fy, ox, oy, levels, out))
         return [Pyramid(self, out[i]) for i in range(n)]
 
-    def pyramid_bgr_batch(self, host_ptrs, depth_scale, intrinsics, levels: int, masks=None) -> list[Pyramid]:
+    def pyramid_bgr_batch(self, host_ptrs, depth_scale, intrinsics, levels: int, masks=None, mask_roles="reference") -> list[Pyramid]:
         """host_ptrs = (ptr_bgr_u8x3, ptr_depth_u16, n, h, w): n consecutive interleaved-BGR images and raw depth images
         in (pinned) host memory; grey conversion (OpenCV BGR2GRAY) and depth scaling run on the device."""
         pC, pD, n, h, w = host_ptrs
         if masks is not None:
-            return self._create_masked(n, "bgr8_depth16", pC, pD, depth_scale, masks, w, h, intrinsics, levels)
+            return self._create_masked(n, "bgr8_depth16", pC, pD, depth_scale, masks, w, h, intrinsics, levels, mask_roles)
         fx, fy, ox, oy = intrinsics
         out = (C.c_void_p * n)()
         self._check(self.lib.dvo_b200_pyramid_create_bgr_batch(self.ctx, n, pC, pD, depth_scale, w, h, fx, fy, ox, oy, levels, out))
         return [Pyramid(self, out[i]) for i in range(n)]
 
-    def pyramid_raw(self, grey_u8, depth_u16, depth_scale, intrinsics, levels: int, mask=None) -> Pyramid:
+    def pyramid_raw(self, grey_u8, depth_u16, depth_scale, intrinsics, levels: int, mask=None, mask_roles="reference") -> Pyramid:
         G = np.ascontiguousarray(grey_u8, dtype=np.uint8)
         D = np.ascontiguousarray(depth_u16, dtype=np.uint16)
         assert G.ndim == 2 and G.shape == D.shape
         h, w = G.shape
         if mask is not None:
-            p = self._create_masked(1, "grey8_depth16", G.ctypes.data, D.ctypes.data, depth_scale, mask, w, h, intrinsics, levels)[0]
+            p = self._create_masked(1, "grey8_depth16", G.ctypes.data, D.ctypes.data, depth_scale, mask, w, h, intrinsics, levels,
+                                    mask_roles)[0]
             self.synchronize()
             return p
         fx, fy, ox, oy = intrinsics

@@ -40,7 +40,7 @@ const RgbdCamera& RgbdCameraPyramid::level(size_t level) const { return *levels_
 
 // ---- image pyramid ----------------------------------------------------------------------------------
 RgbdImagePyramid::RgbdImagePyramid(RgbdCameraPyramid& camera, const cv::Mat& intensity, const cv::Mat& depth)
-    : camera_(camera), device_(0), device_ctx_(0), device_levels_(0), requested_levels_(1) {
+    : camera_(camera), mask_current_(false), device_(0), device_ctx_(0), device_levels_(0), requested_levels_(1) {
   levels_.push_back(camera_.level(0).create(intensity, depth));
 }
 RgbdImagePyramid::~RgbdImagePyramid() {
@@ -54,12 +54,20 @@ void RgbdImagePyramid::build(const size_t num_levels) {
 }
 double RgbdImagePyramid::timestamp() const { return !levels_.empty() ? levels_[0]->timestamp : 0.0; }
 
-bool RgbdImagePyramid::setReferenceMask(const cv::Mat& mask) {
+bool RgbdImagePyramid::setReferenceMask(const cv::Mat& mask) { return setMask(mask, false); }
+
+bool RgbdImagePyramid::setMask(const cv::Mat& mask, bool current_role_too) {
   std::lock_guard<std::mutex> lock(mutex_);
   const RgbdImage& l0 = *levels_[0];
   if (device_ || mask.type() != CV_8UC1 || mask.rows != l0.intensity.rows || mask.cols != l0.intensity.cols) return false;
   mask_ = mask.clone();
+  mask_current_ = current_role_too;
   return true;
+}
+
+// the role set of a pyramid's mask (dvo_b200_pyramid_create_masked_batch_roles)
+static int32_t mask_roles(bool current_role_too) {
+  return current_role_too ? DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT : DVO_B200_MASK_ROLE_REFERENCE;
 }
 
 // the reference mask as n*h*w contiguous bytes (a cv::Mat need not be continuous), or empty without one
@@ -81,10 +89,11 @@ dvo_b200_pyramid* RgbdImagePyramid::device(dvo_b200_ctx* ctx, size_t levels) {
   const IntrinsicMatrix& k = camera_.level(0).intrinsics();
   std::vector<uint8_t> mask;
   if (!mask_.empty()) append_mask(mask_, l0.intensity.cols, l0.intensity.rows, mask);
-  int rc = dvo_b200_pyramid_create_masked_batch(ctx, 1, DVO_B200_INPUT_FLOAT32, l0.intensity.ptr<float>(), l0.depth.ptr<float>(), 0.f,
-                                                mask.empty() ? nullptr : mask.data(), l0.intensity.cols, l0.intensity.rows,
-                                                k.fx(), k.fy(), k.ox(), k.oy(), int(levels), &device_);
-  if (rc != 0) throw std::runtime_error(std::string("dvo_b200_pyramid_create_masked_batch: ") + dvo_b200_last_error(ctx));
+  int rc = dvo_b200_pyramid_create_masked_batch_roles(ctx, 1, DVO_B200_INPUT_FLOAT32, l0.intensity.ptr<float>(), l0.depth.ptr<float>(),
+                                                      0.f, mask.empty() ? nullptr : mask.data(), mask_roles(mask_current_),
+                                                      l0.intensity.cols, l0.intensity.rows, k.fx(), k.fy(), k.ox(), k.oy(), int(levels),
+                                                      &device_);
+  if (rc != 0) throw std::runtime_error(std::string("dvo_b200_pyramid_create_masked_batch_roles: ") + dvo_b200_last_error(ctx));
   dvo_b200_synchronize(ctx);   // the host cv::Mat may be released by the caller
   device_ctx_ = ctx;
   device_levels_ = levels;
@@ -109,34 +118,48 @@ void RgbdImagePyramid::deviceBatch(dvo_b200_ctx* ctx, const std::vector<RgbdImag
     todo.push_back(p);
   }
   if (todo.size() >= 2) {
-    const size_t npx = size_t(w) * h, n = todo.size();
+    const size_t npx = size_t(w) * h;
     size_t lv = levels;
-    for (size_t i = 0; i < n; ++i) lv = std::max(lv, todo[i]->requested_levels_);
-    std::vector<float> I(n * npx), Z(n * npx);
-    bool any_mask = false;
-    for (size_t i = 0; i < n; ++i) {
-      for (int y = 0; y < h; ++y) {   // row by row: a cv::Mat need not be continuous
-        std::memcpy(&I[i * npx + size_t(y) * w], todo[i]->levels_[0]->intensity.ptr<float>(y), sizeof(float) * w);
-        std::memcpy(&Z[i * npx + size_t(y) * w], todo[i]->levels_[0]->depth.ptr<float>(y), sizeof(float) * w);
-      }
-      any_mask = any_mask || !todo[i]->mask_.empty();
-    }
-    std::vector<uint8_t> masks;   // one upload for the batch: the pyramids without a mask get an all-usable one
-    if (any_mask)
-      for (size_t i = 0; i < n; ++i) append_mask(todo[i]->mask_, w, h, masks);
+    for (size_t i = 0; i < todo.size(); ++i) lv = std::max(lv, todo[i]->requested_levels_);
+    // One create call per role set (masks that also act in the current role need their own call), then ONE synchronisation
+    // for the whole upload.  The staging vectors live until then.
+    std::vector<RgbdImagePyramid*> groups[2];
+    for (size_t i = 0; i < todo.size(); ++i) groups[!todo[i]->mask_.empty() && todo[i]->mask_current_ ? 1 : 0].push_back(todo[i]);
+    std::vector<float> I[2], Z[2];
+    std::vector<uint8_t> masks[2];   // per call: the pyramids without a mask get an all-usable one
+    std::vector<dvo_b200_pyramid*> handles[2];
     const IntrinsicMatrix& k = todo[0]->camera_.level(0).intrinsics();
-    std::vector<dvo_b200_pyramid*> handles(n);
-    int rc = dvo_b200_pyramid_create_masked_batch(ctx, int(n), DVO_B200_INPUT_FLOAT32, I.data(), Z.data(), 0.f, any_mask ? masks.data() : nullptr,
-                                                  w, h, k.fx(), k.fy(), k.ox(), k.oy(), int(lv), handles.data());
-    if (rc != 0) throw std::runtime_error(std::string("dvo_b200_pyramid_create_masked_batch: ") + dvo_b200_last_error(ctx));
-    dvo_b200_synchronize(ctx);   // one synchronisation for the whole upload: the staging vectors go out of scope
-    for (size_t i = 0; i < n; ++i) {
-      std::lock_guard<std::mutex> lock(todo[i]->mutex_);
-      if (todo[i]->device_) dvo_b200_pyramid_release(todo[i]->device_);
-      todo[i]->device_ = handles[i];
-      todo[i]->device_ctx_ = ctx;
-      todo[i]->device_levels_ = lv;
+    for (int gi = 0; gi < 2; ++gi) {
+      const std::vector<RgbdImagePyramid*>& g = groups[gi];
+      const size_t n = g.size();
+      if (n == 0) continue;
+      I[gi].resize(n * npx); Z[gi].resize(n * npx);
+      bool any_mask = false;
+      for (size_t i = 0; i < n; ++i) {
+        for (int y = 0; y < h; ++y) {   // row by row: a cv::Mat need not be continuous
+          std::memcpy(&I[gi][i * npx + size_t(y) * w], g[i]->levels_[0]->intensity.ptr<float>(y), sizeof(float) * w);
+          std::memcpy(&Z[gi][i * npx + size_t(y) * w], g[i]->levels_[0]->depth.ptr<float>(y), sizeof(float) * w);
+        }
+        any_mask = any_mask || !g[i]->mask_.empty();
+      }
+      if (any_mask)
+        for (size_t i = 0; i < n; ++i) append_mask(g[i]->mask_, w, h, masks[gi]);
+      handles[gi].resize(n);
+      int rc = dvo_b200_pyramid_create_masked_batch_roles(ctx, int(n), DVO_B200_INPUT_FLOAT32, I[gi].data(), Z[gi].data(), 0.f,
+                                                          any_mask ? masks[gi].data() : nullptr, mask_roles(gi == 1), w, h, k.fx(),
+                                                          k.fy(), k.ox(), k.oy(), int(lv), handles[gi].data());
+      if (rc != 0) throw std::runtime_error(std::string("dvo_b200_pyramid_create_masked_batch_roles: ") + dvo_b200_last_error(ctx));
     }
+    dvo_b200_synchronize(ctx);   // one synchronisation for the whole upload: the staging vectors go out of scope
+    for (int gi = 0; gi < 2; ++gi)
+      for (size_t i = 0; i < groups[gi].size(); ++i) {
+        RgbdImagePyramid* p = groups[gi][i];
+        std::lock_guard<std::mutex> lock(p->mutex_);
+        if (p->device_) dvo_b200_pyramid_release(p->device_);
+        p->device_ = handles[gi][i];
+        p->device_ctx_ = ctx;
+        p->device_levels_ = lv;
+      }
   }
   for (size_t i = 0; i < pyramids.size(); ++i) out[i] = pyramids[i]->device(ctx, levels);   // the rest one by one
 }

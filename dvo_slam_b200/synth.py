@@ -171,6 +171,16 @@ def make_sequence(seed: int, n_frames: int, cfg: SceneConfig | None = None, devi
     return frames, poses
 
 
+def _patch_texture(rng, pw: int, ph: int, amplitude: float) -> np.ndarray:
+    """A (ph, pw) float32 texture of twelve random plane waves around mid-grey, rounded to 8-bit levels."""
+    yy, xx = np.mgrid[0:ph, 0:pw]
+    tex = np.zeros((ph, pw))
+    for _ in range(12):
+        kx, ky = rng.uniform(-0.25, 0.25, 2)
+        tex += rng.uniform(0.3, 1.0) * np.sin(kx * xx + ky * yy + rng.uniform(0, 2 * math.pi))
+    return np.round(np.clip(127.5 + amplitude * tex, 0, 255)).astype(np.float32)
+
+
 def make_moving_object_pair(seed: int, cfg: SceneConfig | None = None, patch=(150, 120), corner=(250, 200), shift=(24, 10),
                             z_obj: float = 0.9, margin: int = 8):
     """make_pair plus an object that moves on its own: a textured fronto-parallel patch (patch = (w, h) pixels at depth
@@ -185,11 +195,7 @@ def make_moving_object_pair(seed: int, cfg: SceneConfig | None = None, patch=(15
     rng = np.random.default_rng(1000 + seed)
     pw, ph = patch
     yy, xx = np.mgrid[0:ph, 0:pw]
-    tex = np.zeros((ph, pw))
-    for _ in range(12):
-        kx, ky = rng.uniform(-0.25, 0.25, 2)
-        tex += rng.uniform(0.3, 1.0) * np.sin(kx * xx + ky * yy + rng.uniform(0, 2 * math.pi))
-    tex = np.round(np.clip(127.5 + 40.0 * tex, 0, 255)).astype(np.float32)
+    tex = _patch_texture(rng, pw, ph, 40.0)
     zt = (np.float32(z_obj) + np.float32(0.0002) * np.round(xx / 8.0)).astype(np.float32)
     x0, y0 = corner
     x1, y1 = x0 + shift[0], y0 + shift[1]
@@ -197,6 +203,28 @@ def make_moving_object_pair(seed: int, cfg: SceneConfig | None = None, patch=(15
     out["Z_ref"][y0:y0 + ph, x0:x0 + pw] = zt
     out["I_cur"][y1:y1 + ph, x1:x1 + pw] = tex
     out["Z_cur"][y1:y1 + ph, x1:x1 + pw] = zt
+    mask = np.ones(out["I_ref"].shape, np.uint8)
+    mask[max(y0 - margin, 0):y0 + ph + margin, max(x0 - margin, 0):x0 + pw + margin] = 0
+    out["mask"] = mask
+    return out
+
+
+def make_overlay_pair(seed: int, size=(160, 120), corner=(420, 300), margin: int = 8, cfg: SceneConfig | None = None):
+    """make_pair plus a textured overlay fixed in the image: size = (w, h) pixels at corner = (x, y), written into the
+    intensity of BOTH frames at the same position, with the scene's depth left as it is -- a logo or timestamp burnt into
+    the colour image, a lens smudge or a glare patch.  Its pixels have the right depth and the wrong intensity, so the
+    occlusion test cannot reject taps on them.  Returns make_pair's dict (float32 numpy images, T_true of the camera) plus
+    "mask": the uint8 mask of either frame that excludes the overlay and a margin of `margin` pixels around it (0 =
+    excluded)."""
+    p = make_pair(seed, cfg)
+    out = dict(p)
+    for k in ("I_ref", "Z_ref", "I_cur", "Z_cur"):
+        out[k] = p[k].cpu().numpy().copy()
+    pw, ph = size
+    tex = _patch_texture(np.random.default_rng(2000 + seed), pw, ph, 60.0)
+    x0, y0 = corner
+    out["I_ref"][y0:y0 + ph, x0:x0 + pw] = tex[:out["I_ref"].shape[0] - y0, :out["I_ref"].shape[1] - x0]
+    out["I_cur"][y0:y0 + ph, x0:x0 + pw] = tex[:out["I_cur"].shape[0] - y0, :out["I_cur"].shape[1] - x0]
     mask = np.ones(out["I_ref"].shape, np.uint8)
     mask[max(y0 - margin, 0):y0 + ph + margin, max(x0 - margin, 0):x0 + pw + margin] = 0
     out["mask"] = mask

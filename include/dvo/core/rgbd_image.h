@@ -86,10 +86,15 @@ class RgbdImagePyramid {   // rgbd_image.h:242-262
   // footprint is; dvo_b200_pyramid_create_masked_batch).  The mask is copied.  Returns false and changes nothing once the
   // device mirror exists (after the first match) or if the size or type is wrong. ---
   bool setReferenceMask(const cv::Mat& mask);
+  // --- extension: the same mask, and with current_role_too also in the current role: while this pyramid is the current
+  // image of an alignment, a warped point is rejected iff one of its four bilinear taps is unusable at that level
+  // (dvo_b200_pyramid_create_masked_batch_roles).  The same rules as setReferenceMask, which is setMask(mask, false). ---
+  bool setMask(const cv::Mat& mask, bool current_role_too);
  private:
   RgbdCameraPyramid& camera_;
   std::vector<RgbdImagePtr> levels_;
-  cv::Mat mask_;   // setReferenceMask; empty: no mask
+  cv::Mat mask_;   // setMask; empty: no mask
+  bool mask_current_;   // setMask(mask, true): the mask also acts in the current role
   dvo_b200_pyramid* device_;
   dvo_b200_ctx* device_ctx_;
   size_t device_levels_, requested_levels_;

@@ -187,11 +187,33 @@ typedef enum dvo_b200_input_format {
  *     (dropped by the reference estimator, re-admitted by the corrected one), dvo_b200_pyramid_select, the residual and
  *     intensity error images.  max_valid_pixels does not change.
  *   Reference role only: the mask does not change the pyramid as the CURRENT image of an alignment (its pixels stay valid
- *     bilinear taps) nor dvo_b200_pyramid_download.
+ *     bilinear taps) nor dvo_b200_pyramid_download.  dvo_b200_pyramid_create_masked_batch_roles with
+ *     DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT makes the mask act in both roles.
  *   Fixed at creation: a pyramid's mask never changes, so sharing it across contexts and threads needs no new rule. */
 int dvo_b200_pyramid_create_masked_batch(dvo_b200_ctx* ctx, int32_t n, int32_t format, const void* image, const void* depth,
                                          float depth_scale, const uint8_t* masks, int32_t width, int32_t height, float fx,
                                          float fy, float ox, float oy, int32_t levels, dvo_b200_pyramid** out /* n handles */);
+/* Roles of a mask (bit set) */
+#define DVO_B200_MASK_ROLE_REFERENCE 1   /* the selection: dvo_b200_pyramid_create_masked_batch */
+#define DVO_B200_MASK_ROLE_CURRENT 2     /* the bilinear taps when the pyramid is the current image of an alignment */
+/* dvo_b200_pyramid_create_masked_batch with a role set.  roles = DVO_B200_MASK_ROLE_REFERENCE: that call, bit for bit.
+ * roles = DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT ("both"): the same pyramid as the reference of an
+ * alignment (selection, S, odd last point, dvo_b200_pyramid_select unchanged), and as the CURRENT image a warped point is
+ * rejected iff any of its four bilinear taps (u0, v0), (u0+1, v0), (u0, v0+1), (u0+1, v0+1) is unusable at that level, on
+ * top of the bounds, NaN and occlusion tests -- the same rejection as a NaN depth at that tap.  The gradients of the usable
+ * taps keep reading the true intensity and depth of unusable neighbours, so the ring of valid pixels next to an excluded
+ * region stays.  Both stages of an iteration see the same points: n, P_k, the log-likelihood, A and b, and the test hooks
+ * (dvo_b200_residual_image, dvo_b200_intensity_error_image, dvo_b200_linearize) follow, with both estimators.
+ * dvo_b200_pyramid_download of such a pyramid returns Z = NaN at the unusable pixels of each level; the other planes are
+ * those of the unmasked build.  Any other roles value -> DVO_B200_ERR_INVALID_ARGUMENT, nothing is created.
+ * masks == NULL: the unmasked pyramids whatever the roles.  Fixed at creation, as the mask itself. */
+int dvo_b200_pyramid_create_masked_batch_roles(dvo_b200_ctx* ctx, int32_t n, int32_t format, const void* image,
+                                               const void* depth, float depth_scale, const uint8_t* masks, int32_t roles,
+                                               int32_t width, int32_t height, float fx, float fy, float ox, float oy,
+                                               int32_t levels, dvo_b200_pyramid** out /* n handles */);
+/* Role set a pyramid was created with: 0 (no mask), DVO_B200_MASK_ROLE_REFERENCE, or
+ * DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT; DVO_B200_ERR_INVALID_ARGUMENT for a null handle. */
+int dvo_b200_pyramid_mask_roles(const dvo_b200_pyramid* p);
 int dvo_b200_pyramid_device(const dvo_b200_pyramid* p);   /* CUDA ordinal the pyramid lives on (-1: null handle) */
 int dvo_b200_pyramid_retain(dvo_b200_pyramid* p);   /* boost::shared_ptr semantics of RgbdImagePyramidPtr */
 /* Any context may use a pyramid, also while its build is still queued on the building context's stream: every call
