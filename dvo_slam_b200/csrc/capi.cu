@@ -160,9 +160,8 @@ int dvo_b200_destroy(dvo_b200_ctx* ctx) {
   drain_profile(ctx);
   for (cudaEvent_t e : ctx->event_pool) cudaEventDestroy(e);
   Workspace& ws = ctx->ws;
-  cudaFree(ws.d_pair_level); cudaFree(ws.d_state); cudaFree(ws.d_row_exports); cudaFree(ws.d_row_base);
-  cudaFree(ws.d_strip_exports); cudaFree(ws.d_strip_base); cudaFree(ws.d_row_partial); cudaFree(ws.d_strip_partial); cudaFree(ws.d_dump); cudaFree(ws.d_tinit);
-  cudaFree(ws.d_iter_log); cudaFree(ws.d_squads); cudaFree(ws.d_csat);
+  cudaFree(ws.d_pair_level); cudaFree(ws.d_state); cudaFree(ws.d_scratch); cudaFree(ws.d_dump); cudaFree(ws.d_tinit);
+  cudaFree(ws.d_iter_log); cudaFree(ws.d_csat);
   if (ws.h_active) cudaFreeHost(ws.h_active);
   pool_close(ctx);
   cudaFree(ctx->d_stage);

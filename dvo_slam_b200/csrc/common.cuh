@@ -188,26 +188,18 @@ struct PairState {
   int iter_log_count;
   int pad_;
   LevelSummary levels[kMaxLevels];
-  double result_T[16], result_info[36], result_ll;
 };
 
 struct Workspace {              // per-ctx scratch of the level kernel
   PairLevel* d_pair_level = nullptr;
   const int** d_csat = nullptr;      // per descriptor of d_pair_level: CurPairLevel::csat (only written for kCurMask launches)
   PairState* d_state = nullptr;
-  float* d_row_exports = nullptr;    // per squad: one scale summary per image row (kSegExportFloats)
-  int* d_row_base = nullptr;         // per squad, per row: valid points before the row inside its CTA
-  double* d_strip_exports = nullptr; // per squad, per strip: scale summary of the strip's rows (fp64, kStripExportDoubles)
-  int* d_strip_base = nullptr;       // per squad: nstrips + 1 exclusive prefixes of the strips' valid counts
-  float* d_row_partial = nullptr;    // per squad, per image row: log-likelihood sum, 21 upper-triangular A, 6 b of the row
-  double* d_strip_partial = nullptr; // per squad, per strip: the same, summed over the strip's rows in fp64
+  char* d_scratch = nullptr;         // the level kernel's per-launch scratch (tracker.cu: ScratchLayout)
   float* d_dump = nullptr;           // test hook: seven residual-record planes of one level
   double* d_tinit = nullptr;         // per pair initial estimate (4x4)
   dvo_b200_iteration_stats* d_iter_log = nullptr;
-  int* h_active = nullptr;           // pinned: per level, the kernel's error flag
-  char* d_squads = nullptr;          // persistent kernel: SquadState[nsquads] + {queue head, error flag}
-  size_t cap_pairs = 0, cap_row_exports = 0, cap_row_base = 0, cap_strip_exports = 0, cap_strip_base = 0, cap_row_partial = 0, cap_strip_partial = 0,
-         cap_squads = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0;
+  int* h_active = nullptr;           // pinned: per launch of a call, the kernel's error flag
+  size_t cap_pairs = 0, cap_scratch = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0;
 };
 
 }  // namespace dvo_b200

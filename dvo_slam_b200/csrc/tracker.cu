@@ -18,6 +18,7 @@
 // order fixed by the level's geometry, so every plan returns the same bits.
 #include "common.cuh"
 #include "stages.cuh"
+#include "launch_plan.h"
 
 #include <cstdio>
 #include <cstring>
@@ -122,7 +123,7 @@ __global__ void k_stage_words(const uint4* __restrict__ src, uint4* __restrict__
 // e: the level's nstrips strip summaries; strip_base: nstrips + 1 exclusive prefixes of their valid counts (output).
 // kCorrected: the summaries hold the plain sum of w r r^T (no pairing, no odd tail term) and every point is kept.
 template <bool kCorrected>
-__device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double* e, int* strip_base, int nstrips, int* active,
+__device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double* e, int* strip_base, int nstrips,
                                            const LevelLaunch& lp, dvo_b200_iteration_stats* ilog, int max_log, SegCombineSmem& sm) {
   const int lane = threadIdx.x & 31;
   const SegT<double> all = combine_strip_exports_warp(e, nstrips, strip_base, sm);
@@ -159,7 +160,6 @@ __device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double
       if (ls.has_inc) { ls.last_inc_n = n; ls.last_inc_nll = 0.0; }
       st.have_done = (st.termination == DVO_B200_TERM_TOO_FEW_CONSTRAINTS) ? -1 : st.have_done;
       st.level_active = 0;
-      if (active) atomicSub(active, 1);
     } else {
       // tail term for odd n, normaliser 1/(n-3) (dense_tracking_impl.cpp:596), symmetric 2x2
       double c[3];
@@ -193,7 +193,7 @@ struct PairEndSmem {
 
 template <typename Release>
 __device__ __noinline__ void pair_end_cta(PairState& st, const PairLevel& pl, int pair, const double* partial, int ntiles,
-                                             int* active, const LevelLaunch& lp, dvo_b200_iteration_stats* ilog, int max_log,
+                                             const LevelLaunch& lp, dvo_b200_iteration_stats* ilog, int max_log,
                                              PairEndSmem& sm, Release release, unsigned long long* tcrit = nullptr) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   unsigned long long tc0 = 0;
@@ -322,7 +322,6 @@ __device__ __noinline__ void pair_end_cta(PairState& st, const PairLevel& pl, in
     int need = (st.termination == DVO_B200_TERM_LOG_LIKELIHOOD_DECREASED ||
                 st.termination == DVO_B200_TERM_TOO_FEW_CONSTRAINTS) ? 2 : 1;
     ls.has_inc = ls.num_iterations >= need;
-    if (active) atomicSub(active, 1);
   } else {
     st.inc = inc;
     st.initial_old = st.initial;
@@ -364,7 +363,6 @@ constexpr size_t kLevelSmemBytes = sizeof(TilePipe) + sizeof(LevelTail);
 // has one segment, or two (the coarse levels with one CTA per pair, then the fine levels with squads of g CTAs) that the
 // grid runs back to back WITHOUT a grid-wide barrier: a CTA that finds the coarse queue empty moves on to the fine
 // segment, and fine squads take their pairs from a ring of pairs whose coarse levels are done (`ready`).
-constexpr int kMaxSeg = 4;   // segments of one launch: the coarse levels, then up to three slices of the fine levels
 struct Segment {
   const PairLevel* pls;   // descriptors of this segment's levels: [level][pair]
   float* row_exports;     // per squad: h segment summaries (one per image row)
@@ -601,7 +599,7 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
       if (squad_arrive(sq, episode, S.g, lt.s_flag)) {
         DVO_TOCK(2);
         if (warp == 0) {
-          pair_mid_warp<kCorrected>(st, pair, strip_exports, strip_base, lp.nstrips, nullptr, lp, a.ilog, a.max_log, lt.comb);
+          pair_mid_warp<kCorrected>(st, pair, strip_exports, strip_base, lp.nstrips, lp, a.ilog, a.max_log, lt.comb);
           if (lane == 0) squad_release(sq, episode);
         }
         __syncthreads();
@@ -651,7 +649,7 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
       DVO_TOCK(1);
       if (squad_arrive(sq, episode, S.g, lt.s_flag)) {
         DVO_TOCK(3);
-        pair_end_cta(st, pl, pair, strip_partial, lp.nstrips, nullptr, lp, a.ilog, a.max_log, lt.end, [&] { squad_release(sq, episode); }, S.dbg2 ? S.dbg2 + 64 : nullptr);
+        pair_end_cta(st, pl, pair, strip_partial, lp.nstrips, lp, a.ilog, a.max_log, lt.end, [&] { squad_release(sq, episode); }, S.dbg2 ? S.dbg2 + 64 : nullptr);
         __syncthreads();
         DVO_TOCK(5);
       } else {
@@ -753,7 +751,6 @@ __global__ void k_set_state(PairState* states, const PairLevel* pls, const doubl
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-inline int level_flag_slot(int li) { return li < 8 ? li : 7; }
 template <typename T>
 int grow(dvo_b200_ctx* ctx, T*& ptr, size_t& cap, size_t need) {
   if (need <= cap) return 0;
@@ -763,33 +760,58 @@ int grow(dvo_b200_ctx* ctx, T*& ptr, size_t& cap, size_t need) {
   return 0;
 }
 
-struct ScratchNeed {
-  size_t row_export_floats = 0, row_base_ints = 0, strip_export_doubles = 0, strip_base_ints = 0, row_partial_floats = 0,
-         strip_partial_doubles = 0, squads = 0;
-  size_t dump_floats = 0;
+// Byte offsets of one launch's scratch in the workspace arena, every region on a 128-byte boundary.  Per segment, for each
+// of its squads and sized for the segment's tallest level: the row and strip scale summaries, the valid-count prefixes of
+// rows and strips, and the row and strip partials of the normal equations.  Then the squad states of every segment, the
+// counter line and the ready ring, back to back so that one memset zeroes them before the launch.
+struct ScratchLayout {
+  size_t row_exports[kMaxSeg], row_base[kMaxSeg], strip_exports[kMaxSeg], strip_base[kMaxSeg], row_partial[kMaxSeg],
+         strip_partial[kMaxSeg], squads[kMaxSeg];
+  size_t counters;   // one 128-byte line: {queue[kMaxSeg], ready tail[kMaxSeg], arrivals[kMaxSeg], error flag}
+  size_t ring;       // npairs slots: the ready rings of the fine segments, by pair range
+  size_t bytes;
 };
 
-int ensure_workspace(dvo_b200_ctx* ctx, int npairs, const ScratchNeed& need, int max_log_per_pair) {
+ScratchLayout scratch_layout(const PlanLaunch& L, int npairs) {
+  ScratchLayout o;
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t off = at; at += (bytes + 127) / 128 * 128; return off; };
+  for (int s = 0; s < L.nseg; ++s) {
+    const PlanSegment& S = L.seg[s];
+    const size_t rows = (size_t)S.nsquads * S.hmax, strips = (size_t)S.nsquads * ((S.hmax + kTileH - 1) / kTileH);
+    o.row_exports[s] = take(sizeof(float) * kSegExportFloats * rows);
+    o.row_base[s] = take(sizeof(int) * rows);
+    o.strip_exports[s] = take(sizeof(double) * kStripExportDoubles * strips);
+    o.strip_base[s] = take(sizeof(int) * (strips + S.nsquads));   // nstrips + 1 per squad
+    o.row_partial[s] = take(sizeof(float) * kNormalValues * rows);
+    o.strip_partial[s] = take(sizeof(double) * kNormalValues * strips);
+  }
+  for (int s = 0; s < L.nseg; ++s) o.squads[s] = take(sizeof(SquadState) * L.seg[s].nsquads);
+  o.counters = take(sizeof(SquadState));
+  o.ring = take(sizeof(int) * (size_t)npairs);
+  o.bytes = at;
+  return o;
+}
+
+// ndesc pair descriptors and states, the scratch arena of the plan's largest launch, the residual-record dump of the test
+// hook and the iteration log.
+int ensure_workspace(dvo_b200_ctx* ctx, int ndesc, const LaunchPlan& plan, int npairs, size_t dump_floats, int max_log_per_pair) {
   Workspace& ws = ctx->ws;
-  if ((size_t)npairs > ws.cap_pairs) {
+  if ((size_t)ndesc > ws.cap_pairs) {
     if (ws.d_pair_level) { cudaStreamSynchronize(ctx->stream); cudaFree(ws.d_pair_level); cudaFree(ws.d_state); }
     ws.d_pair_level = nullptr; ws.d_state = nullptr; ws.cap_pairs = 0;
-    DVO_CUDA(ctx, cudaMalloc((void**)&ws.d_pair_level, sizeof(PairLevel) * npairs + 16));   // k_stage_words copies whole 16-byte words
-    DVO_CUDA(ctx, cudaMalloc((void**)&ws.d_state, sizeof(PairState) * npairs));
-    ws.cap_pairs = npairs;
+    DVO_CUDA(ctx, cudaMalloc((void**)&ws.d_pair_level, sizeof(PairLevel) * ndesc + 16));   // k_stage_words copies whole 16-byte words
+    DVO_CUDA(ctx, cudaMalloc((void**)&ws.d_state, sizeof(PairState) * ndesc));
+    ws.cap_pairs = ndesc;
   }
+  size_t scratch = 0;
+  for (int i = 0; i < plan.nlaunch; ++i) scratch = std::max(scratch, scratch_layout(plan.launch[i], npairs).bytes);
   int rc;
-  if ((rc = grow(ctx, ws.d_row_exports, ws.cap_row_exports, need.row_export_floats))) return rc;
-  if ((rc = grow(ctx, ws.d_row_base, ws.cap_row_base, need.row_base_ints))) return rc;
-  if ((rc = grow(ctx, ws.d_strip_exports, ws.cap_strip_exports, need.strip_export_doubles))) return rc;
-  if ((rc = grow(ctx, ws.d_strip_base, ws.cap_strip_base, need.strip_base_ints))) return rc;
-  if ((rc = grow(ctx, ws.d_row_partial, ws.cap_row_partial, need.row_partial_floats))) return rc;
-  if ((rc = grow(ctx, ws.d_strip_partial, ws.cap_strip_partial, need.strip_partial_doubles))) return rc;
-  if ((rc = grow(ctx, ws.d_squads, ws.cap_squads, need.squads * sizeof(SquadState)))) return rc;
-  if ((rc = grow(ctx, ws.d_dump, ws.cap_dump, need.dump_floats))) return rc;
+  if ((rc = grow(ctx, ws.d_scratch, ws.cap_scratch, scratch))) return rc;
+  if ((rc = grow(ctx, ws.d_dump, ws.cap_dump, dump_floats))) return rc;
   if (!ws.h_active) DVO_CUDA(ctx, cudaMallocHost((void**)&ws.h_active, sizeof(int) * 8));
   if (max_log_per_pair > 0) {
-    size_t n = (size_t)npairs * max_log_per_pair;
+    size_t n = (size_t)ndesc * max_log_per_pair;
     if ((rc = grow(ctx, ws.d_iter_log, ws.cap_iter_log, n))) return rc;
   }
   return 0;
@@ -814,86 +836,12 @@ int ensure_geometry(dvo_b200_ctx* ctx) {
   return 0;
 }
 
-// How a group of consecutive pyramid levels is spread over the persistent grid: one launch walks every pair through the
-// group's levels (coarse to fine) inside the kernel.
-struct GroupPlan {
-  int first_li, nlev;   // levels [first_li, first_li + nlev) of the match (index 0 = coarsest)
-  int g;                // CTAs per squad
-  int nsquads;          // squads in the grid
-  int strips_per_cta[kMaxLevels];
-  int pair_begin, npairs;   // the pairs this segment's queue hands out (a slice of the batch for the fine segments of a fused launch)
-};
-
-// Squad size for one level on its own.  A squad of g CTAs gives each CTA spc = ceil(nstrips / g) strips.  Small squads keep
-// many pairs in flight and amortise the two barriers and the serial P_k / solve sections of an iteration over more tiles
-// per CTA; but the batch is processed in waves of nsquads pairs, and a last wave that is mostly empty wastes more than
-// that.  Pairs are handed out from a queue, so a level takes about (pairs per squad + tail) x time per pair, where the
-// tail (pairs that need two or three times the mean number of iterations) is worth a bit more than one pair and the time
-// per pair goes with (tiles per CTA + per-iteration overhead in tile units).
-int level_squad_size(int nstrips, int nbands, int grid, int npairs) {
-  const char* env = getenv("DVO_B200_STRIPS_PER_CTA");     // developer override (experiments)
-  const int forced_spc = env ? atoi(env) : 0;
-  // per stage: squad barrier + serial step + pipeline fill, in tile-times.  Fitted on an H100 at batch 512 (DESIGN §6): level 0
-  // with g = 2 is 1.3 % faster than g = 3, g = 1 and g >= 4 are slower; the model picks g = 2 there for 43 .. 100.
-  const double overhead_tiles = 45.0;
-  int best_g = 1;
-  double best_cost = -1.0;
-  for (int spc = 1; spc <= nstrips; ++spc) {
-    const int g = (nstrips + spc - 1) / spc;
-    if (g > grid) continue;
-    if (spc > 1 && (nstrips + spc - 2) / (spc - 1) == g) continue;   // same g as the previous spc: more work per CTA, nothing gained
-    const int nsquads = std::min(grid / g, std::max(npairs, 1));
-    const double per_squad = (double)npairs / nsquads;
-    double cost = (std::max(per_squad, 1.0) + (npairs > nsquads ? 1.2 : 0.0)) * ((double)spc * nbands + overhead_tiles);
-    if (forced_spc > 0) cost = std::abs(spc - forced_spc);
-    if (best_cost < 0 || cost < best_cost - 1e-9) { best_cost = cost; best_g = g; }
-  }
-  return best_g;
-}
-
-// Levels small enough for one CTA per pair (no squad barriers at all) form one group: a CTA takes a pair from the queue and
-// runs it through all of them, so a pair that needs many iterations on one coarse level delays nobody.  The remaining
-// (fine) levels form a second group with the squad size of the finest level; a squad likewise walks its pair through both.
-// With few pairs every level gets its own launch and the squad size that minimises its latency.
-int plan_groups(const dvo_b200_pyramid* ref, int first, int last, int grid, int npairs, GroupPlan* out) {
-  const int nlev = first - last + 1;
-  int g_level[kMaxLevels];
-  for (int li = 0; li < nlev; ++li) {
-    const LevelInfo& L = ref->L[first - li];
-    g_level[li] = level_squad_size(L.nstrips, L.nbands, grid, npairs);
-  }
-  int ngroups = 0;
-  const bool walk = npairs >= grid / 4 && !getenv("DVO_B200_NO_WALK");
-  const int coarse_tiles = getenv("DVO_B200_COARSE_TILES") ? atoi(getenv("DVO_B200_COARSE_TILES")) : 110;   // levels up to 320x240 (105 tiles): one CTA per pair; env = developer override
-  for (int li = 0; li < nlev;) {
-    GroupPlan& G = out[ngroups++];
-    G.first_li = li; G.nlev = 1; G.g = g_level[li];
-    if (walk) {
-      const LevelInfo& L0 = ref->L[first - li];
-      const bool coarse = L0.nstrips * L0.nbands <= coarse_tiles;
-      if (coarse) G.g = 1;
-      while (li + G.nlev < nlev) {
-        const LevelInfo& Ln = ref->L[first - (li + G.nlev)];
-        const bool coarse_n = Ln.nstrips * Ln.nbands <= coarse_tiles;
-        if (coarse_n != coarse) break;
-        if (!coarse) G.g = g_level[li + G.nlev];      // the finest level of the group decides
-        G.nlev++;
-      }
-    }
-    if (const char* fg = getenv("DVO_B200_FINE_G")) {     // developer override (experiments): squad size of the non-coarse groups
-      const LevelInfo& L0 = ref->L[first - li];
-      if (L0.nstrips * L0.nbands > coarse_tiles && atoi(fg) > 0) G.g = std::min(atoi(fg), grid);
-    }
-    for (int k = 0; k < G.nlev; ++k) {
-      const LevelInfo& L = ref->L[first - (li + k)];
-      const int g_eff = std::min(G.g, L.nstrips);
-      G.strips_per_cta[k] = (L.nstrips + g_eff - 1) / g_eff;
-    }
-    G.nsquads = std::min(grid / G.g, std::max(npairs, 1));
-    G.pair_begin = 0; G.npairs = npairs;
-    li += G.nlev;
-  }
-  return ngroups;
+// The launch plan (launch_plan.h) of a match over levels first .. last of npairs pairs shaped like `ref`, with the plan
+// overrides of the environment as they are now.
+LaunchPlan plan_launches(const dvo_b200_ctx* ctx, const dvo_b200_pyramid* ref, int first, int last, int npairs) {
+  LevelShape shape[kMaxLevels];
+  for (int l = 0; l <= first; ++l) shape[l] = {ref->L[l].h, ref->L[l].nbands, ref->L[l].nstrips};
+  return make_launch_plan(shape, first, last, ctx->num_sms * ctx->ctas_per_sm, npairs, plan_knobs_from_env());
 }
 
 // One pyramid of each distinct slab among the batch's pyramids (a batch built in one call shares one slab), in slab order.
@@ -972,89 +920,50 @@ LevelLaunch make_level_launch(const LevelInfo& L, const dvo_b200_config* cfg, in
   return lp;
 }
 
-// scratch of one launch = the sum over its segments (they are live at the same time); the workspace keeps the maximum
-ScratchNeed segment_need(int hmax, const GroupPlan& pl) {
-  ScratchNeed s;
-  s.row_export_floats = (size_t)pl.nsquads * hmax * kSegExportFloats;
-  s.row_base_ints = (size_t)pl.nsquads * hmax;
-  const size_t smax = (size_t)(hmax + kTileH - 1) / kTileH;
-  s.strip_export_doubles = (size_t)pl.nsquads * smax * kStripExportDoubles;
-  s.strip_base_ints = (size_t)pl.nsquads * (smax + 1);
-  s.row_partial_floats = (size_t)pl.nsquads * hmax * kNormalValues;
-  s.strip_partial_doubles = (size_t)pl.nsquads * smax * kNormalValues;
-  s.squads = (size_t)pl.nsquads;
-  return s;
-}
-void add_launch_need(ScratchNeed& need, int nseg, const int* hmax, const GroupPlan* plans, int npairs) {
-  ScratchNeed sum;
-  for (int s = 0; s < nseg; ++s) {
-    const ScratchNeed q = segment_need(hmax[s], plans[s]);
-    sum.row_export_floats += q.row_export_floats; sum.row_base_ints += q.row_base_ints; sum.strip_export_doubles += q.strip_export_doubles;
-    sum.strip_base_ints += q.strip_base_ints; sum.row_partial_floats += q.row_partial_floats;
-    sum.strip_partial_doubles += q.strip_partial_doubles; sum.squads += q.squads;
-  }
-  sum.squads += 1 + ((size_t)npairs * sizeof(int) + sizeof(SquadState) - 1) / sizeof(SquadState);   // counters + ready ring
-  need.row_export_floats = std::max(need.row_export_floats, sum.row_export_floats);
-  need.row_base_ints = std::max(need.row_base_ints, sum.row_base_ints);
-  need.strip_export_doubles = std::max(need.strip_export_doubles, sum.strip_export_doubles);
-  need.strip_base_ints = std::max(need.strip_base_ints, sum.strip_base_ints);
-  need.row_partial_floats = std::max(need.row_partial_floats, sum.row_partial_floats);
-  need.strip_partial_doubles = std::max(need.strip_partial_doubles, sum.strip_partial_doubles);
-  need.squads = std::max(need.squads, sum.squads);
-}
-
-// Enqueue one persistent launch of nseg (1 or 2) segments; squad states, queues, the ready ring and the error flag are
-// zeroed first.  lps / d_pls: per segment.  `flag_out` receives the device address of the launch's error flag.
-int launch_segments(dvo_b200_ctx* ctx, int nseg, const LevelLaunch (*lps)[kMaxLevels], const GroupPlan* plans, const int* hmax,
-                    const PairLevel* const* d_pls, const double* d_Tinit, int npairs, int max_log, float* dump, int skip_begin,
-                    int group_index, bool cur_mask, int** flag_out) {
+// Enqueue launch `index` of a plan whose level li is pyramid level first - li of `levels`.  Squad states, queues, the ready
+// ring and the error flag are zeroed first; the error flag is copied to ws.h_active[index] after the launch.
+int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo_b200_config* cfg, const LevelInfo* levels,
+                    int first, const double* d_Tinit, int npairs, int max_log, float* dump, int skip_begin, bool cur_mask) {
   Workspace& ws = ctx->ws;
   cudaStream_t st = ctx->stream;
-  size_t nsq = 0;
-  for (int s = 0; s < nseg; ++s) nsq += plans[s].nsquads;
-  const size_t ring_states = ((size_t)npairs * sizeof(int) + sizeof(SquadState) - 1) / sizeof(SquadState);
-  DVO_CUDA(ctx, cudaMemsetAsync(ws.d_squads, 0, sizeof(SquadState) * (nsq + 1 + ring_states), st));
+  const ScratchLayout o = scratch_layout(L, npairs);
+  char* const base = ws.d_scratch;
+  DVO_CUDA(ctx, cudaMemsetAsync(base + o.squads[0], 0, o.bytes - o.squads[0], st));
   PersistentArgs pa;
   pa.states = ws.d_state;
-  SquadState* squads = reinterpret_cast<SquadState*>(ws.d_squads);
-  int* counters = reinterpret_cast<int*>(squads + nsq);      // one zeroed 128-byte line: {queue[4], ready tail[4], arrivals[4], error flag}
-  int* ring = reinterpret_cast<int*>(squads + nsq + 1);      // npairs slots: the ready rings of the fine segments, by pair range
+  int* counters = reinterpret_cast<int*>(base + o.counters);
   pa.error_flag = counters + 3 * kMaxSeg;
   pa.ilog = ws.d_iter_log; pa.max_log = max_log;
   pa.T_init = d_Tinit; pa.skip_begin = skip_begin;
   pa.dump = dump;
-  pa.npairs = npairs; pa.nseg = nseg;
+  pa.npairs = npairs; pa.nseg = L.nseg;
   pa.pls0 = ws.d_pair_level; pa.csat = ws.d_csat;
-  ScratchNeed off;
-  size_t sq_off = 0;
-  for (int s = 0; s < nseg; ++s) {
+  for (int s = 0; s < L.nseg; ++s) {
+    const PlanSegment& P = L.seg[s];
     Segment& S = pa.seg[s];
-    const GroupPlan& plan = plans[s];
-    S.pls = d_pls[s];
-    S.row_exports = ws.d_row_exports + off.row_export_floats; S.row_base = ws.d_row_base + off.row_base_ints;
-    S.strip_exports = ws.d_strip_exports + off.strip_export_doubles; S.strip_base = ws.d_strip_base + off.strip_base_ints;
-    S.row_partial = ws.d_row_partial + off.row_partial_floats; S.strip_partial = ws.d_strip_partial + off.strip_partial_doubles;
-    S.squads = squads + sq_off;
+    S.pls = ws.d_pair_level + (size_t)P.first_li * npairs;
+    S.row_exports = reinterpret_cast<float*>(base + o.row_exports[s]);
+    S.row_base = reinterpret_cast<int*>(base + o.row_base[s]);
+    S.strip_exports = reinterpret_cast<double*>(base + o.strip_exports[s]);
+    S.strip_base = reinterpret_cast<int*>(base + o.strip_base[s]);
+    S.row_partial = reinterpret_cast<float*>(base + o.row_partial[s]);
+    S.strip_partial = reinterpret_cast<double*>(base + o.strip_partial[s]);
+    S.squads = reinterpret_cast<SquadState*>(base + o.squads[s]);
     S.queue = counters + s; S.ready_tail = counters + kMaxSeg + s; S.arrivals = counters + 2 * kMaxSeg + s;
-    S.pair_begin = plan.pair_begin; S.npairs_seg = plan.npairs;
-    S.cyclic = getenv("DVO_B200_CONTIGUOUS") ? 0 : 1;          // developer switch (results are identical either way)
-    S.ready = ring + plan.pair_begin;
-    const int slot = std::min(group_index + s, 7);
-    S.dbg = ctx->d_dbg ? ctx->d_dbg + 16 * slot : nullptr;
-    S.dbg2 = ctx->d_dbg ? ctx->d_dbg + 128 + 8 * slot : nullptr;
-    S.nlev = plan.nlev; S.g = plan.g; S.nsquads = plan.nsquads;
-    for (int k = 0; k < kMaxLevels; ++k) {
-      S.strips_per_cta[k] = k < plan.nlev ? plan.strips_per_cta[k] : 0;
-      if (k < plan.nlev) S.lp[k] = lps[s][k];
+    S.ready = reinterpret_cast<int*>(base + o.ring) + P.pair_begin;
+    S.cyclic = P.cyclic; S.pair_begin = P.pair_begin; S.npairs_seg = P.npairs;
+    S.dbg = ctx->d_dbg ? ctx->d_dbg + 16 * (index + s) : nullptr;
+    S.dbg2 = ctx->d_dbg ? ctx->d_dbg + 128 + 8 * (index + s) : nullptr;
+    S.nlev = P.nlev; S.g = P.g; S.nsquads = P.nsquads;
+    for (int k = 0; k < kMaxLevels; ++k) S.strips_per_cta[k] = P.strips_per_cta[k];
+    for (int k = 0; k < P.nlev; ++k) {
+      const int li = P.first_li + k;
+      S.lp[k] = make_level_launch(levels[first - li], cfg, li, first - li);
     }
-    const ScratchNeed q = segment_need(hmax[s], plan);
-    off.row_export_floats += q.row_export_floats; off.row_base_ints += q.row_base_ints; off.strip_export_doubles += q.strip_export_doubles;
-    off.strip_base_ints += q.strip_base_ints; off.row_partial_floats += q.row_partial_floats; off.strip_partial_doubles += q.strip_partial_doubles;
-    sq_off += plan.nsquads;
   }
   {
     ProfScope prof(ctx, 0);
-    ProfScope prof_level(ctx, 8 + std::min(group_index, 7));
+    ProfScope prof_level(ctx, 8 + index);
     void* args[] = {&pa};
     const bool corrected = ctx->estimator == DVO_B200_ESTIMATOR_CORRECTED;
     const void* kern = cur_mask ? (corrected ? (const void*)k_level_persistent<true, true> : (const void*)k_level_persistent<false, true>)
@@ -1063,7 +972,7 @@ int launch_segments(dvo_b200_ctx* ctx, int nseg, const LevelLaunch (*lps)[kMaxLe
                                               dim3(kCtaThreads), args, kLevelSmemBytes, st));
     ctx->launches++;
   }
-  *flag_out = pa.error_flag;
+  DVO_CUDA(ctx, cudaMemcpyAsync(&ws.h_active[index], pa.error_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
   return 0;
 }
 
@@ -1080,68 +989,8 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   const int max_log = iter_stats ? max_iter_stats : 0;
   if ((rc = ensure_geometry(ctx))) return rc;
   const int nlev = first - last + 1;
-  const int grid = ctx->num_sms * ctx->ctas_per_sm;
-  GroupPlan groups[kMaxLevels];
-  const int ngroups = plan_groups(refs[0], first, last, grid, n, groups);
-  int hmaxs[kMaxLevels];
-  for (int gi = 0; gi < ngroups; ++gi) {
-    hmaxs[gi] = 0;
-    for (int k = 0; k < groups[gi].nlev; ++k) hmaxs[gi] = std::max(hmaxs[gi], refs[0]->L[first - (groups[gi].first_li + k)].h);
-  }
-  // A coarse group (one CTA per pair) followed by a fine group runs as ONE launch of two segments: no grid-wide barrier and
-  // no launch boundary between them, so the CTAs that run out of coarse pairs start on fine pairs while the long coarse
-  // pairs are still iterating.
-  const bool fuse = ngroups == 2 && groups[0].g == 1 && !getenv("DVO_B200_NO_FUSE");
-  // Fused launch: the fine group is cut into up to three slices of the pair index with squads of g, 2g and 4g CTAs.  Pairs
-  // come off a queue, so with one squad size the launch ends with most squads idle while a few finish pairs that need two
-  // or three times the mean number of iterations.  The last pairs of the
-  // batch, which also leave the coarse segment last, therefore go to wider squads that finish a pair in a half / a quarter
-  // of the time; the slice a pair belongs to is fixed by its index, so results do not depend on timing.
-  GroupPlan segs[kMaxSeg];
-  int seg_hmax[kMaxSeg];
-  int nseg = 1;
-  if (fuse) {
-    segs[0] = groups[0]; seg_hmax[0] = hmaxs[0];
-    const GroupPlan& F = groups[1];
-    int min_strips = 1 << 30;
-    for (int k = 0; k < F.nlev; ++k) min_strips = std::min(min_strips, refs[0]->L[first - (F.first_li + k)].nstrips);
-    int counts[3] = {n, 0, 0};
-    {
-      int c2 = 0, c3 = 0;
-      const int g2 = 2 * F.g, g3 = 4 * F.g;
-      if (g2 <= min_strips && g2 <= grid) c2 = (int)(1.8 * (grid / g2) + 0.5);
-      if (c2 && g3 <= min_strips && g3 <= grid) c3 = (int)(1.8 * (grid / g3) + 0.5);
-      if (const char* e = getenv("DVO_B200_TAIL")) {       // developer override: "c2,c3" pairs for the 2g and 4g slices
-        int a2 = 0, a3 = 0;
-        if (sscanf(e, "%d,%d", &a2, &a3) >= 1) { c2 = (g2 <= min_strips && g2 <= grid) ? a2 : 0; c3 = (c2 && g3 <= min_strips && g3 <= grid) ? a3 : 0; }
-      }
-      const int keep = 2 * (grid / F.g);                     // the first slice keeps at least two pairs per squad
-      if (n - c2 - c3 < keep) c3 = 0;
-      if (n - c2 < keep) c2 = 0;
-      counts[0] = n - c2 - c3; counts[1] = c2; counts[2] = c3;
-    }
-    int begin = 0;
-    for (int k = 0; k < 3; ++k) {
-      if (counts[k] <= 0) continue;
-      GroupPlan& G = segs[nseg];
-      G = F;
-      G.g = F.g << k;
-      for (int j = 0; j < G.nlev; ++j) {
-        const LevelInfo& L = refs[0]->L[first - (G.first_li + j)];
-        const int g_eff = std::min(G.g, L.nstrips);
-        G.strips_per_cta[j] = (L.nstrips + g_eff - 1) / g_eff;
-      }
-      G.pair_begin = begin; G.npairs = counts[k];
-      G.nsquads = std::min(grid / G.g, std::max(counts[k], 1));
-      seg_hmax[nseg] = hmaxs[1];
-      begin += counts[k];
-      ++nseg;
-    }
-  }
-  ScratchNeed need;
-  if (fuse) add_launch_need(need, nseg, seg_hmax, segs, n);
-  else for (int gi = 0; gi < ngroups; ++gi) add_launch_need(need, 1, hmaxs + gi, groups + gi, n);
-  rc = ensure_workspace(ctx, n * nlev, need, max_log);     // d_pair_level holds the descriptors of every level
+  const LaunchPlan plan = plan_launches(ctx, refs[0], first, last, n);
+  rc = ensure_workspace(ctx, n * nlev, plan, n, 0, max_log);     // d_pair_level holds the descriptors of every level
   if (rc) return rc;
 
   // selection masks for non-default thresholds (PointSelection caches per pyramid, point_selection.cpp:100-113)
@@ -1185,39 +1034,10 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
 
   for (int i = 0; i < 8; ++i) ws.h_active[i] = 0;
   if (max_log > 0) DVO_CUDA(ctx, cudaMemsetAsync(ws.d_iter_log, 0, sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log, st));
-  LevelLaunch lps[kMaxLevels][kMaxLevels];
-  const PairLevel* d_pls[kMaxLevels];
-  for (int gi = 0; gi < ngroups; ++gi) {
-    const GroupPlan& G = groups[gi];
-    for (int k = 0; k < G.nlev; ++k) {
-      const int li = G.first_li + k, level = first - li;
-      lps[gi][k] = make_level_launch(refs[0]->L[level], cfg, li, level);
-    }
-    d_pls[gi] = ws.d_pair_level + (size_t)G.first_li * n;
-  }
-  const int nlaunch = fuse ? 1 : ngroups;
-  if (fuse) {
-    LevelLaunch seg_lps[kMaxSeg][kMaxLevels];
-    const PairLevel* seg_pls[kMaxSeg];
-    for (int sgi = 0; sgi < nseg; ++sgi) {
-      const int gi = sgi == 0 ? 0 : 1;
-      for (int k = 0; k < groups[gi].nlev; ++k) seg_lps[sgi][k] = lps[gi][k];
-      seg_pls[sgi] = d_pls[gi];
-    }
-    int* flag = nullptr;
-    if ((rc = launch_segments(ctx, nseg, seg_lps, segs, seg_hmax, seg_pls, have_init ? ws.d_tinit : nullptr, n, max_log, nullptr, 0, 0,
-                              cur_mask, &flag)))
+  for (int i = 0; i < plan.nlaunch; ++i)
+    if ((rc = launch_segments(ctx, plan.launch[i], i, cfg, refs[0]->L, first, have_init ? ws.d_tinit : nullptr, n, max_log,
+                              nullptr, 0, cur_mask)))
       return rc;
-    DVO_CUDA(ctx, cudaMemcpyAsync(&ws.h_active[level_flag_slot(0)], flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-  } else {
-    for (int gi = 0; gi < nlaunch; ++gi) {
-      int* flag = nullptr;
-      if ((rc = launch_segments(ctx, 1, lps + gi, groups + gi, hmaxs + gi, d_pls + gi, have_init ? ws.d_tinit : nullptr, n, max_log,
-                                nullptr, 0, gi, cur_mask, &flag)))
-        return rc;
-      DVO_CUDA(ctx, cudaMemcpyAsync(&ws.h_active[level_flag_slot(gi)], flag, sizeof(int), cudaMemcpyDeviceToHost, st));
-    }
-  }
   // results
   dvo_b200_result* d_res = (dvo_b200_result*)d_results_user;
   if (!d_res) {
@@ -1232,7 +1052,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   }
   DVO_CUDA(ctx, cudaGetLastError());
   if ((rc = note_foreign_uses(ctx, n, refs, curs))) return rc;   // the caller may release the pyramids once this returns
-  ctx->pending_level_flags = nlaunch;   // checked at the next synchronisation point (device-results variant)
+  ctx->pending_level_flags = plan.nlaunch;   // checked at the next synchronisation point (device-results variant)
   if (h_results) {
     size_t bytes = sizeof(dvo_b200_result) * n;
     if (bytes > ctx->h_results_bytes) {
@@ -1288,21 +1108,12 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
   Workspace& ws = ctx->ws;
   const LevelInfo& L = ref->L[level];
   if ((rc = ensure_geometry(ctx))) return rc;
-  GroupPlan plan;
-  {
-    GroupPlan tmp[kMaxLevels];
-    plan_groups(ref, level, level, ctx->num_sms * ctx->ctas_per_sm, 1, tmp);
-    plan = tmp[0];
-    ScratchNeed need;
-    const int hm = L.h;
-    add_launch_need(need, 1, &hm, &plan, 1);
-    if (planes7) need.dump_floats = 7 * (size_t)L.n;
-    if ((rc = ensure_workspace(ctx, 1, need, 0))) return rc;
-  }
+  const LaunchPlan plan = plan_launches(ctx, ref, level, level, 1);
+  if ((rc = ensure_workspace(ctx, 1, plan, 1, planes7 ? 7 * (size_t)L.n : 0, 0))) return rc;
   if ((rc = pyramid_reselect(ctx, ref, cfg->intensity_derivative_threshold, cfg->depth_derivative_threshold))) return rc;
-  LevelLaunch lp = make_level_launch(L, &c, 0, level);
-  lp.max_iterations = use_weights ? 2 : 1;    // k_set_state starts at iteration 1 / 0: exactly one iteration runs
-  lp.first_level = 1; lp.use_initial_estimate = 0; lp.precision = 0.0; lp.mu = 0.0;
+  c.max_iterations_per_level = use_weights ? 2 : 1;    // k_set_state starts at iteration 1 / 0: exactly one iteration runs
+  c.use_initial_estimate = 0; c.precision = 0.0; c.mu = 0.0;
+  const LevelLaunch lp = make_level_launch(L, &c, 0, level);
   if ((rc = ensure_stage(ctx, 1024, sizeof(PairLevel) + 1024))) return rc;
   const bool cur_mask = any_current_mask(1, curs);
   if (cur_mask && (rc = grow(ctx, ws.d_csat, ws.cap_csat, 2))) return rc;
@@ -1324,15 +1135,9 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
   k_set_state<<<1, 1, 0, st>>>(ws.d_state, ws.d_pair_level, (const double*)ctx->d_stage,
                                (const float*)((char*)ctx->d_stage + 128), use_weights, lp);
   ctx->launches += 1;
-  int* flag = nullptr;
   ws.h_active[0] = 0;
-  LevelLaunch lps[1][kMaxLevels];
-  lps[0][0] = lp;
-  const int hm = L.h;
-  const PairLevel* d_pls[1] = {ws.d_pair_level};
-  if ((rc = launch_segments(ctx, 1, lps, &plan, &hm, d_pls, nullptr, 1, 0, planes7 ? ws.d_dump : nullptr, 1, 0, cur_mask, &flag)))
+  if ((rc = launch_segments(ctx, plan.launch[0], 0, &c, ref->L, level, nullptr, 1, 0, planes7 ? ws.d_dump : nullptr, 1, cur_mask)))
     return rc;
-  DVO_CUDA(ctx, cudaMemcpyAsync(&ws.h_active[0], flag, sizeof(int), cudaMemcpyDeviceToHost, st));
   DVO_CUDA(ctx, cudaGetLastError());
   if ((rc = note_foreign_uses(ctx, 1, refs, curs))) return rc;
   PairState* hs = nullptr;

@@ -17,7 +17,7 @@ from test_gpu_generic_tiles import TILE_H, TILE_W, _rot_z, _shift_z
 
 pytestmark = pytest.mark.gpu
 
-COARSE_TILES = 110          # plan_groups (csrc/tracker.cu): a level of at most this many tiles runs one CTA per pair
+COARSE_TILES = 110          # make_launch_plan (csrc/launch_plan.h): a level of at most this many tiles runs one CTA per pair
 CTAS_PER_SM = 2             # the level kernel's occupancy on an H100 (DESIGN.md)
 PP = np.array([[2000.0, -30.0], [-30.0, 9000.0]], dtype=np.float32)
 
