@@ -54,21 +54,31 @@ static void drain_profile(dvo_b200_ctx* ctx) {
 
 namespace {
 
-__global__ void k_convert_bgr(const uint8_t* __restrict__ bgr, uint8_t* __restrict__ grey, int n) {
+__global__ void k_convert_bgr(SrcPlane bgr, uint8_t* __restrict__ grey, int w, int h) {
   // benchmark_slam.cpp:58-68: cv::cvtColor(rgb, grey, CV_BGR2GRAY) on CV_8UC3 (convertTo(CV_32F) happens in the pyramid
   // kernels' loads).  OpenCV's 8-bit path is fixed point: (B*1868 + G*9617 + R*4899 + (1 << 13)) >> 14.
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint8_t* p = bgr + 3 * (size_t)i;
-  grey[i] = (uint8_t)((1868 * (int)p[0] + 9617 * (int)p[1] + 4899 * (int)p[2] + 8192) >> 14);
+  // bgr: interleaved, 3 elements per pixel; grey: packed, image img at img * w * h.
+  const int img = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= w * h) return;
+  const int y = i / w, x = i - y * w;
+  const uint8_t* p = reinterpret_cast<const uint8_t*>(bgr.data) + bgr.at(img, y, 3 * x);
+  grey[(size_t)img * w * h + i] = (uint8_t)((1868 * (int)p[0] + 9617 * (int)p[1] + 4899 * (int)p[2] + 8192) >> 14);
+}
+
+// n BGR images -> n packed 8-bit grey images, as cv::cvtColor leaves them.  The level-0 kernels then read the grey plane (each
+// grey pixel several times: the 2x2 mean and the five taps of the central differences).
+void convert_bgr(dvo_b200_ctx* ctx, int n, int w, int h, SrcPlane bgr, uint8_t* grey) {
+  k_convert_bgr<<<dim3((unsigned)(((size_t)w * h + 255) / 256), n), 256, 0, ctx->stream>>>(bgr, grey, w, h);
+  ctx->launches++;
 }
 
 }  // namespace
 
 // Uploads n frames of one dvo_b200_input_format (and their reference masks, if any) into the context's device staging
-// area and builds their pyramids.  The frames stay in their file representation there: the pyramid kernels convert in
-// their loads (no float32 copy of a raw frame is written); BGR is reduced to 8-bit grey first, as cv::cvtColor leaves it.
-// Masks add one byte per pixel after the frames.
+// area and builds their pyramids from there, packed.  The frames stay in their file representation: the pyramid kernels
+// convert in their loads (no float32 copy of a raw frame is written); BGR is reduced to 8-bit grey first, as cv::cvtColor
+// leaves it.  Masks add one byte per pixel after the frames.
 static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image, const void* depth, float depth_scale,
                          const uint8_t* masks, int mask_roles, int width, int height, float fx, float fy, float ox, float oy,
                          int levels, dvo_b200_pyramid** out) {
@@ -86,11 +96,11 @@ static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image
   int rc = ensure_stage(ctx, masks ? mask_off + npx : frames, 0);
   if (rc) return rc;
   char* stage = (char*)ctx->d_stage;
-  const uint8_t* dM = nullptr;
+  SrcPlane dM{nullptr, 0, 0};
   if (masks) {
     DVO_CUDA(ctx, cudaMemcpyAsync(stage + mask_off, masks, npx, cudaMemcpyHostToDevice, ctx->stream));
     ctx->h2d_bytes += npx;
-    dM = (const uint8_t*)(stage + mask_off);
+    dM = packed_plane(stage + mask_off, width, height);
   }
   if (format == DVO_B200_INPUT_FLOAT32) {
     float* dI = (float*)stage;
@@ -98,7 +108,8 @@ static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image
     DVO_CUDA(ctx, cudaMemcpyAsync(dI, image, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     DVO_CUDA(ctx, cudaMemcpyAsync(dZ, depth, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     ctx->h2d_bytes += 2 * npx * sizeof(float);
-    return pyramid_build_batch_input(ctx, n, dI, dZ, 0, 0.f, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM, mask_roles);
+    return pyramid_build_batch_input(ctx, n, packed_plane(dI, width, height), packed_plane(dZ, width, height), 0, 0.f, width, height,
+                                     fx, fy, ox, oy, levels, 0.f, 0.f, out, dM, mask_roles);
   }
   uint16_t* dR = (uint16_t*)stage;
   uint8_t* dG = (uint8_t*)(stage + grey_off);
@@ -110,10 +121,45 @@ static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image
     uint8_t* dC = (uint8_t*)(stage + bgr_off);
     DVO_CUDA(ctx, cudaMemcpyAsync(dC, image, npx * 3, cudaMemcpyHostToDevice, ctx->stream));
     ctx->h2d_bytes += npx * 5;
-    k_convert_bgr<<<(unsigned)((npx + 255) / 256), 256, 0, ctx->stream>>>(dC, dG, (int)npx);   // 8-bit grey, as cv::cvtColor leaves it
-    ctx->launches++;
+    convert_bgr(ctx, n, width, height, packed_plane(dC, 3 * width, height), dG);
   }
-  return pyramid_build_batch_input(ctx, n, dG, dR, 1, depth_scale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM, mask_roles);
+  return pyramid_build_batch_input(ctx, n, packed_plane(dG, width, height), packed_plane(dR, width, height), 1, depth_scale, width,
+                                   height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM, mask_roles);
+}
+
+// One dvo_b200_device_plane of n images of width x height pixels, elem bytes per element and per_px elements per pixel ->
+// the SrcPlane the pyramid kernels read.  Every check of the header's list; the pointer checks look at the first and the
+// last byte of the plane's extent.
+static int device_plane(dvo_b200_ctx* ctx, const dvo_b200_device_plane* p, const char* name, int elem, int per_px, int n,
+                        int width, int height, SrcPlane* out) {
+  auto bad = [&](const std::string& why) {
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string("pyramid_create_device: ") + name + ": " + why);
+  };
+  if (!p || !p->data) return bad("null plane or data pointer");
+  const int64_t row = (int64_t)width * per_px * elem;
+  if (p->row_bytes < row)
+    return bad("row_bytes " + std::to_string(p->row_bytes) + " < width * bytes per pixel = " + std::to_string(row));
+  if (p->row_bytes % elem) return bad("row_bytes " + std::to_string(p->row_bytes) + " is not a multiple of " + std::to_string(elem));
+  if (p->image_bytes < 0) return bad("negative image_bytes " + std::to_string(p->image_bytes));
+  if (p->image_bytes % elem)
+    return bad("image_bytes " + std::to_string(p->image_bytes) + " is not a multiple of " + std::to_string(elem));
+  if ((uintptr_t)p->data % elem) return bad("data is not aligned to its " + std::to_string(elem) + "-byte elements");
+  int64_t a = 0, b = 0, last = 0;
+  if (__builtin_mul_overflow((int64_t)(n - 1), p->image_bytes, &a) || __builtin_mul_overflow((int64_t)(height - 1), p->row_bytes, &b) ||
+      __builtin_add_overflow(a, b, &last) || __builtin_add_overflow(last, row - 1, &last) ||
+      (uintptr_t)p->data + (uint64_t)last < (uintptr_t)p->data)
+    return bad("the extent of the plane overflows");
+  const char* ends[2] = {(const char*)p->data, (const char*)p->data + last};
+  for (const char* q : ends) {
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, q) != cudaSuccess) { cudaGetLastError(); return bad("not a CUDA pointer"); }
+    if (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)
+      return bad(attr.type == cudaMemoryTypeHost ? "pinned host memory, not device memory" : "host memory, not device memory");
+    if (attr.device != ctx->device)
+      return bad("memory of device " + std::to_string(attr.device) + ", the context is on device " + std::to_string(ctx->device));
+  }
+  *out = SrcPlane{p->data, p->row_bytes / elem, p->image_bytes / elem};
+  return 0;
 }
 
 }  // namespace dvo_b200
@@ -257,6 +303,32 @@ int dvo_b200_pyramid_create_masked_batch_roles(dvo_b200_ctx* ctx, int32_t n, int
   if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked_roles: unsupported role set " + std::to_string(roles));
   return create_staged(ctx, n, format, image, depth, depth_scale, masks, roles, width, height, fx, fy, ox, oy, levels, out);
+}
+
+int dvo_b200_pyramid_create_device_batch(dvo_b200_ctx* ctx, int32_t n, int32_t format, const dvo_b200_device_plane* image,
+                                         const dvo_b200_device_plane* depth, float depth_scale, const dvo_b200_device_plane* masks,
+                                         int32_t roles, int32_t width, int32_t height, float fx, float fy, float ox, float oy,
+                                         int32_t levels, dvo_b200_pyramid** out) {
+  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_device: null/invalid argument");
+  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_device: unknown input format " + std::to_string(format));
+  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_device: unsupported role set " + std::to_string(roles));
+  cudaSetDevice(ctx->device);
+  const bool f32 = format == DVO_B200_INPUT_FLOAT32;
+  SrcPlane I, Z, M{nullptr, 0, 0};
+  int rc = device_plane(ctx, image, "image", f32 ? 4 : 1, format == DVO_B200_INPUT_BGR8_DEPTH16 ? 3 : 1, n, width, height, &I);
+  if (!rc) rc = device_plane(ctx, depth, "depth", f32 ? 4 : 2, 1, n, width, height, &Z);
+  if (!rc && masks) rc = device_plane(ctx, masks, "masks", 1, 1, n, width, height, &M);
+  if (rc) return rc;
+  if (format == DVO_B200_INPUT_BGR8_DEPTH16) {   // grey into staging, as the host path; depth and masks stay in place
+    if ((rc = ensure_stage(ctx, (size_t)width * height * n, 0))) return rc;
+    convert_bgr(ctx, n, width, height, I, (uint8_t*)ctx->d_stage);
+    I = packed_plane(ctx->d_stage, width, height);
+  }
+  return pyramid_build_batch_input(ctx, n, I, Z, f32 ? 0 : 1, f32 ? 0.f : depth_scale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f,
+                                   out, M, roles);
 }
 
 int dvo_b200_pyramid_mask_roles(const dvo_b200_pyramid* p) { return p ? p->mask_roles : DVO_B200_ERR_INVALID_ARGUMENT; }

@@ -249,13 +249,25 @@ struct ProfScope {
   ~ProfScope();
 };
 
+// One plane of level-0 input in device memory: element (img, y, x) of the plane is data[img * stride + y * pitch + x], in
+// elements of the plane's type (a pixel of interleaved BGR is 3 elements).  Packed planes: pitch = row elements, stride =
+// pitch * h.  stride = 0: every image reads the same plane.
+struct SrcPlane {
+  const void* data;
+  int64_t pitch, stride;
+  __host__ __device__ size_t at(int img, int y, int x) const { return (size_t)((int64_t)img * stride + (int64_t)y * pitch + x); }
+};
+inline SrcPlane packed_plane(const void* data, int row_elems, int h) { return {data, row_elems, (int64_t)row_elems * h}; }
+
 // pyramid.cu
 int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float* d_Z, int w, int h, float fx, float fy,
                         float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out);
-int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const void* d_Z, int raw, float zscale, int w, int h,
+// I / Z: level-0 intensity and depth (raw == 0: float32 / float32 metres; raw == 1: 8-bit grey / 16-bit raw depth).  M: the
+// masks (bytes, nonzero = usable), or M.data == NULL for none; mask_roles: DVO_B200_MASK_ROLE_* bits (ignored without masks).
+// The build reads I, Z and M in place until its last kernel has run.
+int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, SrcPlane I, SrcPlane Z, int raw, float zscale, int w, int h,
                               float fx, float fy, float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out,
-                              const uint8_t* d_masks, int mask_roles);   // d_masks: n*h*w device bytes, nonzero = usable; or NULL
-                                                                         // mask_roles: DVO_B200_MASK_ROLE_* bits (ignored without masks)
+                              SrcPlane M, int mask_roles);
 int pyramid_reselect(dvo_b200_ctx* ctx, dvo_b200_pyramid* p, float ti, float td);
 void wait_for_pyramid(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p);   // order ctx's stream after the pyramid's build / re-selection
 int note_foreign_use(dvo_b200_ctx* ctx, const dvo_b200_pyramid* p);    // after enqueueing work that reads p (see Slab::foreign_uses)

@@ -14,7 +14,8 @@ namespace {
 
 __device__ __forceinline__ bool is_nan(float v) { return v != v; }
 
-// Level-0 pixels as they were uploaded.  kRaw = false: float32 intensity and float32 depth in metres (NaN = invalid), what
+// Level-0 pixels as the caller's planes hold them (uploaded into staging, or in place in the caller's device memory; i is
+// the element index of a SrcPlane).  kRaw = false: float32 intensity and float32 depth in metres (NaN = invalid), what
 // benchmark_slam.cpp:46-93 hands to RgbdCameraPyramid::create.  kRaw = true: 8-bit grey and 16-bit raw depth straight from
 // the image files; the loader's conversions -- convertTo(CV_32F) and SurfacePyramid::convertRawDepthImageSse
 // (surface_pyramid.cpp:65-105: u16 * scale, 0 -> NaN) -- happen in the load, no float32 copy of the frame is ever written.
@@ -33,12 +34,13 @@ __device__ __forceinline__ float load_depth(const void* Z, size_t i, float scale
 }
 
 // level l intensity = ((a+b)+c)+d)/4 of the 2x2 block of level l-1 (rgbd_image.cpp:38-55), into P0.x (the Z slot is
-// filled by the finish pass).  kFromInput: level 1 reads the input image, which is level 0's intensity.
-// sp / dp: row pitch of the source / destination planes (float2 elements).
+// filled by the finish pass).  kFromInput: level 1 reads the input plane I0, which is level 0's intensity.  aligned: the
+// base address, row pitch and image stride of I0 are all multiples of two elements, so every 2x2 block starts at a
+// two-element boundary (packed planes: even w and w*h).  sp / dp: row pitch of the source / destination planes (float2
+// elements).
 template <bool kFromInput, bool kRaw>
-__global__ void k_pyr_intensity_down(const void* __restrict__ I0, size_t in_stride, int aligned, float2* __restrict__ planes,
-                                     size_t planes_per_image, size_t src_off, int sw, int sp, size_t dst_off, int dw, int dh,
-                                     int dp) {
+__global__ void k_pyr_intensity_down(SrcPlane I0, int aligned, float2* __restrict__ planes, size_t planes_per_image,
+                                     size_t src_off, int sp, size_t dst_off, int dw, int dh, int dp) {
   int img = blockIdx.y;
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= dw * dh) return;
@@ -46,22 +48,23 @@ __global__ void k_pyr_intensity_down(const void* __restrict__ I0, size_t in_stri
   float2* D = planes + img * planes_per_image + dst_off;
   float a, b, c, d;
   if (kFromInput) {
-    const size_t i0 = (size_t)img * in_stride + (size_t)(2 * y) * sw + 2 * x;
+    const size_t i0 = I0.at(img, 2 * y, 2 * x);
+    const int64_t r = I0.pitch;
     if (kRaw) {
-      const uint8_t* g = reinterpret_cast<const uint8_t*>(I0) + i0;
-      if (aligned) {   // even width and image stride: every 2x2 block starts 2-byte aligned
-        const uchar2 u = __ldg(reinterpret_cast<const uchar2*>(g)), v = __ldg(reinterpret_cast<const uchar2*>(g + sw));
+      const uint8_t* g = reinterpret_cast<const uint8_t*>(I0.data) + i0;
+      if (aligned) {
+        const uchar2 u = __ldg(reinterpret_cast<const uchar2*>(g)), v = __ldg(reinterpret_cast<const uchar2*>(g + r));
         a = (float)u.x; b = (float)u.y; c = (float)v.x; d = (float)v.y;
       } else {
-        a = (float)__ldg(g); b = (float)__ldg(g + 1); c = (float)__ldg(g + sw); d = (float)__ldg(g + sw + 1);
+        a = (float)__ldg(g); b = (float)__ldg(g + 1); c = (float)__ldg(g + r); d = (float)__ldg(g + r + 1);
       }
     } else {
-      const float* p0 = reinterpret_cast<const float*>(I0) + i0;
-      if (aligned) {   // even width and image stride: every 2x2 block starts 8-byte aligned
-        const float2 u = __ldg(reinterpret_cast<const float2*>(p0)), v = __ldg(reinterpret_cast<const float2*>(p0 + sw));
+      const float* p0 = reinterpret_cast<const float*>(I0.data) + i0;
+      if (aligned) {
+        const float2 u = __ldg(reinterpret_cast<const float2*>(p0)), v = __ldg(reinterpret_cast<const float2*>(p0 + r));
         a = u.x; b = u.y; c = v.x; d = v.y;
       } else {
-        a = __ldg(p0); b = __ldg(p0 + 1); c = __ldg(p0 + sw); d = __ldg(p0 + sw + 1);
+        a = __ldg(p0); b = __ldg(p0 + 1); c = __ldg(p0 + r); d = __ldg(p0 + r + 1);
       }
     }
   } else {
@@ -79,21 +82,22 @@ __global__ void k_pyr_intensity_down(const void* __restrict__ I0, size_t in_stri
 __device__ __forceinline__ bool bit_set(const uint32_t* __restrict__ words, size_t i) { return (__ldg(words + (i >> 5)) >> (i & 31)) & 1u; }
 
 // Usable bits of one level of a pyramid built with a reference mask, in the word layout of the selection masks (bit i of
-// word k = linear pixel 32k+i).  Level 0: the caller's h*w bytes, nonzero = usable.  Level l: a pixel is usable iff the
-// four pixels of its 2x2 block in level l-1 are -- the chain of the 2x2 intensity mean -- so iff every level-0 pixel of
-// its footprint [x 2^l, (x+1) 2^l) x [y 2^l, (y+1) 2^l) is.  Runs before k_pyr_finish of the same level.
+// word k = linear pixel 32k+i).  Level 0: the caller's mask plane of bytes, nonzero = usable.  Level l: a pixel is usable
+// iff the four pixels of its 2x2 block in level l-1 are -- the chain of the 2x2 intensity mean -- so iff every level-0 pixel
+// of its footprint [x 2^l, (x+1) 2^l) x [y 2^l, (y+1) 2^l) is.  Runs before k_pyr_finish of the same level.
 template <bool kLevel0>
 __global__ void __launch_bounds__(256)
-k_usable(const uint8_t* __restrict__ mask0, uint32_t* __restrict__ usable, size_t words_per_image, size_t src_off, int sw,
-         size_t dst_off, int w, int h) {
+k_usable(SrcPlane mask0, uint32_t* __restrict__ usable, size_t words_per_image, size_t src_off, int sw, size_t dst_off, int w,
+         int h) {
   const int img = blockIdx.y;
   const int n = w * h;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   uint32_t* U = usable + img * words_per_image;
   bool u = false;
   if (idx < n) {
-    if (kLevel0) {
-      u = __ldg(mask0 + (size_t)img * n + idx) != 0;
+    if (kLevel0) {   // rows packed (the staged masks): the linear index needs no division
+      const size_t i = mask0.pitch == w ? (size_t)((int64_t)img * mask0.stride) + idx : mask0.at(img, idx / w, idx % w);
+      u = __ldg(reinterpret_cast<const uint8_t*>(mask0.data) + i) != 0;
     } else {
       const int y = idx / w, x = idx - y * w;
       const size_t j = (size_t)(2 * y) * sw + 2 * x;   // top-left pixel of the block in level l-1
@@ -115,10 +119,9 @@ k_usable(const uint8_t* __restrict__ mask0, uint32_t* __restrict__ usable, size_
 // bit (k_usable); only the reference role changes, P0 / P2 are written as without a mask.
 template <bool kLevel0, bool kRaw, bool kMasked>
 __global__ void __launch_bounds__(256)
-k_pyr_finish(const void* __restrict__ I0, const void* __restrict__ Z0, float zscale, int w0, int n0, float2* __restrict__ planes,
-             size_t planes_per_image, size_t plane_off, size_t rec_off, int nbands, int w, int h, int pitch, int level,
-             uint32_t* __restrict__ masks, size_t mask_words_per_image, size_t mask_off, float ti, float td,
-             const uint32_t* __restrict__ usable) {
+k_pyr_finish(SrcPlane I0, SrcPlane Z0, float zscale, float2* __restrict__ planes, size_t planes_per_image, size_t plane_off,
+             size_t rec_off, int nbands, int w, int h, int pitch, int level, uint32_t* __restrict__ masks,
+             size_t mask_words_per_image, size_t mask_off, float ti, float td, const uint32_t* __restrict__ usable) {
   const int img = blockIdx.y;
   const int n = w * h;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -130,12 +133,13 @@ k_pyr_finish(const void* __restrict__ I0, const void* __restrict__ Z0, float zsc
     float2* P0 = planes + img * planes_per_image + plane_off;
     float2* P2 = P0 + plane;   // P2 = (I, Z); the depth gradients are not stored
     float2* rec = planes + img * planes_per_image + rec_off;   // reference tile records: (I, Zsel) and (Ix, Iy)
-    const size_t zb = (size_t)img * n0;
     const int xp = max(x - 1, 0), xn = min(x + 1, w - 1), yp = max(y - 1, 0), yn = min(y + 1, h - 1);
     float I, ixp, ixn, iyp, iyn;
     if (kLevel0) {
-      I = load_intensity<kRaw>(I0, zb + idx); ixp = load_intensity<kRaw>(I0, zb + y * w + xp); ixn = load_intensity<kRaw>(I0, zb + y * w + xn);
-      iyp = load_intensity<kRaw>(I0, zb + yp * w + x); iyn = load_intensity<kRaw>(I0, zb + yn * w + x);
+      const void* g = I0.data;
+      I = load_intensity<kRaw>(g, I0.at(img, y, x)); ixp = load_intensity<kRaw>(g, I0.at(img, y, xp));
+      ixn = load_intensity<kRaw>(g, I0.at(img, y, xn));
+      iyp = load_intensity<kRaw>(g, I0.at(img, yp, x)); iyn = load_intensity<kRaw>(g, I0.at(img, yn, x));
     } else {
       const size_t row = (size_t)y * pitch;
       I = P0[row + x].x; ixp = P0[row + xp].x; ixn = P0[row + xn].x;
@@ -143,11 +147,12 @@ k_pyr_finish(const void* __restrict__ I0, const void* __restrict__ Z0, float zsc
     }
     const float ix = (ixn - ixp) * 0.5f;
     const float iy = (iyn - iyp) * 0.5f;
-    const size_t zr = (size_t)(y << level) * w0;
-    const float z = load_depth<kRaw>(Z0, zb + zr + (x << level), zscale);
-    const float zx = (load_depth<kRaw>(Z0, zb + zr + (xn << level), zscale) - load_depth<kRaw>(Z0, zb + zr + (xp << level), zscale)) * 0.5f;
-    const float zy = (load_depth<kRaw>(Z0, zb + (size_t)(yn << level) * w0 + (x << level), zscale) -
-                      load_depth<kRaw>(Z0, zb + (size_t)(yp << level) * w0 + (x << level), zscale)) * 0.5f;
+    const void* zp = Z0.data;
+    const float z = load_depth<kRaw>(zp, Z0.at(img, y << level, x << level), zscale);
+    const float zx = (load_depth<kRaw>(zp, Z0.at(img, y << level, xn << level), zscale) -
+                      load_depth<kRaw>(zp, Z0.at(img, y << level, xp << level), zscale)) * 0.5f;
+    const float zy = (load_depth<kRaw>(zp, Z0.at(img, yn << level, x << level), zscale) -
+                      load_depth<kRaw>(zp, Z0.at(img, yp << level, x << level), zscale)) * 0.5f;
     const bool bad = is_nan(I) || is_nan(ix) || is_nan(iy) || is_nan(z) || is_nan(zx) || is_nan(zy);
     const float zm = bad ? __int_as_float(0x7fc00000) : z;
     const size_t o = (size_t)y * pitch + x;
@@ -441,17 +446,19 @@ void pool_close(dvo_b200_ctx* ctx) {
 
 int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float* d_Z, int w, int h, float fx, float fy,
                         float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out) {
-  return pyramid_build_batch_input(ctx, n, d_I, d_Z, 0, 0.f, w, h, fx, fy, ox, oy, levels, ti, td, out, nullptr, 0);
+  return pyramid_build_batch_input(ctx, n, packed_plane(d_I, w, h), packed_plane(d_Z, w, h), 0, 0.f, w, h, fx, fy, ox, oy, levels,
+                                   ti, td, out, SrcPlane{nullptr, 0, 0}, 0);
 }
 
-// d_I / d_Z: raw == 0: float32 intensity / float32 depth; raw == 1: 8-bit grey / 16-bit raw depth (depth = raw * zscale, 0 -> NaN)
-// d_masks: n consecutive h*w byte reference masks (nonzero = usable) or NULL.  Without masks the slab holds no usable bits
-// and the build runs exactly the kernels it ran before masks existed.  mask_roles with DVO_B200_MASK_ROLE_CURRENT: the
-// masks also act in the current role (k_cur_mask, k_cur_sat after the other kernels of each level); otherwise the build is
-// the reference-mask build, kernel for kernel.
-int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const void* d_Z, int raw, float zscale, int w, int h,
+// I / Z: raw == 0: float32 intensity / float32 depth; raw == 1: 8-bit grey / 16-bit raw depth (depth = raw * zscale, 0 -> NaN)
+// M: reference masks of bytes (nonzero = usable), or M.data == NULL.  Without masks the slab holds no usable bits and the
+// build runs exactly the kernels it ran before masks existed.  mask_roles with DVO_B200_MASK_ROLE_CURRENT: the masks also
+// act in the current role (k_cur_mask, k_cur_sat after the other kernels of each level); otherwise the build is the
+// reference-mask build, kernel for kernel.  The planes are read where they lie, with their pitch and stride: staged
+// uploads and the caller's device memory take the same kernels.
+int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, SrcPlane I, SrcPlane Z, int raw, float zscale, int w, int h,
                               float fx, float fy, float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out,
-                              const uint8_t* d_masks, int mask_roles) {
+                              SrcPlane M, int mask_roles) {
   if (n <= 0 || levels < 1 || levels > kMaxLevels || w < 32 || h < 2)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid: bad geometry");
   LevelInfo L[kMaxLevels];
@@ -490,7 +497,7 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
   size_t bytes_tmpl = (size_t)n * tmpl_floats * sizeof(float);
   size_t bytes_sel = align_up((size_t)n * sel_ints * sizeof(int), 256);
   size_t bytes_range = (size_t)n * range_f2 * sizeof(float2);
-  const bool masked = d_masks != nullptr;
+  const bool masked = M.data != nullptr;
   size_t bytes_usable = masked ? bytes_masks : 0;   // usable bits: the layout of the selection masks
   const bool cur_masked = masked && (mask_roles & DVO_B200_MASK_ROLE_CURRENT) != 0;
   size_t bytes_sat = cur_masked ? (size_t)n * sat_ints * sizeof(int) : 0;   // unusable-pixel summaries, after the usable bits
@@ -510,6 +517,10 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
   {
     ProfScope prof(ctx, 3, (cur_masked ? 9 : masked ? 7 : 6) * levels - 1);
     const int T = 256;
+    // the 2x2 blocks of level 0 start at two-element boundaries: base address, row pitch and image stride even (in elements)
+    const size_t two_elems = raw ? 2 : 2 * sizeof(float);
+    const int aligned = (uintptr_t)I.data % two_elems == 0 && I.pitch % 2 == 0 && I.stride % 2 == 0 ? 1 : 0;
+    const SrcPlane none{nullptr, 0, 0};
     for (int l = 0; l < levels; ++l) {
       const LevelInfo& q = L[l];
       dim3 gt((q.w + q.h + T - 1) / T, n);
@@ -517,24 +528,23 @@ int pyramid_build_batch_input(dvo_b200_ctx* ctx, int n, const void* d_I, const v
       ctx->launches += 1;
       if (l == 0) continue;   // level 0 takes its intensity from the input image
       dim3 g((q.n + T - 1) / T, n);
-      const int aligned = (((size_t)w * h) | (size_t)w) % 2 == 0 ? 1 : 0;
-      if (l == 1 && raw) k_pyr_intensity_down<true, true><<<g, T, 0, st>>>(d_I, (size_t)w * h, aligned, planes, plane_f2, 0, L[0].w, L[0].pitch, q.plane_off, q.w, q.h, q.pitch);
-      else if (l == 1) k_pyr_intensity_down<true, false><<<g, T, 0, st>>>(d_I, (size_t)w * h, aligned, planes, plane_f2, 0, L[0].w, L[0].pitch, q.plane_off, q.w, q.h, q.pitch);
-      else k_pyr_intensity_down<false, false><<<g, T, 0, st>>>(nullptr, 0, 0, planes, plane_f2, L[l - 1].plane_off, L[l - 1].w, L[l - 1].pitch, q.plane_off, q.w, q.h, q.pitch);
+      if (l == 1 && raw) k_pyr_intensity_down<true, true><<<g, T, 0, st>>>(I, aligned, planes, plane_f2, 0, L[0].pitch, q.plane_off, q.w, q.h, q.pitch);
+      else if (l == 1) k_pyr_intensity_down<true, false><<<g, T, 0, st>>>(I, aligned, planes, plane_f2, 0, L[0].pitch, q.plane_off, q.w, q.h, q.pitch);
+      else k_pyr_intensity_down<false, false><<<g, T, 0, st>>>(none, 0, planes, plane_f2, L[l - 1].plane_off, L[l - 1].pitch, q.plane_off, q.w, q.h, q.pitch);
       ctx->launches += 1;
     }
     for (int l = 0; l < levels; ++l) {
       const LevelInfo& q = L[l];
       dim3 g((q.words * 32 + T - 1) / T, n);
       if (masked) {
-        if (l == 0) k_usable<true><<<g, T, 0, st>>>(d_masks, usable, mask_words, 0, 0, q.mask_off, q.w, q.h);
-        else k_usable<false><<<g, T, 0, st>>>(nullptr, usable, mask_words, L[l - 1].mask_off, L[l - 1].w, q.mask_off, q.w, q.h);
+        if (l == 0) k_usable<true><<<g, T, 0, st>>>(M, usable, mask_words, 0, 0, q.mask_off, q.w, q.h);
+        else k_usable<false><<<g, T, 0, st>>>(none, usable, mask_words, L[l - 1].mask_off, L[l - 1].w, q.mask_off, q.w, q.h);
         ctx->launches += 1;
       }
-      if (l == 0 && raw) launch_finish<true, true>(masked, g, st, d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
-      else if (l == 0) launch_finish<true, false>(masked, g, st, d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
-      else if (raw) launch_finish<false, true>(masked, g, st, d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
-      else launch_finish<false, false>(masked, g, st, d_I, d_Z, zscale, w, w * h, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
+      if (l == 0 && raw) launch_finish<true, true>(masked, g, st, I, Z, zscale, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
+      else if (l == 0) launch_finish<true, false>(masked, g, st, I, Z, zscale, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
+      else if (raw) launch_finish<false, true>(masked, g, st, I, Z, zscale, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
+      else launch_finish<false, false>(masked, g, st, I, Z, zscale, planes, plane_f2, q.plane_off, q.rec_off, q.nbands, q.w, q.h, q.pitch, l, masks, mask_words, q.mask_off, ti, td, usable);
       k_sel_info<<<n, 32, 0, st>>>(masks, mask_words, q.mask_off, q.words, sel, sel_ints, l);
       k_drop_odd_last<<<(n + 127) / 128, 128, 0, st>>>(planes, plane_f2, q.rec_off, q.nbands, q.w, sel, sel_ints, l, n);
       const int ntiles = q.nbands * q.nstrips;

@@ -30,7 +30,7 @@ ABI_SYMBOLS = [
     "dvo_b200_sharded_num_shards", "dvo_b200_sharded_ctx", "dvo_b200_sharded_last_error", "dvo_b200_shard_range",
     "dvo_b200_sharded_pyramid_create_batch", "dvo_b200_sharded_pyramid_create_raw_batch", "dvo_b200_match_batch_sharded",
     "dvo_b200_set_estimator", "dvo_b200_get_estimator", "dvo_b200_pyramid_create_masked_batch",
-    "dvo_b200_pyramid_create_masked_batch_roles", "dvo_b200_pyramid_mask_roles",
+    "dvo_b200_pyramid_create_masked_batch_roles", "dvo_b200_pyramid_mask_roles", "dvo_b200_pyramid_create_device_batch",
 ]
 
 # dvo_b200_estimator
@@ -58,6 +58,62 @@ class Config(C.Structure):
             if not hasattr(self, k):
                 raise AttributeError(k)
             setattr(self, k, v)
+
+
+class DevicePlane(C.Structure):
+    """dvo_b200_device_plane: one plane of a batch of images in device memory"""
+    _fields_ = [("data", C.c_void_p), ("row_bytes", C.c_int64), ("image_bytes", C.c_int64)]
+
+
+def device_planes(image, depth, masks=None):
+    """The arguments of dvo_b200_pyramid_create_device_batch for torch tensors, from their shapes, dtypes and strides alone
+    (nothing is copied, and the tensors may live on any device):
+        float32 [n,h,w] image + float32 [n,h,w] depth   -> "float32"
+        uint8 [n,h,w] grey + uint16 [n,h,w] raw depth   -> "grey8_depth16"
+        uint8 [n,h,w,3] BGR + uint16 [n,h,w] raw depth  -> "bgr8_depth16" (pixel stride 3, channel stride 1)
+    masks: None, or bool / uint8 [n,h,w] or [h,w] (nonzero = usable); a [h,w] mask, or one expanded along n, is one mask
+    for the whole batch (image_bytes 0).  Strided views such as a crop big[:, y0:y0+h, x0:x0+w] become a plane with the
+    larger image's row pitch.  Returns (format, (n, h, w), image, depth, masks) with each plane a (data_ptr, row_bytes,
+    image_bytes) tuple, masks None without a mask.  A layout that one row pitch and one image stride per plane cannot
+    express (a column stride other than one pixel, rows that overlap) raises ValueError."""
+    import torch
+    if image.dtype == torch.float32 and image.dim() == 3:
+        fmt, depth_dtype, px = "float32", torch.float32, 1
+    elif image.dtype == torch.uint8 and image.dim() == 3:
+        fmt, depth_dtype, px = "grey8_depth16", torch.uint16, 1
+    elif image.dtype == torch.uint8 and image.dim() == 4 and image.shape[3] == 3:
+        fmt, depth_dtype, px = "bgr8_depth16", torch.uint16, 3
+    else:
+        raise ValueError(f"image: {image.dtype} {tuple(image.shape)} is none of float32 [n,h,w], uint8 [n,h,w] (grey) or "
+                         "uint8 [n,h,w,3] (BGR)")
+    n, h, w = (int(v) for v in image.shape[:3])
+    if depth.dtype != depth_dtype or tuple(depth.shape) != (n, h, w):
+        raise ValueError(f"depth: {depth.dtype} {tuple(depth.shape)}, want {depth_dtype} {(n, h, w)} with a {fmt} image")
+    if px == 3 and image.stride(3) != 1:
+        raise ValueError(f"image: BGR channel stride {image.stride(3)}, want 1 (interleaved pixels)")
+
+    def plane(t, name, per_px, shared=False):
+        es = t.element_size()
+        if w > 1 and t.stride(-1 if per_px == 1 else -2) != per_px:
+            raise ValueError(f"{name}: column stride {t.stride(-1 if per_px == 1 else -2)} elements, want {per_px} (pixels packed "
+                             "within a row)")
+        row = t.stride(-2 if per_px == 1 else -3) if h > 1 else w * per_px
+        if row < w * per_px:
+            raise ValueError(f"{name}: row stride {row} elements is below the {w * per_px} of a row (rows overlap)")
+        img = 0 if shared or n == 1 else t.stride(0)
+        return (t.data_ptr(), row * es, img * es)
+
+    pm = None
+    if masks is not None:
+        if masks.dtype not in (torch.bool, torch.uint8):
+            raise ValueError(f"masks: {masks.dtype}, want bool or uint8")
+        if tuple(masks.shape) == (h, w):
+            pm = plane(masks, "masks", 1, shared=True)
+        elif tuple(masks.shape) == (n, h, w):
+            pm = plane(masks, "masks", 1)
+        else:
+            raise ValueError(f"masks: shape {tuple(masks.shape)}, want {(n, h, w)} or {(h, w)}")
+    return fmt, (n, h, w), plane(image, "image", px), plane(depth, "depth", 1), pm
 
 
 class IterationStats(C.Structure):
@@ -135,6 +191,9 @@ def load_library():
                                                        C.c_float, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_create_masked_batch_roles.argtypes = [vp, i32, i32, vp, vp, C.c_float, vp, i32, i32, i32, C.c_float, C.c_float,
                                                              C.c_float, C.c_float, i32, C.POINTER(vp)]
+    L.dvo_b200_pyramid_create_device_batch.argtypes = [vp, i32, i32, C.POINTER(DevicePlane), C.POINTER(DevicePlane), C.c_float,
+                                                       C.POINTER(DevicePlane), i32, i32, i32, C.c_float, C.c_float, C.c_float,
+                                                       C.c_float, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_mask_roles.argtypes = [vp]
     L.dvo_b200_pyramid_device.argtypes = [vp]
     L.dvo_b200_sharded_create.argtypes = [i32, C.POINTER(i32), C.POINTER(vp)]
@@ -367,6 +426,40 @@ class Engine:
         fx, fy, ox, oy = intrinsics
         out = (C.c_void_p * n)()
         self._check(self.lib.dvo_b200_pyramid_create_bgr_batch(self.ctx, n, pC, pD, depth_scale, w, h, fx, fy, ox, oy, levels, out))
+        return [Pyramid(self, out[i]) for i in range(n)]
+
+    def pyramid_batch_device(self, image, depth, intrinsics, levels: int, depth_scale=None, masks=None,
+                             mask_roles="reference") -> list[Pyramid]:
+        """Pyramids from torch CUDA tensors on the engine's device, read in place (dvo_b200_pyramid_create_device_batch): no
+        host round trip and no host synchronisation.  The format follows from the dtypes and shapes (device_planes);
+        depth_scale (metres per raw depth unit) is required for uint16 depth.  masks / mask_roles as in pyramid_batch.
+        Ordered with torch: the engine's stream waits for the current stream before the build, and the current stream waits
+        for the build after it, so the inputs may be produced and overwritten on the current stream."""
+        import torch
+        if mask_roles not in MASK_ROLES:
+            raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
+        fmt, (n, h, w), pI, pZ, pM = device_planes(image, depth, masks)
+        if fmt != "float32" and depth_scale is None:
+            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
+        dev = torch.device("cuda", self.device)
+        inputs = [t for t in (image, depth, masks) if t is not None]
+        for t in inputs:
+            if t.device != dev:
+                raise ValueError(f"a tensor on {t.device}: the engine runs on {dev}")
+        I, Z = DevicePlane(*pI), DevicePlane(*pZ)
+        M = DevicePlane(*pM) if pM is not None else None
+        fx, fy, ox, oy = intrinsics
+        out = (C.c_void_p * n)()
+        current = torch.cuda.current_stream(dev)
+        ext = torch.cuda.ExternalStream(self.stream, device=dev)
+        ext.wait_stream(current)
+        for t in inputs:
+            t.record_stream(ext)     # the caching allocator keeps the memory until the build has read it
+        rc = self.lib.dvo_b200_pyramid_create_device_batch(self.ctx, n, INPUT_FORMATS[fmt], C.byref(I), C.byref(Z),
+                                                           float(depth_scale or 0.0), C.byref(M) if M is not None else None,
+                                                           MASK_ROLES[mask_roles], w, h, fx, fy, ox, oy, levels, out)
+        current.wait_stream(ext)
+        self._check(rc)
         return [Pyramid(self, out[i]) for i in range(n)]
 
     def pyramid_raw(self, grey_u8, depth_u16, depth_scale, intrinsics, levels: int, mask=None, mask_roles="reference") -> Pyramid:

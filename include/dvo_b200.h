@@ -211,6 +211,41 @@ int dvo_b200_pyramid_create_masked_batch_roles(dvo_b200_ctx* ctx, int32_t n, int
                                                const void* depth, float depth_scale, const uint8_t* masks, int32_t roles,
                                                int32_t width, int32_t height, float fx, float fy, float ox, float oy,
                                                int32_t levels, dvo_b200_pyramid** out /* n handles */);
+/* One plane of a batch of images in DEVICE memory (dvo_b200_pyramid_create_device_batch): row y of image i starts at
+ * (const char*)data + i * image_bytes + y * row_bytes, its pixels packed.  A cropped view of a larger image is a plane
+ * whose data points at the crop's first pixel, with the larger image's row_bytes. */
+typedef struct dvo_b200_device_plane {
+  const void* data;     /* device (or managed) memory on the context's device, aligned to the element size */
+  int64_t row_bytes;    /* >= width * bytes per pixel of the plane, a multiple of the element size */
+  int64_t image_bytes;  /* image i starts at data + i * image_bytes; >= 0, a multiple of the element size (0: every image
+                         * reads the same plane, e.g. one mask of the robot's body or a vignette for the whole batch) */
+} dvo_b200_device_plane;
+/* dvo_b200_pyramid_create_masked_batch_roles from planes already in device memory (frames decoded, rendered, rectified or
+ * cropped on the GPU; masks from a segmentation network), without a host round trip: the same pyramids, bit for bit, as
+ * that call with the same format, values, masks and roles -- every plane, the selection, S, the odd last point, the usable
+ * bits and the current-role masking.
+ *   Planes by format (element size, bytes per pixel): FLOAT32 image and depth (4, 4); GREY8_DEPTH16 grey (1, 1) and raw
+ *     depth (2, 2); BGR8_DEPTH16 interleaved BGR (1, 3) and raw depth (2, 2); masks (1, 1), nonzero = usable, NULL: no mask
+ *     (the unmasked pyramids of the format).  depth_scale is ignored for FLOAT32.
+ *   Reads in place: depth and masks are read by the build's kernels where they lie (depth by every level's kernels); only
+ *     BGR is reduced to 8-bit grey in the context's staging memory first.  Nothing is copied from the host:
+ *     dvo_b200_h2d_bytes does not move.
+ *   Stream order: all work is enqueued on dvo_b200_stream(ctx), and the call does not synchronise.  The inputs must be
+ *     ready in that stream's order: make that stream wait for their producer (cudaStreamWaitEvent), or create the context
+ *     on the producer's stream (dvo_b200_create(device, stream, ...)).  The caller must not modify or free the inputs until
+ *     the work this call enqueued has completed (record an event on dvo_b200_stream(ctx) after the call and wait for it),
+ *     as with the source of cudaMemcpyAsync.  The pyramids themselves follow the rules of every other pyramid.
+ *   Validation (DVO_B200_ERR_INVALID_ARGUMENT with dvo_b200_last_error set, and nothing is created): a NULL
+ *     image, depth or data pointer; an unknown format or role set (as dvo_b200_pyramid_create_masked_batch_roles); a
+ *     row_bytes below width * bytes per pixel or not a multiple of the element size; a negative image_bytes or one that is
+ *     not a multiple of the element size; a data pointer not aligned to the element size; and a first or last byte of a
+ *     plane's extent that cudaPointerGetAttributes does not report as device or managed memory of the context's device --
+ *     pageable or pinned host memory is refused, never copied. */
+int dvo_b200_pyramid_create_device_batch(dvo_b200_ctx* ctx, int32_t n, int32_t format, const dvo_b200_device_plane* image,
+                                         const dvo_b200_device_plane* depth, float depth_scale,
+                                         const dvo_b200_device_plane* masks /* NULL: no mask */, int32_t roles, int32_t width,
+                                         int32_t height, float fx, float fy, float ox, float oy, int32_t levels,
+                                         dvo_b200_pyramid** out /* n handles */);
 /* Role set a pyramid was created with: 0 (no mask), DVO_B200_MASK_ROLE_REFERENCE, or
  * DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT; DVO_B200_ERR_INVALID_ARGUMENT for a null handle. */
 int dvo_b200_pyramid_mask_roles(const dvo_b200_pyramid* p);
