@@ -1,6 +1,7 @@
 // capi.cu -- the extern "C" surface declared in include/dvo_b200.h.
 #include "common.cuh"
 
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -75,13 +76,35 @@ void convert_bgr(dvo_b200_ctx* ctx, int n, int w, int h, SrcPlane bgr, uint8_t* 
 
 }  // namespace
 
+// The last step of every create: build the pyramids from level-0 planes in device memory.  With a rectifier, the planes are
+// first remapped into packed float32 planes (and byte masks) in the staging memory at rect_off, which the caller has sized
+// with rectified_bytes, and the build reads those with the rectifier's size and intrinsics.
+static size_t rectified_bytes(const dvo_b200_rectifier* rect, int n, bool masked) {
+  return rect ? (size_t)rect->w * rect->h * n * (2 * sizeof(float) + (masked ? 1 : 0)) : 0;
+}
+
+static int build_planes(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, size_t rect_off, int n, SrcPlane I, SrcPlane Z, int raw,
+                        float zscale, SrcPlane M, int roles, int width, int height, float fx, float fy, float ox, float oy, int levels,
+                        dvo_b200_pyramid** out) {
+  if (!rect)
+    return pyramid_build_batch_input(ctx, n, I, Z, raw, zscale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, M, roles);
+  const size_t npx = (size_t)rect->w * rect->h * n;
+  float* dI = (float*)((char*)ctx->d_stage + rect_off);
+  float* dZ = dI + npx;
+  uint8_t* dM = M.data ? (uint8_t*)(dZ + npx) : nullptr;
+  rectify_batch(ctx, rect, n, I, Z, raw, zscale, M, dI, dZ, dM);
+  return pyramid_build_batch_input(ctx, n, packed_plane(dI, rect->w, rect->h), packed_plane(dZ, rect->w, rect->h), 0, 0.f, rect->w,
+                                   rect->h, rect->K[0], rect->K[1], rect->K[2], rect->K[3], levels, 0.f, 0.f, out,
+                                   dM ? packed_plane(dM, rect->w, rect->h) : SrcPlane{nullptr, 0, 0}, roles);
+}
+
 // Uploads n frames of one dvo_b200_input_format (and their reference masks, if any) into the context's device staging
 // area and builds their pyramids from there, packed.  The frames stay in their file representation: the pyramid kernels
 // convert in their loads (no float32 copy of a raw frame is written); BGR is reduced to 8-bit grey first, as cv::cvtColor
-// leaves it.  Masks add one byte per pixel after the frames.
+// leaves it.  Masks add one byte per pixel after the frames.  rect: the rectified planes follow the upload.
 static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image, const void* depth, float depth_scale,
                          const uint8_t* masks, int mask_roles, int width, int height, float fx, float fy, float ox, float oy,
-                         int levels, dvo_b200_pyramid** out) {
+                         int levels, dvo_b200_pyramid** out, const dvo_b200_rectifier* rect = nullptr) {
   cudaSetDevice(ctx->device);
   const size_t npx = (size_t)width * height * n;
   size_t frames = 0, grey_off = 0, bgr_off = 0;   // bytes of the staged frames; offsets of the grey and BGR images
@@ -93,7 +116,8 @@ static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image
     frames = (format == DVO_B200_INPUT_BGR8_DEPTH16 ? bgr_off + npx * 3 : grey_off + npx) + 64;
   }
   const size_t mask_off = (frames + 255) / 256 * 256;
-  int rc = ensure_stage(ctx, masks ? mask_off + npx : frames, 0);
+  const size_t rect_off = ((masks ? mask_off + npx : frames) + 255) / 256 * 256;
+  int rc = ensure_stage(ctx, rect ? rect_off + rectified_bytes(rect, n, masks != nullptr) : masks ? mask_off + npx : frames, 0);
   if (rc) return rc;
   char* stage = (char*)ctx->d_stage;
   SrcPlane dM{nullptr, 0, 0};
@@ -108,8 +132,8 @@ static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image
     DVO_CUDA(ctx, cudaMemcpyAsync(dI, image, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     DVO_CUDA(ctx, cudaMemcpyAsync(dZ, depth, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     ctx->h2d_bytes += 2 * npx * sizeof(float);
-    return pyramid_build_batch_input(ctx, n, packed_plane(dI, width, height), packed_plane(dZ, width, height), 0, 0.f, width, height,
-                                     fx, fy, ox, oy, levels, 0.f, 0.f, out, dM, mask_roles);
+    return build_planes(ctx, rect, rect_off, n, packed_plane(dI, width, height), packed_plane(dZ, width, height), 0, 0.f, dM, mask_roles,
+                        width, height, fx, fy, ox, oy, levels, out);
   }
   uint16_t* dR = (uint16_t*)stage;
   uint8_t* dG = (uint8_t*)(stage + grey_off);
@@ -123,17 +147,17 @@ static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image
     ctx->h2d_bytes += npx * 5;
     convert_bgr(ctx, n, width, height, packed_plane(dC, 3 * width, height), dG);
   }
-  return pyramid_build_batch_input(ctx, n, packed_plane(dG, width, height), packed_plane(dR, width, height), 1, depth_scale, width,
-                                   height, fx, fy, ox, oy, levels, 0.f, 0.f, out, dM, mask_roles);
+  return build_planes(ctx, rect, rect_off, n, packed_plane(dG, width, height), packed_plane(dR, width, height), 1, depth_scale, dM,
+                      mask_roles, width, height, fx, fy, ox, oy, levels, out);
 }
 
 // One dvo_b200_device_plane of n images of width x height pixels, elem bytes per element and per_px elements per pixel ->
 // the SrcPlane the pyramid kernels read.  Every check of the header's list; the pointer checks look at the first and the
 // last byte of the plane's extent.
-static int device_plane(dvo_b200_ctx* ctx, const dvo_b200_device_plane* p, const char* name, int elem, int per_px, int n,
-                        int width, int height, SrcPlane* out) {
+static int device_plane(dvo_b200_ctx* ctx, const char* fn, const dvo_b200_device_plane* p, const char* name, int elem, int per_px,
+                        int n, int width, int height, SrcPlane* out) {
   auto bad = [&](const std::string& why) {
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string("pyramid_create_device: ") + name + ": " + why);
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": " + name + ": " + why);
   };
   if (!p || !p->data) return bad("null plane or data pointer");
   const int64_t row = (int64_t)width * per_px * elem;
@@ -160,6 +184,38 @@ static int device_plane(dvo_b200_ctx* ctx, const dvo_b200_device_plane* p, const
   }
   *out = SrcPlane{p->data, p->row_bytes / elem, p->image_bytes / elem};
   return 0;
+}
+
+
+// dvo_b200_pyramid_create_device_batch, and with a rectifier its rectified form.  fn names the entry point in the errors.
+static int create_device(dvo_b200_ctx* ctx, const char* fn, const dvo_b200_rectifier* rect, int n, int format,
+                         const dvo_b200_device_plane* image, const dvo_b200_device_plane* depth, float depth_scale,
+                         const dvo_b200_device_plane* masks, int roles, int width, int height, float fx, float fy, float ox, float oy,
+                         int levels, dvo_b200_pyramid** out) {
+  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": null/invalid argument");
+  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": unknown input format " + std::to_string(format));
+  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": unsupported role set " + std::to_string(roles));
+  cudaSetDevice(ctx->device);
+  const bool f32 = format == DVO_B200_INPUT_FLOAT32;
+  SrcPlane I, Z, M{nullptr, 0, 0};
+  int rc = device_plane(ctx, fn, image, "image", f32 ? 4 : 1, format == DVO_B200_INPUT_BGR8_DEPTH16 ? 3 : 1, n, width, height, &I);
+  if (!rc) rc = device_plane(ctx, fn, depth, "depth", f32 ? 4 : 2, 1, n, width, height, &Z);
+  if (!rc && masks) rc = device_plane(ctx, fn, masks, "masks", 1, 1, n, width, height, &M);
+  if (rc) return rc;
+  const size_t grey = format == DVO_B200_INPUT_BGR8_DEPTH16 ? (size_t)width * height * n : 0;   // BGR reduced to grey in staging
+  const size_t rect_off = (grey + 255) / 256 * 256;
+  if (grey || rect) {
+    if ((rc = ensure_stage(ctx, rect ? rect_off + rectified_bytes(rect, n, masks != nullptr) : grey, 0))) return rc;
+  }
+  if (grey) {   // grey into staging, as the host path; depth and masks stay in place
+    convert_bgr(ctx, n, width, height, I, (uint8_t*)ctx->d_stage);
+    I = packed_plane(ctx->d_stage, width, height);
+  }
+  return build_planes(ctx, rect, rect_off, n, I, Z, f32 ? 0 : 1, f32 ? 0.f : depth_scale, M, roles, width, height, fx, fy, ox, oy,
+                      levels, out);
 }
 
 }  // namespace dvo_b200
@@ -309,26 +365,100 @@ int dvo_b200_pyramid_create_device_batch(dvo_b200_ctx* ctx, int32_t n, int32_t f
                                          const dvo_b200_device_plane* depth, float depth_scale, const dvo_b200_device_plane* masks,
                                          int32_t roles, int32_t width, int32_t height, float fx, float fy, float ox, float oy,
                                          int32_t levels, dvo_b200_pyramid** out) {
-  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_device: null/invalid argument");
-  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_device: unknown input format " + std::to_string(format));
-  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_device: unsupported role set " + std::to_string(roles));
-  cudaSetDevice(ctx->device);
-  const bool f32 = format == DVO_B200_INPUT_FLOAT32;
-  SrcPlane I, Z, M{nullptr, 0, 0};
-  int rc = device_plane(ctx, image, "image", f32 ? 4 : 1, format == DVO_B200_INPUT_BGR8_DEPTH16 ? 3 : 1, n, width, height, &I);
-  if (!rc) rc = device_plane(ctx, depth, "depth", f32 ? 4 : 2, 1, n, width, height, &Z);
-  if (!rc && masks) rc = device_plane(ctx, masks, "masks", 1, 1, n, width, height, &M);
-  if (rc) return rc;
-  if (format == DVO_B200_INPUT_BGR8_DEPTH16) {   // grey into staging, as the host path; depth and masks stay in place
-    if ((rc = ensure_stage(ctx, (size_t)width * height * n, 0))) return rc;
-    convert_bgr(ctx, n, width, height, I, (uint8_t*)ctx->d_stage);
-    I = packed_plane(ctx->d_stage, width, height);
+  return create_device(ctx, "pyramid_create_device", nullptr, n, format, image, depth, depth_scale, masks, roles, width, height, fx, fy,
+                       ox, oy, levels, out);
+}
+
+int dvo_b200_undistort_map(int32_t width, int32_t height, const double K[4], const double dist[5], const double K_new[4],
+                           float* map_x, float* map_y) {
+  if (width <= 0 || height <= 0 || !K || !dist || !K_new || !map_x || !map_y) return DVO_B200_ERR_INVALID_ARGUMENT;
+  for (int i = 0; i < 5; ++i)
+    if (!std::isfinite(dist[i]) || (i < 4 && (!std::isfinite(K[i]) || !std::isfinite(K_new[i])))) return DVO_B200_ERR_INVALID_ARGUMENT;
+  const double fx = K[0], fy = K[1], cx = K[2], cy = K[3], nfx = K_new[0], nfy = K_new[1], ncx = K_new[2], ncy = K_new[3];
+  const double k1 = dist[0], k2 = dist[1], p1 = dist[2], p2 = dist[3], k3 = dist[4];
+  const double sx = fx / nfx, sy = fy / nfy;
+  for (int v = 0; v < height; ++v) {
+    const double y = (v - ncy) / nfy;
+    for (int u = 0; u < width; ++u) {
+      // the order of the header comment, term by term
+      const double x = (u - ncx) / nfx;
+      const double r2 = x * x + y * y;
+      const double kr = ((k3 * r2 + k2) * r2 + k1) * r2;
+      const double dx = x * kr + ((2 * p1) * x * y + p2 * (r2 + 2 * x * x));
+      const double dy = y * kr + (p1 * (r2 + 2 * y * y) + (2 * p2) * x * y);
+      map_x[(size_t)v * width + u] = (float)((cx + sx * (u - ncx)) + fx * dx);
+      map_y[(size_t)v * width + u] = (float)((cy + sy * (v - ncy)) + fy * dy);
+    }
   }
-  return pyramid_build_batch_input(ctx, n, I, Z, f32 ? 0 : 1, f32 ? 0.f : depth_scale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f,
-                                   out, M, roles);
+  return 0;
+}
+
+int dvo_b200_rectifier_create(dvo_b200_ctx* ctx, int32_t in_width, int32_t in_height, int32_t width, int32_t height,
+                              const float* map_x, const float* map_y, const float K_new[4], dvo_b200_rectifier** out) {
+  if (out) *out = nullptr;
+  if (!ctx || !map_x || !map_y || !K_new || !out || in_width < 2 || in_height < 2 || width <= 0 || height <= 0)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "rectifier_create: null/invalid argument");
+  cudaSetDevice(ctx->device);
+  const size_t npx = (size_t)width * height;
+  float* d = nullptr;
+  DVO_CUDA(ctx, cudaMallocAsync((void**)&d, 2 * npx * sizeof(float), ctx->stream));
+  cudaError_t e = cudaMemcpyAsync(d, map_x, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d + npx, map_y, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);   // the caller's arrays may go when this returns
+  if (e != cudaSuccess) {
+    cudaFreeAsync(d, ctx->stream);
+    return check_cuda(ctx, e, "rectifier_create: map upload");
+  }
+  ctx->h2d_bytes += 2 * npx * sizeof(float);
+  dvo_b200_rectifier* r = new dvo_b200_rectifier;
+  r->ctx = ctx; r->in_w = in_width; r->in_h = in_height; r->w = width; r->h = height; r->map = d;
+  for (int i = 0; i < 4; ++i) r->K[i] = K_new[i];
+  *out = r;
+  return 0;
+}
+
+int dvo_b200_rectifier_release(dvo_b200_rectifier* r) {
+  if (!r) return DVO_B200_ERR_INVALID_ARGUMENT;
+  DeviceScope dev(r->ctx->device);
+  // every create that read the map was enqueued on this stream before this call: the free follows them in stream order
+  const cudaError_t e = cudaFreeAsync(r->map, r->ctx->stream);
+  const int rc = check_cuda(r->ctx, e, "rectifier_release");
+  delete r;
+  return rc;
+}
+
+// The rectifier's checks shared by both rectified creates: it exists, belongs to ctx and takes frames of width x height.
+static int check_rectifier(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, int width, int height, const char* fn) {
+  if (!rect) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": null rectifier");
+  if (rect->ctx != ctx) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": the rectifier belongs to another context");
+  if (width != rect->in_w || height != rect->in_h)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": frames of " + std::to_string(width) + "x" +
+                                                             std::to_string(height) + ", the rectifier takes " + std::to_string(rect->in_w) +
+                                                             "x" + std::to_string(rect->in_h));
+  return 0;
+}
+
+int dvo_b200_pyramid_create_rectified_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, int32_t n, int32_t format,
+                                            const void* image, const void* depth, float depth_scale, const uint8_t* masks,
+                                            int32_t roles, int32_t width, int32_t height, int32_t levels, dvo_b200_pyramid** out) {
+  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_rectified: null/invalid argument");
+  if (int rc = check_rectifier(ctx, rect, width, height, "pyramid_create_rectified")) return rc;
+  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_rectified: unknown input format " + std::to_string(format));
+  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_rectified: unsupported role set " + std::to_string(roles));
+  return create_staged(ctx, n, format, image, depth, depth_scale, masks, roles, width, height, 0.f, 0.f, 0.f, 0.f, levels, out, rect);
+}
+
+int dvo_b200_pyramid_create_rectified_device_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, int32_t n, int32_t format,
+                                                   const dvo_b200_device_plane* image, const dvo_b200_device_plane* depth,
+                                                   float depth_scale, const dvo_b200_device_plane* masks, int32_t roles, int32_t width,
+                                                   int32_t height, int32_t levels, dvo_b200_pyramid** out) {
+  if (!ctx) return DVO_B200_ERR_INVALID_ARGUMENT;
+  if (int rc = check_rectifier(ctx, rect, width, height, "pyramid_create_rectified_device")) return rc;
+  return create_device(ctx, "pyramid_create_rectified_device", rect, n, format, image, depth, depth_scale, masks, roles, width, height,
+                       0.f, 0.f, 0.f, 0.f, levels, out);
 }
 
 int dvo_b200_pyramid_mask_roles(const dvo_b200_pyramid* p) { return p ? p->mask_roles : DVO_B200_ERR_INVALID_ARGUMENT; }

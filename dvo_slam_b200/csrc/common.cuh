@@ -259,6 +259,23 @@ struct SrcPlane {
 };
 inline SrcPlane packed_plane(const void* data, int row_elems, int h) { return {data, row_elems, (int64_t)row_elems * h}; }
 
+}  // namespace dvo_b200
+
+struct dvo_b200_rectifier {      // a remap to a pinhole camera (dvo_b200_rectifier_create)
+  dvo_b200_ctx* ctx = nullptr;   // the owning context: its stream orders every use and the free
+  int in_w = 0, in_h = 0;        // input frames
+  int w = 0, h = 0;              // rectified frames = level 0
+  float K[4] = {0, 0, 0, 0};     // K_new: fx, fy, cx, cy of level 0
+  float* map = nullptr;          // device, stream-ordered allocation: map_x[w*h] then map_y[w*h]
+};
+
+namespace dvo_b200 {
+
+// pyramid.cu: the rectifying remap of n frames into packed float32 planes dI / dZ (w*h floats per image) and, if M.data,
+// packed byte masks dM (1 = usable).  raw as in pyramid_build_batch_input: 8-bit grey + 16-bit depth, else float32.
+void rectify_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* r, int n, SrcPlane I, SrcPlane Z, int raw, float zscale, SrcPlane M,
+                   float* dI, float* dZ, uint8_t* dM);
+
 // pyramid.cu
 int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float* d_Z, int w, int h, float fx, float fy,
                         float ox, float oy, int levels, float ti, float td, dvo_b200_pyramid** out);

@@ -342,6 +342,43 @@ __global__ void k_template(float* __restrict__ tmpl, size_t tmpl_per_image, size
   else if (i < w + h) t[i] = __fdiv_rn((float)(i - w) - oy, fy);
 }
 
+// The rectifying remap (dvo_b200_pyramid_create_rectified_batch): one thread per output pixel of one image.  Bilinear
+// intensity in a fixed order with every operation rounded to nearest (no contraction), the nearest tap's depth, NaN / NaN
+// where the map points outside [0, in_w-1] x [0, in_h-1].  kMasked: the pixel is usable iff it is valid and its four taps
+// are.  The outputs are packed planes of w*h elements per image, the layout of a staged FLOAT32 upload.
+template <bool kRaw, bool kMasked>
+__global__ void __launch_bounds__(256)
+k_rectify(SrcPlane I, SrcPlane Z, float zscale, SrcPlane M, const float* __restrict__ map_x, const float* __restrict__ map_y,
+          int in_w, int in_h, int n, float* __restrict__ dI, float* __restrict__ dZ, uint8_t* __restrict__ dM) {
+  const int img = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float sx = __ldg(map_x + i), sy = __ldg(map_y + i);
+  const float nanv = __int_as_float(0x7fc00000);
+  float v = nanv, z = nanv;
+  bool usable = false;
+  if (sx >= 0.f && sx <= (float)(in_w - 1) && sy >= 0.f && sy <= (float)(in_h - 1)) {
+    const int x0 = min((int)floorf(sx), in_w - 2), y0 = min((int)floorf(sy), in_h - 2);
+    const float ax = __fsub_rn(sx, (float)x0), ay = __fsub_rn(sy, (float)y0);
+    const float bx = __fsub_rn(1.f, ax), by = __fsub_rn(1.f, ay);
+    const size_t o = I.at(img, y0, x0);
+    const float i00 = load_intensity<kRaw>(I.data, o), i10 = load_intensity<kRaw>(I.data, o + 1);
+    const float i01 = load_intensity<kRaw>(I.data, o + I.pitch), i11 = load_intensity<kRaw>(I.data, o + I.pitch + 1);
+    const float top = __fadd_rn(__fmul_rn(bx, i00), __fmul_rn(ax, i10));
+    const float bot = __fadd_rn(__fmul_rn(bx, i01), __fmul_rn(ax, i11));
+    v = __fadd_rn(__fmul_rn(by, top), __fmul_rn(ay, bot));
+    z = load_depth<kRaw>(Z.data, Z.at(img, y0 + (ay >= 0.5f), x0 + (ax >= 0.5f)), zscale);
+    if (kMasked) {
+      const uint8_t* m = reinterpret_cast<const uint8_t*>(M.data) + M.at(img, y0, x0);
+      usable = __ldg(m) && __ldg(m + 1) && __ldg(m + M.pitch) && __ldg(m + M.pitch + 1);
+    }
+  }
+  const size_t out = (size_t)img * n + i;
+  dI[out] = v;
+  dZ[out] = z;
+  if (kMasked) dM[out] = usable ? 1 : 0;
+}
+
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 template <bool kLevel0, bool kRaw, typename... Args>
@@ -442,6 +479,22 @@ void pool_close(dvo_b200_ctx* ctx) {
   for (auto& kv : ctx->pool->free) destroy_slab(kv.second);
   ctx->pool->free.clear();
   ctx->pool->closed = true;
+}
+
+void rectify_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* r, int n, SrcPlane I, SrcPlane Z, int raw, float zscale, SrcPlane M,
+                   float* dI, float* dZ, uint8_t* dM) {
+  ProfScope prof(ctx, 3, 1);
+  const int npx = r->w * r->h;
+  const dim3 g((npx + 255) / 256, n);
+  const float* mx = r->map;
+  const float* my = r->map + npx;
+  cudaStream_t st = ctx->stream;
+  const bool masked = M.data != nullptr;
+  if (raw && masked) k_rectify<true, true><<<g, 256, 0, st>>>(I, Z, zscale, M, mx, my, r->in_w, r->in_h, npx, dI, dZ, dM);
+  else if (raw) k_rectify<true, false><<<g, 256, 0, st>>>(I, Z, zscale, M, mx, my, r->in_w, r->in_h, npx, dI, dZ, dM);
+  else if (masked) k_rectify<false, true><<<g, 256, 0, st>>>(I, Z, zscale, M, mx, my, r->in_w, r->in_h, npx, dI, dZ, dM);
+  else k_rectify<false, false><<<g, 256, 0, st>>>(I, Z, zscale, M, mx, my, r->in_w, r->in_h, npx, dI, dZ, dM);
+  ctx->launches += 1;
 }
 
 int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float* d_Z, int w, int h, float fx, float fy,

@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import weakref
 
 import numpy as np
 
@@ -31,6 +32,8 @@ ABI_SYMBOLS = [
     "dvo_b200_sharded_pyramid_create_batch", "dvo_b200_sharded_pyramid_create_raw_batch", "dvo_b200_match_batch_sharded",
     "dvo_b200_set_estimator", "dvo_b200_get_estimator", "dvo_b200_pyramid_create_masked_batch",
     "dvo_b200_pyramid_create_masked_batch_roles", "dvo_b200_pyramid_mask_roles", "dvo_b200_pyramid_create_device_batch",
+    "dvo_b200_undistort_map", "dvo_b200_rectifier_create", "dvo_b200_rectifier_release", "dvo_b200_pyramid_create_rectified_batch",
+    "dvo_b200_pyramid_create_rectified_device_batch",
 ]
 
 # dvo_b200_estimator
@@ -195,6 +198,12 @@ def load_library():
                                                        C.POINTER(DevicePlane), i32, i32, i32, C.c_float, C.c_float, C.c_float,
                                                        C.c_float, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_mask_roles.argtypes = [vp]
+    L.dvo_b200_undistort_map.argtypes = [i32, i32, dp, dp, dp, fp, fp]
+    L.dvo_b200_rectifier_create.argtypes = [vp, i32, i32, i32, i32, fp, fp, fp, C.POINTER(vp)]
+    L.dvo_b200_rectifier_release.argtypes = [vp]
+    L.dvo_b200_pyramid_create_rectified_batch.argtypes = [vp, vp, i32, i32, vp, vp, C.c_float, vp, i32, i32, i32, i32, C.POINTER(vp)]
+    L.dvo_b200_pyramid_create_rectified_device_batch.argtypes = [vp, vp, i32, i32, C.POINTER(DevicePlane), C.POINTER(DevicePlane),
+                                                                 C.c_float, C.POINTER(DevicePlane), i32, i32, i32, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_device.argtypes = [vp]
     L.dvo_b200_sharded_create.argtypes = [i32, C.POINTER(i32), C.POINTER(vp)]
     L.dvo_b200_sharded_destroy.argtypes = [vp]
@@ -280,6 +289,42 @@ class Pyramid:
             pass
 
 
+def undistort_map(width: int, height: int, K, dist, K_new=None):
+    """dvo_b200_undistort_map: (map_x, map_y), float32 [height, width] each, of OpenCV's plumb-bob model with R = I
+    (cv2.initUndistortRectifyMap(K, dist, None, K_new, (width, height), cv2.CV_32FC1)).  K, K_new: (fx, fy, cx, cy), K_new
+    defaults to K; dist: (k1, k2, p1, p2, k3).  Host only: no context and no GPU."""
+    K = np.ascontiguousarray(K, dtype=np.float64).reshape(4)
+    Kn = np.ascontiguousarray(K if K_new is None else K_new, dtype=np.float64).reshape(4)
+    d = np.ascontiguousarray(dist, dtype=np.float64).reshape(5)
+    mx, my = np.empty((height, width), np.float32), np.empty((height, width), np.float32)
+    dp, fp = C.POINTER(C.c_double), C.POINTER(C.c_float)
+    rc = load_library().dvo_b200_undistort_map(width, height, K.ctypes.data_as(dp), d.ctypes.data_as(dp), Kn.ctypes.data_as(dp),
+                                               mx.ctypes.data_as(fp), my.ctypes.data_as(fp))
+    if rc != 0:
+        raise ValueError(f"dvo_b200_undistort_map: status {rc} (sizes {width}x{height}, K {K}, dist {d}, K_new {Kn})")
+    return mx, my
+
+
+class Rectifier:
+    """Owning handle of a dvo_b200_rectifier: a remap of in_size = (w, h) frames to a pinhole camera K_new of size
+    (w, h) = size.  Released with release(), when collected, or when its engine closes."""
+
+    def __init__(self, engine: "Engine", handle: int, in_size, size, K_new):
+        self.engine, self.handle = engine, handle
+        self.in_size, self.size, self.K_new = tuple(in_size), tuple(size), tuple(K_new)
+
+    def release(self):
+        if self.handle:
+            load_library().dvo_b200_rectifier_release(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+
 class Engine:
     """One dvo_b200_ctx (one CUDA stream on one device).  estimator: "reference" (dvo::DenseTracker::match()'s numbers) or
     "corrected" (the same algorithm without the reference's scale-pairing, log-likelihood-tail and odd-point quirks; see
@@ -296,6 +341,7 @@ class Engine:
                                "(the engine has no CPU fallback)")
         self.ctx = ctx
         self.device = device
+        self._rectifiers = weakref.WeakSet()
         self.set_estimator(estimator)
 
     def set_estimator(self, estimator: str):
@@ -311,6 +357,8 @@ class Engine:
 
     def close(self):
         if getattr(self, "ctx", None):
+            for r in list(getattr(self, "_rectifiers", ())):   # a rectifier is freed on its context's stream
+                r.release()
             self.lib.dvo_b200_destroy(self.ctx)
             self.ctx = None
 
@@ -458,6 +506,96 @@ class Engine:
         rc = self.lib.dvo_b200_pyramid_create_device_batch(self.ctx, n, INPUT_FORMATS[fmt], C.byref(I), C.byref(Z),
                                                            float(depth_scale or 0.0), C.byref(M) if M is not None else None,
                                                            MASK_ROLES[mask_roles], w, h, fx, fy, ox, oy, levels, out)
+        current.wait_stream(ext)
+        self._check(rc)
+        return [Pyramid(self, out[i]) for i in range(n)]
+
+    # ---- distorted cameras ----
+    undistort_map = staticmethod(undistort_map)
+
+    def rectifier(self, in_size, map_x, map_y, K_new) -> Rectifier:
+        """dvo_b200_rectifier_create: frames of in_size = (w, h) remapped through map_x / map_y (float32 [h', w'] input pixel
+        coordinates, e.g. from undistort_map or cv2.initUndistortRectifyMap(..., cv2.CV_32FC1)) to a pinhole camera K_new =
+        (fx, fy, cx, cy) of size (w', h').  The map is uploaded once."""
+        mx = np.ascontiguousarray(map_x, dtype=np.float32)
+        my = np.ascontiguousarray(map_y, dtype=np.float32)
+        if mx.ndim != 2 or mx.shape != my.shape:
+            raise ValueError(f"map_x {mx.shape} and map_y {my.shape}: want two [h, w] arrays")
+        h, w = mx.shape
+        K = (C.c_float * 4)(*[float(v) for v in K_new])
+        out = C.c_void_p()
+        fp = C.POINTER(C.c_float)
+        self._check(self.lib.dvo_b200_rectifier_create(self.ctx, int(in_size[0]), int(in_size[1]), w, h, mx.ctypes.data_as(fp),
+                                                       my.ctypes.data_as(fp), K, C.byref(out)))
+        r = Rectifier(self, out.value, in_size, (w, h), tuple(K))
+        self._rectifiers.add(r)
+        return r
+
+    def pyramid_rectified_batch(self, rect: Rectifier, image, depth, levels: int, depth_scale=None, masks=None,
+                                mask_roles="reference") -> list[Pyramid]:
+        """Pyramids of frames remapped through rect (dvo_b200_pyramid_create_rectified_batch): level 0 has rect's size and
+        intrinsics.  Host arrays: float32 [n,h,w] image + float32 depth in metres, uint8 [n,h,w] grey + uint16 raw depth, or
+        uint8 [n,h,w,3] BGR + uint16 raw depth, the format from the dtypes; synchronises before returning.  torch CUDA
+        tensors: through device_planes and dvo_b200_pyramid_create_rectified_device_batch, ordered with torch's current
+        stream as in pyramid_batch_device, without a host synchronisation.  depth_scale (metres per raw unit) is required
+        with uint16 depth.  masks ([n,h,w] or [h,w], nonzero = usable, in the input geometry) / mask_roles as in
+        pyramid_batch."""
+        if mask_roles not in MASK_ROLES:
+            raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
+        if not isinstance(image, np.ndarray) and hasattr(image, "is_cuda") and image.is_cuda:
+            return self._rectified_device(rect, image, depth, levels, depth_scale, masks, mask_roles)
+        image, depth = np.asarray(image), np.asarray(depth)
+        if image.dtype == np.float32 and image.ndim == 3 and depth.dtype == np.float32:
+            fmt = "float32"
+        elif image.dtype == np.uint8 and image.ndim == 3 and depth.dtype == np.uint16:
+            fmt = "grey8_depth16"
+        elif image.dtype == np.uint8 and image.ndim == 4 and image.shape[3] == 3 and depth.dtype == np.uint16:
+            fmt = "bgr8_depth16"
+        else:
+            raise ValueError(f"image {image.dtype} {image.shape} with depth {depth.dtype}: want float32 [n,h,w] + float32, uint8 "
+                             "[n,h,w] + uint16 or uint8 [n,h,w,3] + uint16")
+        n, h, w = image.shape[:3]
+        if depth.shape != (n, h, w):
+            raise ValueError(f"depth {depth.shape}, want {(n, h, w)}")
+        if fmt != "float32" and depth_scale is None:
+            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
+        I, Z = np.ascontiguousarray(image), np.ascontiguousarray(depth)
+        M = None
+        if masks is not None:
+            M = np.asarray(masks)
+            M = np.broadcast_to(M, (n, h, w)) if M.shape == (h, w) else M
+            if M.shape != (n, h, w):
+                raise ValueError(f"masks {M.shape}, want {(n, h, w)} or {(h, w)}")
+            M = np.ascontiguousarray(M if M.dtype == np.uint8 else M != 0, dtype=np.uint8)
+        out = (C.c_void_p * n)()
+        self._check(self.lib.dvo_b200_pyramid_create_rectified_batch(self.ctx, rect.handle, n, INPUT_FORMATS[fmt], I.ctypes.data,
+                                                                     Z.ctypes.data, float(depth_scale or 0.0),
+                                                                     M.ctypes.data if M is not None else None, MASK_ROLES[mask_roles],
+                                                                     w, h, levels, out))
+        self.synchronize()   # the staged host arrays may die with this call
+        return [Pyramid(self, out[i]) for i in range(n)]
+
+    def _rectified_device(self, rect, image, depth, levels, depth_scale, masks, mask_roles):
+        import torch
+        fmt, (n, h, w), pI, pZ, pM = device_planes(image, depth, masks)
+        if fmt != "float32" and depth_scale is None:
+            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
+        dev = torch.device("cuda", self.device)
+        inputs = [t for t in (image, depth, masks) if t is not None]
+        for t in inputs:
+            if t.device != dev:
+                raise ValueError(f"a tensor on {t.device}: the engine runs on {dev}")
+        I, Z = DevicePlane(*pI), DevicePlane(*pZ)
+        M = DevicePlane(*pM) if pM is not None else None
+        out = (C.c_void_p * n)()
+        current = torch.cuda.current_stream(dev)
+        ext = torch.cuda.ExternalStream(self.stream, device=dev)
+        ext.wait_stream(current)
+        for t in inputs:
+            t.record_stream(ext)     # the caching allocator keeps the memory until the build has read it
+        rc = self.lib.dvo_b200_pyramid_create_rectified_device_batch(self.ctx, rect.handle, n, INPUT_FORMATS[fmt], C.byref(I), C.byref(Z),
+                                                                     float(depth_scale or 0.0), C.byref(M) if M is not None else None,
+                                                                     MASK_ROLES[mask_roles], w, h, levels, out)
         current.wait_stream(ext)
         self._check(rc)
         return [Pyramid(self, out[i]) for i in range(n)]

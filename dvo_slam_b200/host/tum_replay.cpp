@@ -184,7 +184,18 @@ void quaternion_of(const dvo::core::AffineTransformd& T, double q[4]) {
 
 std::string dir_of(const std::string& path) { size_t s = path.find_last_of('/'); return s == std::string::npos ? std::string() : path.substr(0, s + 1); }
 
-struct Frame { double stamp; dvo::core::RgbdImagePyramidPtr pyramid; };
+struct Frame { double stamp; dvo::core::RgbdImagePyramidPtr pyramid; dvo_b200_pyramid* rectified; };
+
+// --distortion: the frames go through a rectifier (dvo_b200_rectifier) on a context of this program's own, and the pairs
+// are aligned through the C ABI with the tracker's configuration, as DenseTracker::matchBatch aligns them.
+struct Rectified {
+  dvo_b200_ctx* ctx = nullptr;
+  dvo_b200_rectifier* rect = nullptr;
+  ~Rectified() {
+    if (rect) dvo_b200_rectifier_release(rect);
+    if (ctx) dvo_b200_destroy(ctx);
+  }
+};
 
 }  // namespace
 
@@ -193,6 +204,8 @@ int main(int argc, char** argv) {
   float K[4] = {517.3f, 516.5f, 318.6f, 255.3f};     // TUM freiburg1 (benchmark_slam.cpp:384)
   int first = 3, last = 1, batch = 32, max_frames = -1;
   bool parse_only = false;
+  bool distorted = false;
+  double dist[5] = {0, 0, 0, 0, 0};   // k1 k2 p1 p2 k3 (plumb bob)
   for (int i = 1; i < argc; ++i) {
     const std::string a = argv[i];
     if (a == "--assoc" && i + 1 < argc) assoc = argv[++i];
@@ -204,8 +217,17 @@ int main(int argc, char** argv) {
     else if (a == "--batch" && i + 1 < argc) batch = std::max(1, std::atoi(argv[++i]));
     else if (a == "--max-frames" && i + 1 < argc) max_frames = std::atoi(argv[++i]);
     else if (a == "--parse-only") parse_only = true;
+    else if (a == "--distortion" && i + 5 < argc) {
+      distorted = true;
+      for (int k = 0; k < 5; ++k) {
+        char* end = nullptr;
+        dist[k] = std::strtod(argv[++i], &end);
+        if (end == argv[i] || *end) { std::fprintf(stderr, "tum_replay: --distortion takes five numbers k1 k2 p1 p2 k3\n"); return 2; }
+      }
+    }
     else { std::fprintf(stderr, "usage: tum_replay --assoc assoc.txt [--groundtruth gt.txt] [--out traj.txt] [--intrinsics fx fy ox oy]\n"
-                                "                  [--first L] [--last L] [--batch N] [--max-frames N] [--parse-only]\n"); return 2; }
+                                "                  [--distortion k1 k2 p1 p2 k3] [--first L] [--last L] [--batch N] [--max-frames N]\n"
+                                "                  [--parse-only]\n"); return 2; }
   }
   if (assoc.empty()) { std::fprintf(stderr, "tum_replay: --assoc is required\n"); return 2; }
   std::vector<RgbdPair> pairs;
@@ -236,9 +258,11 @@ int main(int argc, char** argv) {
     double q[4];
     quaternion_of(trajectory, q);
     std::printf("{\"pairs\": %zu, \"groundtruth\": %zu, \"gt_first\": %zu, \"first_stamp\": \"%s\", \"rgb\": [%d, %d, %d, %d], \"depth\": [%d, %d, %d, %d], "
-                "\"grey_sum\": %.17g, \"depth_sum\": %.17g, \"depth_nan\": %lld, \"pose0\": [%.17g, %.17g, %.17g, %.17g, %.17g, %.17g, %.17g]}\n",
+                "\"grey_sum\": %.17g, \"depth_sum\": %.17g, \"depth_nan\": %lld, \"pose0\": [%.17g, %.17g, %.17g, %.17g, %.17g, %.17g, %.17g]%s}\n",
                 pairs.size(), gt.size(), gt_first, stamp_text(pairs[0].rgb_stamp).c_str(), rgb.w, rgb.h, rgb.channels, rgb.bits, depth.w, depth.h,
-                depth.channels, depth.bits, gsum, zsum, znan, trajectory.matrix()(0, 3), trajectory.matrix()(1, 3), trajectory.matrix()(2, 3), q[0], q[1], q[2], q[3]);
+                depth.channels, depth.bits, gsum, zsum, znan, trajectory.matrix()(0, 3), trajectory.matrix()(1, 3), trajectory.matrix()(2, 3), q[0], q[1], q[2], q[3],
+                distorted ? (", \"distortion\": [" + std::to_string(dist[0]) + ", " + std::to_string(dist[1]) + ", " + std::to_string(dist[2]) + ", " +
+                             std::to_string(dist[3]) + ", " + std::to_string(dist[4]) + "]").c_str() : "");
     return 0;
   }
 
@@ -257,6 +281,24 @@ int main(int argc, char** argv) {
     if (!load_png(folder + pairs[0].rgb_file, first_rgb, why)) { std::fprintf(stderr, "tum_replay: %s\n", why.c_str()); return 2; }
     dvo::core::RgbdCameraPyramid camera(size_t(first_rgb.w), size_t(first_rgb.h), dvo::core::IntrinsicMatrix::create(K[0], K[1], K[2], K[3]));
     dvo::DenseTracker tracker(cfg);
+    Rectified rectified;
+    dvo_b200_config ccfg;
+    if (distorted) {   // one rectifier for the sequence: K_new = --intrinsics, the frames' size
+      const int w = first_rgb.w, h = first_rgb.h;
+      const double Kd[4] = {K[0], K[1], K[2], K[3]};
+      std::vector<float> mx(size_t(w) * h), my(size_t(w) * h);
+      const char* dev = std::getenv("DVO_B200_DEVICE");
+      if (dvo_b200_undistort_map(w, h, Kd, dist, Kd, mx.data(), my.data()) != 0 ||
+          dvo_b200_create(dev ? std::atoi(dev) : 0, 0, &rectified.ctx) != 0 ||
+          dvo_b200_rectifier_create(rectified.ctx, w, h, w, h, mx.data(), my.data(), K, &rectified.rect) != 0) {
+        std::fprintf(stderr, "tum_replay: cannot set up the rectifier: %s\n", rectified.ctx ? dvo_b200_last_error(rectified.ctx) : "no CUDA device");
+        return 3;
+      }
+      dvo_b200_config_default(&ccfg);   // the fields DenseTracker::matchBatch passes
+      ccfg.first_level = cfg.FirstLevel; ccfg.last_level = cfg.LastLevel; ccfg.max_iterations_per_level = cfg.MaxIterationsPerLevel;
+      ccfg.use_initial_estimate = 0; ccfg.precision = cfg.Precision; ccfg.mu = cfg.Mu;
+      ccfg.intensity_derivative_threshold = cfg.IntensityDerivativeThreshold; ccfg.depth_derivative_threshold = cfg.DepthDerivativeThreshold;
+    }
     for (size_t next = 0; next < pairs.size();) {
       // load up to `batch` new frames behind the current reference
       while (next < pairs.size() && frames.size() < size_t(batch) + 1) {
@@ -268,16 +310,45 @@ int main(int argc, char** argv) {
           ++next;
           continue;
         }
-        Frame f = {pairs[next].rgb_stamp, camera.create(grey, z)};
+        Frame f = {pairs[next].rgb_stamp, dvo::core::RgbdImagePyramidPtr(), nullptr};
+        if (distorted) {
+          if (grey.cols != first_rgb.w || grey.rows != first_rgb.h) { std::fprintf(stderr, "tum_replay: frame %zu: size differs from the first frame\n", next); return 2; }
+          if (dvo_b200_pyramid_create_rectified_batch(rectified.ctx, rectified.rect, 1, DVO_B200_INPUT_FLOAT32, grey.ptr<float>(), z.ptr<float>(), 0.f,
+                                                      nullptr, DVO_B200_MASK_ROLE_REFERENCE, grey.cols, grey.rows, int(cfg.getNumLevels()),
+                                                      &f.rectified) != 0 ||
+              dvo_b200_synchronize(rectified.ctx) != 0) {   // the frame's host images go out of scope
+            std::fprintf(stderr, "tum_replay: %s\n", dvo_b200_last_error(rectified.ctx));
+            return 3;
+          }
+        } else {
+          f.pyramid = camera.create(grey, z);
+        }
         frames.push_back(f);
         ++next;
       }
       if (frames.size() < 2) break;
-      std::vector<dvo::core::RgbdImagePyramid*> references, currents;
-      for (size_t i = 1; i < frames.size(); ++i) { references.push_back(frames[i - 1].pyramid.get()); currents.push_back(frames[i].pyramid.get()); }
-      std::vector<dvo::DenseTracker::Result> results(references.size());
+      std::vector<dvo::DenseTracker::Result> results(frames.size() - 1);
       const auto t0 = std::chrono::steady_clock::now();
-      tracker.matchBatch(references, currents, results);
+      if (distorted) {
+        std::vector<dvo_b200_pyramid*> references, currents;
+        for (size_t i = 1; i < frames.size(); ++i) { references.push_back(frames[i - 1].rectified); currents.push_back(frames[i].rectified); }
+        std::vector<dvo_b200_result> raw(references.size());
+        if (dvo_b200_match_batch(rectified.ctx, &ccfg, int(raw.size()), references.data(), currents.data(), nullptr, raw.data(), nullptr, 0) != 0) {
+          std::fprintf(stderr, "tum_replay: dvo_b200_match_batch: %s\n", dvo_b200_last_error(rectified.ctx));
+          return 3;
+        }
+        for (size_t i = 0; i < raw.size(); ++i) {   // what Result::isNaN and the trajectory read, as fill_result copies them
+          for (int a = 0; a < 4; ++a)
+            for (int b = 0; b < 4; ++b) results[i].Transformation.matrix()(a, b) = raw[i].transformation[a * 4 + b];
+          for (int a = 0; a < 6; ++a)
+            for (int b = 0; b < 6; ++b) results[i].Information(a, b) = raw[i].information[a * 6 + b];
+        }
+        for (size_t i = 0; i + 1 < frames.size(); ++i) dvo_b200_pyramid_release(frames[i].rectified);   // the last one is the next reference
+      } else {
+        std::vector<dvo::core::RgbdImagePyramid*> references, currents;
+        for (size_t i = 1; i < frames.size(); ++i) { references.push_back(frames[i - 1].pyramid.get()); currents.push_back(frames[i].pyramid.get()); }
+        tracker.matchBatch(references, currents, results);
+      }
       match_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
       for (size_t i = 0; i < results.size(); ++i) {
         if (results[i].isNaN()) { ++failed; results[i].setIdentity(); }
@@ -292,6 +363,7 @@ int main(int argc, char** argv) {
       frames.clear();
       frames.push_back(keep);
     }
+    if (distorted && !frames.empty()) dvo_b200_pyramid_release(frames.back().rectified);
   } catch (const std::exception& e) {
     std::fprintf(stderr, "%s\n", e.what());
     return 3;

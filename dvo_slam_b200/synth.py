@@ -65,6 +65,7 @@ class SceneConfig:
     depth_quantum: float = 1.0 / 5000.0
     intensity_noise_sigma: float = 0.0
     quantize_intensity: bool = True
+    distortion: tuple | None = None  # (k1, k2, p1, p2, k3) plumb-bob lens; None: a pinhole camera
 
     def scaled(self, factor: int) -> "SceneConfig":
         """Same camera at ``factor`` x the resolution (config 5: 1280x960 = 2 x fr1)."""
@@ -72,7 +73,31 @@ class SceneConfig:
         return SceneConfig(self.width * factor, self.height * factor,
                            (fx * factor, fy * factor, ox * factor, oy * factor), self.n_sinusoids,
                            self.max_translation, self.max_rotation, self.hole_fraction, self.max_depth,
-                           self.depth_quantum, self.intensity_noise_sigma, self.quantize_intensity)
+                           self.depth_quantum, self.intensity_noise_sigma, self.quantize_intensity, self.distortion)
+
+
+FR1_DISTORTION = (0.2624, -0.9531, -0.0054, 0.0026, 1.1633)   # TUM fr1 plumb-bob k1, k2, p1, p2, k3
+
+
+def undistort_points(xd, yd, dist, tol: float = 1e-12, max_iter: int = 100):
+    """Normalised pinhole coordinates (x, y) whose plumb-bob distortion (OpenCV's model, dist = (k1, k2, p1, p2, k3)) is
+    (xd, yd): Newton's method in float64 from (xd, yd) until the residual is below tol."""
+    k1, k2, p1, p2, k3 = (float(v) for v in dist)
+    x, y = xd.clone(), yd.clone()
+    for _ in range(max_iter):
+        r2 = x * x + y * y
+        R = 1 + ((k3 * r2 + k2) * r2 + k1) * r2
+        dR = k1 + (2 * k2 + 3 * k3 * r2) * r2           # dR / dr2
+        fx = x * R + 2 * p1 * x * y + p2 * (r2 + 2 * x * x) - xd
+        fy = y * R + p1 * (r2 + 2 * y * y) + 2 * p2 * x * y - yd
+        if max(float(fx.abs().max()), float(fy.abs().max())) < tol:
+            return x, y
+        a = R + 2 * x * x * dR + 2 * p1 * y + 6 * p2 * x  # Jacobian [[a, b], [c, d]]
+        b = 2 * x * y * dR + 2 * p1 * x + 2 * p2 * y
+        d = R + 2 * y * y * dR + 6 * p1 * y + 2 * p2 * x
+        det = a * d - b * b
+        x, y = x - (d * fx - b * fy) / det, y - (a * fy - b * fx) / det
+    raise RuntimeError(f"undistort_points: no convergence to {tol} in {max_iter} iterations")
 
 
 def _render(cfg: SceneConfig, T_cam: np.ndarray, tex, box, rng: np.random.Generator, device):
@@ -84,7 +109,10 @@ def _render(cfg: SceneConfig, T_cam: np.ndarray, tex, box, rng: np.random.Genera
     R, t = T[:3, :3], T[:3, 3]
     xs = (torch.arange(w, dtype=f64, device=device) - ox) / fx
     ys = (torch.arange(h, dtype=f64, device=device) - oy) / fy
-    dc = torch.stack([xs[None, :].expand(h, w), ys[:, None].expand(h, w), torch.ones(h, w, dtype=f64, device=device)], -1)
+    xs, ys = xs[None, :].expand(h, w), ys[:, None].expand(h, w)
+    if cfg.distortion is not None:   # pixel (u, v) of the lens sees the ray of the pinhole point it distorts from
+        xs, ys = undistort_points(xs.contiguous(), ys.contiguous(), cfg.distortion)
+    dc = torch.stack([xs, ys, torch.ones(h, w, dtype=f64, device=device)], -1)   # d_cam.z = 1: depth stays the z-distance
     d = dc @ R            # rows: R^T d_cam  (direction in the reference frame)
     o = -(R.T @ t)        # camera centre in the reference frame
     # back plane: z - 0.3x - 0.2y = 2.5

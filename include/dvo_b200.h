@@ -246,6 +246,71 @@ int dvo_b200_pyramid_create_device_batch(dvo_b200_ctx* ctx, int32_t n, int32_t f
                                          const dvo_b200_device_plane* masks /* NULL: no mask */, int32_t roles, int32_t width,
                                          int32_t height, float fx, float fy, float ox, float oy, int32_t levels,
                                          dvo_b200_pyramid** out /* n handles */);
+/* ---- distorted cameras: undistortion through a remap in the pyramid build -------------------------------------------
+ * The tracker projects with a pinhole K.  Frames of a real lens are first remapped to a pinhole camera K_new: output pixel
+ * (x, y) of a rectified frame reads the input frame at (sx, sy) = (map_x[y*w + x], map_y[y*w + x]).
+ *
+ * dvo_b200_undistort_map: the map of OpenCV's plumb-bob model with R = I, as cv::initUndistortRectifyMap(K, dist, I, K_new,
+ * (width, height), CV_32FC1) computes it.  Host only: no context, no GPU.  K and K_new are fx, fy, cx, cy; dist is k1, k2,
+ * p1, p2, k3.  For each output pixel (u, v), in double precision and in this order (a*b+c means (a*b)+c, no fused
+ * multiply-add):
+ *   x  = (u - cx') / fx'                       y  = (v - cy') / fy'            (K_new = fx', fy', cx', cy')
+ *   r2 = x*x + y*y
+ *   kr = ((k3*r2 + k2)*r2 + k1)*r2                                             (the radial factor minus 1)
+ *   dx = x*kr + ((2*p1)*x*y + p2*(r2 + 2*x*x))  dy = y*kr + (p1*(r2 + 2*y*y) + (2*p2)*x*y)
+ *   map_x = (cx + (fx/fx')*(u - cx')) + fx*dx  map_y = (cy + (fy/fy')*(v - cy')) + fy*dy
+ * then each map value is rounded once to float.  This is fx*(x*(1 + kr) + tangential) + cx, the plumb-bob model, written
+ * so that zero coefficients with K_new = K give exact integer coordinates (dx = 0 and cx + (u - cx) = u).  width*height
+ * floats per map.  A NULL pointer, a non-positive size or a non-finite K, K_new or dist -> DVO_B200_ERR_INVALID_ARGUMENT. */
+int dvo_b200_undistort_map(int32_t width, int32_t height, const double K[4], const double dist[5], const double K_new[4],
+                           float* map_x, float* map_y);
+/* A rectifier: one map, uploaded once to the context's device, through which later create calls remap their frames.  Any
+ * camera model works through its map (fisheye maps or stereo rectification from OpenCV, say).
+ *   in_width x in_height: the frames the create calls take (>= 2 x 2).  width x height: the rectified frames, i.e. level 0 of
+ *     the pyramids; map_x / map_y: HOST arrays of width*height floats, input pixel coordinates (pixel centres at integers,
+ *     OpenCV's convention).  K_new: fx, fy, cx, cy of the rectified camera, level 0's intrinsics.  Copied: the caller's
+ *     arrays may be freed when the call returns.  Synchronises.  dvo_b200_h2d_bytes grows by the 8*width*height bytes of
+ *     the map, once.
+ *   A rectifier belongs to its context: only create calls on that context take it.  dvo_b200_rectifier_release may be
+ *   called as soon as the create calls that used it have returned, with their work still queued; its memory is freed in
+ *   the context's stream order after that work, with no host synchronisation.  Release every rectifier of a context before
+ *   destroying the context. */
+typedef struct dvo_b200_rectifier dvo_b200_rectifier;
+int dvo_b200_rectifier_create(dvo_b200_ctx* ctx, int32_t in_width, int32_t in_height, int32_t width, int32_t height,
+                              const float* map_x, const float* map_y, const float K_new[4], dvo_b200_rectifier** out);
+int dvo_b200_rectifier_release(dvo_b200_rectifier* r);
+/* Rectified creates: the frames (in_width x in_height, given as width / height, which must equal the rectifier's) are
+ * remapped into the context's staging memory, then built exactly as dvo_b200_pyramid_create_masked_batch_roles builds
+ * FLOAT32 frames of the rectifier's width x height with intrinsics K_new.  format, masks (nonzero = usable, in the INPUT
+ * geometry), roles, depth_scale and levels as in that call.
+ *   For output pixel (x, y) with (sx, sy) = map(x, y), in float32:
+ *     valid iff 0 <= sx <= in_width - 1 and 0 <= sy <= in_height - 1 (a NaN or infinite coordinate is invalid);
+ *     taps x0 = min(floor(sx), in_width - 2), ax = sx - x0, y0 = min(floor(sy), in_height - 2), ay = sy - y0;
+ *     intensity = bilinear, each operation rounded to nearest, no contraction:
+ *       top = (1-ax)*I(x0,y0) + ax*I(x0+1,y0), bot = (1-ax)*I(x0,y0+1) + ax*I(x0+1,y0+1), I = (1-ay)*top + ay*bot
+ *       from 8-bit grey or float32; BGR is first reduced to 8-bit grey exactly as dvo_b200_pyramid_create_bgr_batch does;
+ *     depth = the nearest tap, never blended (a blend across a depth edge invents a surface): Z(x0 + (ax >= 0.5),
+ *       y0 + (ay >= 0.5)), float32 metres as given or u16 * depth_scale with 0 -> NaN, as the raw create calls convert;
+ *     an invalid pixel gets I = NaN and Z = NaN: it is never a point or a tap, and the 2x2 mean carries the NaN into every
+ *       coarse pixel whose footprint touches the area without source (a zero would be a false intensity there);
+ *     mask: usable iff the pixel is valid and its four intensity taps are usable.
+ *   The pyramids equal, bit for bit, those of dvo_b200_pyramid_create_masked_batch_roles(FLOAT32) on the rectified planes
+ *   and mask (masks == NULL: no mask, whatever the roles), with the rectifier's size and K_new.
+ * dvo_b200_pyramid_create_rectified_batch: HOST pointers to n frames, staged like dvo_b200_pyramid_create_masked_batch_roles
+ *   (dvo_b200_h2d_bytes grows by the input bytes only).
+ * dvo_b200_pyramid_create_rectified_device_batch: dvo_b200_device_plane inputs, validated and ordered exactly as in
+ *   dvo_b200_pyramid_create_device_batch; nothing is copied from the host.
+ * A NULL ctx or rectifier, a rectifier of another context, a width / height other than the rectifier's input size, or any
+ * argument the corresponding unrectified call refuses -> DVO_B200_ERR_INVALID_ARGUMENT, and nothing is created. */
+int dvo_b200_pyramid_create_rectified_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, int32_t n, int32_t format,
+                                            const void* image, const void* depth, float depth_scale, const uint8_t* masks,
+                                            int32_t roles, int32_t width, int32_t height, int32_t levels,
+                                            dvo_b200_pyramid** out /* n handles */);
+int dvo_b200_pyramid_create_rectified_device_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, int32_t n, int32_t format,
+                                                   const dvo_b200_device_plane* image, const dvo_b200_device_plane* depth,
+                                                   float depth_scale, const dvo_b200_device_plane* masks /* NULL: no mask */,
+                                                   int32_t roles, int32_t width, int32_t height, int32_t levels,
+                                                   dvo_b200_pyramid** out /* n handles */);
 /* Role set a pyramid was created with: 0 (no mask), DVO_B200_MASK_ROLE_REFERENCE, or
  * DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT; DVO_B200_ERR_INVALID_ARGUMENT for a null handle. */
 int dvo_b200_pyramid_mask_roles(const dvo_b200_pyramid* p);
