@@ -76,48 +76,60 @@ void convert_bgr(dvo_b200_ctx* ctx, int n, int w, int h, SrcPlane bgr, uint8_t* 
 
 }  // namespace
 
-// The last step of every create: build the pyramids from level-0 planes in device memory.  With a rectifier, the planes are
-// first remapped into packed float32 planes (and byte masks) in the staging memory at rect_off, which the caller has sized
-// with rectified_bytes, and the build reads those with the rectifier's size and intrinsics.
-static size_t rectified_bytes(const dvo_b200_rectifier* rect, int n, bool masked) {
+// The last step of every create: build the pyramids from level-0 planes in device memory.  With a rectifier or a depth
+// registration, the planes are first remapped or registered into packed float32 planes (and, through a rectifier, byte
+// masks) in the staging memory at rect_off, which the caller has sized with rectified_bytes, and the build reads those with
+// the target's size and intrinsics.  Registered without a rectifier, the build reads the colour geometry's masks in place.
+static size_t rectified_bytes(const dvo_b200_rectifier* rect, const dvo_b200_depth_registration* reg, int n, bool masked) {
+  if (reg) return (size_t)reg->w * reg->h * n * (2 * sizeof(float) + (rect && masked ? 1 : 0));
   return rect ? (size_t)rect->w * rect->h * n * (2 * sizeof(float) + (masked ? 1 : 0)) : 0;
 }
 
-static int build_planes(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, size_t rect_off, int n, SrcPlane I, SrcPlane Z, int raw,
-                        float zscale, SrcPlane M, int roles, int width, int height, float fx, float fy, float ox, float oy, int levels,
-                        dvo_b200_pyramid** out) {
-  if (!rect)
+static int build_planes(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, const dvo_b200_depth_registration* reg, size_t rect_off,
+                        int n, SrcPlane I, SrcPlane Z, int raw, float zscale, SrcPlane M, int roles, int width, int height, float fx,
+                        float fy, float ox, float oy, int levels, dvo_b200_pyramid** out) {
+  if (!rect && !reg)
     return pyramid_build_batch_input(ctx, n, I, Z, raw, zscale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, M, roles);
-  const size_t npx = (size_t)rect->w * rect->h * n;
+  const int w = reg ? reg->w : rect->w, h = reg ? reg->h : rect->h;
+  const float* K = reg ? reg->K : rect->K;
+  const size_t npx = (size_t)w * h * n;
   float* dI = (float*)((char*)ctx->d_stage + rect_off);
   float* dZ = dI + npx;
-  uint8_t* dM = M.data ? (uint8_t*)(dZ + npx) : nullptr;
-  rectify_batch(ctx, rect, n, I, Z, raw, zscale, M, dI, dZ, dM);
-  return pyramid_build_batch_input(ctx, n, packed_plane(dI, rect->w, rect->h), packed_plane(dZ, rect->w, rect->h), 0, 0.f, rect->w,
-                                   rect->h, rect->K[0], rect->K[1], rect->K[2], rect->K[3], levels, 0.f, 0.f, out,
-                                   dM ? packed_plane(dM, rect->w, rect->h) : SrcPlane{nullptr, 0, 0}, roles);
+  uint8_t* dM = rect && M.data ? (uint8_t*)(dZ + npx) : nullptr;
+  if (reg) {
+    if (int rc = register_batch(ctx, reg, rect, n, I, Z, raw, zscale, M, dI, dZ, dM)) return rc;
+  } else {
+    rectify_batch(ctx, rect, n, I, Z, raw, zscale, M, dI, dZ, dM);
+  }
+  const SrcPlane mask = rect ? (dM ? packed_plane(dM, w, h) : SrcPlane{nullptr, 0, 0}) : M;
+  return pyramid_build_batch_input(ctx, n, packed_plane(dI, w, h), packed_plane(dZ, w, h), 0, 0.f, w, h, K[0], K[1], K[2], K[3], levels,
+                                   0.f, 0.f, out, mask, roles);
 }
 
 // Uploads n frames of one dvo_b200_input_format (and their reference masks, if any) into the context's device staging
 // area and builds their pyramids from there, packed.  The frames stay in their file representation: the pyramid kernels
 // convert in their loads (no float32 copy of a raw frame is written); BGR is reduced to 8-bit grey first, as cv::cvtColor
-// leaves it.  Masks add one byte per pixel after the frames.  rect: the rectified planes follow the upload.
+// leaves it.  Masks add one byte per pixel after the frames.  rect / reg: the rectified or registered planes follow the
+// upload; with reg the depth frames have the depth camera's dw x dh.
 static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image, const void* depth, float depth_scale,
                          const uint8_t* masks, int mask_roles, int width, int height, float fx, float fy, float ox, float oy,
-                         int levels, dvo_b200_pyramid** out, const dvo_b200_rectifier* rect = nullptr) {
+                         int levels, dvo_b200_pyramid** out, const dvo_b200_rectifier* rect = nullptr,
+                         const dvo_b200_depth_registration* reg = nullptr) {
   cudaSetDevice(ctx->device);
   const size_t npx = (size_t)width * height * n;
+  const int dw = reg ? reg->dw : width, dh = reg ? reg->dh : height;
+  const size_t dnpx = (size_t)dw * dh * n;         // depth pixels
   size_t frames = 0, grey_off = 0, bgr_off = 0;   // bytes of the staged frames; offsets of the grey and BGR images
   if (format == DVO_B200_INPUT_FLOAT32) {
-    frames = 2 * npx * sizeof(float);
+    frames = (npx + dnpx) * sizeof(float);
   } else {
-    grey_off = (npx * 2 + 255) / 256 * 256;
+    grey_off = (dnpx * 2 + 255) / 256 * 256;
     bgr_off = grey_off + (npx + 255) / 256 * 256;
     frames = (format == DVO_B200_INPUT_BGR8_DEPTH16 ? bgr_off + npx * 3 : grey_off + npx) + 64;
   }
   const size_t mask_off = (frames + 255) / 256 * 256;
   const size_t rect_off = ((masks ? mask_off + npx : frames) + 255) / 256 * 256;
-  int rc = ensure_stage(ctx, rect ? rect_off + rectified_bytes(rect, n, masks != nullptr) : masks ? mask_off + npx : frames, 0);
+  int rc = ensure_stage(ctx, rect || reg ? rect_off + rectified_bytes(rect, reg, n, masks != nullptr) : masks ? mask_off + npx : frames, 0);
   if (rc) return rc;
   char* stage = (char*)ctx->d_stage;
   SrcPlane dM{nullptr, 0, 0};
@@ -130,24 +142,24 @@ static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image
     float* dI = (float*)stage;
     float* dZ = dI + npx;
     DVO_CUDA(ctx, cudaMemcpyAsync(dI, image, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    DVO_CUDA(ctx, cudaMemcpyAsync(dZ, depth, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    ctx->h2d_bytes += 2 * npx * sizeof(float);
-    return build_planes(ctx, rect, rect_off, n, packed_plane(dI, width, height), packed_plane(dZ, width, height), 0, 0.f, dM, mask_roles,
+    DVO_CUDA(ctx, cudaMemcpyAsync(dZ, depth, dnpx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    ctx->h2d_bytes += (npx + dnpx) * sizeof(float);
+    return build_planes(ctx, rect, reg, rect_off, n, packed_plane(dI, width, height), packed_plane(dZ, dw, dh), 0, 0.f, dM, mask_roles,
                         width, height, fx, fy, ox, oy, levels, out);
   }
   uint16_t* dR = (uint16_t*)stage;
   uint8_t* dG = (uint8_t*)(stage + grey_off);
-  DVO_CUDA(ctx, cudaMemcpyAsync(dR, depth, npx * 2, cudaMemcpyHostToDevice, ctx->stream));
+  DVO_CUDA(ctx, cudaMemcpyAsync(dR, depth, dnpx * 2, cudaMemcpyHostToDevice, ctx->stream));
   if (format == DVO_B200_INPUT_GREY8_DEPTH16) {
     DVO_CUDA(ctx, cudaMemcpyAsync(dG, image, npx, cudaMemcpyHostToDevice, ctx->stream));
-    ctx->h2d_bytes += npx * 3;
+    ctx->h2d_bytes += npx + dnpx * 2;
   } else {
     uint8_t* dC = (uint8_t*)(stage + bgr_off);
     DVO_CUDA(ctx, cudaMemcpyAsync(dC, image, npx * 3, cudaMemcpyHostToDevice, ctx->stream));
-    ctx->h2d_bytes += npx * 5;
+    ctx->h2d_bytes += npx * 3 + dnpx * 2;
     convert_bgr(ctx, n, width, height, packed_plane(dC, 3 * width, height), dG);
   }
-  return build_planes(ctx, rect, rect_off, n, packed_plane(dG, width, height), packed_plane(dR, width, height), 1, depth_scale, dM,
+  return build_planes(ctx, rect, reg, rect_off, n, packed_plane(dG, width, height), packed_plane(dR, dw, dh), 1, depth_scale, dM,
                       mask_roles, width, height, fx, fy, ox, oy, levels, out);
 }
 
@@ -187,11 +199,12 @@ static int device_plane(dvo_b200_ctx* ctx, const char* fn, const dvo_b200_device
 }
 
 
-// dvo_b200_pyramid_create_device_batch, and with a rectifier its rectified form.  fn names the entry point in the errors.
+// dvo_b200_pyramid_create_device_batch, and with a rectifier or a registration its rectified or registered form.  fn names
+// the entry point in the errors.
 static int create_device(dvo_b200_ctx* ctx, const char* fn, const dvo_b200_rectifier* rect, int n, int format,
                          const dvo_b200_device_plane* image, const dvo_b200_device_plane* depth, float depth_scale,
                          const dvo_b200_device_plane* masks, int roles, int width, int height, float fx, float fy, float ox, float oy,
-                         int levels, dvo_b200_pyramid** out) {
+                         int levels, dvo_b200_pyramid** out, const dvo_b200_depth_registration* reg = nullptr) {
   if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": null/invalid argument");
   if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
@@ -202,19 +215,19 @@ static int create_device(dvo_b200_ctx* ctx, const char* fn, const dvo_b200_recti
   const bool f32 = format == DVO_B200_INPUT_FLOAT32;
   SrcPlane I, Z, M{nullptr, 0, 0};
   int rc = device_plane(ctx, fn, image, "image", f32 ? 4 : 1, format == DVO_B200_INPUT_BGR8_DEPTH16 ? 3 : 1, n, width, height, &I);
-  if (!rc) rc = device_plane(ctx, fn, depth, "depth", f32 ? 4 : 2, 1, n, width, height, &Z);
+  if (!rc) rc = device_plane(ctx, fn, depth, "depth", f32 ? 4 : 2, 1, n, reg ? reg->dw : width, reg ? reg->dh : height, &Z);
   if (!rc && masks) rc = device_plane(ctx, fn, masks, "masks", 1, 1, n, width, height, &M);
   if (rc) return rc;
   const size_t grey = format == DVO_B200_INPUT_BGR8_DEPTH16 ? (size_t)width * height * n : 0;   // BGR reduced to grey in staging
   const size_t rect_off = (grey + 255) / 256 * 256;
-  if (grey || rect) {
-    if ((rc = ensure_stage(ctx, rect ? rect_off + rectified_bytes(rect, n, masks != nullptr) : grey, 0))) return rc;
+  if (grey || rect || reg) {
+    if ((rc = ensure_stage(ctx, rect || reg ? rect_off + rectified_bytes(rect, reg, n, masks != nullptr) : grey, 0))) return rc;
   }
   if (grey) {   // grey into staging, as the host path; depth and masks stay in place
     convert_bgr(ctx, n, width, height, I, (uint8_t*)ctx->d_stage);
     I = packed_plane(ctx->d_stage, width, height);
   }
-  return build_planes(ctx, rect, rect_off, n, I, Z, f32 ? 0 : 1, f32 ? 0.f : depth_scale, M, roles, width, height, fx, fy, ox, oy,
+  return build_planes(ctx, rect, reg, rect_off, n, I, Z, f32 ? 0 : 1, f32 ? 0.f : depth_scale, M, roles, width, height, fx, fy, ox, oy,
                       levels, out);
 }
 
@@ -459,6 +472,157 @@ int dvo_b200_pyramid_create_rectified_device_batch(dvo_b200_ctx* ctx, const dvo_
   if (int rc = check_rectifier(ctx, rect, width, height, "pyramid_create_rectified_device")) return rc;
   return create_device(ctx, "pyramid_create_rectified_device", rect, n, format, image, depth, depth_scale, masks, roles, width, height,
                        0.f, 0.f, 0.f, 0.f, levels, out);
+}
+
+int dvo_b200_depth_rays(int32_t dw, int32_t dh, const double K[4], const double dist[5], float* cx_ray, float* cy_ray, float* kx_ray,
+                        float* ky_ray) {
+  if (dw < 2 || dh < 2 || !K || !cx_ray || !cy_ray || !kx_ray || !ky_ray) return DVO_B200_ERR_INVALID_ARGUMENT;
+  for (int i = 0; i < 5; ++i)
+    if ((i < 4 && !std::isfinite(K[i])) || (dist && !std::isfinite(dist[i]))) return DVO_B200_ERR_INVALID_ARGUMENT;
+  const double fx = K[0], fy = K[1], cx = K[2], cy = K[3];
+  if (!(fx > 0) || !(fy > 0)) return DVO_B200_ERR_INVALID_ARGUMENT;
+  // the ray through pixel coordinates (u, v): the order of the header comment, term by term
+  auto ray = [&](double u, double v, float* rx, float* ry) {
+    const double xd = (u - cx) / fx, yd = (v - cy) / fy;
+    double x = xd, y = yd;
+    if (dist) {
+      const double k1 = dist[0], k2 = dist[1], p1 = dist[2], p2 = dist[3], k3 = dist[4];
+      for (int it = 0;; ++it) {
+        const double r2 = x * x + y * y;
+        const double R = 1 + ((k3 * r2 + k2) * r2 + k1) * r2;
+        const double dR = k1 + (2 * k2 + 3 * k3 * r2) * r2;
+        const double ex = x * R + 2 * p1 * x * y + p2 * (r2 + 2 * x * x) - xd;
+        const double ey = y * R + p1 * (r2 + 2 * y * y) + 2 * p2 * x * y - yd;
+        if (std::fabs(ex) < 1e-12 && std::fabs(ey) < 1e-12) break;
+        if (it == DVO_B200_DEPTH_RAYS_MAX_ITER) return false;
+        const double a = R + 2 * x * x * dR + 2 * p1 * y + 6 * p2 * x;
+        const double b = 2 * x * y * dR + 2 * p1 * x + 2 * p2 * y;
+        const double d = R + 2 * y * y * dR + 6 * p1 * y + 2 * p2 * x;
+        const double det = a * d - b * b;
+        const double nx = x - (d * ex - b * ey) / det, ny = y - (a * ey - b * ex) / det;
+        x = nx;
+        y = ny;
+      }
+    }
+    *rx = (float)x;
+    *ry = (float)y;
+    return true;
+  };
+  for (int v = 0; v < dh; ++v)
+    for (int u = 0; u < dw; ++u)
+      if (!ray(u, v, cx_ray + (size_t)v * dw + u, cy_ray + (size_t)v * dw + u)) return DVO_B200_ERR_INVALID_ARGUMENT;
+  for (int v = 0; v <= dh; ++v)
+    for (int u = 0; u <= dw; ++u)
+      if (!ray(u - 0.5, v - 0.5, kx_ray + (size_t)v * (dw + 1) + u, ky_ray + (size_t)v * (dw + 1) + u)) return DVO_B200_ERR_INVALID_ARGUMENT;
+  return 0;
+}
+
+int dvo_b200_depth_registration_create(dvo_b200_ctx* ctx, int32_t dw, int32_t dh, const float* cx_ray, const float* cy_ray,
+                                       const float* kx_ray, const float* ky_ray, const double T[16], int32_t width, int32_t height,
+                                       const float K[4], dvo_b200_depth_registration** out) {
+  if (out) *out = nullptr;
+  auto bad = [&](const char* why) {
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string("depth_registration_create: ") + why);
+  };
+  if (!ctx || !cx_ray || !cy_ray || !kx_ray || !ky_ray || !T || !K || !out || dw < 2 || dh < 2 || width <= 0 || height <= 0)
+    return bad("null/invalid argument");
+  for (int i = 0; i < 16; ++i)
+    if (!std::isfinite(T[i])) return bad("non-finite T_color_depth");
+  if (T[12] != 0 || T[13] != 0 || T[14] != 0 || T[15] != 1) return bad("T_color_depth: bottom row is not (0, 0, 0, 1)");
+  double err = 0;
+  for (int a = 0; a < 3; ++a)
+    for (int b = 0; b < 3; ++b) {
+      double s = 0;
+      for (int k = 0; k < 3; ++k) s += T[4 * k + a] * T[4 * k + b];
+      err = std::max(err, std::fabs(s - (a == b ? 1.0 : 0.0)));
+    }
+  const double det = T[0] * (T[5] * T[10] - T[6] * T[9]) - T[1] * (T[4] * T[10] - T[6] * T[8]) + T[2] * (T[4] * T[9] - T[5] * T[8]);
+  if (!(err <= 1e-6) || !(det > 0)) return bad("T_color_depth is not a rigid transform (R^T R != I or det R <= 0)");
+  for (int i = 0; i < 4; ++i)
+    if (!std::isfinite(K[i])) return bad("non-finite K");
+  if (!(K[0] > 0) || !(K[1] > 0)) return bad("non-positive focal length");
+  const size_t nc = (size_t)dw * dh, nk = (size_t)(dw + 1) * (dh + 1);
+  const float* tables[4] = {cx_ray, cy_ray, kx_ray, ky_ray};
+  for (int t = 0; t < 4; ++t)
+    for (size_t i = 0; i < (t < 2 ? nc : nk); ++i)
+      if (!std::isfinite(tables[t][i])) return bad("non-finite ray");
+  cudaSetDevice(ctx->device);
+  const size_t bytes = (2 * nc + 2 * nk) * sizeof(float);
+  float* d = nullptr;
+  DVO_CUDA(ctx, cudaMallocAsync((void**)&d, bytes, ctx->stream));
+  const size_t offs[4] = {0, nc, 2 * nc, 2 * nc + nk};
+  cudaError_t e = cudaSuccess;
+  for (int t = 0; t < 4 && e == cudaSuccess; ++t)
+    e = cudaMemcpyAsync(d + offs[t], tables[t], (t < 2 ? nc : nk) * sizeof(float), cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);   // the caller's arrays may go when this returns
+  if (e != cudaSuccess) {
+    cudaFreeAsync(d, ctx->stream);
+    return check_cuda(ctx, e, "depth_registration_create: ray upload");
+  }
+  ctx->h2d_bytes += bytes;
+  dvo_b200_depth_registration* r = new dvo_b200_depth_registration;
+  r->ctx = ctx; r->dw = dw; r->dh = dh; r->w = width; r->h = height; r->rays = d;
+  for (int a = 0; a < 3; ++a) {
+    for (int b = 0; b < 3; ++b) r->R[3 * a + b] = (float)T[4 * a + b];
+    r->t[a] = (float)T[4 * a + 3];
+  }
+  for (int i = 0; i < 4; ++i) r->K[i] = K[i];
+  *out = r;
+  return 0;
+}
+
+int dvo_b200_depth_registration_release(dvo_b200_depth_registration* r) {
+  if (!r) return DVO_B200_ERR_INVALID_ARGUMENT;
+  DeviceScope dev(r->ctx->device);
+  // every create that read the rays was enqueued on this stream before this call: the free follows them in stream order
+  const cudaError_t e = cudaFreeAsync(r->rays, r->ctx->stream);
+  const int rc = check_cuda(r->ctx, e, "depth_registration_release");
+  delete r;
+  return rc;
+}
+
+// The checks shared by both registered creates: the registration exists and belongs to ctx; without a rectifier the colour
+// frames have its target size; with one, the rectifier passes check_rectifier and its output is the target.
+static int check_registration(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg, const dvo_b200_rectifier* rect, int width,
+                              int height, const char* fn) {
+  auto bad = [&](const std::string& why) { return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": " + why); };
+  if (!reg) return bad("null depth registration");
+  if (reg->ctx != ctx) return bad("the depth registration belongs to another context");
+  const std::string target = std::to_string(reg->w) + "x" + std::to_string(reg->h);
+  if (rect) {
+    if (int rc = check_rectifier(ctx, rect, width, height, fn)) return rc;
+    if (rect->w != reg->w || rect->h != reg->h) return bad("the rectifier's output is not the registration's target " + target);
+    for (int i = 0; i < 4; ++i)
+      if (rect->K[i] != reg->K[i]) return bad("the rectifier's K_new is not the registration's K");
+  } else if (width != reg->w || height != reg->h) {
+    return bad("colour frames of " + std::to_string(width) + "x" + std::to_string(height) + ", the registration's target is " + target);
+  }
+  return 0;
+}
+
+int dvo_b200_pyramid_create_registered_batch(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg, const dvo_b200_rectifier* rect,
+                                             int32_t n, int32_t format, const void* image, const void* depth, float depth_scale,
+                                             const uint8_t* masks, int32_t roles, int32_t width, int32_t height, int32_t levels,
+                                             dvo_b200_pyramid** out) {
+  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_registered: null/invalid argument");
+  if (int rc = check_registration(ctx, reg, rect, width, height, "pyramid_create_registered")) return rc;
+  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_registered: unknown input format " + std::to_string(format));
+  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_registered: unsupported role set " + std::to_string(roles));
+  return create_staged(ctx, n, format, image, depth, depth_scale, masks, roles, width, height, 0.f, 0.f, 0.f, 0.f, levels, out, rect, reg);
+}
+
+int dvo_b200_pyramid_create_registered_device_batch(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg,
+                                                    const dvo_b200_rectifier* rect, int32_t n, int32_t format,
+                                                    const dvo_b200_device_plane* image, const dvo_b200_device_plane* depth,
+                                                    float depth_scale, const dvo_b200_device_plane* masks, int32_t roles, int32_t width,
+                                                    int32_t height, int32_t levels, dvo_b200_pyramid** out) {
+  if (!ctx) return DVO_B200_ERR_INVALID_ARGUMENT;
+  if (int rc = check_registration(ctx, reg, rect, width, height, "pyramid_create_registered_device")) return rc;
+  return create_device(ctx, "pyramid_create_registered_device", rect, n, format, image, depth, depth_scale, masks, roles, width, height,
+                       0.f, 0.f, 0.f, 0.f, levels, out, reg);
 }
 
 int dvo_b200_pyramid_mask_roles(const dvo_b200_pyramid* p) { return p ? p->mask_roles : DVO_B200_ERR_INVALID_ARGUMENT; }

@@ -269,12 +269,26 @@ struct dvo_b200_rectifier {      // a remap to a pinhole camera (dvo_b200_rectif
   float* map = nullptr;          // device, stream-ordered allocation: map_x[w*h] then map_y[w*h]
 };
 
+struct dvo_b200_depth_registration {   // a depth camera reprojected into a pinhole colour camera (dvo_b200_depth_registration_create)
+  dvo_b200_ctx* ctx = nullptr;          // the owning context: its stream orders every use and the free
+  int dw = 0, dh = 0;                   // depth frames
+  int w = 0, h = 0;                     // colour frames = level 0
+  float R[9] = {}, t[3] = {};           // T_color_depth, each value rounded once
+  float K[4] = {0, 0, 0, 0};            // fx, fy, cx, cy of level 0
+  float* rays = nullptr;                // device, stream-ordered: cx_ray, cy_ray [dw*dh] then kx_ray, ky_ray [(dw+1)*(dh+1)]
+};
+
 namespace dvo_b200 {
 
 // pyramid.cu: the rectifying remap of n frames into packed float32 planes dI / dZ (w*h floats per image) and, if M.data,
 // packed byte masks dM (1 = usable).  raw as in pyramid_build_batch_input: 8-bit grey + 16-bit depth, else float32.
 void rectify_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* r, int n, SrcPlane I, SrcPlane Z, int raw, float zscale, SrcPlane M,
                    float* dI, float* dZ, uint8_t* dM);
+// pyramid.cu: depth registration of n frames into packed float32 planes dI / dZ of the registration's w*h floats per image.
+// Z: depth in the depth camera's dw x dh.  I (and M): the colour frames.  Without a rectifier they are w x h, and the build
+// reads M in place.  With one they have its input size and go through its map, and the remapped byte masks go to dM.
+int register_batch(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg, const dvo_b200_rectifier* rect, int n, SrcPlane I,
+                    SrcPlane Z, int raw, float zscale, SrcPlane M, float* dI, float* dZ, uint8_t* dM);
 
 // pyramid.cu
 int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float* d_Z, int w, int h, float fx, float fy,

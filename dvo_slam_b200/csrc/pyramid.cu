@@ -345,8 +345,10 @@ __global__ void k_template(float* __restrict__ tmpl, size_t tmpl_per_image, size
 // The rectifying remap (dvo_b200_pyramid_create_rectified_batch): one thread per output pixel of one image.  Bilinear
 // intensity in a fixed order with every operation rounded to nearest (no contraction), the nearest tap's depth, NaN / NaN
 // where the map points outside [0, in_w-1] x [0, in_h-1].  kMasked: the pixel is usable iff it is valid and its four taps
-// are.  The outputs are packed planes of w*h elements per image, the layout of a staged FLOAT32 upload.
-template <bool kRaw, bool kMasked>
+// are.  The outputs are packed planes of w*h elements per image, the layout of a staged FLOAT32 upload.  kZbuf (a
+// registered create): Z is not read; dZ holds k_register_scatter's z-buffer, whose untouched pixels become NaN, valid
+// map or not.
+template <bool kRaw, bool kMasked, bool kZbuf = false>
 __global__ void __launch_bounds__(256)
 k_rectify(SrcPlane I, SrcPlane Z, float zscale, SrcPlane M, const float* __restrict__ map_x, const float* __restrict__ map_y,
           int in_w, int in_h, int n, float* __restrict__ dI, float* __restrict__ dZ, uint8_t* __restrict__ dM) {
@@ -367,16 +369,85 @@ k_rectify(SrcPlane I, SrcPlane Z, float zscale, SrcPlane M, const float* __restr
     const float top = __fadd_rn(__fmul_rn(bx, i00), __fmul_rn(ax, i10));
     const float bot = __fadd_rn(__fmul_rn(bx, i01), __fmul_rn(ax, i11));
     v = __fadd_rn(__fmul_rn(by, top), __fmul_rn(ay, bot));
-    z = load_depth<kRaw>(Z.data, Z.at(img, y0 + (ay >= 0.5f), x0 + (ax >= 0.5f)), zscale);
+    if (!kZbuf) z = load_depth<kRaw>(Z.data, Z.at(img, y0 + (ay >= 0.5f), x0 + (ax >= 0.5f)), zscale);
     if (kMasked) {
       const uint8_t* m = reinterpret_cast<const uint8_t*>(M.data) + M.at(img, y0, x0);
       usable = __ldg(m) && __ldg(m + 1) && __ldg(m + M.pitch) && __ldg(m + M.pitch + 1);
     }
   }
   const size_t out = (size_t)img * n + i;
+  if (kZbuf) {
+    const float zb = dZ[out];
+    z = __float_as_uint(zb) == 0xffffffffu ? nanv : zb;
+  }
   dI[out] = v;
   dZ[out] = z;
   if (kMasked) dM[out] = usable ? 1 : 0;
+}
+
+// Depth registration (dvo_b200_pyramid_create_registered_batch): the geometry of a dvo_b200_depth_registration, by value.
+struct RegGeometry {
+  int dw, dh, w, h;
+  float R[9], t[3], K[4];
+};
+
+// ((r0*X + r1*Y) + r2*Z) + t, every operation rounded to nearest
+__device__ __forceinline__ float reg_row(float r0, float r1, float r2, float t, float X, float Y, float Z) {
+  return __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(r0, X), __fmul_rn(r1, Y)), __fmul_rn(r2, Z)), t);
+}
+
+// The forward projection of the header, one thread per depth pixel of one image: Zc of the pixel's centre ray goes into
+// every colour pixel of the footprint of its four corner rays through atomicMin on the float's bits, which order as
+// unsigned ints for positive floats.  zbuf: packed w*h words per image, 0xffffffff where nothing has landed.  The result is
+// the minimum over the covering pixels, whatever order the threads run in.
+template <bool kRaw>
+__global__ void __launch_bounds__(256)
+k_register_scatter(SrcPlane Z, float zscale, RegGeometry g, const float* __restrict__ rays, unsigned* __restrict__ zbuf) {
+  const int img = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int npx = g.dw * g.dh;
+  if (i >= npx) return;
+  const int v = i / g.dw, u = i - v * g.dw;
+  const float d = load_depth<kRaw>(Z.data, Z.at(img, v, u), zscale);
+  if (!(d > 0.f) || !isfinite(d)) return;
+  const float zc = reg_row(g.R[6], g.R[7], g.R[8], g.t[2], __fmul_rn(__ldg(rays + i), d), __fmul_rn(__ldg(rays + npx + i), d), d);
+  if (!(zc > 0.f)) return;
+  const float* kx = rays + 2 * (size_t)npx;
+  const float* ky = kx + (size_t)(g.dw + 1) * (g.dh + 1);
+  float xmin = INFINITY, xmax = -INFINITY, ymin = INFINITY, ymax = -INFINITY;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) {
+    const size_t k = (size_t)(v + (c >> 1)) * (g.dw + 1) + u + (c & 1);
+    const float X = __fmul_rn(__ldg(kx + k), d), Y = __fmul_rn(__ldg(ky + k), d);
+    const float zk = reg_row(g.R[6], g.R[7], g.R[8], g.t[2], X, Y, d);
+    if (!(zk > 0.f)) return;
+    const float x = __fadd_rn(__fmul_rn(g.K[0], __fdiv_rn(reg_row(g.R[0], g.R[1], g.R[2], g.t[0], X, Y, d), zk)), g.K[2]);
+    const float y = __fadd_rn(__fmul_rn(g.K[1], __fdiv_rn(reg_row(g.R[3], g.R[4], g.R[5], g.t[1], X, Y, d), zk)), g.K[3]);
+    if (!(fabsf(x) < 1048576.f) || !(fabsf(y) < 1048576.f)) return;
+    xmin = fminf(xmin, x); xmax = fmaxf(xmax, x);
+    ymin = fminf(ymin, y); ymax = fmaxf(ymax, y);
+  }
+  const int x0 = (int)ceilf(xmin), x1 = (int)ceilf(xmax), y0 = (int)ceilf(ymin), y1 = (int)ceilf(ymax);
+  if (x1 - x0 > DVO_B200_REGISTRATION_MAX_FOOTPRINT || y1 - y0 > DVO_B200_REGISTRATION_MAX_FOOTPRINT) return;
+  const int xa = max(x0, 0), xb = min(x1, g.w), ya = max(y0, 0), yb = min(y1, g.h);
+  unsigned* zb = zbuf + (size_t)img * g.w * g.h;
+  const unsigned bits = __float_as_uint(zc);
+  for (int y = ya; y < yb; ++y)
+    for (int x = xa; x < xb; ++x) atomicMin(zb + (size_t)y * g.w + x, bits);
+}
+
+// The registered create's finish without a rectifier, one thread per colour pixel of one image: the packed float32
+// intensity of the colour frame (as given, or 8-bit grey converted exactly), and NaN depth where the z-buffer is untouched.
+template <bool kRaw>
+__global__ void __launch_bounds__(256)
+k_register_finish(SrcPlane I, int w, int n, float* __restrict__ dI, float* __restrict__ dZ) {
+  const int img = blockIdx.y;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int y = i / w, x = i - y * w;
+  const size_t out = (size_t)img * n + i;
+  dI[out] = load_intensity<kRaw>(I.data, I.at(img, y, x));
+  if (__float_as_uint(dZ[out]) == 0xffffffffu) dZ[out] = __int_as_float(0x7fc00000);
 }
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -495,6 +566,38 @@ void rectify_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* r, int n, SrcPla
   else if (masked) k_rectify<false, true><<<g, 256, 0, st>>>(I, Z, zscale, M, mx, my, r->in_w, r->in_h, npx, dI, dZ, dM);
   else k_rectify<false, false><<<g, 256, 0, st>>>(I, Z, zscale, M, mx, my, r->in_w, r->in_h, npx, dI, dZ, dM);
   ctx->launches += 1;
+}
+
+int register_batch(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg, const dvo_b200_rectifier* rect, int n, SrcPlane I,
+                   SrcPlane Z, int raw, float zscale, SrcPlane M, float* dI, float* dZ, uint8_t* dM) {
+  ProfScope prof(ctx, 3, 2);
+  const int npx = reg->w * reg->h, dpx = reg->dw * reg->dh;
+  cudaStream_t st = ctx->stream;
+  DVO_CUDA(ctx, cudaMemsetAsync(dZ, 0xff, (size_t)npx * n * sizeof(float), st));   // the empty z-buffer
+  RegGeometry geo;
+  geo.dw = reg->dw; geo.dh = reg->dh; geo.w = reg->w; geo.h = reg->h;
+  for (int k = 0; k < 9; ++k) geo.R[k] = reg->R[k];
+  for (int k = 0; k < 3; ++k) geo.t[k] = reg->t[k];
+  for (int k = 0; k < 4; ++k) geo.K[k] = reg->K[k];
+  const dim3 gs((dpx + 255) / 256, n), gc((npx + 255) / 256, n);
+  unsigned* zbuf = reinterpret_cast<unsigned*>(dZ);
+  if (raw) k_register_scatter<true><<<gs, 256, 0, st>>>(Z, zscale, geo, reg->rays, zbuf);
+  else k_register_scatter<false><<<gs, 256, 0, st>>>(Z, zscale, geo, reg->rays, zbuf);
+  if (rect) {   // intensity and masks through the rectifier's map, depth from the z-buffer
+    const float* mx = rect->map;
+    const float* my = rect->map + npx;
+    const bool masked = M.data != nullptr;
+    if (raw && masked) k_rectify<true, true, true><<<gc, 256, 0, st>>>(I, Z, 0.f, M, mx, my, rect->in_w, rect->in_h, npx, dI, dZ, dM);
+    else if (raw) k_rectify<true, false, true><<<gc, 256, 0, st>>>(I, Z, 0.f, M, mx, my, rect->in_w, rect->in_h, npx, dI, dZ, dM);
+    else if (masked) k_rectify<false, true, true><<<gc, 256, 0, st>>>(I, Z, 0.f, M, mx, my, rect->in_w, rect->in_h, npx, dI, dZ, dM);
+    else k_rectify<false, false, true><<<gc, 256, 0, st>>>(I, Z, 0.f, M, mx, my, rect->in_w, rect->in_h, npx, dI, dZ, dM);
+  } else if (raw) {
+    k_register_finish<true><<<gc, 256, 0, st>>>(I, reg->w, npx, dI, dZ);
+  } else {
+    k_register_finish<false><<<gc, 256, 0, st>>>(I, reg->w, npx, dI, dZ);
+  }
+  ctx->launches += 2;
+  return 0;
 }
 
 int pyramid_build_batch(dvo_b200_ctx* ctx, int n, const float* d_I, const float* d_Z, int w, int h, float fx, float fy,

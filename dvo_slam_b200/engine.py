@@ -33,7 +33,9 @@ ABI_SYMBOLS = [
     "dvo_b200_set_estimator", "dvo_b200_get_estimator", "dvo_b200_pyramid_create_masked_batch",
     "dvo_b200_pyramid_create_masked_batch_roles", "dvo_b200_pyramid_mask_roles", "dvo_b200_pyramid_create_device_batch",
     "dvo_b200_undistort_map", "dvo_b200_rectifier_create", "dvo_b200_rectifier_release", "dvo_b200_pyramid_create_rectified_batch",
-    "dvo_b200_pyramid_create_rectified_device_batch",
+    "dvo_b200_pyramid_create_rectified_device_batch", "dvo_b200_depth_rays", "dvo_b200_depth_registration_create",
+    "dvo_b200_depth_registration_release", "dvo_b200_pyramid_create_registered_batch",
+    "dvo_b200_pyramid_create_registered_device_batch",
 ]
 
 # dvo_b200_estimator
@@ -68,7 +70,7 @@ class DevicePlane(C.Structure):
     _fields_ = [("data", C.c_void_p), ("row_bytes", C.c_int64), ("image_bytes", C.c_int64)]
 
 
-def device_planes(image, depth, masks=None):
+def device_planes(image, depth, masks=None, depth_size=None):
     """The arguments of dvo_b200_pyramid_create_device_batch for torch tensors, from their shapes, dtypes and strides alone
     (nothing is copied, and the tensors may live on any device):
         float32 [n,h,w] image + float32 [n,h,w] depth   -> "float32"
@@ -78,7 +80,8 @@ def device_planes(image, depth, masks=None):
     for the whole batch (image_bytes 0).  Strided views such as a crop big[:, y0:y0+h, x0:x0+w] become a plane with the
     larger image's row pitch.  Returns (format, (n, h, w), image, depth, masks) with each plane a (data_ptr, row_bytes,
     image_bytes) tuple, masks None without a mask.  A layout that one row pitch and one image stride per plane cannot
-    express (a column stride other than one pixel, rows that overlap) raises ValueError."""
+    express (a column stride other than one pixel, rows that overlap) raises ValueError.  depth_size = (dw, dh): the depth
+    planes are [n, dh, dw], a depth camera of its own (dvo_b200_pyramid_create_registered_device_batch)."""
     import torch
     if image.dtype == torch.float32 and image.dim() == 3:
         fmt, depth_dtype, px = "float32", torch.float32, 1
@@ -90,12 +93,14 @@ def device_planes(image, depth, masks=None):
         raise ValueError(f"image: {image.dtype} {tuple(image.shape)} is none of float32 [n,h,w], uint8 [n,h,w] (grey) or "
                          "uint8 [n,h,w,3] (BGR)")
     n, h, w = (int(v) for v in image.shape[:3])
-    if depth.dtype != depth_dtype or tuple(depth.shape) != (n, h, w):
-        raise ValueError(f"depth: {depth.dtype} {tuple(depth.shape)}, want {depth_dtype} {(n, h, w)} with a {fmt} image")
+    dw, dh = (w, h) if depth_size is None else (int(depth_size[0]), int(depth_size[1]))
+    if depth.dtype != depth_dtype or tuple(depth.shape) != (n, dh, dw):
+        raise ValueError(f"depth: {depth.dtype} {tuple(depth.shape)}, want {depth_dtype} {(n, dh, dw)} with a {fmt} image")
     if px == 3 and image.stride(3) != 1:
         raise ValueError(f"image: BGR channel stride {image.stride(3)}, want 1 (interleaved pixels)")
 
     def plane(t, name, per_px, shared=False):
+        h, w = t.shape[1:3] if t.dim() >= 3 else t.shape
         es = t.element_size()
         if w > 1 and t.stride(-1 if per_px == 1 else -2) != per_px:
             raise ValueError(f"{name}: column stride {t.stride(-1 if per_px == 1 else -2)} elements, want {per_px} (pixels packed "
@@ -204,6 +209,13 @@ def load_library():
     L.dvo_b200_pyramid_create_rectified_batch.argtypes = [vp, vp, i32, i32, vp, vp, C.c_float, vp, i32, i32, i32, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_create_rectified_device_batch.argtypes = [vp, vp, i32, i32, C.POINTER(DevicePlane), C.POINTER(DevicePlane),
                                                                  C.c_float, C.POINTER(DevicePlane), i32, i32, i32, i32, C.POINTER(vp)]
+    L.dvo_b200_depth_rays.argtypes = [i32, i32, dp, dp, fp, fp, fp, fp]
+    L.dvo_b200_depth_registration_create.argtypes = [vp, i32, i32, fp, fp, fp, fp, dp, i32, i32, fp, C.POINTER(vp)]
+    L.dvo_b200_depth_registration_release.argtypes = [vp]
+    L.dvo_b200_pyramid_create_registered_batch.argtypes = [vp, vp, vp, i32, i32, vp, vp, C.c_float, vp, i32, i32, i32, i32,
+                                                           C.POINTER(vp)]
+    L.dvo_b200_pyramid_create_registered_device_batch.argtypes = [vp, vp, vp, i32, i32, C.POINTER(DevicePlane), C.POINTER(DevicePlane),
+                                                                  C.c_float, C.POINTER(DevicePlane), i32, i32, i32, i32, C.POINTER(vp)]
     L.dvo_b200_pyramid_device.argtypes = [vp]
     L.dvo_b200_sharded_create.argtypes = [i32, C.POINTER(i32), C.POINTER(vp)]
     L.dvo_b200_sharded_destroy.argtypes = [vp]
@@ -325,6 +337,44 @@ class Rectifier:
             pass
 
 
+def depth_rays(size, K, dist=None):
+    """dvo_b200_depth_rays: the ray tables (cx_ray, cy_ray, kx_ray, ky_ray) of a depth camera of size = (dw, dh) with
+    intrinsics K = (fx, fy, cx, cy): float32 [dh, dw] rays through the pixel centres and [dh+1, dw+1] rays through the pixel
+    corners (u - 0.5, v - 0.5), normalised to z = 1.  dist: None (pinhole) or plumb-bob (k1, k2, p1, p2, k3), inverted by
+    Newton's method.  Host only: no context and no GPU."""
+    dw, dh = (int(v) for v in size)
+    Kd = np.ascontiguousarray(K, dtype=np.float64).reshape(4)
+    d = None if dist is None else np.ascontiguousarray(dist, dtype=np.float64).reshape(5)
+    cx, cy = np.empty((dh, dw), np.float32), np.empty((dh, dw), np.float32)
+    kx, ky = np.empty((dh + 1, dw + 1), np.float32), np.empty((dh + 1, dw + 1), np.float32)
+    dp, fp = C.POINTER(C.c_double), C.POINTER(C.c_float)
+    rc = load_library().dvo_b200_depth_rays(dw, dh, Kd.ctypes.data_as(dp), None if d is None else d.ctypes.data_as(dp),
+                                            *(a.ctypes.data_as(fp) for a in (cx, cy, kx, ky)))
+    if rc != 0:
+        raise ValueError(f"dvo_b200_depth_rays: status {rc} (size {dw}x{dh}, K {Kd}, dist {d})")
+    return cx, cy, kx, ky
+
+
+class DepthRegistration:
+    """Owning handle of a dvo_b200_depth_registration: a depth camera of depth_size = (dw, dh) reprojected into a pinhole
+    colour camera K of size = (w, h).  Released with release(), when collected, or when its engine closes."""
+
+    def __init__(self, engine: "Engine", handle: int, depth_size, size, K):
+        self.engine, self.handle = engine, handle
+        self.depth_size, self.size, self.K = tuple(depth_size), tuple(size), tuple(K)
+
+    def release(self):
+        if self.handle:
+            load_library().dvo_b200_depth_registration_release(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
+
+
 class Engine:
     """One dvo_b200_ctx (one CUDA stream on one device).  estimator: "reference" (dvo::DenseTracker::match()'s numbers) or
     "corrected" (the same algorithm without the reference's scale-pairing, log-likelihood-tail and odd-point quirks; see
@@ -342,6 +392,7 @@ class Engine:
         self.ctx = ctx
         self.device = device
         self._rectifiers = weakref.WeakSet()
+        self._registrations = weakref.WeakSet()
         self.set_estimator(estimator)
 
     def set_estimator(self, estimator: str):
@@ -358,6 +409,8 @@ class Engine:
     def close(self):
         if getattr(self, "ctx", None):
             for r in list(getattr(self, "_rectifiers", ())):   # a rectifier is freed on its context's stream
+                r.release()
+            for r in list(getattr(self, "_registrations", ())):   # so is a depth registration
                 r.release()
             self.lib.dvo_b200_destroy(self.ctx)
             self.ctx = None
@@ -596,6 +649,102 @@ class Engine:
         rc = self.lib.dvo_b200_pyramid_create_rectified_device_batch(self.ctx, rect.handle, n, INPUT_FORMATS[fmt], C.byref(I), C.byref(Z),
                                                                      float(depth_scale or 0.0), C.byref(M) if M is not None else None,
                                                                      MASK_ROLES[mask_roles], w, h, levels, out)
+        current.wait_stream(ext)
+        self._check(rc)
+        return [Pyramid(self, out[i]) for i in range(n)]
+
+    # ---- unregistered depth ----
+    depth_rays = staticmethod(depth_rays)
+
+    def depth_registration(self, depth_size, rays, T_color_depth, size, K) -> DepthRegistration:
+        """dvo_b200_depth_registration_create: a depth camera of depth_size = (dw, dh) given by rays = (cx_ray, cy_ray, kx_ray,
+        ky_ray) as depth_rays returns them, at T_color_depth (4x4, p_color = T p_depth, metres) from a pinhole colour camera
+        K = (fx, fy, cx, cy) of size = (w, h).  The tables are uploaded once."""
+        dw, dh = (int(v) for v in depth_size)
+        shapes = [(dh, dw), (dh, dw), (dh + 1, dw + 1), (dh + 1, dw + 1)]
+        tabs = [np.ascontiguousarray(r, dtype=np.float32) for r in rays]
+        if len(tabs) != 4 or [t.shape for t in tabs] != shapes:
+            raise ValueError(f"rays {[t.shape for t in tabs]}: want {shapes}")
+        T = np.ascontiguousarray(T_color_depth, dtype=np.float64).reshape(16)
+        Kf = (C.c_float * 4)(*[float(v) for v in K])
+        out = C.c_void_p()
+        fp = C.POINTER(C.c_float)
+        self._check(self.lib.dvo_b200_depth_registration_create(self.ctx, dw, dh, *(t.ctypes.data_as(fp) for t in tabs),
+                                                                T.ctypes.data_as(C.POINTER(C.c_double)), int(size[0]), int(size[1]),
+                                                                Kf, C.byref(out)))
+        r = DepthRegistration(self, out.value, (dw, dh), size, tuple(Kf))
+        self._registrations.add(r)
+        return r
+
+    def pyramid_registered_batch(self, reg: DepthRegistration, image, depth, levels: int, depth_scale=None, masks=None,
+                                 mask_roles="reference", rectifier: Rectifier | None = None) -> list[Pyramid]:
+        """Pyramids of colour frames with the depth of a separate depth camera reprojected into them
+        (dvo_b200_pyramid_create_registered_batch): level 0 has reg's colour size and K.  image: the colour frames, [n,h,w]
+        float32 or uint8 grey, or uint8 [n,h,w,3] BGR, of reg's size or, with a rectifier, of its input size; depth: [n,dh,dw]
+        float32 metres (with float32 images) or uint16 raw (then depth_scale), in the depth camera's geometry.  masks
+        ([n,h,w] or [h,w], nonzero = usable, in the colour frames' geometry) / mask_roles as in pyramid_batch.  numpy arrays:
+        staged from the host, synchronises before returning.  torch CUDA tensors: through
+        dvo_b200_pyramid_create_registered_device_batch, ordered with torch's current stream as in pyramid_batch_device,
+        without a host synchronisation."""
+        if mask_roles not in MASK_ROLES:
+            raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
+        rh = rectifier.handle if rectifier is not None else None
+        if not isinstance(image, np.ndarray) and hasattr(image, "is_cuda") and image.is_cuda:
+            return self._registered_device(reg, rh, image, depth, levels, depth_scale, masks, mask_roles)
+        image, depth = np.asarray(image), np.asarray(depth)
+        if image.dtype == np.float32 and image.ndim == 3 and depth.dtype == np.float32:
+            fmt = "float32"
+        elif image.dtype == np.uint8 and image.ndim == 3 and depth.dtype == np.uint16:
+            fmt = "grey8_depth16"
+        elif image.dtype == np.uint8 and image.ndim == 4 and image.shape[3] == 3 and depth.dtype == np.uint16:
+            fmt = "bgr8_depth16"
+        else:
+            raise ValueError(f"image {image.dtype} {image.shape} with depth {depth.dtype}: want float32 [n,h,w] + float32, uint8 "
+                             "[n,h,w] + uint16 or uint8 [n,h,w,3] + uint16")
+        n, h, w = image.shape[:3]
+        dw, dh = reg.depth_size
+        if depth.shape != (n, dh, dw):
+            raise ValueError(f"depth {depth.shape}, want {(n, dh, dw)} (the depth camera's size)")
+        if fmt != "float32" and depth_scale is None:
+            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
+        I, Z = np.ascontiguousarray(image), np.ascontiguousarray(depth)
+        M = None
+        if masks is not None:
+            M = np.asarray(masks)
+            M = np.broadcast_to(M, (n, h, w)) if M.shape == (h, w) else M
+            if M.shape != (n, h, w):
+                raise ValueError(f"masks {M.shape}, want {(n, h, w)} or {(h, w)}")
+            M = np.ascontiguousarray(M if M.dtype == np.uint8 else M != 0, dtype=np.uint8)
+        out = (C.c_void_p * n)()
+        self._check(self.lib.dvo_b200_pyramid_create_registered_batch(self.ctx, reg.handle, rh, n, INPUT_FORMATS[fmt], I.ctypes.data,
+                                                                      Z.ctypes.data, float(depth_scale or 0.0),
+                                                                      M.ctypes.data if M is not None else None, MASK_ROLES[mask_roles],
+                                                                      w, h, levels, out))
+        self.synchronize()   # the staged host arrays may die with this call
+        return [Pyramid(self, out[i]) for i in range(n)]
+
+    def _registered_device(self, reg, rh, image, depth, levels, depth_scale, masks, mask_roles):
+        import torch
+        fmt, (n, h, w), pI, pZ, pM = device_planes(image, depth, masks, depth_size=reg.depth_size)
+        if fmt != "float32" and depth_scale is None:
+            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
+        dev = torch.device("cuda", self.device)
+        inputs = [t for t in (image, depth, masks) if t is not None]
+        for t in inputs:
+            if t.device != dev:
+                raise ValueError(f"a tensor on {t.device}: the engine runs on {dev}")
+        I, Z = DevicePlane(*pI), DevicePlane(*pZ)
+        M = DevicePlane(*pM) if pM is not None else None
+        out = (C.c_void_p * n)()
+        current = torch.cuda.current_stream(dev)
+        ext = torch.cuda.ExternalStream(self.stream, device=dev)
+        ext.wait_stream(current)
+        for t in inputs:
+            t.record_stream(ext)     # the caching allocator keeps the memory until the build has read it
+        rc = self.lib.dvo_b200_pyramid_create_registered_device_batch(self.ctx, reg.handle, rh, n, INPUT_FORMATS[fmt], C.byref(I),
+                                                                      C.byref(Z), float(depth_scale or 0.0),
+                                                                      C.byref(M) if M is not None else None, MASK_ROLES[mask_roles], w,
+                                                                      h, levels, out)
         current.wait_stream(ext)
         self._check(rc)
         return [Pyramid(self, out[i]) for i in range(n)]

@@ -12,7 +12,7 @@ Runs on any torch device (CPU in the unit tests, CUDA when the bench builds its 
 from __future__ import annotations
 
 import math
-from dataclasses import dataclass
+from dataclasses import dataclass, replace
 
 import numpy as np
 import torch
@@ -66,6 +66,7 @@ class SceneConfig:
     intensity_noise_sigma: float = 0.0
     quantize_intensity: bool = True
     distortion: tuple | None = None  # (k1, k2, p1, p2, k3) plumb-bob lens; None: a pinhole camera
+    depth_camera: "DepthCamera | None" = None   # depth from a camera of its own; None: depth along the colour rays
 
     def scaled(self, factor: int) -> "SceneConfig":
         """Same camera at ``factor`` x the resolution (config 5: 1280x960 = 2 x fr1)."""
@@ -73,7 +74,26 @@ class SceneConfig:
         return SceneConfig(self.width * factor, self.height * factor,
                            (fx * factor, fy * factor, ox * factor, oy * factor), self.n_sinusoids,
                            self.max_translation, self.max_rotation, self.hole_fraction, self.max_depth,
-                           self.depth_quantum, self.intensity_noise_sigma, self.quantize_intensity, self.distortion)
+                           self.depth_quantum, self.intensity_noise_sigma, self.quantize_intensity, self.distortion,
+                           self.depth_camera)
+
+
+@dataclass
+class DepthCamera:
+    """A depth camera apart from the colour camera (a time-of-flight or stereo depth sensor): its own size, intrinsics and
+    optional plumb-bob distortion, at T_color_depth (4x4, p_color = T_color_depth @ p_depth, metres)."""
+    width: int
+    height: int
+    intrinsics: tuple
+    T_color_depth: np.ndarray
+    distortion: tuple | None = None
+
+
+def baseline(tx: float, ty: float = 0.0, tz: float = 0.0) -> np.ndarray:
+    """T_color_depth of a depth camera mounted parallel to the colour camera at (tx, ty, tz) metres in its frame"""
+    T = np.eye(4)
+    T[:3, 3] = (tx, ty, tz)
+    return T
 
 
 FR1_DISTORTION = (0.2624, -0.9531, -0.0054, 0.0026, 1.1633)   # TUM fr1 plumb-bob k1, k2, p1, p2, k3
@@ -149,7 +169,8 @@ def _render(cfg: SceneConfig, T_cam: np.ndarray, tex, box, rng: np.random.Genera
 
 def make_pair(seed: int, cfg: SceneConfig | None = None, device="cpu"):
     """Returns dict with float32 [h,w] tensors I_ref, Z_ref, I_cur, Z_cur on ``device`` and
-    float64 numpy ``T_true`` (p_cur = T_true p_ref) and ``xi``."""
+    float64 numpy ``T_true`` (p_cur = T_true p_ref) and ``xi``.  With ``cfg.depth_camera``, Z_ref / Z_cur are that camera's
+    depth frames in its own geometry, and Z_ref_color / Z_cur_color the colour camera's own depth."""
     cfg = cfg or SceneConfig()
     rng = np.random.default_rng(seed)
     xi = np.concatenate([rng.uniform(-cfg.max_translation, cfg.max_translation, 3),
@@ -168,8 +189,19 @@ def make_pair(seed: int, cfg: SceneConfig | None = None, device="cpu"):
     box = (1.2 + rng.uniform(-0.1, 0.1), rng.uniform(-0.2, 0.2), rng.uniform(-0.15, 0.15), 0.28, 0.22)
     I_ref, Z_ref = _render(cfg, np.eye(4), tex, box, rng, device)
     I_cur, Z_cur = _render(cfg, T_true, tex, box, rng, device)
-    return {"I_ref": I_ref, "Z_ref": Z_ref, "I_cur": I_cur, "Z_cur": Z_cur, "T_true": T_true, "xi": xi,
-            "intrinsics": cfg.intrinsics, "width": cfg.width, "height": cfg.height}
+    out = {"I_ref": I_ref, "Z_ref": Z_ref, "I_cur": I_cur, "Z_cur": Z_cur, "T_true": T_true, "xi": xi,
+           "intrinsics": cfg.intrinsics, "width": cfg.width, "height": cfg.height}
+    if cfg.depth_camera is not None:
+        # Z_ref / Z_cur come from the depth camera, in its own geometry, after the colour frames have drawn from rng;
+        # the colour camera's own depth stays as Z_ref_color / Z_cur_color
+        dc = cfg.depth_camera
+        dcfg = replace(cfg, width=dc.width, height=dc.height, intrinsics=tuple(dc.intrinsics), distortion=dc.distortion,
+                       depth_camera=None)
+        T_dc = np.linalg.inv(np.asarray(dc.T_color_depth, dtype=np.float64))   # p_depth = T_dc p_color
+        out["Z_ref_color"], out["Z_cur_color"] = Z_ref, Z_cur
+        out["Z_ref"] = _render(dcfg, T_dc, tex, box, rng, device)[1]
+        out["Z_cur"] = _render(dcfg, T_dc @ T_true, tex, box, rng, device)[1]
+    return out
 
 
 def make_sequence(seed: int, n_frames: int, cfg: SceneConfig | None = None, device="cpu"):

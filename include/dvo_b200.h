@@ -311,6 +311,88 @@ int dvo_b200_pyramid_create_rectified_device_batch(dvo_b200_ctx* ctx, const dvo_
                                                    float depth_scale, const dvo_b200_device_plane* masks /* NULL: no mask */,
                                                    int32_t roles, int32_t width, int32_t height, int32_t levels,
                                                    dvo_b200_pyramid** out /* n handles */);
+/* ---- unregistered depth: a separate depth camera reprojected into the colour camera in the pyramid build --------------
+ * The tracker needs every pixel's depth measured along the ray of its intensity.  A sensor whose depth comes from its own
+ * camera (time of flight, a stereo pair) some centimetres from the colour camera first has its depth registered: every depth
+ * pixel is moved into the colour camera, whose geometry the pyramids keep.
+ *
+ * dvo_b200_depth_rays: the ray tables of a depth camera of dw x dh pixels, in normalised coordinates (z = 1), rounded once
+ * to float.  Host only: no context, no GPU.  K_depth = fx, fy, cx, cy.  cx_ray / cy_ray [dh][dw]: the ray through pixel
+ * centre (u, v); kx_ray / ky_ray [dh+1][dw+1]: the ray through pixel corner (u - 0.5, v - 0.5), u in 0..dw, v in 0..dh.
+ *   dist == NULL (pinhole): x = (u - cx) / fx, y = (v - cy) / fy in double.
+ *   dist = k1, k2, p1, p2, k3 (OpenCV's plumb-bob model): the pixel's distorted coordinates xd = (u - cx) / fx,
+ *     yd = (v - cy) / fy are undistorted by Newton's method in double, from (x, y) = (xd, yd), per point, in this order (a*b+c
+ *     means (a*b)+c, products left to right, no fused multiply-add):
+ *       r2 = x*x + y*y;  R = 1 + ((k3*r2 + k2)*r2 + k1)*r2;  dR = k1 + (2*k2 + 3*k3*r2)*r2
+ *       ex = x*R + 2*p1*x*y + p2*(r2 + 2*x*x) - xd;  ey = y*R + p1*(r2 + 2*y*y) + 2*p2*x*y - yd
+ *       stop when |ex| < 1e-12 and |ey| < 1e-12; otherwise, after DVO_B200_DEPTH_RAYS_MAX_ITER updates, fail;
+ *       a = R + 2*x*x*dR + 2*p1*y + 6*p2*x;  b = 2*x*y*dR + 2*p1*x + 2*p2*y;  d = R + 2*y*y*dR + 6*p1*y + 2*p2*x
+ *       det = a*d - b*b;  x' = x - (d*ex - b*ey) / det;  y' = y - (a*ey - b*ex) / det
+ *   A NULL table or K_depth, dw or dh < 2, a non-finite K_depth or dist, fx or fy <= 0, or a point that does not converge
+ *   -> DVO_B200_ERR_INVALID_ARGUMENT (the tables are then undefined). */
+#define DVO_B200_DEPTH_RAYS_MAX_ITER 100
+int dvo_b200_depth_rays(int32_t dw, int32_t dh, const double K_depth[4], const double dist[5] /* NULL: pinhole */, float* cx_ray,
+                        float* cy_ray, float* kx_ray, float* ky_ray);
+/* A depth registration: a depth camera given by its ray tables (any camera model works through them, as any remap works
+ * through a rectifier's map), the rigid transform T_color_depth (row-major 4x4 double, p_color = T * p_depth, metres) and the
+ * target pinhole colour camera of width x height pixels and intrinsics K = fx, fy, cx, cy (level 0 of the pyramids).
+ *   The tables are HOST arrays as dvo_b200_depth_rays writes them; they are uploaded once to the context's device and the
+ *   call synchronises, so the caller's arrays may be freed when it returns.  dvo_b200_h2d_bytes grows by their
+ *   4 * (2*dw*dh + 2*(dw+1)*(dh+1)) bytes, once.  T is stored as float R (9 values) and t (3 values), each rounded once.
+ *   Refused with DVO_B200_ERR_INVALID_ARGUMENT: a NULL pointer, dw or dh < 2, a non-positive width or height, a non-finite
+ *   ray, T or K, fx or fy <= 0, a bottom row of T other than (0, 0, 0, 1), max|R^T R - I| > 1e-6 or det R <= 0.
+ *   A registration belongs to its context, and dvo_b200_depth_registration_release frees it in the context's stream order
+ *   with no host synchronisation, exactly as dvo_b200_rectifier_release does.  Release every registration of a context
+ *   before destroying the context. */
+typedef struct dvo_b200_depth_registration dvo_b200_depth_registration;
+int dvo_b200_depth_registration_create(dvo_b200_ctx* ctx, int32_t dw, int32_t dh, const float* cx_ray, const float* cy_ray,
+                                       const float* kx_ray, const float* ky_ray, const double T_color_depth[16], int32_t width,
+                                       int32_t height, const float K[4], dvo_b200_depth_registration** out);
+int dvo_b200_depth_registration_release(dvo_b200_depth_registration* reg);
+/* Registered creates.  In float32, every operation rounded to nearest (no fused multiply-add), for each depth pixel (u, v)
+ * of image i:
+ *   d: float32 metres as given, or u16 * depth_scale with 0 -> NaN as the raw creates convert; skipped unless d is finite
+ *     and d > 0.
+ *   For a ray (rx, ry): P = (rx*d, ry*d, d), Pc = R*P + t with each component ((r0*X + r1*Y) + r2*Z) + t.
+ *   The value is Zc of the centre ray; skipped unless Zc > 0.
+ *   Footprint: the four corner rays of the pixel project to x = fx*(Xc/Zc) + cx, y = fy*(Yc/Zc) + cy (divide, multiply,
+ *     add).  Skipped unless all four corners have Zc > 0 and every |x|, |y| < 2^20.  It covers the colour columns
+ *     ceil(xmin) .. ceil(xmax) - 1 and rows ceil(ymin) .. ceil(ymax) - 1 (half-open, so neighbours on a continuous surface
+ *     tile without cracks); skipped if either extent exceeds DVO_B200_REGISTRATION_MAX_FOOTPRINT; then clipped to the image.
+ *   Depth test: each colour pixel keeps the minimum Zc of the depth pixels that cover it, whatever their order.  A colour
+ *     pixel nothing covers gets NaN depth: it is never a point or a tap (the part of the scene the colour camera sees and
+ *     the depth camera does not).
+ * Intensity and masks (nonzero = usable) stay in the colour geometry:
+ *   rect == NULL: the colour frames are width x height = the registration's target size; the intensity is used as given
+ *     (float32, 8-bit grey converted exactly, BGR reduced as dvo_b200_pyramid_create_bgr_batch reduces it).
+ *   rect != NULL (a distorted colour camera): its output size and K_new equal the registration's target, width x height is
+ *     its input size, and intensity and masks go through its map with the rules of the rectified creates.  Depth comes from
+ *     the registration, never from the map.
+ * The pyramids equal, bit for bit, those of dvo_b200_pyramid_create_masked_batch_roles(FLOAT32) on the registered
+ * intensity and depth planes (and mask), with the registration's width x height and K.  With the identity registration
+ * (the same size, the pinhole rays of K, T = I) every colour pixel is covered by its own depth pixel alone and Zc = d, so
+ * the pyramids are those of the unregistered create of the same format.
+ * dvo_b200_pyramid_create_registered_batch: HOST pointers to n colour frames of width x height and n depth frames of the
+ *   registration's dw x dh, staged like dvo_b200_pyramid_create_masked_batch_roles (dvo_b200_h2d_bytes grows by the input
+ *   bytes only).
+ * dvo_b200_pyramid_create_registered_device_batch: dvo_b200_device_plane inputs, validated and ordered exactly as in
+ *   dvo_b200_pyramid_create_device_batch, the depth plane against dw x dh; nothing is copied from the host.
+ * A NULL ctx or registration, a registration or rectifier of another context, a colour size other than the target (or the
+ * rectifier's input size), a rectifier whose output size or K_new differs from the target, or any argument the
+ * corresponding unregistered call refuses -> DVO_B200_ERR_INVALID_ARGUMENT, and nothing is created. */
+#define DVO_B200_REGISTRATION_MAX_FOOTPRINT 8
+int dvo_b200_pyramid_create_registered_batch(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg,
+                                             const dvo_b200_rectifier* rect /* NULL: pinhole colour camera */, int32_t n,
+                                             int32_t format, const void* image, const void* depth, float depth_scale,
+                                             const uint8_t* masks, int32_t roles, int32_t width, int32_t height, int32_t levels,
+                                             dvo_b200_pyramid** out /* n handles */);
+int dvo_b200_pyramid_create_registered_device_batch(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg,
+                                                    const dvo_b200_rectifier* rect /* NULL: pinhole colour camera */, int32_t n,
+                                                    int32_t format, const dvo_b200_device_plane* image,
+                                                    const dvo_b200_device_plane* depth, float depth_scale,
+                                                    const dvo_b200_device_plane* masks /* NULL: no mask */, int32_t roles,
+                                                    int32_t width, int32_t height, int32_t levels,
+                                                    dvo_b200_pyramid** out /* n handles */);
 /* Role set a pyramid was created with: 0 (no mask), DVO_B200_MASK_ROLE_REFERENCE, or
  * DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT; DVO_B200_ERR_INVALID_ARGUMENT for a null handle. */
 int dvo_b200_pyramid_mask_roles(const dvo_b200_pyramid* p);
