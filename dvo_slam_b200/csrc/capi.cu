@@ -76,93 +76,6 @@ void convert_bgr(dvo_b200_ctx* ctx, int n, int w, int h, SrcPlane bgr, uint8_t* 
 
 }  // namespace
 
-// The last step of every create: build the pyramids from level-0 planes in device memory.  With a rectifier or a depth
-// registration, the planes are first remapped or registered into packed float32 planes (and, through a rectifier, byte
-// masks) in the staging memory at rect_off, which the caller has sized with rectified_bytes, and the build reads those with
-// the target's size and intrinsics.  Registered without a rectifier, the build reads the colour geometry's masks in place.
-static size_t rectified_bytes(const dvo_b200_rectifier* rect, const dvo_b200_depth_registration* reg, int n, bool masked) {
-  if (reg) return (size_t)reg->w * reg->h * n * (2 * sizeof(float) + (rect && masked ? 1 : 0));
-  return rect ? (size_t)rect->w * rect->h * n * (2 * sizeof(float) + (masked ? 1 : 0)) : 0;
-}
-
-static int build_planes(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, const dvo_b200_depth_registration* reg, size_t rect_off,
-                        int n, SrcPlane I, SrcPlane Z, int raw, float zscale, SrcPlane M, int roles, int width, int height, float fx,
-                        float fy, float ox, float oy, int levels, dvo_b200_pyramid** out) {
-  if (!rect && !reg)
-    return pyramid_build_batch_input(ctx, n, I, Z, raw, zscale, width, height, fx, fy, ox, oy, levels, 0.f, 0.f, out, M, roles);
-  const int w = reg ? reg->w : rect->w, h = reg ? reg->h : rect->h;
-  const float* K = reg ? reg->K : rect->K;
-  const size_t npx = (size_t)w * h * n;
-  float* dI = (float*)((char*)ctx->d_stage + rect_off);
-  float* dZ = dI + npx;
-  uint8_t* dM = rect && M.data ? (uint8_t*)(dZ + npx) : nullptr;
-  if (reg) {
-    if (int rc = register_batch(ctx, reg, rect, n, I, Z, raw, zscale, M, dI, dZ, dM)) return rc;
-  } else {
-    rectify_batch(ctx, rect, n, I, Z, raw, zscale, M, dI, dZ, dM);
-  }
-  const SrcPlane mask = rect ? (dM ? packed_plane(dM, w, h) : SrcPlane{nullptr, 0, 0}) : M;
-  return pyramid_build_batch_input(ctx, n, packed_plane(dI, w, h), packed_plane(dZ, w, h), 0, 0.f, w, h, K[0], K[1], K[2], K[3], levels,
-                                   0.f, 0.f, out, mask, roles);
-}
-
-// Uploads n frames of one dvo_b200_input_format (and their reference masks, if any) into the context's device staging
-// area and builds their pyramids from there, packed.  The frames stay in their file representation: the pyramid kernels
-// convert in their loads (no float32 copy of a raw frame is written); BGR is reduced to 8-bit grey first, as cv::cvtColor
-// leaves it.  Masks add one byte per pixel after the frames.  rect / reg: the rectified or registered planes follow the
-// upload; with reg the depth frames have the depth camera's dw x dh.
-static int create_staged(dvo_b200_ctx* ctx, int n, int format, const void* image, const void* depth, float depth_scale,
-                         const uint8_t* masks, int mask_roles, int width, int height, float fx, float fy, float ox, float oy,
-                         int levels, dvo_b200_pyramid** out, const dvo_b200_rectifier* rect = nullptr,
-                         const dvo_b200_depth_registration* reg = nullptr) {
-  cudaSetDevice(ctx->device);
-  const size_t npx = (size_t)width * height * n;
-  const int dw = reg ? reg->dw : width, dh = reg ? reg->dh : height;
-  const size_t dnpx = (size_t)dw * dh * n;         // depth pixels
-  size_t frames = 0, grey_off = 0, bgr_off = 0;   // bytes of the staged frames; offsets of the grey and BGR images
-  if (format == DVO_B200_INPUT_FLOAT32) {
-    frames = (npx + dnpx) * sizeof(float);
-  } else {
-    grey_off = (dnpx * 2 + 255) / 256 * 256;
-    bgr_off = grey_off + (npx + 255) / 256 * 256;
-    frames = (format == DVO_B200_INPUT_BGR8_DEPTH16 ? bgr_off + npx * 3 : grey_off + npx) + 64;
-  }
-  const size_t mask_off = (frames + 255) / 256 * 256;
-  const size_t rect_off = ((masks ? mask_off + npx : frames) + 255) / 256 * 256;
-  int rc = ensure_stage(ctx, rect || reg ? rect_off + rectified_bytes(rect, reg, n, masks != nullptr) : masks ? mask_off + npx : frames, 0);
-  if (rc) return rc;
-  char* stage = (char*)ctx->d_stage;
-  SrcPlane dM{nullptr, 0, 0};
-  if (masks) {
-    DVO_CUDA(ctx, cudaMemcpyAsync(stage + mask_off, masks, npx, cudaMemcpyHostToDevice, ctx->stream));
-    ctx->h2d_bytes += npx;
-    dM = packed_plane(stage + mask_off, width, height);
-  }
-  if (format == DVO_B200_INPUT_FLOAT32) {
-    float* dI = (float*)stage;
-    float* dZ = dI + npx;
-    DVO_CUDA(ctx, cudaMemcpyAsync(dI, image, npx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    DVO_CUDA(ctx, cudaMemcpyAsync(dZ, depth, dnpx * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    ctx->h2d_bytes += (npx + dnpx) * sizeof(float);
-    return build_planes(ctx, rect, reg, rect_off, n, packed_plane(dI, width, height), packed_plane(dZ, dw, dh), 0, 0.f, dM, mask_roles,
-                        width, height, fx, fy, ox, oy, levels, out);
-  }
-  uint16_t* dR = (uint16_t*)stage;
-  uint8_t* dG = (uint8_t*)(stage + grey_off);
-  DVO_CUDA(ctx, cudaMemcpyAsync(dR, depth, dnpx * 2, cudaMemcpyHostToDevice, ctx->stream));
-  if (format == DVO_B200_INPUT_GREY8_DEPTH16) {
-    DVO_CUDA(ctx, cudaMemcpyAsync(dG, image, npx, cudaMemcpyHostToDevice, ctx->stream));
-    ctx->h2d_bytes += npx + dnpx * 2;
-  } else {
-    uint8_t* dC = (uint8_t*)(stage + bgr_off);
-    DVO_CUDA(ctx, cudaMemcpyAsync(dC, image, npx * 3, cudaMemcpyHostToDevice, ctx->stream));
-    ctx->h2d_bytes += npx * 3 + dnpx * 2;
-    convert_bgr(ctx, n, width, height, packed_plane(dC, 3 * width, height), dG);
-  }
-  return build_planes(ctx, rect, reg, rect_off, n, packed_plane(dG, width, height), packed_plane(dR, dw, dh), 1, depth_scale, dM,
-                      mask_roles, width, height, fx, fy, ox, oy, levels, out);
-}
-
 // One dvo_b200_device_plane of n images of width x height pixels, elem bytes per element and per_px elements per pixel ->
 // the SrcPlane the pyramid kernels read.  Every check of the header's list; the pointer checks look at the first and the
 // last byte of the plane's extent.
@@ -199,36 +112,119 @@ static int device_plane(dvo_b200_ctx* ctx, const char* fn, const dvo_b200_device
 }
 
 
-// dvo_b200_pyramid_create_device_batch, and with a rectifier or a registration its rectified or registered form.  fn names
-// the entry point in the errors.
-static int create_device(dvo_b200_ctx* ctx, const char* fn, const dvo_b200_rectifier* rect, int n, int format,
-                         const dvo_b200_device_plane* image, const dvo_b200_device_plane* depth, float depth_scale,
-                         const dvo_b200_device_plane* masks, int roles, int width, int height, float fx, float fy, float ox, float oy,
-                         int levels, dvo_b200_pyramid** out, const dvo_b200_depth_registration* reg = nullptr) {
-  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": null/invalid argument");
-  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": unknown input format " + std::to_string(format));
-  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": unsupported role set " + std::to_string(roles));
+// The context's staging memory for one create, in 256-byte aligned sections: the uploaded frames (depth, then the image, then
+// 64 bytes of slack), the uploaded masks, the grey reduced from BGR, then the remapped or registered planes (float32
+// intensity and depth of level 0 and, through a rectifier, its byte masks).  A section the call does not need has size 0;
+// a device create uploads nothing.
+struct StageLayout {
+  size_t image, masks, grey, remap, total;   // byte offsets (the depth frames start at 0) and the bytes of all sections
+};
+
+static StageLayout stage_layout(const CreateArgs& a, int w0, int h0) {
+  auto up = [](size_t v) { return (v + 255) / 256 * 256; };
+  const bool f32 = a.format == DVO_B200_INPUT_FLOAT32, bgr = a.format == DVO_B200_INPUT_BGR8_DEPTH16;
+  const bool masked = a.device ? a.mask_plane != nullptr : a.masks != nullptr;
+  const size_t npx = (size_t)a.width * a.height * a.n;
+  const size_t dnpx = a.reg ? (size_t)a.reg->dw * a.reg->dh * a.n : npx;
+  StageLayout s{};
+  size_t end = 0;
+  if (!a.device) {
+    s.image = up(dnpx * (f32 ? 4 : 2));
+    end = s.image + npx * (f32 ? 4 : bgr ? 3 : 1) + 64;
+    s.masks = up(end);
+    if (masked) end = s.masks + npx;
+  }
+  s.grey = up(end);
+  if (bgr) end = s.grey + npx;
+  s.remap = up(end);
+  if (a.rect || a.reg) end = s.remap + (size_t)w0 * h0 * a.n * (2 * sizeof(float) + (a.rect && masked ? 1 : 0));
+  s.total = end;
+  return s;
+}
+
+// Every create: the checks of create_args.h and the device planes' before any device work, then the upload into staging
+// (host forms), the BGR reduction, the remap or registration, and the build.  The frames stay in their file representation:
+// the pyramid kernels convert in their loads (no float32 copy of a raw frame is written); BGR is reduced to 8-bit grey
+// first, as cv::cvtColor leaves it.  Device planes are read in place.
+static int create_pyramids(dvo_b200_ctx* ctx, const CreateArgs& a, dvo_b200_pyramid** out) {
+  const std::string why = create_args_error(ctx, a, out);
+  if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
   cudaSetDevice(ctx->device);
-  const bool f32 = format == DVO_B200_INPUT_FLOAT32;
+  const bool f32 = a.format == DVO_B200_INPUT_FLOAT32, bgr = a.format == DVO_B200_INPUT_BGR8_DEPTH16;
+  const int n = a.n, w = a.width, h = a.height;
+  const int dw = a.reg ? a.reg->dw : w, dh = a.reg ? a.reg->dh : h;   // with a registration, depth has the depth camera's size
   SrcPlane I, Z, M{nullptr, 0, 0};
-  int rc = device_plane(ctx, fn, image, "image", f32 ? 4 : 1, format == DVO_B200_INPUT_BGR8_DEPTH16 ? 3 : 1, n, width, height, &I);
-  if (!rc) rc = device_plane(ctx, fn, depth, "depth", f32 ? 4 : 2, 1, n, reg ? reg->dw : width, reg ? reg->dh : height, &Z);
-  if (!rc && masks) rc = device_plane(ctx, fn, masks, "masks", 1, 1, n, width, height, &M);
-  if (rc) return rc;
-  const size_t grey = format == DVO_B200_INPUT_BGR8_DEPTH16 ? (size_t)width * height * n : 0;   // BGR reduced to grey in staging
-  const size_t rect_off = (grey + 255) / 256 * 256;
-  if (grey || rect || reg) {
-    if ((rc = ensure_stage(ctx, rect || reg ? rect_off + rectified_bytes(rect, reg, n, masks != nullptr) : grey, 0))) return rc;
+  if (a.device) {
+    int rc = device_plane(ctx, a.fn, a.image_plane, "image", f32 ? 4 : 1, bgr ? 3 : 1, n, w, h, &I);
+    if (!rc) rc = device_plane(ctx, a.fn, a.depth_plane, "depth", f32 ? 4 : 2, 1, n, dw, dh, &Z);
+    if (!rc && a.mask_plane) rc = device_plane(ctx, a.fn, a.mask_plane, "masks", 1, 1, n, w, h, &M);
+    if (rc) return rc;
   }
-  if (grey) {   // grey into staging, as the host path; depth and masks stay in place
-    convert_bgr(ctx, n, width, height, I, (uint8_t*)ctx->d_stage);
-    I = packed_plane(ctx->d_stage, width, height);
+  int w0, h0;
+  const float* K;
+  create_level0(a, &w0, &h0, &K);
+  const StageLayout s = stage_layout(a, w0, h0);
+  if (int rc = ensure_stage(ctx, s.total, 0)) return rc;
+  char* stage = (char*)ctx->d_stage;
+  if (!a.device) {
+    const size_t npx = (size_t)w * h * n;
+    const size_t zbytes = (size_t)dw * dh * n * (f32 ? 4 : 2), ibytes = npx * (f32 ? 4 : bgr ? 3 : 1);
+    DVO_CUDA(ctx, cudaMemcpyAsync(stage, a.depth, zbytes, cudaMemcpyHostToDevice, ctx->stream));
+    DVO_CUDA(ctx, cudaMemcpyAsync(stage + s.image, a.image, ibytes, cudaMemcpyHostToDevice, ctx->stream));
+    ctx->h2d_bytes += zbytes + ibytes;
+    Z = packed_plane(stage, dw, dh);
+    I = packed_plane(stage + s.image, bgr ? 3 * w : w, h);
+    if (a.masks) {
+      DVO_CUDA(ctx, cudaMemcpyAsync(stage + s.masks, a.masks, npx, cudaMemcpyHostToDevice, ctx->stream));
+      ctx->h2d_bytes += npx;
+      M = packed_plane(stage + s.masks, w, h);
+    }
   }
-  return build_planes(ctx, rect, reg, rect_off, n, I, Z, f32 ? 0 : 1, f32 ? 0.f : depth_scale, M, roles, width, height, fx, fy, ox, oy,
-                      levels, out);
+  if (bgr) {
+    convert_bgr(ctx, n, w, h, I, (uint8_t*)stage + s.grey);
+    I = packed_plane(stage + s.grey, w, h);
+  }
+  int raw = f32 ? 0 : 1;
+  float zscale = f32 ? 0.f : a.depth_scale;
+  if (a.rect || a.reg) {   // the build reads the packed float32 planes of level 0 (and the remapped masks through a rectifier)
+    const size_t npx0 = (size_t)w0 * h0 * n;
+    float* dI = (float*)(stage + s.remap);
+    float* dZ = dI + npx0;
+    uint8_t* dM = a.rect && M.data ? (uint8_t*)(dZ + npx0) : nullptr;
+    if (int rc = remap_batch(ctx, a.rect, a.reg, n, I, Z, raw, zscale, M, dI, dZ, dM)) return rc;
+    I = packed_plane(dI, w0, h0);
+    Z = packed_plane(dZ, w0, h0);
+    raw = 0;
+    zscale = 0.f;
+    if (a.rect) M = dM ? packed_plane(dM, w0, h0) : SrcPlane{nullptr, 0, 0};
+  }
+  return pyramid_build_batch_input(ctx, n, I, Z, raw, zscale, w0, h0, K, a.levels, out, M, a.roles);
+}
+
+static CreateArgs host_args(const char* fn, int n, int format, const void* image, const void* depth, float depth_scale,
+                            const uint8_t* masks, int roles, int width, int height, int levels) {
+  CreateArgs a;
+  a.fn = fn; a.n = n; a.format = format; a.image = image; a.depth = depth; a.depth_scale = depth_scale; a.masks = masks;
+  a.roles = roles; a.width = width; a.height = height; a.levels = levels;
+  return a;
+}
+
+static CreateArgs device_args(const char* fn, int n, int format, const dvo_b200_device_plane* image, const dvo_b200_device_plane* depth,
+                              float depth_scale, const dvo_b200_device_plane* masks, int roles, int width, int height, int levels) {
+  CreateArgs a = host_args(fn, n, format, nullptr, nullptr, depth_scale, nullptr, roles, width, height, levels);
+  a.device = true; a.image_plane = image; a.depth_plane = depth; a.mask_plane = masks;
+  return a;
+}
+
+static CreateArgs with_K(CreateArgs a, float fx, float fy, float ox, float oy) {
+  a.K[0] = fx; a.K[1] = fy; a.K[2] = ox; a.K[3] = oy;
+  return a;
+}
+
+static CreateArgs with_remap(CreateArgs a, int remap, const dvo_b200_rectifier* rect, const dvo_b200_depth_registration* reg) {
+  a.remap = remap;
+  a.rect = rect; a.reg = reg;
+  return a;
 }
 
 }  // namespace dvo_b200
@@ -322,9 +318,8 @@ int dvo_b200_get_estimator(const dvo_b200_ctx* ctx) { return ctx ? ctx->estimato
 int dvo_b200_pyramid_create_batch(dvo_b200_ctx* ctx, int32_t n, const float* intensity, const float* depth, int32_t width,
                                   int32_t height, float fx, float fy, float ox, float oy, int32_t levels,
                                   dvo_b200_pyramid** out) {
-  if (!ctx || !intensity || !depth || !out || n <= 0 || width <= 0 || height <= 0)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create: null/invalid argument");
-  return create_staged(ctx, n, DVO_B200_INPUT_FLOAT32, intensity, depth, 0.f, nullptr, 0, width, height, fx, fy, ox, oy, levels, out);
+  return create_pyramids(ctx, with_K(host_args("pyramid_create", n, DVO_B200_INPUT_FLOAT32, intensity, depth, 0.f, nullptr,
+                                               DVO_B200_MASK_ROLE_REFERENCE, width, height, levels), fx, fy, ox, oy), out);
 }
 
 int dvo_b200_pyramid_create(dvo_b200_ctx* ctx, const float* intensity, const float* depth, int32_t width, int32_t height,
@@ -335,51 +330,38 @@ int dvo_b200_pyramid_create(dvo_b200_ctx* ctx, const float* intensity, const flo
 int dvo_b200_pyramid_create_raw_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_t* grey, const uint16_t* raw_depth,
                                       float depth_scale, int32_t width, int32_t height, float fx, float fy, float ox,
                                       float oy, int32_t levels, dvo_b200_pyramid** out) {
-  if (!ctx || !grey || !raw_depth || !out || n <= 0 || width <= 0 || height <= 0)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_raw: null/invalid argument");
-  return create_staged(ctx, n, DVO_B200_INPUT_GREY8_DEPTH16, grey, raw_depth, depth_scale, nullptr, 0, width, height, fx, fy, ox, oy,
-                       levels, out);
+  return create_pyramids(ctx, with_K(host_args("pyramid_create_raw", n, DVO_B200_INPUT_GREY8_DEPTH16, grey, raw_depth, depth_scale,
+                                               nullptr, DVO_B200_MASK_ROLE_REFERENCE, width, height, levels), fx, fy, ox, oy), out);
 }
 
 int dvo_b200_pyramid_create_bgr_batch(dvo_b200_ctx* ctx, int32_t n, const uint8_t* bgr, const uint16_t* raw_depth,
                                       float depth_scale, int32_t width, int32_t height, float fx, float fy, float ox,
                                       float oy, int32_t levels, dvo_b200_pyramid** out) {
-  if (!ctx || !bgr || !raw_depth || !out || n <= 0 || width <= 0 || height <= 0)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_bgr: null/invalid argument");
-  return create_staged(ctx, n, DVO_B200_INPUT_BGR8_DEPTH16, bgr, raw_depth, depth_scale, nullptr, 0, width, height, fx, fy, ox, oy,
-                       levels, out);
+  return create_pyramids(ctx, with_K(host_args("pyramid_create_bgr", n, DVO_B200_INPUT_BGR8_DEPTH16, bgr, raw_depth, depth_scale,
+                                               nullptr, DVO_B200_MASK_ROLE_REFERENCE, width, height, levels), fx, fy, ox, oy), out);
 }
 
 int dvo_b200_pyramid_create_masked_batch(dvo_b200_ctx* ctx, int32_t n, int32_t format, const void* image, const void* depth,
                                          float depth_scale, const uint8_t* masks, int32_t width, int32_t height, float fx,
                                          float fy, float ox, float oy, int32_t levels, dvo_b200_pyramid** out) {
-  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked: null/invalid argument");
-  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked: unknown input format " + std::to_string(format));
-  return create_staged(ctx, n, format, image, depth, depth_scale, masks, DVO_B200_MASK_ROLE_REFERENCE, width, height, fx, fy, ox,
-                       oy, levels, out);
+  return create_pyramids(ctx, with_K(host_args("pyramid_create_masked", n, format, image, depth, depth_scale, masks,
+                                               DVO_B200_MASK_ROLE_REFERENCE, width, height, levels), fx, fy, ox, oy), out);
 }
 
 int dvo_b200_pyramid_create_masked_batch_roles(dvo_b200_ctx* ctx, int32_t n, int32_t format, const void* image,
                                                const void* depth, float depth_scale, const uint8_t* masks, int32_t roles,
                                                int32_t width, int32_t height, float fx, float fy, float ox, float oy,
                                                int32_t levels, dvo_b200_pyramid** out) {
-  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked_roles: null/invalid argument");
-  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked_roles: unknown input format " + std::to_string(format));
-  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_masked_roles: unsupported role set " + std::to_string(roles));
-  return create_staged(ctx, n, format, image, depth, depth_scale, masks, roles, width, height, fx, fy, ox, oy, levels, out);
+  return create_pyramids(ctx, with_K(host_args("pyramid_create_masked_roles", n, format, image, depth, depth_scale, masks, roles,
+                                               width, height, levels), fx, fy, ox, oy), out);
 }
 
 int dvo_b200_pyramid_create_device_batch(dvo_b200_ctx* ctx, int32_t n, int32_t format, const dvo_b200_device_plane* image,
                                          const dvo_b200_device_plane* depth, float depth_scale, const dvo_b200_device_plane* masks,
                                          int32_t roles, int32_t width, int32_t height, float fx, float fy, float ox, float oy,
                                          int32_t levels, dvo_b200_pyramid** out) {
-  return create_device(ctx, "pyramid_create_device", nullptr, n, format, image, depth, depth_scale, masks, roles, width, height, fx, fy,
-                       ox, oy, levels, out);
+  return create_pyramids(ctx, with_K(device_args("pyramid_create_device", n, format, image, depth, depth_scale, masks, roles, width,
+                                                 height, levels), fx, fy, ox, oy), out);
 }
 
 int dvo_b200_undistort_map(int32_t width, int32_t height, const double K[4], const double dist[5], const double K_new[4],
@@ -440,38 +422,19 @@ int dvo_b200_rectifier_release(dvo_b200_rectifier* r) {
   return rc;
 }
 
-// The rectifier's checks shared by both rectified creates: it exists, belongs to ctx and takes frames of width x height.
-static int check_rectifier(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, int width, int height, const char* fn) {
-  if (!rect) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": null rectifier");
-  if (rect->ctx != ctx) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": the rectifier belongs to another context");
-  if (width != rect->in_w || height != rect->in_h)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": frames of " + std::to_string(width) + "x" +
-                                                             std::to_string(height) + ", the rectifier takes " + std::to_string(rect->in_w) +
-                                                             "x" + std::to_string(rect->in_h));
-  return 0;
-}
-
 int dvo_b200_pyramid_create_rectified_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, int32_t n, int32_t format,
                                             const void* image, const void* depth, float depth_scale, const uint8_t* masks,
                                             int32_t roles, int32_t width, int32_t height, int32_t levels, dvo_b200_pyramid** out) {
-  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_rectified: null/invalid argument");
-  if (int rc = check_rectifier(ctx, rect, width, height, "pyramid_create_rectified")) return rc;
-  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_rectified: unknown input format " + std::to_string(format));
-  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_rectified: unsupported role set " + std::to_string(roles));
-  return create_staged(ctx, n, format, image, depth, depth_scale, masks, roles, width, height, 0.f, 0.f, 0.f, 0.f, levels, out, rect);
+  return create_pyramids(ctx, with_remap(host_args("pyramid_create_rectified", n, format, image, depth, depth_scale, masks, roles,
+                                                   width, height, levels), kRemapRectify, rect, nullptr), out);
 }
 
 int dvo_b200_pyramid_create_rectified_device_batch(dvo_b200_ctx* ctx, const dvo_b200_rectifier* rect, int32_t n, int32_t format,
                                                    const dvo_b200_device_plane* image, const dvo_b200_device_plane* depth,
                                                    float depth_scale, const dvo_b200_device_plane* masks, int32_t roles, int32_t width,
                                                    int32_t height, int32_t levels, dvo_b200_pyramid** out) {
-  if (!ctx) return DVO_B200_ERR_INVALID_ARGUMENT;
-  if (int rc = check_rectifier(ctx, rect, width, height, "pyramid_create_rectified_device")) return rc;
-  return create_device(ctx, "pyramid_create_rectified_device", rect, n, format, image, depth, depth_scale, masks, roles, width, height,
-                       0.f, 0.f, 0.f, 0.f, levels, out);
+  return create_pyramids(ctx, with_remap(device_args("pyramid_create_rectified_device", n, format, image, depth, depth_scale, masks,
+                                                     roles, width, height, levels), kRemapRectify, rect, nullptr), out);
 }
 
 int dvo_b200_depth_rays(int32_t dw, int32_t dh, const double K[4], const double dist[5], float* cx_ray, float* cy_ray, float* kx_ray,
@@ -581,37 +544,12 @@ int dvo_b200_depth_registration_release(dvo_b200_depth_registration* r) {
   return rc;
 }
 
-// The checks shared by both registered creates: the registration exists and belongs to ctx; without a rectifier the colour
-// frames have its target size; with one, the rectifier passes check_rectifier and its output is the target.
-static int check_registration(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg, const dvo_b200_rectifier* rect, int width,
-                              int height, const char* fn) {
-  auto bad = [&](const std::string& why) { return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, std::string(fn) + ": " + why); };
-  if (!reg) return bad("null depth registration");
-  if (reg->ctx != ctx) return bad("the depth registration belongs to another context");
-  const std::string target = std::to_string(reg->w) + "x" + std::to_string(reg->h);
-  if (rect) {
-    if (int rc = check_rectifier(ctx, rect, width, height, fn)) return rc;
-    if (rect->w != reg->w || rect->h != reg->h) return bad("the rectifier's output is not the registration's target " + target);
-    for (int i = 0; i < 4; ++i)
-      if (rect->K[i] != reg->K[i]) return bad("the rectifier's K_new is not the registration's K");
-  } else if (width != reg->w || height != reg->h) {
-    return bad("colour frames of " + std::to_string(width) + "x" + std::to_string(height) + ", the registration's target is " + target);
-  }
-  return 0;
-}
-
 int dvo_b200_pyramid_create_registered_batch(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg, const dvo_b200_rectifier* rect,
                                              int32_t n, int32_t format, const void* image, const void* depth, float depth_scale,
                                              const uint8_t* masks, int32_t roles, int32_t width, int32_t height, int32_t levels,
                                              dvo_b200_pyramid** out) {
-  if (!ctx || !image || !depth || !out || n <= 0 || width <= 0 || height <= 0)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_registered: null/invalid argument");
-  if (int rc = check_registration(ctx, reg, rect, width, height, "pyramid_create_registered")) return rc;
-  if (format != DVO_B200_INPUT_FLOAT32 && format != DVO_B200_INPUT_GREY8_DEPTH16 && format != DVO_B200_INPUT_BGR8_DEPTH16)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_registered: unknown input format " + std::to_string(format));
-  if (roles != DVO_B200_MASK_ROLE_REFERENCE && roles != (DVO_B200_MASK_ROLE_REFERENCE | DVO_B200_MASK_ROLE_CURRENT))
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "pyramid_create_registered: unsupported role set " + std::to_string(roles));
-  return create_staged(ctx, n, format, image, depth, depth_scale, masks, roles, width, height, 0.f, 0.f, 0.f, 0.f, levels, out, rect, reg);
+  return create_pyramids(ctx, with_remap(host_args("pyramid_create_registered", n, format, image, depth, depth_scale, masks, roles,
+                                                   width, height, levels), kRemapRegister, rect, reg), out);
 }
 
 int dvo_b200_pyramid_create_registered_device_batch(dvo_b200_ctx* ctx, const dvo_b200_depth_registration* reg,
@@ -619,10 +557,8 @@ int dvo_b200_pyramid_create_registered_device_batch(dvo_b200_ctx* ctx, const dvo
                                                     const dvo_b200_device_plane* image, const dvo_b200_device_plane* depth,
                                                     float depth_scale, const dvo_b200_device_plane* masks, int32_t roles, int32_t width,
                                                     int32_t height, int32_t levels, dvo_b200_pyramid** out) {
-  if (!ctx) return DVO_B200_ERR_INVALID_ARGUMENT;
-  if (int rc = check_registration(ctx, reg, rect, width, height, "pyramid_create_registered_device")) return rc;
-  return create_device(ctx, "pyramid_create_registered_device", rect, n, format, image, depth, depth_scale, masks, roles, width, height,
-                       0.f, 0.f, 0.f, 0.f, levels, out, reg);
+  return create_pyramids(ctx, with_remap(device_args("pyramid_create_registered_device", n, format, image, depth, depth_scale, masks,
+                                                     roles, width, height, levels), kRemapRegister, rect, reg), out);
 }
 
 int dvo_b200_pyramid_mask_roles(const dvo_b200_pyramid* p) { return p ? p->mask_roles : DVO_B200_ERR_INVALID_ARGUMENT; }

@@ -124,6 +124,55 @@ def device_planes(image, depth, masks=None, depth_size=None):
     return fmt, (n, h, w), plane(image, "image", px), plane(depth, "depth", 1), pm
 
 
+def _host_frames(image, depth, depth_size=None):
+    """Host arrays of n frames -> (format, (n, h, w), image, depth) with C-contiguous arrays, the format from the dtypes:
+        float32 [n,h,w] image + float32 depth, uint8 [n,h,w] grey + uint16 raw depth, uint8 [n,h,w,3] BGR + uint16 raw depth.
+    depth: [n,h,w], or [n,dh,dw] with depth_size = (dw, dh).  Raises ValueError for anything else."""
+    image, depth = np.asarray(image), np.asarray(depth)
+    if image.dtype == np.float32 and image.ndim == 3 and depth.dtype == np.float32:
+        fmt = "float32"
+    elif image.dtype == np.uint8 and image.ndim == 3 and depth.dtype == np.uint16:
+        fmt = "grey8_depth16"
+    elif image.dtype == np.uint8 and image.ndim == 4 and image.shape[3] == 3 and depth.dtype == np.uint16:
+        fmt = "bgr8_depth16"
+    else:
+        raise ValueError(f"image {image.dtype} {image.shape} with depth {depth.dtype}: want float32 [n,h,w] + float32, uint8 "
+                         "[n,h,w] + uint16 or uint8 [n,h,w,3] + uint16")
+    n, h, w = image.shape[:3]
+    dw, dh = (w, h) if depth_size is None else depth_size
+    if depth.shape != (n, dh, dw):
+        raise ValueError(f"depth {depth.shape}, want {(n, dh, dw)}" + ("" if depth_size is None else " (the depth camera's size)"))
+    return fmt, (n, h, w), np.ascontiguousarray(image), np.ascontiguousarray(depth)
+
+
+def _depth_scale(fmt, depth_scale) -> float:
+    """depth_scale as the creates take it: required with raw depth"""
+    if fmt != "float32" and depth_scale is None:
+        raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
+    return float(depth_scale or 0.0)
+
+
+def _host_masks(masks, n, h, w):
+    """Host masks of n images of h x w -> (pointer, array): an int is a host pointer to n*h*w bytes (array None); an array
+    of [h, w] is one mask for the whole batch; any other array must hold n*h*w values (nonzero = usable).  The array is the
+    caller's own when it is C-contiguous uint8, else a converted copy that must outlive the create's upload."""
+    if isinstance(masks, int):
+        return masks, None
+    M = np.asarray(masks)
+    if M.size != n * h * w:
+        if M.shape != (h, w):
+            raise ValueError(f"masks {M.shape} for {n} images of {h}x{w}: want {(n, h, w)}, {(h, w)} or {n * h * w} values")
+        M = np.broadcast_to(M, (n, h, w))
+    M = np.ascontiguousarray(M if M.dtype == np.uint8 else M != 0, dtype=np.uint8)
+    return M.ctypes.data, M
+
+
+def _mask_roles(mask_roles) -> int:
+    if mask_roles not in MASK_ROLES:
+        raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
+    return MASK_ROLES[mask_roles]
+
+
 class IterationStats(C.Structure):
     _fields_ = [("level", C.c_int32), ("id", C.c_int32), ("valid_constraints", C.c_int64),
                 ("tdist_log_likelihood", C.c_double), ("tdist_precision", C.c_double * 4),
@@ -443,25 +492,18 @@ class Engine:
 
     # ---- pyramids ----
     # mask= / masks=: reference masks (dvo_b200_pyramid_create_masked_batch): None, an array of n*h*w values (nonzero = usable
-    # reference pixel; shape [h, w] or [n, h, w]) or, for the host-pointer forms, a host pointer (int) to n*h*w bytes.
+    # reference pixel; shape [n, h, w], or [h, w] for one mask of the whole batch) or, for the host-pointer forms, a host
+    # pointer (int) to n*h*w bytes.
     # mask_roles="reference" (default): the mask keeps its pixels out of the point selection; "both": also out of the
     # bilinear taps when the pyramid is the current image of an alignment (dvo_b200_pyramid_create_masked_batch_roles).
     def _create_masked(self, n, fmt, pI, pZ, depth_scale, masks, w, h, intrinsics, levels, mask_roles="reference") -> list[Pyramid]:
-        if mask_roles not in MASK_ROLES:
-            raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
-        keep = None
-        if isinstance(masks, int):
-            pM = masks
-        else:
-            keep = np.asarray(masks)
-            keep = np.ascontiguousarray(keep if keep.dtype == np.uint8 else (keep != 0).astype(np.uint8))
-            assert keep.size == n * h * w, f"masks: {keep.shape} for {n} images of {h}x{w}"
-            pM = keep.ctypes.data
+        roles = _mask_roles(mask_roles)
+        pM, M = _host_masks(masks, n, h, w)
         fx, fy, ox, oy = intrinsics
         out = (C.c_void_p * n)()
         self._check(self.lib.dvo_b200_pyramid_create_masked_batch_roles(self.ctx, n, INPUT_FORMATS[fmt], pI, pZ, depth_scale, pM,
-                                                                        MASK_ROLES[mask_roles], w, h, fx, fy, ox, oy, levels, out))
-        if keep is not None and keep is not masks:
+                                                                        roles, w, h, fx, fy, ox, oy, levels, out))
+        if M is not None and M is not masks:
             self.synchronize()   # the converted copy dies with this call
         return [Pyramid(self, out[i]) for i in range(n)]
 
@@ -536,12 +578,19 @@ class Engine:
         depth_scale (metres per raw depth unit) is required for uint16 depth.  masks / mask_roles as in pyramid_batch.
         Ordered with torch: the engine's stream waits for the current stream before the build, and the current stream waits
         for the build after it, so the inputs may be produced and overwritten on the current stream."""
+        roles = _mask_roles(mask_roles)
+        fx, fy, ox, oy = intrinsics
+        return self._create_device(image, depth, masks, depth_scale, None, lambda n, fmt, I, Z, scale, M, w, h, out:
+                                   self.lib.dvo_b200_pyramid_create_device_batch(self.ctx, n, fmt, I, Z, scale, M, roles, w, h, fx, fy,
+                                                                                 ox, oy, levels, out))
+
+    def _create_device(self, image, depth, masks, depth_scale, depth_size, create) -> list[Pyramid]:
+        """A device create from torch CUDA tensors (device_planes), ordered with torch's current stream: the engine's stream
+        waits for it, the tensors' memory is kept until the build has read it, and the current stream waits for the build.
+        create(n, format, image, depth, depth_scale, masks, w, h, out) calls the entry point with the planes."""
         import torch
-        if mask_roles not in MASK_ROLES:
-            raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
-        fmt, (n, h, w), pI, pZ, pM = device_planes(image, depth, masks)
-        if fmt != "float32" and depth_scale is None:
-            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
+        fmt, (n, h, w), pI, pZ, pM = device_planes(image, depth, masks, depth_size=depth_size)
+        scale = _depth_scale(fmt, depth_scale)
         dev = torch.device("cuda", self.device)
         inputs = [t for t in (image, depth, masks) if t is not None]
         for t in inputs:
@@ -549,16 +598,13 @@ class Engine:
                 raise ValueError(f"a tensor on {t.device}: the engine runs on {dev}")
         I, Z = DevicePlane(*pI), DevicePlane(*pZ)
         M = DevicePlane(*pM) if pM is not None else None
-        fx, fy, ox, oy = intrinsics
         out = (C.c_void_p * n)()
         current = torch.cuda.current_stream(dev)
         ext = torch.cuda.ExternalStream(self.stream, device=dev)
         ext.wait_stream(current)
         for t in inputs:
             t.record_stream(ext)     # the caching allocator keeps the memory until the build has read it
-        rc = self.lib.dvo_b200_pyramid_create_device_batch(self.ctx, n, INPUT_FORMATS[fmt], C.byref(I), C.byref(Z),
-                                                           float(depth_scale or 0.0), C.byref(M) if M is not None else None,
-                                                           MASK_ROLES[mask_roles], w, h, fx, fy, ox, oy, levels, out)
+        rc = create(n, INPUT_FORMATS[fmt], C.byref(I), C.byref(Z), scale, C.byref(M) if M is not None else None, w, h, out)
         current.wait_stream(ext)
         self._check(rc)
         return [Pyramid(self, out[i]) for i in range(n)]
@@ -593,64 +639,32 @@ class Engine:
         stream as in pyramid_batch_device, without a host synchronisation.  depth_scale (metres per raw unit) is required
         with uint16 depth.  masks ([n,h,w] or [h,w], nonzero = usable, in the input geometry) / mask_roles as in
         pyramid_batch."""
-        if mask_roles not in MASK_ROLES:
-            raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
-        if not isinstance(image, np.ndarray) and hasattr(image, "is_cuda") and image.is_cuda:
-            return self._rectified_device(rect, image, depth, levels, depth_scale, masks, mask_roles)
-        image, depth = np.asarray(image), np.asarray(depth)
-        if image.dtype == np.float32 and image.ndim == 3 and depth.dtype == np.float32:
-            fmt = "float32"
-        elif image.dtype == np.uint8 and image.ndim == 3 and depth.dtype == np.uint16:
-            fmt = "grey8_depth16"
-        elif image.dtype == np.uint8 and image.ndim == 4 and image.shape[3] == 3 and depth.dtype == np.uint16:
-            fmt = "bgr8_depth16"
-        else:
-            raise ValueError(f"image {image.dtype} {image.shape} with depth {depth.dtype}: want float32 [n,h,w] + float32, uint8 "
-                             "[n,h,w] + uint16 or uint8 [n,h,w,3] + uint16")
-        n, h, w = image.shape[:3]
-        if depth.shape != (n, h, w):
-            raise ValueError(f"depth {depth.shape}, want {(n, h, w)}")
-        if fmt != "float32" and depth_scale is None:
-            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
-        I, Z = np.ascontiguousarray(image), np.ascontiguousarray(depth)
-        M = None
-        if masks is not None:
-            M = np.asarray(masks)
-            M = np.broadcast_to(M, (n, h, w)) if M.shape == (h, w) else M
-            if M.shape != (n, h, w):
-                raise ValueError(f"masks {M.shape}, want {(n, h, w)} or {(h, w)}")
-            M = np.ascontiguousarray(M if M.dtype == np.uint8 else M != 0, dtype=np.uint8)
-        out = (C.c_void_p * n)()
-        self._check(self.lib.dvo_b200_pyramid_create_rectified_batch(self.ctx, rect.handle, n, INPUT_FORMATS[fmt], I.ctypes.data,
-                                                                     Z.ctypes.data, float(depth_scale or 0.0),
-                                                                     M.ctypes.data if M is not None else None, MASK_ROLES[mask_roles],
-                                                                     w, h, levels, out))
-        self.synchronize()   # the staged host arrays may die with this call
-        return [Pyramid(self, out[i]) for i in range(n)]
+        return self._create_remapped(rect, None, image, depth, levels, depth_scale, masks, mask_roles)
 
-    def _rectified_device(self, rect, image, depth, levels, depth_scale, masks, mask_roles):
-        import torch
-        fmt, (n, h, w), pI, pZ, pM = device_planes(image, depth, masks)
-        if fmt != "float32" and depth_scale is None:
-            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
-        dev = torch.device("cuda", self.device)
-        inputs = [t for t in (image, depth, masks) if t is not None]
-        for t in inputs:
-            if t.device != dev:
-                raise ValueError(f"a tensor on {t.device}: the engine runs on {dev}")
-        I, Z = DevicePlane(*pI), DevicePlane(*pZ)
-        M = DevicePlane(*pM) if pM is not None else None
+    def _create_remapped(self, rect, reg, image, depth, levels, depth_scale, masks, mask_roles) -> list[Pyramid]:
+        """pyramid_rectified_batch (reg None) and pyramid_registered_batch (rect None or a Rectifier), from host arrays or
+        torch CUDA tensors"""
+        roles = _mask_roles(mask_roles)
+        rh = rect.handle if rect is not None else None
+        depth_size = reg.depth_size if reg is not None else None
+        if not isinstance(image, np.ndarray) and hasattr(image, "is_cuda") and image.is_cuda:
+            if reg is None:
+                create = lambda n, fmt, I, Z, scale, M, w, h, out: self.lib.dvo_b200_pyramid_create_rectified_device_batch(
+                    self.ctx, rh, n, fmt, I, Z, scale, M, roles, w, h, levels, out)
+            else:
+                create = lambda n, fmt, I, Z, scale, M, w, h, out: self.lib.dvo_b200_pyramid_create_registered_device_batch(
+                    self.ctx, reg.handle, rh, n, fmt, I, Z, scale, M, roles, w, h, levels, out)
+            return self._create_device(image, depth, masks, depth_scale, depth_size, create)
+        fmt, (n, h, w), I, Z = _host_frames(image, depth, depth_size)
+        scale = _depth_scale(fmt, depth_scale)
+        pM, M = _host_masks(masks, n, h, w) if masks is not None else (None, None)   # M: kept until the upload is done
+        args = (n, INPUT_FORMATS[fmt], I.ctypes.data, Z.ctypes.data, scale, pM, roles, w, h, levels)
         out = (C.c_void_p * n)()
-        current = torch.cuda.current_stream(dev)
-        ext = torch.cuda.ExternalStream(self.stream, device=dev)
-        ext.wait_stream(current)
-        for t in inputs:
-            t.record_stream(ext)     # the caching allocator keeps the memory until the build has read it
-        rc = self.lib.dvo_b200_pyramid_create_rectified_device_batch(self.ctx, rect.handle, n, INPUT_FORMATS[fmt], C.byref(I), C.byref(Z),
-                                                                     float(depth_scale or 0.0), C.byref(M) if M is not None else None,
-                                                                     MASK_ROLES[mask_roles], w, h, levels, out)
-        current.wait_stream(ext)
-        self._check(rc)
+        if reg is None:
+            self._check(self.lib.dvo_b200_pyramid_create_rectified_batch(self.ctx, rh, *args, out))
+        else:
+            self._check(self.lib.dvo_b200_pyramid_create_registered_batch(self.ctx, reg.handle, rh, *args, out))
+        self.synchronize()   # the staged host arrays may die with this call
         return [Pyramid(self, out[i]) for i in range(n)]
 
     # ---- unregistered depth ----
@@ -686,68 +700,7 @@ class Engine:
         staged from the host, synchronises before returning.  torch CUDA tensors: through
         dvo_b200_pyramid_create_registered_device_batch, ordered with torch's current stream as in pyramid_batch_device,
         without a host synchronisation."""
-        if mask_roles not in MASK_ROLES:
-            raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
-        rh = rectifier.handle if rectifier is not None else None
-        if not isinstance(image, np.ndarray) and hasattr(image, "is_cuda") and image.is_cuda:
-            return self._registered_device(reg, rh, image, depth, levels, depth_scale, masks, mask_roles)
-        image, depth = np.asarray(image), np.asarray(depth)
-        if image.dtype == np.float32 and image.ndim == 3 and depth.dtype == np.float32:
-            fmt = "float32"
-        elif image.dtype == np.uint8 and image.ndim == 3 and depth.dtype == np.uint16:
-            fmt = "grey8_depth16"
-        elif image.dtype == np.uint8 and image.ndim == 4 and image.shape[3] == 3 and depth.dtype == np.uint16:
-            fmt = "bgr8_depth16"
-        else:
-            raise ValueError(f"image {image.dtype} {image.shape} with depth {depth.dtype}: want float32 [n,h,w] + float32, uint8 "
-                             "[n,h,w] + uint16 or uint8 [n,h,w,3] + uint16")
-        n, h, w = image.shape[:3]
-        dw, dh = reg.depth_size
-        if depth.shape != (n, dh, dw):
-            raise ValueError(f"depth {depth.shape}, want {(n, dh, dw)} (the depth camera's size)")
-        if fmt != "float32" and depth_scale is None:
-            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
-        I, Z = np.ascontiguousarray(image), np.ascontiguousarray(depth)
-        M = None
-        if masks is not None:
-            M = np.asarray(masks)
-            M = np.broadcast_to(M, (n, h, w)) if M.shape == (h, w) else M
-            if M.shape != (n, h, w):
-                raise ValueError(f"masks {M.shape}, want {(n, h, w)} or {(h, w)}")
-            M = np.ascontiguousarray(M if M.dtype == np.uint8 else M != 0, dtype=np.uint8)
-        out = (C.c_void_p * n)()
-        self._check(self.lib.dvo_b200_pyramid_create_registered_batch(self.ctx, reg.handle, rh, n, INPUT_FORMATS[fmt], I.ctypes.data,
-                                                                      Z.ctypes.data, float(depth_scale or 0.0),
-                                                                      M.ctypes.data if M is not None else None, MASK_ROLES[mask_roles],
-                                                                      w, h, levels, out))
-        self.synchronize()   # the staged host arrays may die with this call
-        return [Pyramid(self, out[i]) for i in range(n)]
-
-    def _registered_device(self, reg, rh, image, depth, levels, depth_scale, masks, mask_roles):
-        import torch
-        fmt, (n, h, w), pI, pZ, pM = device_planes(image, depth, masks, depth_size=reg.depth_size)
-        if fmt != "float32" and depth_scale is None:
-            raise ValueError(f"{fmt}: depth_scale (metres per raw depth unit) is required")
-        dev = torch.device("cuda", self.device)
-        inputs = [t for t in (image, depth, masks) if t is not None]
-        for t in inputs:
-            if t.device != dev:
-                raise ValueError(f"a tensor on {t.device}: the engine runs on {dev}")
-        I, Z = DevicePlane(*pI), DevicePlane(*pZ)
-        M = DevicePlane(*pM) if pM is not None else None
-        out = (C.c_void_p * n)()
-        current = torch.cuda.current_stream(dev)
-        ext = torch.cuda.ExternalStream(self.stream, device=dev)
-        ext.wait_stream(current)
-        for t in inputs:
-            t.record_stream(ext)     # the caching allocator keeps the memory until the build has read it
-        rc = self.lib.dvo_b200_pyramid_create_registered_device_batch(self.ctx, reg.handle, rh, n, INPUT_FORMATS[fmt], C.byref(I),
-                                                                      C.byref(Z), float(depth_scale or 0.0),
-                                                                      C.byref(M) if M is not None else None, MASK_ROLES[mask_roles], w,
-                                                                      h, levels, out)
-        current.wait_stream(ext)
-        self._check(rc)
-        return [Pyramid(self, out[i]) for i in range(n)]
+        return self._create_remapped(rectifier, reg, image, depth, levels, depth_scale, masks, mask_roles)
 
     def pyramid_raw(self, grey_u8, depth_u16, depth_scale, intrinsics, levels: int, mask=None, mask_roles="reference") -> Pyramid:
         G = np.ascontiguousarray(grey_u8, dtype=np.uint8)
