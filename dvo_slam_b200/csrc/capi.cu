@@ -709,6 +709,45 @@ int dvo_b200_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_p
                            A_out, b_out, nullptr);
 }
 
+// ---- photometric mode ----
+static bool all_finite(const double* v, size_t n) {
+  for (size_t i = 0; i < n; ++i)
+    if (!std::isfinite(v[i])) return false;
+  return true;
+}
+
+int dvo_b200_match_batch_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,
+                                     dvo_b200_pyramid* const* currents, const double* T_init, const double* photometric_init,
+                                     dvo_b200_result* results, double* photometric, dvo_b200_iteration_stats* iteration_stats,
+                                     int32_t max_iteration_stats) {
+  if (!ctx || !results || !photometric) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_photometric: null argument");
+  if (photometric_init && n > 0 && !all_finite(photometric_init, 2 * (size_t)n))
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_photometric: photometric_init is not finite");
+  cudaSetDevice(ctx->device);
+  return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
+                             iteration_stats ? max_iteration_stats : 0, photometric_init, photometric);
+}
+
+int dvo_b200_residual_image_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,
+                                        dvo_b200_pyramid* current, int32_t level, const double* T, const double ab[2], float* planes7,
+                                        int64_t* count) {
+  if (!ctx || !cfg || !planes7 || !ab) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "residual_image_photometric: null argument");
+  if (!all_finite(ab, 2)) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "residual_image_photometric: ab is not finite");
+  cudaSetDevice(ctx->device);
+  return tracker_linearize(ctx, cfg, reference, current, level, T, 0, nullptr, count, nullptr, nullptr, nullptr, nullptr, planes7, ab);
+}
+
+int dvo_b200_linearize_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,
+                                   dvo_b200_pyramid* current, int32_t level, const double* T, const double ab[2], int32_t use_weights,
+                                   const float* prev_precision, int64_t* count, float* precision_out, float* ll_out, double* A_out,
+                                   double* b_out) {
+  if (!ctx || !cfg || !ab) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "linearize_photometric: null argument");
+  if (!all_finite(ab, 2)) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "linearize_photometric: ab is not finite");
+  cudaSetDevice(ctx->device);
+  return tracker_linearize(ctx, cfg, reference, current, level, T, use_weights, prev_precision, count, precision_out, ll_out,
+                           A_out, b_out, nullptr, ab);
+}
+
 int dvo_b200_profile_enable(dvo_b200_ctx* ctx, int32_t enable) {
   if (!ctx) return DVO_B200_ERR_INVALID_ARGUMENT;
   ctx->profile = enable != 0;

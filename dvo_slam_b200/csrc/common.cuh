@@ -149,6 +149,15 @@ struct PairState {
   LevelSummary levels[kMaxLevels];
 };
 
+// The affine brightness model of one pair (photometric alignments only: an array of its own, so that PairState and the
+// default instances of the level kernel stay as they are).  (alpha, beta) is what the current iteration's residuals use
+// (as float); old is the Revertable copy, restored together with the pose.  A / b: the 8 x 8 linearisation (no prior), written
+// only for the linearisation hook.
+struct AffineState {
+  double ab[2], ab_old[2];
+  double A[64], b[8];
+};
+
 struct Workspace {              // per-ctx scratch of the level kernel
   PairLevel* d_pair_level = nullptr;
   const int** d_csat = nullptr;      // per descriptor of d_pair_level: CurPairLevel::csat (only written for kCurMask launches)
@@ -157,8 +166,9 @@ struct Workspace {              // per-ctx scratch of the level kernel
   float* d_dump = nullptr;           // test hook: seven residual-record planes of one level
   double* d_tinit = nullptr;         // per pair initial estimate (4x4)
   dvo_b200_iteration_stats* d_iter_log = nullptr;
+  AffineState* d_affine = nullptr;   // per pair of a photometric alignment
   int* h_active = nullptr;           // pinned: per launch of a call, the kernel's error flag
-  size_t cap_pairs = 0, cap_scratch = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0;
+  size_t cap_pairs = 0, cap_scratch = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0, cap_affine = 0;
 };
 
 }  // namespace dvo_b200
@@ -167,6 +177,7 @@ struct dvo_b200_ctx {
   int device = 0;
   uint64_t uid = 0;                   // unique over the process lifetime (a context's address may be reused after destroy)
   int num_sms = 0, ctas_per_sm = 0;   // persistent-kernel grid geometry (queried once)
+  int ctas_per_sm_affine = 0;         // the same for the instances of the photometric mode
   int estimator = DVO_B200_ESTIMATOR_REFERENCE;   // dvo_b200_estimator of every later alignment / test hook on this context
   unsigned long long* d_dbg = nullptr;   // DVO_B200_TIMING=1: per-level phase timers of the persistent kernel (64 slots)
   cudaStream_t stream = nullptr;
@@ -239,12 +250,16 @@ void pool_close(dvo_b200_ctx* ctx);
 int ensure_stage(dvo_b200_ctx* ctx, size_t dev_bytes, size_t host_bytes);
 
 // tracker.cu
+// ab_out != NULL: the photometric mode (8 unknowns: pose, gain, bias), from ab_init (2n doubles, NULL = (1, 0) each); the
+// final (alpha, beta) of each pair go to ab_out (host, 2n doubles).  Needs h_results.
 int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                         dvo_b200_pyramid* const* curs, const double* T_init, dvo_b200_result* h_results,
-                        void* d_results, dvo_b200_iteration_stats* iter_stats, int max_iter_stats);
+                        void* d_results, dvo_b200_iteration_stats* iter_stats, int max_iter_stats,
+                        const double* ab_init = nullptr, double* ab_out = nullptr);
 int check_level_flags(dvo_b200_ctx* ctx);   // after a stream synchronisation: did a level kernel report a timeout?
 int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* ref, dvo_b200_pyramid* cur,
                       int level, const double* T, int use_weights, const float* prev_precision, int64_t* count,
-                      float* precision_out, float* ll_out, double* A_out, double* b_out, float* planes7);
+                      float* precision_out, float* ll_out, double* A_out, double* b_out, float* planes7,
+                      const double* ab = nullptr);   // ab != NULL: photometric mode at (alpha, beta); A_out 8 x 8, b_out 8
 
 }  // namespace dvo_b200

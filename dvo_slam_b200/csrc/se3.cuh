@@ -182,9 +182,12 @@ DVO_HD void se3_log(const SE3d& s, double out[6]) {
 // without pivoting then performs exactly the operations of the in-place pivoted version, with compile-time indices:
 // on the device everything stays in registers (the in-place version indexed a local-memory array through the
 // permutation, ~700 local loads and stores on the critical path of every Gauss-Newton iteration).
-DVO_HD void ldlt_solve6(const double Ain[36], const double bin[6], double x[6]) {
-  constexpr int n = 6;
-  int idx[6] = {0, 1, 2, 3, 4, 5};
+// The same for any symmetric n x n (the 8 x 8 of the affine brightness model, tracker.cu).
+template <int n>
+DVO_HD void ldlt_solve(const double* Ain, const double* bin, double* x) {
+  int idx[n];
+#pragma unroll
+  for (int i = 0; i < n; ++i) idx[i] = i;
 #pragma unroll
   for (int k = 0; k < n; ++k) {
     int piv = k;
@@ -202,7 +205,7 @@ DVO_HD void ldlt_solve6(const double Ain[36], const double bin[6], double x[6]) 
     for (int i = k + 1; i < n; ++i) if (piv == i) idx[i] = ik;
     idx[k] = ip;
   }
-  double A[6][6], y[6], rd[6];     // rd: reciprocal pivots (one division per pivot; Eigen divides element by element,
+  double A[n][n], y[n], rd[n];     // rd: reciprocal pivots (one division per pivot; Eigen divides element by element,
                                    // which differs in the last bit of a double -- far below every tolerance of this path)
 #pragma unroll
   for (int i = 0; i < n; ++i) {
@@ -245,5 +248,6 @@ DVO_HD void ldlt_solve6(const double Ain[36], const double bin[6], double x[6]) 
     for (int t = 0; t < n; ++t) if (idx[i] == t) x[t] = y[i];
   }
 }
+DVO_HD void ldlt_solve6(const double Ain[36], const double bin[6], double x[6]) { ldlt_solve<6>(Ain, bin, x); }
 
 }  // namespace dvo_b200

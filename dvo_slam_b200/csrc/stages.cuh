@@ -850,12 +850,22 @@ __device__ __forceinline__ WinView make_view(unsigned bufs, const int4& d0, cons
 //                   weight reads c.first_iteration).
 // Both loops call the same pixel functions in the same order, so they compute the same bits.
 
+// The affine brightness model of a pair-iteration (kAffine instances): the intensity residual compares the current image
+// with alpha I_ref + beta, formed as fmaf(alpha, I_ref, beta), which is I_ref itself at (1, 0).
+struct Brightness {
+  float alpha, beta;
+};
+template <bool kAffine>
+__device__ __forceinline__ float ref_intensity(float Ir, const Brightness& br) {
+  return kAffine ? __fmaf_rn(br.alpha, Ir, br.beta) : Ir;
+}
+
 // Stage A rounds of one tile row: two rounds per trip, whose projection / tap / blend chains are independent and interleave.
 // kCorrected: plain scale sums; the generic loop also re-admits the odd last point at tile column odd_col (-1: none).
-template <bool kCorrected, bool kExact, bool kFirst>
+template <bool kCorrected, bool kExact, bool kFirst, bool kAffine = false>
 __device__ __forceinline__ void stage_a_rounds(const WinView& wv, int bw, unsigned refa, unsigned txa, float ty, const StageConsts& c,
                                                typename ScaleOf<kCorrected>::type& ss, int lane, unsigned lt_mask, int odd_col,
-                                               float odd_z) {
+                                               float odd_z, const Brightness& br = {1.f, 0.f}) {
   static_assert(kTileW % 64 == 0, "the exact loop takes whole pairs of rounds");
   const int nr = kExact ? kTileW / 32 : (bw + 31) >> 5;
   const int xlim = bw - lane;        // lane's column r*32+lane is inside the band iff r*32 < xlim
@@ -878,8 +888,8 @@ __device__ __forceinline__ void stage_a_rounds(const WinView& wv, int bw, unsign
     const PixelProjection p0 = project_pixel(tx0, ty, z0, c);
     const PixelProjection p1 = project_pixel(tx1, ty, z1, c);
     float ei0, ez0, ei1, ez1;
-    const bool v0 = residual_pixel<kExact>(p0, wv, lo(rz0), z0, c, ei0, ez0);
-    const bool v1 = residual_pixel<kExact>(p1, wv, lo(rz1), z1, c, ei1, ez1);
+    const bool v0 = residual_pixel<kExact>(p0, wv, ref_intensity<kAffine>(lo(rz0), br), z0, c, ei0, ez0);
+    const bool v1 = residual_pixel<kExact>(p1, wv, ref_intensity<kAffine>(lo(rz1), br), z1, c, ei1, ez1);
     const float w0 = student_weight(c, first, ei0, ez0), w1 = student_weight(c, first, ei1, ez1);
     scale_add(ss, lane, lt_mask, v0, w0, ei0, ez0);
     scale_add(ss, lane, lt_mask, v1, w1, ei1, ez1);
@@ -889,9 +899,10 @@ __device__ __forceinline__ void stage_a_rounds(const WinView& wv, int bw, unsign
 // scale state across the bands (they are consecutive pixels of the row) and writes one segment summary per row
 // to row_exports[y * kSegExportFloats].  Warp kConsumerWarps is the producer: it stages the same tiles, kStages ahead.
 // kCorrected: plain scale sums, and the tile row that holds the odd last point takes the generic loop, which re-admits it.
-template <bool kCorrected>
+template <bool kCorrected, bool kAffine = false>
 __device__ __forceinline__ void stage_a_run(TilePipe& tp, const PairLevel& pl, const LevelGeom& g, const StageConsts& c,
-                                            float* row_exports, unsigned& tile_count, int* error_flag, PipeTiming& tm) {
+                                            float* row_exports, unsigned& tile_count, int* error_flag, PipeTiming& tm,
+                                            const Brightness& br = {1.f, 0.f}) {
   const int lane = threadIdx.x & 31, q = threadIdx.x >> 5;
   const unsigned lt_mask = (1u << lane) - 1u;
   const int ntiles = g.nmine * g.nbands;
@@ -931,10 +942,11 @@ __device__ __forceinline__ void stage_a_run(TilePipe& tp, const PairLevel& pl, c
         const unsigned refa = bufs + my_ref, txa = bufs + my_tx;
         const bool odd_tile = kCorrected && y == odd.y && (unsigned)(odd.x - x0) < (unsigned)bw;   // warp-uniform
         if (wv.exact && bw == kTileW && !odd_tile) {   // warp-uniform
-          if (c.first_iteration) stage_a_rounds<kCorrected, true, true>(wv, bw, refa, txa, ty, c, ss, lane, lt_mask, -1, 0.f);
-          else stage_a_rounds<kCorrected, true, false>(wv, bw, refa, txa, ty, c, ss, lane, lt_mask, -1, 0.f);
+          if (c.first_iteration) stage_a_rounds<kCorrected, true, true, kAffine>(wv, bw, refa, txa, ty, c, ss, lane, lt_mask, -1, 0.f, br);
+          else stage_a_rounds<kCorrected, true, false, kAffine>(wv, bw, refa, txa, ty, c, ss, lane, lt_mask, -1, 0.f, br);
         } else {
-          stage_a_rounds<kCorrected, false, false>(wv, bw, refa, txa, ty, c, ss, lane, lt_mask, odd_tile ? odd.x - x0 : -1, odd.z);
+          stage_a_rounds<kCorrected, false, false, kAffine>(wv, bw, refa, txa, ty, c, ss, lane, lt_mask, odd_tile ? odd.x - x0 : -1,
+                                                            odd.z, br);
         }
       }
       __syncwarp();
@@ -950,39 +962,52 @@ struct StageBConsts {
   float l, wd0, wd1;          // P_k = [1 l; 0 1]^T-style factors, see stage_b_pixel
 };
 
-constexpr int kNormalValues = 28;   // log-likelihood sum, 21 upper-triangular A (row-major), 6 b
+// Normal-equation values of one image row: the log-likelihood sum, the upper triangle of A (row-major) and b, over the
+// kCols unknowns: the 6 of the pose, or with the affine brightness model (kAffine) 8 = pose, gain alpha, bias beta.
+template <int kCols> constexpr int kNormalValuesOf = 1 + kCols * (kCols + 1) / 2 + kCols;
+constexpr int kNormalValues = kNormalValuesOf<6>;    // 28
+constexpr int kNormalValuesAffine = kNormalValuesOf<8>;   // 45
+template <bool kAffine> constexpr int kColsOf = kAffine ? 8 : 6;
 
-// Accumulators of stage B for one thread: the 21 entries of the upper triangle of A (row-major: A[r][c], c >= r, is
-// A[tri(r, c)]) and the 6 of b, one register each.
-constexpr int kTriValues = 21;
-__host__ __device__ constexpr int tri(int r, int c) { return r * 6 - r * (r - 1) / 2 + (c - r); }
-struct StageBAcc {
-  float A[kTriValues];
-  float b[6];
+// Accumulators of stage B for one thread: the entries of the upper triangle of A (row-major: A[r][c], c >= r, is
+// A[tri<kCols>(r, c)]) and the kCols of b, one register each.
+template <int kCols>
+__host__ __device__ constexpr int tri(int r, int c) { return r * kCols - r * (r - 1) / 2 + (c - r); }
+template <int kCols>
+struct StageBAccN {
+  static constexpr int kTri = kCols * (kCols + 1) / 2;
+  float A[kTri];
+  float b[kCols];
   float llsum;     // sum of log2(1 + 0.2 r^T P r) over this thread's kept points
 };
+using StageBAcc = StageBAccN<6>;
 
-__device__ __forceinline__ void stage_b_init(StageBAcc& a) {
+template <int kCols>
+__device__ __forceinline__ void stage_b_init(StageBAccN<kCols>& a) {
 #pragma unroll
-  for (int i = 0; i < kTriValues; ++i) a.A[i] = 0.f;
+  for (int i = 0; i < StageBAccN<kCols>::kTri; ++i) a.A[i] = 0.f;
 #pragma unroll
-  for (int i = 0; i < 6; ++i) a.b[i] = 0.f;
+  for (int i = 0; i < kCols; ++i) a.b[i] = 0.f;
   a.llsum = 0.f;
 }
 
-// A += u v^T (upper triangle) and b += u * s for one 6-vector v given as three pairs V, with u = v * wd.
-__device__ __forceinline__ void stage_b_rank1(StageBAcc& acc, const f2 V[3], float wd, float s) {
-  const float v[6] = {lo(V[0]), hi(V[0]), lo(V[1]), hi(V[1]), lo(V[2]), hi(V[2])};
-  float u[6];
+// A += u v^T (upper triangle) and b += u * s with u = v * wd, for v = the 6-vector given as three pairs V, followed (kN = 8)
+// by v6, v7; entries past the first kN are zero.
+template <int kCols, int kN>
+__device__ __forceinline__ void stage_b_rank1(StageBAccN<kCols>& acc, const f2 V[3], float wd, float s, float v6 = 0.f, float v7 = 0.f) {
+  float v[kN];
+  v[0] = lo(V[0]); v[1] = hi(V[0]); v[2] = lo(V[1]); v[3] = hi(V[1]); v[4] = lo(V[2]); v[5] = hi(V[2]);
+  if constexpr (kN == 8) { v[6] = v6; v[7] = v7; }
+  float u[kN];
 #pragma unroll
-  for (int r = 0; r < 6; ++r) u[r] = __fmul_rn(v[r], wd);
+  for (int r = 0; r < kN; ++r) u[r] = __fmul_rn(v[r], wd);
 #pragma unroll
-  for (int r = 0; r < 6; ++r) {
+  for (int r = 0; r < kN; ++r) {
 #pragma unroll
-    for (int c = r; c < 6; ++c) acc.A[tri(r, c)] = __fmaf_rn(u[r], v[c], acc.A[tri(r, c)]);
+    for (int c = r; c < kN; ++c) acc.A[tri<kCols>(r, c)] = __fmaf_rn(u[r], v[c], acc.A[tri<kCols>(r, c)]);
   }
 #pragma unroll
-  for (int r = 0; r < 6; ++r) acc.b[r] = __fmaf_rn(u[r], s, acc.b[r]);
+  for (int r = 0; r < kN; ++r) acc.b[r] = __fmaf_rn(u[r], s, acc.b[r]);
 }
 
 // One valid point: log-likelihood term and normal equations with W = w * P_k.
@@ -992,8 +1017,11 @@ __device__ __forceinline__ void stage_b_rank1(StageBAcc& acc, const f2 V[3], flo
 // (dense_tracking.cpp:448-476): J0 = gx a + gy b, J1 = hx a + hy b - c with
 //   a = [1/z, 0, -x/z^2, a2 y, 1 - a2 x, -y/z], b = [0, 1/z, -y/z^2, b2 y - 1, -a3, x/z], c = [0, 0, 1, y, -x, 0].
 // Branch-free: a rejected point arrives with wgt = 0 and finite stand-in inputs, so it adds exact zeros.
-__device__ __forceinline__ void stage_b_pixel(StageBAcc& acc, const StageBConsts& c, float wgt, bool keep, float ei, float ez, f2 G,
-                                              f2 H, float z, float tx, float ty) {
+// kCols = 8 (affine brightness): the intensity row has two more columns, de_i/dalpha = -c_i I_ref and de_i/dbeta = -c_i, and
+// the depth row zeros there, so j0' grows by those two entries and the second update keeps its 6 columns.  nci = -c_i.
+template <int kCols>
+__device__ __forceinline__ void stage_b_pixel(StageBAccN<kCols>& acc, const StageBConsts& c, float wgt, bool keep, float ei, float ez,
+                                              f2 G, f2 H, float z, float tx, float ty, float Ir = 0.f, float nci = 0.f) {
   // log-likelihood term: log(1 + 0.2 r^T P r); one MUFU.LG2 per point, scaled by ln 2 once at the end
   const float d = (ei * c.P00 + ez * c.P10) * ei + (ei * c.P01 + ez * c.P11) * ez;
   acc.llsum += __log2f(keep ? fmaf(0.2f, d, 1.0f) : 1.0f);
@@ -1014,14 +1042,16 @@ __device__ __forceinline__ void stage_b_pixel(StageBAcc& acc, const StageBConsts
   V1[1] = fma2(bc(hx), A23, fma2(bc(hy), B23, NC23));
   V1[2] = fma2(bc(hx), A45, fma2(bc(hy), B45, NC45));
   // b -= J^T W r
-  stage_b_rank1(acc, V0, wgt * c.wd0, -fmaf(c.l, ez, ei));
-  stage_b_rank1(acc, V1, wgt * c.wd1, -ez);
+  stage_b_rank1<kCols, kCols>(acc, V0, wgt * c.wd0, -fmaf(c.l, ez, ei), nci * Ir, nci);
+  stage_b_rank1<kCols, 6>(acc, V1, wgt * c.wd1, -ez);
 }
 
 // Value k of the row's normal equations (k a compile-time index once unrolled): 0 = log-likelihood sum (the log2 terms
-// scaled by ln 2 once), 1..21 = A upper triangle (row-major), 22..27 = b, 28..31 = zero padding of the exchange.
-__device__ __forceinline__ float stage_b_value(const StageBAcc& acc, int k) {
-  return k == 0 ? acc.llsum * 0.69314718055994531f : k <= kTriValues ? acc.A[k - 1] : k < kNormalValues ? acc.b[k - 1 - kTriValues] : 0.f;
+// scaled by ln 2 once), 1..kTri = A upper triangle (row-major), then b, then zero padding of the exchange.
+template <int kCols>
+__device__ __forceinline__ float stage_b_value(const StageBAccN<kCols>& acc, int k) {
+  constexpr int kTri = StageBAccN<kCols>::kTri;
+  return k == 0 ? acc.llsum * 0.69314718055994531f : k <= kTri ? acc.A[k - 1] : k < kNormalValuesOf<kCols> ? acc.b[k - 1 - kTri] : 0.f;
 }
 
 // One step of the halving exchange of flush_row_partial: a[0 .. 2 kHalf) -> a[0 .. kHalf), partner lane ^ kHalf.
@@ -1037,23 +1067,30 @@ __device__ __forceinline__ void halving_step(float (&a)[16], int lane) {
   }
 }
 
-// Sum the kNormalValues accumulators of a row over the 32 lanes of its warp in a fixed order (halving exchange: partner
-// lane ^ 16, ^ 8, ... ^ 1; 31 shuffles instead of 5 x 28) and store the row's totals: lane l ends up with value l.
-// The first exchange reads the accumulators directly; the later ones halve the 16 partial sums in place.
-__device__ __forceinline__ void flush_row_partial(const StageBAcc& acc, int lane, float* row_out) {
+// Sum the normal-equation values kBase .. kBase + 31 of a row over the 32 lanes of its warp in a fixed order (halving
+// exchange: partner lane ^ 16, ^ 8, ... ^ 1; 31 shuffles instead of 5 x 32) and store the row's totals: lane l ends up with
+// value kBase + l.  The first exchange reads the accumulators directly; the later ones halve the 16 partial sums in place.
+template <int kBase, int kCols>
+__device__ __forceinline__ void flush_row_window(const StageBAccN<kCols>& acc, int lane, float* row_out) {
   float a[16];
   const bool up = (lane & 16) != 0;
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
-    const float mine = up ? stage_b_value(acc, 16 + j) : stage_b_value(acc, j);
-    const float send = up ? stage_b_value(acc, j) : stage_b_value(acc, 16 + j);
+    const float mine = up ? stage_b_value(acc, kBase + 16 + j) : stage_b_value(acc, kBase + j);
+    const float send = up ? stage_b_value(acc, kBase + j) : stage_b_value(acc, kBase + 16 + j);
     a[j] = mine + __shfl_xor_sync(kFullMask, send, 16);
   }
   halving_step<8>(a, lane);
   halving_step<4>(a, lane);
   halving_step<2>(a, lane);
   halving_step<1>(a, lane);
-  if (lane < kNormalValues) row_out[lane] = a[0];
+  if (lane < kNormalValuesOf<kCols> - kBase) row_out[kBase + lane] = a[0];
+}
+// All kNormalValuesOf<kCols> values of a row, 32 at a time.
+template <int kCols>
+__device__ __forceinline__ void flush_row_partial(const StageBAccN<kCols>& acc, int lane, float* row_out) {
+  flush_row_window<0>(acc, lane, row_out);
+  if constexpr (kNormalValuesOf<kCols> > 32) flush_row_window<32>(acc, lane, row_out);
 }
 
 // optional per-pixel dump of the residual records (dvo_b200_residual_image): seven planes of n floats
@@ -1077,11 +1114,13 @@ __device__ __noinline__ void dump_record(const RecordDump& dump, size_t i, bool 
 // re-admits the odd last point at tile column odd_col (-1: none), as stage_a_rounds does.
 // kCurMask, generic loop, cmask (warp-uniform): a valid point also needs four usable taps -- four non-NaN Z' in the current
 // image's P0 (cur0), the very test stage A makes on its blended Z' -- so both stages keep the same points.
-template <bool kCorrected, bool kExact, bool kFirst, bool kDump, bool kCurMask = false>
+// kAffine: the intensity residual against alpha I_ref + beta, and the two brightness columns (stage_b_pixel).
+template <bool kCorrected, bool kExact, bool kFirst, bool kDump, bool kCurMask = false, bool kAffine = false>
 __device__ __forceinline__ void stage_b_rounds(const WinView& wv, int bw, unsigned refa, unsigned txa, float ty, const StageConsts& c,
-                                               const StageBConsts& cb, StageBAcc& acc, bool cta_has_tail, int& rank, int keep_rank,
-                                               const RecordDump& dump, size_t pix, int lane, unsigned lt_mask, int odd_col, float odd_z,
-                                               PipeTiming& tm, bool cmask = false, const float2* cur0 = nullptr) {
+                                               const StageBConsts& cb, StageBAccN<kColsOf<kAffine>>& acc, bool cta_has_tail, int& rank,
+                                               int keep_rank, const RecordDump& dump, size_t pix, int lane, unsigned lt_mask, int odd_col,
+                                               float odd_z, PipeTiming& tm, bool cmask = false, const float2* cur0 = nullptr,
+                                               const Brightness& br = {1.f, 0.f}) {
   const int nr = kExact ? kTileW / 32 : (bw + 31) >> 5;
   const int xlim = bw - lane;
   const bool first = kExact ? kFirst : c.first_iteration != 0;
@@ -1095,7 +1134,7 @@ __device__ __forceinline__ void stage_b_rounds(const WinView& wv, int bw, unsign
     if (kCorrected && !kExact) z = (r * 32 + lane == odd_col) ? odd_z : z;
     const PixelProjection p = project_pixel(tx, ty, z, c);
     f2 E, G, H;
-    bool valid = record_pixel<kExact>(p, wv, lo(rz), z, gr, c, E, G, H);
+    bool valid = record_pixel<kExact>(p, wv, ref_intensity<kAffine>(lo(rz), br), z, gr, c, E, G, H);
     if (kCurMask && !kExact && cmask && valid) {   // valid: the taps lie inside the image
       const float2* t = cur0 + (size_t)p.v0 * wv.pitch + p.u0;   // u0 may be odd: four 8-byte loads
       const float z00 = __ldg(t).y, z10 = __ldg(t + 1).y, z01 = __ldg(t + wv.pitch).y, z11 = __ldg(t + wv.pitch + 1).y;
@@ -1114,7 +1153,8 @@ __device__ __forceinline__ void stage_b_rounds(const WinView& wv, int bw, unsign
     const float wall = student_weight(c, first, ei, ez);
     const float wgt = valid ? wall : 0.f;
     // (tx too: past a partial band it comes from shared memory no copy has written)
-    stage_b_pixel(acc, cb, wgt, keep, ei, ez, valid ? G : bc(0.f), valid ? H : bc(0.f), valid ? z : 1.0f, valid ? tx : 0.f, ty);
+    stage_b_pixel(acc, cb, wgt, keep, ei, ez, valid ? G : bc(0.f), valid ? H : bc(0.f), valid ? z : 1.0f, valid ? tx : 0.f, ty,
+                  valid ? lo(rz) : 0.f, -c.c_i);
   }
 }
 
@@ -1123,11 +1163,12 @@ __device__ __forceinline__ void stage_b_rounds(const WinView& wv, int bw, unsign
 // computeCompleteDataLogLikelihood (dense_tracking_impl.cpp:413-422).  kCorrected: the log-likelihood keeps every point, so
 // no strip has a tail and ranks are never counted; the tile row that holds the odd last point takes the generic loop.
 // kCurMask: tiles with the cmask bit take the generic loop with the per-tap mask test (produce_tiles clears their `exact`).
-template <bool kDump, bool kCorrected, bool kCurMask = false>
+template <bool kDump, bool kCorrected, bool kCurMask = false, bool kAffine = false>
 __device__ __forceinline__ void stage_b_run(TilePipe& tp, const PairLevel& pl, const LevelGeom& g, const StageConsts& c,
                                             const StageBConsts& cb, const int* row_base, const int* strip_base, long long n_keep,
                                             const RecordDump& dump, float* row_partial, unsigned& tile_count, int* error_flag,
-                                            PipeTiming& tm) {
+                                            PipeTiming& tm, const Brightness& br = {1.f, 0.f}) {
+  constexpr int kCols = kColsOf<kAffine>;
   const int lane = threadIdx.x & 31, q = threadIdx.x >> 5;
   const unsigned lt_mask = (1u << lane) - 1u;
   const int ntiles = g.nmine * g.nbands;
@@ -1159,7 +1200,7 @@ __device__ __forceinline__ void stage_b_run(TilePipe& tp, const PairLevel& pl, c
       keep_rank = (int)max(min(n_keep - sbase, (long long)0x7fffffff), (long long)-1);
       if (cta_has_tail && row_ok) rank = __ldcg(row_base + y);
     }
-    StageBAcc acc;             // one image row at a time: the row's sums leave the warp in a fixed order (flush_row_partial)
+    StageBAccN<kCols> acc;     // one image row at a time: the row's sums leave the warp in a fixed order (flush_row_partial)
     stage_b_init(acc);
     for (int b = 0; b < gnb; ++b, ++i) {
       const unsigned t = tbase + i;
@@ -1178,15 +1219,16 @@ __device__ __forceinline__ void stage_b_run(TilePipe& tp, const PairLevel& pl, c
         const bool odd_tile = kCorrected && y == odd.y && (unsigned)(odd.x - x0) < (unsigned)bw;   // warp-uniform
         if (wv.exact && bw == kTileW && !cta_has_tail && !odd_tile) {   // warp-uniform
           if (c.first_iteration)
-            stage_b_rounds<kCorrected, true, true, kDump>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank, dump, pix, lane,
-                                                          lt_mask, -1, 0.f, tm);
+            stage_b_rounds<kCorrected, true, true, kDump, false, kAffine>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank,
+                                                                          dump, pix, lane, lt_mask, -1, 0.f, tm, false, nullptr, br);
           else
-            stage_b_rounds<kCorrected, true, false, kDump>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank, dump, pix, lane,
-                                                           lt_mask, -1, 0.f, tm);
+            stage_b_rounds<kCorrected, true, false, kDump, false, kAffine>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank,
+                                                                           dump, pix, lane, lt_mask, -1, 0.f, tm, false, nullptr, br);
         } else {
-          stage_b_rounds<kCorrected, false, false, kDump, kCurMask>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank, keep_rank, dump,
-                                                                    pix, lane, lt_mask, odd_tile ? odd.x - x0 : -1, odd.z, tm,
-                                                                    kCurMask && d1.w != 0, pl.c0);
+          stage_b_rounds<kCorrected, false, false, kDump, kCurMask, kAffine>(wv, bw, refa, txa, ty, c, cb, acc, cta_has_tail, rank,
+                                                                             keep_rank, dump, pix, lane, lt_mask,
+                                                                             odd_tile ? odd.x - x0 : -1, odd.z, tm,
+                                                                             kCurMask && d1.w != 0, pl.c0, br);
         }
       } else if (kDump && row_ok) {
         for (int xl = lane; xl < bw; xl += 32) dump_record(dump, (size_t)y * gw + x0 + xl, false, bc(0.f), bc(0.f), bc(0.f), 0.f);
@@ -1194,7 +1236,7 @@ __device__ __forceinline__ void stage_b_run(TilePipe& tp, const PairLevel& pl, c
       __syncwarp();
       if (lane == 0) mbar_arrive_s(tp_s + (unsigned)offsetof(TilePipe, empty) + bufi * 8u);
     }
-    if (row_ok) flush_row_partial(acc, lane, row_partial + (size_t)y * kNormalValues);
+    if (row_ok) flush_row_partial(acc, lane, row_partial + (size_t)y * kNormalValuesOf<kCols>);
   }
 }
 

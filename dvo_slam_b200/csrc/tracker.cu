@@ -26,6 +26,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <algorithm>
+#include <type_traits>
 
 namespace dvo_b200 {
 
@@ -188,13 +189,39 @@ __device__ __noinline__ void pair_mid_warp(PairState& st, int pair, const double
 //   deferred : Revertable bookkeeping, statistics, the iteration log.  It finishes before this CTA arrives at
 //              the squad's next barrier, so the next P_k / end step (run by whichever CTA arrives last) sees it.
 struct PairEndSmem {
+  static constexpr bool kAffine = false;
   double part[kEndWarps][32];
 };
+// The photometric mode: 45 values per strip, and the pair's brightness state (set by the kernel before the call).  They
+// travel in the end step's shared block rather than as arguments: an extra argument of the __noinline__ pair_end_cta would
+// change the call sequence, and with it the code, of the default instances.
+struct PairEndSmemAffine {
+  static constexpr bool kAffine = true;
+  double part[kEndWarps][64];
+  AffineState* aff;
+  int keep_system;   // 1: the linearisation hook, which reads the 8 x 8 system back (AffineState::A, b)
+};
 
-template <typename Release>
+// The photometric mode's pose information: the Schur complement A_xx - A_xp A_pp^-1 A_px of the 8 x 8 system onto the pose,
+// in fp64, with the 2 x 2 inverse written out.
+__device__ __forceinline__ void schur_pose(const double A[64], double S[36]) {
+  const double a = A[6 * 8 + 6], c = A[6 * 8 + 7], d = A[7 * 8 + 7];
+  const double rdet = 1.0 / (a * d - c * c);
+  const double i00 = d * rdet, i01 = -c * rdet, i11 = a * rdet;
+  for (int i = 0; i < 6; ++i) {
+    const double g0 = i00 * A[i * 8 + 6] + i01 * A[i * 8 + 7], g1 = i01 * A[i * 8 + 6] + i11 * A[i * 8 + 7];   // (A_pp^-1 A_px)^T row i
+    for (int j = 0; j < 6; ++j) S[i * 6 + j] = A[i * 8 + j] - (g0 * A[j * 8 + 6] + g1 * A[j * 8 + 7]);
+  }
+}
+
+// Smem: PairEndSmem, or PairEndSmemAffine for the photometric mode (8 unknowns: the 8 x 8 solve, the additive update of
+// (alpha, beta), the Schur complement as the information, and the revert of (alpha, beta) with the pose).
+template <typename Smem, typename Release>
 __device__ __noinline__ void pair_end_cta(PairState& st, const PairLevel& pl, int pair, const double* partial, int ntiles,
                                              const LevelLaunch& lp, dvo_b200_iteration_stats* ilog, int max_log,
-                                             PairEndSmem& sm, Release release, unsigned long long* tcrit = nullptr) {
+                                             Smem& sm, Release release, unsigned long long* tcrit = nullptr) {
+  constexpr bool kAffine = Smem::kAffine;
+  constexpr int kNV = kAffine ? kNormalValuesAffine : kNormalValues, kN = kAffine ? 8 : 6;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   unsigned long long tc0 = 0;
   if (tcrit && threadIdx.x == 0) asm volatile("mov.u64 %0, %globaltimer;" : "=l"(tc0));
@@ -203,27 +230,30 @@ __device__ __noinline__ void pair_end_cta(PairState& st, const PairLevel& pl, in
   auto phase = [&](int k) {
     if (tcrit) { unsigned long long tn; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(tn)); atomicAdd(tcrit + k, tn - tph); tph = tn; }
   };
-  {   // fp64 sum of the level's strip partials in a fixed order: warp q takes strips q, q+4, ... with independent loads in flight
+  // fp64 sum of the level's strip partials in a fixed order: warp q takes strips q, q+4, ... with independent loads in flight;
+  // lane l sums value l (and l + 32 in the photometric mode)
+#pragma unroll
+  for (int w0 = 0; w0 < kNV; w0 += 32) {
     double v = 0.0;
-    if (lane < kNormalValues && warp < kEndWarps) {
-      const double* p = partial + lane;
+    if (w0 + lane < kNV && warp < kEndWarps) {
+      const double* p = partial + (w0 + lane);
       int t = warp;
       for (; t + 3 * kEndWarps < ntiles; t += 4 * kEndWarps) {
-        const double a0 = __ldcg(p + (size_t)t * kNormalValues);
-        const double a1 = __ldcg(p + (size_t)(t + kEndWarps) * kNormalValues);
-        const double a2 = __ldcg(p + (size_t)(t + 2 * kEndWarps) * kNormalValues);
-        const double a3 = __ldcg(p + (size_t)(t + 3 * kEndWarps) * kNormalValues);
+        const double a0 = __ldcg(p + (size_t)t * kNV);
+        const double a1 = __ldcg(p + (size_t)(t + kEndWarps) * kNV);
+        const double a2 = __ldcg(p + (size_t)(t + 2 * kEndWarps) * kNV);
+        const double a3 = __ldcg(p + (size_t)(t + 3 * kEndWarps) * kNV);
         v += a0; v += a1; v += a2; v += a3;
       }
-      for (; t < ntiles; t += kEndWarps) v += __ldcg(p + (size_t)t * kNormalValues);
+      for (; t < ntiles; t += kEndWarps) v += __ldcg(p + (size_t)t * kNV);
     }
-    if (warp < kEndWarps) sm.part[warp][lane] = v;
+    if (warp < kEndWarps) sm.part[warp][w0 + lane] = v;
   }
   __syncthreads();
   if (threadIdx.x != 0) return;
-  double vals[kNormalValues];
+  double vals[kNV];
 #pragma unroll
-  for (int i = 0; i < kNormalValues; ++i) {
+  for (int i = 0; i < kNV; ++i) {
     double v = sm.part[0][i];
 #pragma unroll
     for (int q = 1; q < kEndWarps; ++q) v += sm.part[q][i];
@@ -247,23 +277,25 @@ __device__ __noinline__ void pair_end_cta(PairState& st, const PairLevel& pl, in
   const double last_error = st.error;              // dense_tracking.cpp:306-307
   const double error = -(double)ll;
   const bool accept = error < last_error;          // dense_tracking.cpp:312
-  double A[36], bvec[6], x[6];
+  double A[kN * kN], bvec[kN], x[kN];
   {
     int k = 1;
-    for (int i = 0; i < 6; ++i)
-      for (int j = i; j < 6; ++j) { A[i * 6 + j] = vals[k]; A[j * 6 + i] = vals[k]; ++k; }
-    for (int i = 0; i < 6; ++i) bvec[i] = vals[22 + i];
+    for (int i = 0; i < kN; ++i)
+      for (int j = i; j < kN; ++j) { A[i * kN + j] = vals[k]; A[j * kN + i] = vals[k]; ++k; }
+    for (int i = 0; i < kN; ++i) bvec[i] = vals[1 + kN * (kN + 1) / 2 + i];
   }
   int iteration = st.iteration;
   const int it_id = iteration;                     // IterationStats.Id = itctx_.Iteration before the increment (dense_tracking.cpp:251)
   if (accept) {
-    double As[36], bs[6];
-    for (int i = 0; i < 36; ++i) As[i] = A[i];
-    for (int i = 0; i < 6; ++i) { As[i * 6 + i] += lp.mu; bs[i] = bvec[i] + lp.mu * li[i]; }   // lines 345-346
-    ldlt_solve6(As, bs, x);                                                                    // line 347
-    iteration += 1;                                                                            // line 353
+    double As[kN * kN], bs[kN];
+    for (int i = 0; i < kN * kN; ++i) As[i] = A[i];
+    for (int i = 0; i < 6; ++i) { As[i * kN + i] += lp.mu; bs[i] = bvec[i] + lp.mu * li[i]; }   // lines 345-346 (the pose only)
+    if constexpr (kAffine) { bs[6] = bvec[6]; bs[7] = bvec[7]; }
+    ldlt_solve<kN>(As, bs, x);                                                                   // line 347
+    iteration += 1;                                                                              // line 353
   } else {
     for (int i = 0; i < 6; ++i) x[i] = st.x[i];
+    if constexpr (kAffine) x[6] = x[7] = 0.0;
   }
   phase(2);   // accept test, LDL^T
   double m = 0; bool nanx = false;
@@ -285,8 +317,18 @@ __device__ __noinline__ void pair_end_cta(PairState& st, const PairLevel& pl, in
       st.kt[8 + j] = t2;
     }
     st.iteration = iteration;
+    if constexpr (kAffine) {   // alpha += dalpha, beta += dbeta, with the pose
+      AffineState& af = *sm.aff;
+      const double a0 = af.ab[0], b0 = af.ab[1];
+      af.ab_old[0] = a0; af.ab_old[1] = b0;
+      af.ab[0] = a0 + x[6]; af.ab[1] = b0 + x[7];
+    }
   } else {
     st.level_active = 0;
+    if constexpr (kAffine) {   // a rejected iteration reverts (alpha, beta) with the pose
+      AffineState& af = *sm.aff;
+      if (!accept) { af.ab[0] = af.ab_old[0]; af.ab[1] = af.ab_old[1]; }
+    }
   }
   phase(3);   // exp, pose product, K*T
   if (tcrit) { unsigned long long tc1; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(tc1)); atomicAdd(tcrit + 7, tc1 - tc0); }
@@ -300,16 +342,34 @@ __device__ __noinline__ void pair_end_cta(PairState& st, const PairLevel& pl, in
   st.prior_cur = lp.mu * sq;                       // dense_tracking.cpp:302
   st.last_error = last_error;
   st.error = error;
-  for (int i = 0; i < 36; ++i) st.A[i] = A[i];
+  if constexpr (kAffine) {
+    for (int i = 0; i < 6; ++i)
+      for (int j = 0; j < 6; ++j) st.A[i * 6 + j] = A[i * kN + j];
+  } else {
+    for (int i = 0; i < 36; ++i) st.A[i] = A[i];
+  }
   for (int i = 0; i < 6; ++i) st.b[i] = bvec[i];
+  if constexpr (kAffine) {
+    if (sm.keep_system) {
+      for (int i = 0; i < 64; ++i) sm.aff->A[i] = A[i];
+      for (int i = 0; i < 8; ++i) sm.aff->b[i] = bvec[i];
+    }
+  }
   if (!accept) {
     st.initial = st.initial_old; st.estimate = st.estimate_old;   // dense_tracking.cpp:314-321
     st.termination = DVO_B200_TERM_LOG_LIKELIHOOD_DECREASED;
     log_iteration(ilog, max_log, pair, st, it_id, lp.level_id, false);
   } else {
     for (int i = 0; i < 6; ++i) st.x[i] = x[i];
-    for (int i = 0; i < 36; ++i) st.A_done[i] = A[i];
-    for (int i = 0; i < 6; ++i) st.A_done[i * 6 + i] += lp.mu;
+    if constexpr (kAffine) {
+      double Ap[64];
+      for (int i = 0; i < 64; ++i) Ap[i] = A[i];
+      for (int i = 0; i < 6; ++i) Ap[i * 8 + i] += lp.mu;
+      schur_pose(Ap, st.A_done);
+    } else {
+      for (int i = 0; i < 36; ++i) st.A_done[i] = A[i];
+      for (int i = 0; i < 6; ++i) st.A_done[i * 6 + i] += lp.mu;
+    }
     st.nll_done = st.nll_cur; st.prior_done = st.prior_cur; st.have_done = 1;
     ls.last_inc_n = st.n; ls.last_inc_nll = st.nll_cur;
     log_iteration(ilog, max_log, pair, st, it_id, lp.level_id, true);
@@ -352,12 +412,14 @@ struct SquadState {
   int pad_[29];   // one 128-byte line per squad
 };
 
-struct LevelTail {      // shared memory after the tile pipeline
+template <bool kAffine>
+struct LevelTailOf {    // shared memory after the tile pipeline
   SegCombineSmem comb;
-  PairEndSmem end;
+  typename std::conditional<kAffine, PairEndSmemAffine, PairEndSmem>::type end;
   int s_flag[2];
 };
-constexpr size_t kLevelSmemBytes = sizeof(TilePipe) + sizeof(LevelTail);
+template <bool kAffine> constexpr size_t kLevelSmemBytesOf = sizeof(TilePipe) + sizeof(LevelTailOf<kAffine>);
+constexpr size_t kLevelSmemBytes = kLevelSmemBytesOf<false>;
 
 // One segment of a launch: a group of consecutive pyramid levels that a squad of g CTAs walks a pair through.  A launch
 // has one segment, or two (the coarse levels with one CTA per pair, then the fine levels with squads of g CTAs) that the
@@ -400,6 +462,7 @@ struct PersistentArgs {
   Segment seg[kMaxSeg];
   const PairLevel* pls0;  // kCurMask: csat[i] belongs to the descriptor pls0[i]
   const int* const* csat;
+  AffineState* affine;    // kAffine: per pair
 };
 
 // The descriptor of one pair at one level of a segment: a PairLevel, or with kCurMask a CurPairLevel.
@@ -464,12 +527,20 @@ __device__ __forceinline__ void squad_wait(SquadState* sq, unsigned episode, int
 // kCurMask: some pair's current image has a mask in the current role (PairLevel::csat); stage B then tests the taps of the
 // tiles whose window touches an unusable pixel (produce_tiles, stage_b_rounds).  Without it the instance is the one that
 // existed before current-role masks.
-template <bool kCorrected, bool kCurMask = false>
-__global__ void __launch_bounds__(kCtaThreads, 2)
+// kAffine: the photometric mode (include/dvo_b200.h): a gain and a bias per pair (PersistentArgs::affine) estimated with the
+// pose, 45 normal-equation values per row instead of 28.  Its stage-B loop holds 17 more accumulators; it is compiled for
+// kAffineCtasPerSm resident CTAs (DESIGN §4.8), and the launch plan of a photometric match uses that occupancy.
+#ifndef DVO_AFFINE_CTAS_PER_SM
+#define DVO_AFFINE_CTAS_PER_SM 2
+#endif
+constexpr int kAffineCtasPerSm = DVO_AFFINE_CTAS_PER_SM;
+template <bool kCorrected, bool kCurMask = false, bool kAffine = false>
+__global__ void __launch_bounds__(kCtaThreads, kAffine ? kAffineCtasPerSm : 2)
 k_level_persistent(const __grid_constant__ PersistentArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   TilePipe& tp = *reinterpret_cast<TilePipe*>(smem_raw);
-  LevelTail& lt = *reinterpret_cast<LevelTail*>(smem_raw + sizeof(TilePipe));
+  LevelTailOf<kAffine>& lt = *reinterpret_cast<LevelTailOf<kAffine>*>(smem_raw + sizeof(TilePipe));
+  constexpr int kNV = kAffine ? kNormalValuesAffine : kNormalValues;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -506,8 +577,8 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
   const int smax = (hmax + kTileH - 1) / kTileH;      // strips of the tallest level of the segment
   double* strip_exports = S.strip_exports + (size_t)squad * smax * kStripExportDoubles;
   int* strip_base = S.strip_base + (size_t)squad * (smax + 1);
-  float* row_partial = S.row_partial + (size_t)squad * hmax * kNormalValues;
-  double* strip_partial = S.strip_partial + (size_t)squad * smax * kNormalValues;
+  float* row_partial = S.row_partial + (size_t)squad * hmax * kNV;
+  double* strip_partial = S.strip_partial + (size_t)squad * smax * kNV;
   unsigned episode = 0;
   unsigned long long t_acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, t0 = 0, t1 = 0;
   const bool timing = S.dbg != nullptr && threadIdx.x == 0;
@@ -550,6 +621,12 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
     const int pair = __ldcg(&sq->pair);
     if (pair < 0 || *reinterpret_cast<volatile int*>(a.error_flag)) break;
     PairState& st = a.states[pair];
+    // (alpha, beta) of the pair's current iteration, read like the pose (written between stages by another SM)
+    auto brightness = [&]() {
+      Brightness br{1.f, 0.f};
+      if constexpr (kAffine) br = Brightness{(float)__ldcg(&a.affine[pair].ab[0]), (float)__ldcg(&a.affine[pair].ab[1])};
+      return br;
+    };
 
     // ---- the squad walks its pair through the levels of this launch, coarse to fine ----
     for (int li = 0; li < S.nlev; ++li) {
@@ -569,6 +646,10 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
       if (squad_arrive(sq, episode, S.g, lt.s_flag)) {
         if (threadIdx.x == 0) {
           level_begin(st, pl, a.T_init, pair, lp);
+          if constexpr (kAffine) {   // the level's first iteration reverts (alpha, beta) to where the level starts
+            AffineState& af = a.affine[pair];
+            af.ab_old[0] = af.ab[0]; af.ab_old[1] = af.ab[1];
+          }
           squad_release(sq, episode);
         }
       } else {
@@ -585,7 +666,7 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
         StageConsts c;
         load_stage_consts(st, pl, lp.w, lp.h, false, c);
         const long long ts0 = DVO_CLOCK(tm);
-        stage_a_run<kCorrected>(tp, pl, geo, c, row_exports, tile_count, a.error_flag, tm);
+        stage_a_run<kCorrected, kAffine>(tp, pl, geo, c, row_exports, tile_count, a.error_flag, tm, brightness());
         DVO_ADD(tm, rounds_a, DVO_CLOCK(tm) - ts0);
       }
       __syncthreads();
@@ -600,6 +681,16 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
         DVO_TOCK(2);
         if (warp == 0) {
           pair_mid_warp<kCorrected>(st, pair, strip_exports, strip_base, lp.nstrips, lp, a.ilog, a.max_log, lt.comb);
+          if constexpr (kAffine) {   // too few constraints: the pose was reverted, and (alpha, beta) go with it
+            AffineState& af = a.affine[pair];
+            if (lane == 0 && !st.level_active) {   // and, as the pose's, no normal equations for the linearisation hook
+              af.ab[0] = af.ab_old[0]; af.ab[1] = af.ab_old[1];
+              if (a.skip_begin) {
+                for (int i = 0; i < 64; ++i) af.A[i] = 0.0;
+                for (int i = 0; i < 8; ++i) af.b[i] = 0.0;
+              }
+            }
+          }
           if (lane == 0) squad_release(sq, episode);
         }
         __syncthreads();
@@ -626,29 +717,33 @@ k_level_persistent(const __grid_constant__ PersistentArgs a) {
         RecordDump dump;
         dump.planes = a.dump; dump.n = lp.n;
         const long long ts0 = DVO_CLOCK(tm);
-        if (a.dump) stage_b_run<true, kCorrected, kCurMask>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
-        else stage_b_run<false, kCorrected, kCurMask>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm);
+        const Brightness br = brightness();
+        if (a.dump) stage_b_run<true, kCorrected, kCurMask, kAffine>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm, br);
+        else stage_b_run<false, kCorrected, kCurMask, kAffine>(tp, pl, geo, c, cb, row_base, strip_base, n_keep, dump, row_partial, tile_count, a.error_flag, tm, br);
         DVO_ADD(tm, rounds_b, DVO_CLOCK(tm) - ts0);
       }
       __syncthreads();
       if (level_ends) break;
       // the rows of each of this CTA's strips, in order, in fp64: one thread per (strip, value)
-      for (int it = threadIdx.x; it < geo.nmine * kNormalValues; it += kCtaThreads) {
-        const int j = it / kNormalValues, i = it - j * kNormalValues;
+      for (int it = threadIdx.x; it < geo.nmine * kNV; it += kCtaThreads) {
+        const int j = it / kNV, i = it - j * kNV;
         const int sj = geo.strip0 + j * geo.strip_step;
         const int nrow = min(kTileH, lp.h - sj * kTileH);
-        const float* rp = row_partial + (size_t)sj * kTileH * kNormalValues + i;
+        const float* rp = row_partial + (size_t)sj * kTileH * kNV + i;
         float r[kTileH];
 #pragma unroll
-        for (int k = 0; k < kTileH; ++k) r[k] = k < nrow ? __ldcg(rp + (size_t)k * kNormalValues) : 0.f;   // independent loads
+        for (int k = 0; k < kTileH; ++k) r[k] = k < nrow ? __ldcg(rp + (size_t)k * kNV) : 0.f;   // independent loads
         double v = 0.0;
 #pragma unroll
         for (int k = 0; k < kTileH; ++k) v += (double)r[k];      // a missing row adds an exact zero
-        strip_partial[(size_t)sj * kNormalValues + i] = v;
+        strip_partial[(size_t)sj * kNV + i] = v;
       }
       DVO_TOCK(1);
       if (squad_arrive(sq, episode, S.g, lt.s_flag)) {
         DVO_TOCK(3);
+        if constexpr (kAffine) {
+          if (threadIdx.x == 0) { lt.end.aff = a.affine + pair; lt.end.keep_system = a.skip_begin; }
+        }
         pair_end_cta(st, pl, pair, strip_partial, lp.nstrips, lp, a.ilog, a.max_log, lt.end, [&] { squad_release(sq, episode); }, S.dbg2 ? S.dbg2 + 64 : nullptr);
         __syncthreads();
         DVO_TOCK(5);
@@ -748,6 +843,15 @@ __global__ void k_set_state(PairState* states, const PairLevel* pls, const doubl
   }
 }
 
+// (alpha, beta) of the photometric mode at the start of a match or test hook: ab (2n doubles, pinned host memory read over
+// PCIe, or NULL = (1, 0) each)
+__global__ void k_affine_init(AffineState* s, const double* ab, int n) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const double a = ab ? ab[2 * p] : 1.0, b = ab ? ab[2 * p + 1] : 0.0;
+  s[p].ab[0] = a; s[p].ab[1] = b; s[p].ab_old[0] = a; s[p].ab_old[1] = b;
+}
+
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
@@ -772,7 +876,8 @@ struct ScratchLayout {
   size_t bytes;
 };
 
-ScratchLayout scratch_layout(const PlanLaunch& L, int npairs) {
+// nvals: normal-equation values per row and strip (kNormalValues, or kNormalValuesAffine in the photometric mode)
+ScratchLayout scratch_layout(const PlanLaunch& L, int npairs, int nvals) {
   ScratchLayout o;
   size_t at = 0;
   auto take = [&](size_t bytes) { const size_t off = at; at += (bytes + 127) / 128 * 128; return off; };
@@ -783,8 +888,8 @@ ScratchLayout scratch_layout(const PlanLaunch& L, int npairs) {
     o.row_base[s] = take(sizeof(int) * rows);
     o.strip_exports[s] = take(sizeof(double) * kStripExportDoubles * strips);
     o.strip_base[s] = take(sizeof(int) * (strips + S.nsquads));   // nstrips + 1 per squad
-    o.row_partial[s] = take(sizeof(float) * kNormalValues * rows);
-    o.strip_partial[s] = take(sizeof(double) * kNormalValues * strips);
+    o.row_partial[s] = take(sizeof(float) * nvals * rows);
+    o.strip_partial[s] = take(sizeof(double) * nvals * strips);
   }
   for (int s = 0; s < L.nseg; ++s) o.squads[s] = take(sizeof(SquadState) * L.seg[s].nsquads);
   o.counters = take(sizeof(SquadState));
@@ -795,7 +900,8 @@ ScratchLayout scratch_layout(const PlanLaunch& L, int npairs) {
 
 // ndesc pair descriptors and states, the scratch arena of the plan's largest launch, the residual-record dump of the test
 // hook and the iteration log.
-int ensure_workspace(dvo_b200_ctx* ctx, int ndesc, const LaunchPlan& plan, int npairs, size_t dump_floats, int max_log_per_pair) {
+int ensure_workspace(dvo_b200_ctx* ctx, int ndesc, const LaunchPlan& plan, int npairs, size_t dump_floats, int max_log_per_pair,
+                     bool affine = false) {
   Workspace& ws = ctx->ws;
   if ((size_t)ndesc > ws.cap_pairs) {
     if (ws.d_pair_level) { cudaStreamSynchronize(ctx->stream); cudaFree(ws.d_pair_level); cudaFree(ws.d_state); }
@@ -805,8 +911,10 @@ int ensure_workspace(dvo_b200_ctx* ctx, int ndesc, const LaunchPlan& plan, int n
     ws.cap_pairs = ndesc;
   }
   size_t scratch = 0;
-  for (int i = 0; i < plan.nlaunch; ++i) scratch = std::max(scratch, scratch_layout(plan.launch[i], npairs).bytes);
+  const int nvals = affine ? kNormalValuesAffine : kNormalValues;
+  for (int i = 0; i < plan.nlaunch; ++i) scratch = std::max(scratch, scratch_layout(plan.launch[i], npairs, nvals).bytes);
   int rc;
+  if (affine && (rc = grow(ctx, ws.d_affine, ws.cap_affine, (size_t)npairs))) return rc;
   if ((rc = grow(ctx, ws.d_scratch, ws.cap_scratch, scratch))) return rc;
   if ((rc = grow(ctx, ws.d_dump, ws.cap_dump, dump_floats))) return rc;
   if (!ws.h_active) DVO_CUDA(ctx, cudaMallocHost((void**)&ws.h_active, sizeof(int) * 8));
@@ -817,7 +925,27 @@ int ensure_workspace(dvo_b200_ctx* ctx, int ndesc, const LaunchPlan& plan, int n
   return 0;
 }
 
-int ensure_geometry(dvo_b200_ctx* ctx) {
+// The photometric instances: queried on their first use, so that the default path's grid stays what it was.
+int ensure_geometry_affine(dvo_b200_ctx* ctx) {
+  if (ctx->ctas_per_sm_affine != 0) return 0;
+  int per_sm = 1 << 30;
+  for (auto kern : {k_level_persistent<false, false, true>, k_level_persistent<true, false, true>, k_level_persistent<false, true, true>,
+                    k_level_persistent<true, true, true>}) {
+    DVO_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLevelSmemBytesOf<true>));
+    int k_per_sm = 0;
+    DVO_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k_per_sm, kern, kCtaThreads, kLevelSmemBytesOf<true>));
+    per_sm = std::min(per_sm, k_per_sm);
+  }
+  if (per_sm < 1) return set_error(ctx, DVO_B200_ERR_CUDA, "persistent kernel (photometric) does not fit on an SM");
+  ctx->ctas_per_sm_affine = per_sm;
+  return 0;
+}
+
+int ensure_geometry(dvo_b200_ctx* ctx, bool affine = false) {
+  if (affine) {
+    if (int rc = ensure_geometry(ctx)) return rc;
+    return ensure_geometry_affine(ctx);
+  }
   if (ctx->num_sms != 0) return 0;
   cudaDeviceProp prop;
   DVO_CUDA(ctx, cudaGetDeviceProperties(&prop, ctx->device));
@@ -838,10 +966,12 @@ int ensure_geometry(dvo_b200_ctx* ctx) {
 
 // The launch plan (launch_plan.h) of a match over levels first .. last of npairs pairs shaped like `ref`, with the plan
 // overrides of the environment as they are now.
-LaunchPlan plan_launches(const dvo_b200_ctx* ctx, const dvo_b200_pyramid* ref, int first, int last, int npairs) {
+// The grid is that of the instance launched: ctas_per_sm, or ctas_per_sm_affine in the photometric mode.
+int grid_ctas(const dvo_b200_ctx* ctx, bool affine) { return ctx->num_sms * (affine ? ctx->ctas_per_sm_affine : ctx->ctas_per_sm); }
+LaunchPlan plan_launches(const dvo_b200_ctx* ctx, const dvo_b200_pyramid* ref, int first, int last, int npairs, bool affine = false) {
   LevelShape shape[kMaxLevels];
   for (int l = 0; l <= first; ++l) shape[l] = {ref->L[l].h, ref->L[l].nbands, ref->L[l].nstrips};
-  return make_launch_plan(shape, first, last, ctx->num_sms * ctx->ctas_per_sm, npairs, plan_knobs_from_env());
+  return make_launch_plan(shape, first, last, grid_ctas(ctx, affine), npairs, plan_knobs_from_env());
 }
 
 // One pyramid of each distinct slab among the batch's pyramids (a batch built in one call shares one slab), in slab order.
@@ -923,10 +1053,11 @@ LevelLaunch make_level_launch(const LevelInfo& L, const dvo_b200_config* cfg, in
 // Enqueue launch `index` of a plan whose level li is pyramid level first - li of `levels`.  Squad states, queues, the ready
 // ring and the error flag are zeroed first; the error flag is copied to ws.h_active[index] after the launch.
 int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo_b200_config* cfg, const LevelInfo* levels,
-                    int first, const double* d_Tinit, int npairs, int max_log, float* dump, int skip_begin, bool cur_mask) {
+                    int first, const double* d_Tinit, int npairs, int max_log, float* dump, int skip_begin, bool cur_mask,
+                    bool affine = false) {
   Workspace& ws = ctx->ws;
   cudaStream_t st = ctx->stream;
-  const ScratchLayout o = scratch_layout(L, npairs);
+  const ScratchLayout o = scratch_layout(L, npairs, affine ? kNormalValuesAffine : kNormalValues);
   char* const base = ws.d_scratch;
   DVO_CUDA(ctx, cudaMemsetAsync(base + o.squads[0], 0, o.bytes - o.squads[0], st));
   PersistentArgs pa;
@@ -938,6 +1069,7 @@ int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo
   pa.dump = dump;
   pa.npairs = npairs; pa.nseg = L.nseg;
   pa.pls0 = ws.d_pair_level; pa.csat = ws.d_csat;
+  pa.affine = affine ? ws.d_affine : nullptr;
   for (int s = 0; s < L.nseg; ++s) {
     const PlanSegment& P = L.seg[s];
     Segment& S = pa.seg[s];
@@ -966,10 +1098,15 @@ int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo
     ProfScope prof_level(ctx, 8 + index);
     void* args[] = {&pa};
     const bool corrected = ctx->estimator == DVO_B200_ESTIMATOR_CORRECTED;
-    const void* kern = cur_mask ? (corrected ? (const void*)k_level_persistent<true, true> : (const void*)k_level_persistent<false, true>)
-                                : (corrected ? (const void*)k_level_persistent<true, false> : (const void*)k_level_persistent<false, false>);
-    DVO_CUDA(ctx, cudaLaunchCooperativeKernel(kern, dim3(ctx->num_sms * ctx->ctas_per_sm),
-                                              dim3(kCtaThreads), args, kLevelSmemBytes, st));
+    const void* kern;
+    if (!affine)
+      kern = cur_mask ? (corrected ? (const void*)k_level_persistent<true, true> : (const void*)k_level_persistent<false, true>)
+                      : (corrected ? (const void*)k_level_persistent<true, false> : (const void*)k_level_persistent<false, false>);
+    else
+      kern = cur_mask ? (corrected ? (const void*)k_level_persistent<true, true, true> : (const void*)k_level_persistent<false, true, true>)
+                      : (corrected ? (const void*)k_level_persistent<true, false, true> : (const void*)k_level_persistent<false, false, true>);
+    DVO_CUDA(ctx, cudaLaunchCooperativeKernel(kern, dim3(grid_ctas(ctx, affine)), dim3(kCtaThreads), args,
+                                              affine ? kLevelSmemBytesOf<true> : kLevelSmemBytes, st));
     ctx->launches++;
   }
   DVO_CUDA(ctx, cudaMemcpyAsync(&ws.h_active[index], pa.error_flag, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -980,17 +1117,19 @@ int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo
 
 int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                         dvo_b200_pyramid* const* curs, const double* T_init, dvo_b200_result* h_results,
-                        void* d_results_user, dvo_b200_iteration_stats* iter_stats, int max_iter_stats) {
+                        void* d_results_user, dvo_b200_iteration_stats* iter_stats, int max_iter_stats, const double* ab_init,
+                        double* ab_out) {
   int rc = check_batch(ctx, cfg, n, refs, curs);
   if (rc) return rc;
   cudaStream_t st = ctx->stream;
   Workspace& ws = ctx->ws;
   const int last = cfg->last_level, first = cfg->first_level;
   const int max_log = iter_stats ? max_iter_stats : 0;
-  if ((rc = ensure_geometry(ctx))) return rc;
+  const bool affine = ab_out != nullptr;
+  if ((rc = ensure_geometry(ctx, affine))) return rc;
   const int nlev = first - last + 1;
-  const LaunchPlan plan = plan_launches(ctx, refs[0], first, last, n);
-  rc = ensure_workspace(ctx, n * nlev, plan, n, 0, max_log);     // d_pair_level holds the descriptors of every level
+  const LaunchPlan plan = plan_launches(ctx, refs[0], first, last, n, affine);
+  rc = ensure_workspace(ctx, n * nlev, plan, n, 0, max_log, affine);     // d_pair_level holds the descriptors of every level
   if (rc) return rc;
 
   // selection masks for non-default thresholds (PointSelection caches per pyramid, point_selection.cpp:100-113)
@@ -1004,7 +1143,8 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   const size_t init_bytes = have_init ? sizeof(double) * 16 * (size_t)n : 0;
   const bool cur_mask = any_current_mask(n, curs);
   const size_t csat_bytes = cur_mask ? (sizeof(const int*) * (size_t)n * nlev + 15) / 16 * 16 : 0;
-  if ((rc = ensure_stage(ctx, 0, desc_bytes + init_bytes + csat_bytes))) return rc;
+  const size_t ab_bytes = affine && ab_init ? sizeof(double) * 2 * (size_t)n : 0;
+  if ((rc = ensure_stage(ctx, 0, desc_bytes + init_bytes + csat_bytes + ab_bytes))) return rc;
   if (cur_mask && (rc = grow(ctx, ws.d_csat, ws.cap_csat, csat_bytes / sizeof(const int*)))) return rc;
   if ((rc = grow(ctx, ws.d_tinit, ws.cap_tinit, (size_t)16 * n))) return rc;
   DVO_CUDA(ctx, cudaStreamSynchronize(st));   // previous use of the pinned stage has drained
@@ -1014,7 +1154,9 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   const int** h_csat = (const int**)((char*)ctx->h_stage + desc_bytes + init_bytes);
   if (cur_mask)
     for (int level = first, li = 0; level >= last; --level, ++li) fill_pair_csat(h_csat + (size_t)li * n, n, curs, level);
-  ctx->h2d_bytes += desc_bytes + init_bytes + csat_bytes;
+  const double* h_ab = (const double*)((char*)ctx->h_stage + desc_bytes + init_bytes + csat_bytes);
+  if (ab_bytes) std::memcpy((void*)h_ab, ab_init, ab_bytes);
+  ctx->h2d_bytes += desc_bytes + init_bytes + csat_bytes + ab_bytes;
   {
     ProfScope prof(ctx, 2);
     const size_t n16 = desc_bytes / 16;
@@ -1030,13 +1172,17 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
       k_stage_words<<<(unsigned)((c16 + 255) / 256), 256, 0, st>>>((const uint4*)h_csat, (uint4*)ws.d_csat, c16);
       ctx->launches++;
     }
+    if (affine) {
+      k_affine_init<<<(n + 255) / 256, 256, 0, st>>>(ws.d_affine, ab_bytes ? h_ab : nullptr, n);
+      ctx->launches++;
+    }
   }
 
   for (int i = 0; i < 8; ++i) ws.h_active[i] = 0;
   if (max_log > 0) DVO_CUDA(ctx, cudaMemsetAsync(ws.d_iter_log, 0, sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log, st));
   for (int i = 0; i < plan.nlaunch; ++i)
     if ((rc = launch_segments(ctx, plan.launch[i], i, cfg, refs[0]->L, first, have_init ? ws.d_tinit : nullptr, n, max_log,
-                              nullptr, 0, cur_mask)))
+                              nullptr, 0, cur_mask, affine)))
       return rc;
   // results
   dvo_b200_result* d_res = (dvo_b200_result*)d_results_user;
@@ -1055,13 +1201,19 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   ctx->pending_level_flags = plan.nlaunch;   // checked at the next synchronisation point (device-results variant)
   if (h_results) {
     size_t bytes = sizeof(dvo_b200_result) * n;
-    if (bytes > ctx->h_results_bytes) {
+    const size_t pinned = bytes + (affine ? sizeof(double) * 2 * (size_t)n : 0);   // the results, then (alpha, beta) of each pair
+    if (pinned > ctx->h_results_bytes) {
       if (ctx->h_results) cudaFreeHost(ctx->h_results);
       ctx->h_results = nullptr; ctx->h_results_bytes = 0;
-      DVO_CUDA(ctx, cudaMallocHost(&ctx->h_results, bytes));
-      ctx->h_results_bytes = bytes;
+      DVO_CUDA(ctx, cudaMallocHost(&ctx->h_results, pinned));
+      ctx->h_results_bytes = pinned;
     }
     DVO_CUDA(ctx, cudaMemcpyAsync(ctx->h_results, d_res, bytes, cudaMemcpyDeviceToHost, st));
+    if (affine) {
+      DVO_CUDA(ctx, cudaMemcpy2DAsync((char*)ctx->h_results + bytes, 2 * sizeof(double), ws.d_affine[0].ab, sizeof(AffineState),
+                                      2 * sizeof(double), (size_t)n, cudaMemcpyDeviceToHost, st));
+      ctx->d2h_bytes += sizeof(double) * 2 * (size_t)n;
+    }
     if (iter_stats) {
       DVO_CUDA(ctx, cudaMemcpyAsync(iter_stats, ws.d_iter_log, sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log,
                                     cudaMemcpyDeviceToHost, st));
@@ -1069,6 +1221,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
     }
     DVO_CUDA(ctx, cudaStreamSynchronize(st));
     std::memcpy(h_results, ctx->h_results, bytes);
+    if (affine) std::memcpy(ab_out, (char*)ctx->h_results + bytes, sizeof(double) * 2 * (size_t)n);
     ctx->d2h_bytes += bytes;
     return check_level_flags(ctx);
   }
@@ -1096,7 +1249,7 @@ int check_level_flags(dvo_b200_ctx* ctx) {
 // pair at a fixed transform: stage A, P_k, stage B (optionally dumping the residual records), end step.
 int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* ref, dvo_b200_pyramid* cur,
                       int level, const double* T, int use_weights, const float* prev_precision, int64_t* count,
-                      float* precision_out, float* ll_out, double* A_out, double* b_out, float* planes7) {
+                      float* precision_out, float* ll_out, double* A_out, double* b_out, float* planes7, const double* ab) {
   dvo_b200_config c = *cfg;
   c.first_level = level; c.last_level = level;
   dvo_b200_pyramid* refs[1] = {ref};
@@ -1107,9 +1260,10 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
   cudaStream_t st = ctx->stream;
   Workspace& ws = ctx->ws;
   const LevelInfo& L = ref->L[level];
-  if ((rc = ensure_geometry(ctx))) return rc;
-  const LaunchPlan plan = plan_launches(ctx, ref, level, level, 1);
-  if ((rc = ensure_workspace(ctx, 1, plan, 1, planes7 ? 7 * (size_t)L.n : 0, 0))) return rc;
+  const bool affine = ab != nullptr;
+  if ((rc = ensure_geometry(ctx, affine))) return rc;
+  const LaunchPlan plan = plan_launches(ctx, ref, level, level, 1, affine);
+  if ((rc = ensure_workspace(ctx, 1, plan, 1, planes7 ? 7 * (size_t)L.n : 0, 0, affine))) return rc;
   if ((rc = pyramid_reselect(ctx, ref, cfg->intensity_derivative_threshold, cfg->depth_derivative_threshold))) return rc;
   c.max_iterations_per_level = use_weights ? 2 : 1;    // k_set_state starts at iteration 1 / 0: exactly one iteration runs
   c.use_initial_estimate = 0; c.precision = 0.0; c.mu = 0.0;
@@ -1130,28 +1284,36 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
   float pp[4] = {0, 0, 0, 0};
   if (use_weights && prev_precision) std::memcpy(pp, prev_precision, sizeof(pp));
   std::memcpy((char*)ctx->h_stage + 128, pp, sizeof(pp));
+  if (affine) std::memcpy((char*)ctx->h_stage + 160, ab, 2 * sizeof(double));
   DVO_CUDA(ctx, cudaMemcpyAsync(ctx->d_stage, ctx->h_stage, 256, cudaMemcpyHostToDevice, st));
   ctx->h2d_bytes += sizeof(PairLevel) + 256;
   k_set_state<<<1, 1, 0, st>>>(ws.d_state, ws.d_pair_level, (const double*)ctx->d_stage,
                                (const float*)((char*)ctx->d_stage + 128), use_weights, lp);
   ctx->launches += 1;
+  if (affine) {
+    k_affine_init<<<1, 32, 0, st>>>(ws.d_affine, (const double*)((char*)ctx->d_stage + 160), 1);
+    ctx->launches += 1;
+  }
   ws.h_active[0] = 0;
-  if ((rc = launch_segments(ctx, plan.launch[0], 0, &c, ref->L, level, nullptr, 1, 0, planes7 ? ws.d_dump : nullptr, 1, cur_mask)))
+  if ((rc = launch_segments(ctx, plan.launch[0], 0, &c, ref->L, level, nullptr, 1, 0, planes7 ? ws.d_dump : nullptr, 1, cur_mask,
+                            affine)))
     return rc;
   DVO_CUDA(ctx, cudaGetLastError());
   if ((rc = note_foreign_uses(ctx, 1, refs, curs))) return rc;
   PairState* hs = nullptr;
-  if ((rc = ensure_stage(ctx, 0, sizeof(PairState) + 64))) return rc;
+  if ((rc = ensure_stage(ctx, 0, sizeof(PairState) + sizeof(AffineState) + 64))) return rc;
   hs = (PairState*)ctx->h_stage;
+  AffineState* ha = (AffineState*)((char*)ctx->h_stage + (sizeof(PairState) + 15) / 16 * 16);
   DVO_CUDA(ctx, cudaMemcpyAsync(hs, ws.d_state, sizeof(PairState), cudaMemcpyDeviceToHost, st));
+  if (affine) DVO_CUDA(ctx, cudaMemcpyAsync(ha, ws.d_affine, sizeof(AffineState), cudaMemcpyDeviceToHost, st));
   DVO_CUDA(ctx, cudaStreamSynchronize(st));
   ctx->pending_level_flags = 1;
   if ((rc = check_level_flags(ctx))) return rc;
   if (count) *count = hs->n;
   if (precision_out) std::memcpy(precision_out, hs->precision, sizeof(float) * 4);
   if (ll_out) *ll_out = hs->ll;
-  if (A_out) std::memcpy(A_out, hs->A, sizeof(double) * 36);
-  if (b_out) std::memcpy(b_out, hs->b, sizeof(double) * 6);
+  if (A_out) std::memcpy(A_out, affine ? ha->A : hs->A, sizeof(double) * (affine ? 64 : 36));
+  if (b_out) std::memcpy(b_out, affine ? ha->b : hs->b, sizeof(double) * (affine ? 8 : 6));
   if (planes7) {
     // {ei, ez, gx, gy, hx, hy, z_ref}; invalid -> NaN in every plane
     DVO_CUDA(ctx, cudaMemcpy(planes7, ws.d_dump, sizeof(float) * 7 * (size_t)L.n, cudaMemcpyDeviceToHost));

@@ -26,7 +26,8 @@ ABI_SYMBOLS = [
     "dvo_b200_pyramid_create_raw_batch", "dvo_b200_pyramid_create_bgr_batch",
     "dvo_b200_pyramid_retain", "dvo_b200_pyramid_release", "dvo_b200_pyramid_num_levels", "dvo_b200_pyramid_level_info",
     "dvo_b200_pyramid_download", "dvo_b200_pyramid_select", "dvo_b200_match", "dvo_b200_match_batch",
-    "dvo_b200_match_batch_device", "dvo_b200_residual_image", "dvo_b200_intensity_error_image", "dvo_b200_linearize", "dvo_b200_profile_enable",
+    "dvo_b200_match_batch_device", "dvo_b200_residual_image", "dvo_b200_intensity_error_image", "dvo_b200_linearize", "dvo_b200_match_batch_photometric", "dvo_b200_residual_image_photometric",
+    "dvo_b200_linearize_photometric", "dvo_b200_profile_enable",
     "dvo_b200_profile_read", "dvo_b200_pyramid_device", "dvo_b200_sharded_create", "dvo_b200_sharded_destroy",
     "dvo_b200_sharded_num_shards", "dvo_b200_sharded_ctx", "dvo_b200_sharded_last_error", "dvo_b200_shard_range",
     "dvo_b200_sharded_pyramid_create_batch", "dvo_b200_sharded_pyramid_create_raw_batch", "dvo_b200_match_batch_sharded",
@@ -292,6 +293,10 @@ def load_library():
     L.dvo_b200_residual_image.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, fp, C.POINTER(i64)]
     L.dvo_b200_intensity_error_image.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, fp, C.POINTER(i64)]
     L.dvo_b200_linearize.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, i32, fp, C.POINTER(i64), fp, fp, dp, dp]
+    L.dvo_b200_match_batch_photometric.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), dp, dp, C.POINTER(CResult),
+                                                   dp, C.POINTER(IterationStats), i32]
+    L.dvo_b200_residual_image_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, fp, C.POINTER(i64)]
+    L.dvo_b200_linearize_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, i32, fp, C.POINTER(i64), fp, fp, dp, dp]
     L.dvo_b200_set_estimator.argtypes = [vp, i32]
     L.dvo_b200_get_estimator.argtypes = [vp]
     L.dvo_b200_profile_enable.argtypes = [vp, i32]
@@ -723,7 +728,18 @@ class Engine:
     def match(self, ref: Pyramid, cur: Pyramid, cfg: Config, T_init=None, with_iterations: bool = False) -> Result:
         return self.match_batch([ref], [cur], cfg, None if T_init is None else [T_init], with_iterations)[0]
 
-    def match_batch(self, refs, curs, cfg: Config, T_init=None, with_iterations: bool = False, raw: bool = False):
+    def match_batch_photometric(self, refs, curs, cfg: Config, T_init=None, photometric_init=None, with_iterations: bool = False):
+        """match_batch in the photometric mode (include/dvo_b200.h): the pose and an intensity gain and bias per pair.
+        photometric_init: [n, 2] (alpha, beta) or None = (1, 0).  Returns (results, [n, 2] float64 final (alpha, beta))."""
+        n = len(refs)
+        ab0 = None
+        if photometric_init is not None:
+            ab0 = np.ascontiguousarray(np.asarray(photometric_init, dtype=np.float64).reshape(n, 2))
+        ab = np.zeros((n, 2), dtype=np.float64)
+        out = self.match_batch(refs, curs, cfg, T_init, with_iterations, _photometric=(ab0, ab))
+        return out, ab
+
+    def match_batch(self, refs, curs, cfg: Config, T_init=None, with_iterations: bool = False, raw: bool = False, _photometric=None):
         n = len(refs)
         assert n == len(curs) and n > 0
         rh = (C.c_void_p * n)(*[p.handle for p in refs])
@@ -737,9 +753,14 @@ class Engine:
         if with_iterations:
             max_log = (cfg.first_level - cfg.last_level + 1) * (cfg.max_iterations_per_level + 1)
             log = (IterationStats * (n * max_log))()
-        self._check(self.lib.dvo_b200_match_batch(self.ctx, C.byref(cfg), n, rh, ch,
-                                                  T.ctypes.data_as(C.POINTER(C.c_double)) if T is not None else None,
-                                                  res, log, max_log))
+        Tp = T.ctypes.data_as(C.POINTER(C.c_double)) if T is not None else None
+        if _photometric is None:
+            self._check(self.lib.dvo_b200_match_batch(self.ctx, C.byref(cfg), n, rh, ch, Tp, res, log, max_log))
+        else:
+            ab0, ab = _photometric
+            self._check(self.lib.dvo_b200_match_batch_photometric(
+                self.ctx, C.byref(cfg), n, rh, ch, Tp, ab0.ctypes.data_as(C.POINTER(C.c_double)) if ab0 is not None else None, res,
+                ab.ctypes.data_as(C.POINTER(C.c_double)), log, max_log))
         if raw:
             return res
         out = []
@@ -765,15 +786,20 @@ class Engine:
                                                          T.ctypes.data_as(C.POINTER(C.c_double)) if T is not None else None,
                                                          C.c_void_p(d_results_ptr)))
 
-    def residual_image(self, ref: Pyramid, cur: Pyramid, level: int, T, cfg: Config | None = None):
+    def residual_image(self, ref: Pyramid, cur: Pyramid, level: int, T, cfg: Config | None = None, ab=None):
+        """ab = (alpha, beta): the photometric mode's hook at that brightness model (dvo_b200_residual_image_photometric)."""
         cfg = cfg or Config()
         w, h, _ = ref.level_info(level)
         out = np.empty((7, h, w), dtype=np.float32)
         T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(16))
         cnt = C.c_int64()
-        self._check(self.lib.dvo_b200_residual_image(self.ctx, C.byref(cfg), ref.handle, cur.handle, level,
-                                                     T.ctypes.data_as(C.POINTER(C.c_double)),
-                                                     out.ctypes.data_as(C.POINTER(C.c_float)), C.byref(cnt)))
+        Tp, op = T.ctypes.data_as(C.POINTER(C.c_double)), out.ctypes.data_as(C.POINTER(C.c_float))
+        if ab is None:
+            self._check(self.lib.dvo_b200_residual_image(self.ctx, C.byref(cfg), ref.handle, cur.handle, level, Tp, op, C.byref(cnt)))
+        else:
+            ab = np.ascontiguousarray(np.asarray(ab, dtype=np.float64).reshape(2))
+            self._check(self.lib.dvo_b200_residual_image_photometric(self.ctx, C.byref(cfg), ref.handle, cur.handle, level, Tp,
+                                                                     ab.ctypes.data_as(C.POINTER(C.c_double)), op, C.byref(cnt)))
         return cnt.value, out
 
     def intensity_error_image(self, ref: Pyramid, cur: Pyramid, level: int, T, cfg: Config | None = None):
@@ -788,21 +814,29 @@ class Engine:
                                                             out.ctypes.data_as(C.POINTER(C.c_float)), C.byref(cnt)))
         return int(cnt.value), out
 
-    def linearize(self, ref: Pyramid, cur: Pyramid, level: int, T, use_weights=False, prev_precision=None, cfg: Config | None = None):
+    def linearize(self, ref: Pyramid, cur: Pyramid, level: int, T, use_weights=False, prev_precision=None, cfg: Config | None = None,
+                  ab=None):
+        """ab = (alpha, beta): the photometric mode's hook (dvo_b200_linearize_photometric); A is then 8 x 8 and b 8."""
         cfg = cfg or Config()
         T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(16))
         pp = np.ascontiguousarray(np.asarray(prev_precision if prev_precision is not None else np.zeros(4), dtype=np.float32).reshape(4))
         P = np.zeros(4, dtype=np.float32)
         ll = C.c_float()
-        A = np.zeros(36)
-        b = np.zeros(6)
+        k = 6 if ab is None else 8
+        A = np.zeros(k * k)
+        b = np.zeros(k)
         cnt = C.c_int64()
-        self._check(self.lib.dvo_b200_linearize(self.ctx, C.byref(cfg), ref.handle, cur.handle, level,
-                                                T.ctypes.data_as(C.POINTER(C.c_double)), int(use_weights),
-                                                pp.ctypes.data_as(C.POINTER(C.c_float)), C.byref(cnt),
-                                                P.ctypes.data_as(C.POINTER(C.c_float)), C.byref(ll),
-                                                A.ctypes.data_as(C.POINTER(C.c_double)), b.ctypes.data_as(C.POINTER(C.c_double))))
-        return {"n": cnt.value, "precision": P.reshape(2, 2), "ll": ll.value, "A": A.reshape(6, 6), "b": b}
+        Tp, ppp = T.ctypes.data_as(C.POINTER(C.c_double)), pp.ctypes.data_as(C.POINTER(C.c_float))
+        Pp, Ap, bp = P.ctypes.data_as(C.POINTER(C.c_float)), A.ctypes.data_as(C.POINTER(C.c_double)), b.ctypes.data_as(C.POINTER(C.c_double))
+        if ab is None:
+            self._check(self.lib.dvo_b200_linearize(self.ctx, C.byref(cfg), ref.handle, cur.handle, level, Tp, int(use_weights), ppp,
+                                                    C.byref(cnt), Pp, C.byref(ll), Ap, bp))
+        else:
+            ab = np.ascontiguousarray(np.asarray(ab, dtype=np.float64).reshape(2))
+            self._check(self.lib.dvo_b200_linearize_photometric(self.ctx, C.byref(cfg), ref.handle, cur.handle, level, Tp,
+                                                                ab.ctypes.data_as(C.POINTER(C.c_double)), int(use_weights), ppp,
+                                                                C.byref(cnt), Pp, C.byref(ll), Ap, bp))
+        return {"n": cnt.value, "precision": P.reshape(2, 2), "ll": ll.value, "A": A.reshape(k, k), "b": b}
 
     # ---- profiling ----
     def profile_enable(self, on: bool = True):

@@ -289,3 +289,10 @@ def make_overlay_pair(seed: int, size=(160, 120), corner=(420, 300), margin: int
     mask[max(y0 - margin, 0):y0 + ph + margin, max(x0 - margin, 0):x0 + pw + margin] = 0
     out["mask"] = mask
     return out
+
+
+def exposure(I, gain: float, bias: float):
+    """An auto-exposure / white-balance change of a frame: clip(round(gain I + bias), 0, 255), in float32 arithmetic (gain and
+    bias rounded to float32, ties to even)."""
+    I = np.asarray(I, dtype=np.float32)
+    return np.clip(np.round(np.float32(gain) * I + np.float32(bias)), 0, 255).astype(np.float32)

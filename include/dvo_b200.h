@@ -488,6 +488,48 @@ int dvo_b200_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_p
                        const float* prev_precision, int64_t* count, float* precision_out, float* ll_out,
                        double* A_out, double* b_out);
 
+/* ---- photometric mode: an affine brightness change per pair, estimated jointly with the pose ----------------------
+ * Auto exposure and white balance change the intensity of consecutive frames by a global gain and offset, which the
+ * brightness-constancy residual cannot absorb.  In this mode every alignment estimates 8 unknowns, the pose xi, a gain
+ * alpha and a bias beta, with the model I_cur(w(x)) ~ alpha I_ref(x) + beta (intensities on the 0..255 scale of the
+ * pyramid).  With either estimator and with current-role masks; the default entry points are unchanged.  Operation by
+ * operation:
+ *   residual   e_i = c_i I_cur(w) - c_i fmaf(alpha, I_ref, beta), c_i = 1/255, with (alpha, beta) rounded to float: at
+ *              (1, 0) it is the default e_i bit for bit.  The depth residual, the validity of a point, the occlusion test
+ *              and the selection do not depend on (alpha, beta).
+ *   weights, scale, log-likelihood: the estimator's own formulas over the new e_i (REFERENCE: with its three quirks).
+ *   normal equations: 8 x 8 over (xi, alpha, beta) with W = w P_k.  The intensity row adds de_i/dalpha = -c_i I_ref and
+ *              de_i/dbeta = -c_i; the depth row has zeros there.  Jacobians at the untransformed point, as by default.
+ *   prior      mu acts on the pose block as by default (A_ii += mu, b_i += mu log(initial)_i for i < 6); none on alpha, beta.
+ *   solve      8 x 8 LDL^T in fp64 with the pivot rule of the 6 x 6.  The pose is updated as by default, alpha += dalpha,
+ *              beta += dbeta (fp64), with the pose: an increment is applied when the pose's is, and a rejected iteration
+ *              (LogLikelihoodDecreased, TooFewConstraints) reverts all 8 together.
+ *   termination IncrementTooSmall tests the 6 pose components only; precision keeps its meaning.  The rest is unchanged.
+ *   levels     (alpha, beta) carry over from level to level unchanged (the 2 x 2 mean commutes with an affine map).
+ *   outputs    transformation and log_likelihood keep their meaning.  information is the Schur complement of the 8 x 8
+ *              (prior included) onto the pose, A_xx - A_xp A_pp^-1 A_px, times 0.008^2 as by default; iteration stats carry
+ *              the pose part of the increment and the same Schur complement; level stats are unchanged.
+ * Not provided in this mode: match_batch_device and the sharded forms. */
+
+/* dvo_b200_match_batch in the photometric mode.  photometric_init: 2n doubles (alpha, beta) per pair, or NULL = (1, 0) each;
+ * photometric: 2n doubles out, the final (alpha, beta) of each pair.  A NULL photometric or a non-finite photometric_init is
+ * refused with DVO_B200_ERR_INVALID_ARGUMENT before anything is uploaded or launched; every other argument is checked as
+ * dvo_b200_match_batch checks it. */
+int dvo_b200_match_batch_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n,
+                                     dvo_b200_pyramid* const* references, dvo_b200_pyramid* const* currents,
+                                     const double* T_init, const double* photometric_init, dvo_b200_result* results,
+                                     double* photometric, dvo_b200_iteration_stats* iteration_stats,
+                                     int32_t max_iteration_stats);
+/* The test hooks at a fixed (alpha, beta) = ab (finite, else DVO_B200_ERR_INVALID_ARGUMENT), on the same kernel instance as
+ * the photometric match.  dvo_b200_linearize_photometric returns the whole 8 x 8 A (row-major, no prior) and the 8 of b. */
+int dvo_b200_residual_image_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,
+                                        dvo_b200_pyramid* current, int32_t level, const double* T, const double ab[2],
+                                        float* planes7, int64_t* count);
+int dvo_b200_linearize_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,
+                                   dvo_b200_pyramid* current, int32_t level, const double* T, const double ab[2],
+                                   int32_t use_weights, const float* prev_precision, int64_t* count, float* precision_out,
+                                   float* ll_out, double A_out[64], double b_out[8]);
+
 /* ---- profiling hooks (bench.py roofline): per-kernel-class accumulated device time measured with
  *      CUDA events on the ctx stream.  classes: 0 residual/scale stage, 1 normal-equation stage,
  *      2 per-pair step kernels, 3 pyramid build, 4 selection. -------------------------------- */
