@@ -1,5 +1,6 @@
 // capi.cu -- the extern "C" surface declared in include/dvo_b200.h.
 #include "common.cuh"
+#include "prior_args.h"
 
 #include <cmath>
 #include <cstdio>
@@ -272,7 +273,7 @@ int dvo_b200_destroy(dvo_b200_ctx* ctx) {
   for (cudaEvent_t e : ctx->event_pool) cudaEventDestroy(e);
   Workspace& ws = ctx->ws;
   cudaFree(ws.d_pair_level); cudaFree(ws.d_state); cudaFree(ws.d_scratch); cudaFree(ws.d_dump); cudaFree(ws.d_tinit);
-  cudaFree(ws.d_iter_log); cudaFree(ws.d_csat);
+  cudaFree(ws.d_iter_log); cudaFree(ws.d_csat); cudaFree(ws.d_prior);
   if (ws.h_active) cudaFreeHost(ws.h_active);
   pool_close(ctx);
   cudaFree(ctx->d_stage);
@@ -726,6 +727,21 @@ int dvo_b200_match_batch_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* c
   cudaSetDevice(ctx->device);
   return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
                              iteration_stats ? max_iteration_stats : 0, photometric_init, photometric);
+}
+
+// ---- motion prior ----
+int dvo_b200_match_batch_prior(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,
+                               dvo_b200_pyramid* const* currents, const double* T_init, const double* prior_information,
+                               const double* photometric_init, double* photometric, dvo_b200_result* results,
+                               dvo_b200_iteration_stats* iteration_stats, int32_t max_iteration_stats) {
+  if (!ctx || !results) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_prior: null argument");
+  const std::string why = prior_args_error(cfg, n, prior_information, photometric_init, photometric);
+  if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
+  if (photometric_init && n > 0 && !all_finite(photometric_init, 2 * (size_t)n))
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_prior: photometric_init is not finite");
+  cudaSetDevice(ctx->device);
+  return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
+                             iteration_stats ? max_iteration_stats : 0, photometric_init, photometric, prior_information);
 }
 
 int dvo_b200_residual_image_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,

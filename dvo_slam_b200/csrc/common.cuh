@@ -167,8 +167,9 @@ struct Workspace {              // per-ctx scratch of the level kernel
   double* d_tinit = nullptr;         // per pair initial estimate (4x4)
   dvo_b200_iteration_stats* d_iter_log = nullptr;
   AffineState* d_affine = nullptr;   // per pair of a photometric alignment
+  double* d_prior = nullptr;         // per pair of an alignment with a motion prior: the 6 x 6 information, row-major
   int* h_active = nullptr;           // pinned: per launch of a call, the kernel's error flag
-  size_t cap_pairs = 0, cap_scratch = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0, cap_affine = 0;
+  size_t cap_pairs = 0, cap_scratch = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0, cap_affine = 0, cap_prior = 0;
 };
 
 }  // namespace dvo_b200
@@ -178,6 +179,7 @@ struct dvo_b200_ctx {
   uint64_t uid = 0;                   // unique over the process lifetime (a context's address may be reused after destroy)
   int num_sms = 0, ctas_per_sm = 0;   // persistent-kernel grid geometry (queried once)
   int ctas_per_sm_affine = 0;         // the same for the instances of the photometric mode
+  int ctas_per_sm_prior[2] = {0, 0};  // the same for the instances with a motion prior: [0] default, [1] photometric mode
   int estimator = DVO_B200_ESTIMATOR_REFERENCE;   // dvo_b200_estimator of every later alignment / test hook on this context
   unsigned long long* d_dbg = nullptr;   // DVO_B200_TIMING=1: per-level phase timers of the persistent kernel (64 slots)
   cudaStream_t stream = nullptr;
@@ -252,10 +254,11 @@ int ensure_stage(dvo_b200_ctx* ctx, size_t dev_bytes, size_t host_bytes);
 // tracker.cu
 // ab_out != NULL: the photometric mode (8 unknowns: pose, gain, bias), from ab_init (2n doubles, NULL = (1, 0) each); the
 // final (alpha, beta) of each pair go to ab_out (host, 2n doubles).  Needs h_results.
+// prior != NULL: a motion prior, n row-major 6 x 6 informations (host) in place of cfg->mu I (which must then be 0).
 int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                         dvo_b200_pyramid* const* curs, const double* T_init, dvo_b200_result* h_results,
                         void* d_results, dvo_b200_iteration_stats* iter_stats, int max_iter_stats,
-                        const double* ab_init = nullptr, double* ab_out = nullptr);
+                        const double* ab_init = nullptr, double* ab_out = nullptr, const double* prior = nullptr);
 int check_level_flags(dvo_b200_ctx* ctx);   // after a stream synchronisation: did a level kernel report a timeout?
 int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* ref, dvo_b200_pyramid* cur,
                       int level, const double* T, int use_weights, const float* prev_precision, int64_t* count,

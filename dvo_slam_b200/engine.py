@@ -36,7 +36,7 @@ ABI_SYMBOLS = [
     "dvo_b200_undistort_map", "dvo_b200_rectifier_create", "dvo_b200_rectifier_release", "dvo_b200_pyramid_create_rectified_batch",
     "dvo_b200_pyramid_create_rectified_device_batch", "dvo_b200_depth_rays", "dvo_b200_depth_registration_create",
     "dvo_b200_depth_registration_release", "dvo_b200_pyramid_create_registered_batch",
-    "dvo_b200_pyramid_create_registered_device_batch",
+    "dvo_b200_pyramid_create_registered_device_batch", "dvo_b200_match_batch_prior",
 ]
 
 # dvo_b200_estimator
@@ -215,6 +215,14 @@ class Result:
         return not (np.isfinite(self.transformation.sum()) and np.isfinite(self.information.sum()))
 
 
+def prior_from_result(result: Result, scale: float = 1.0) -> np.ndarray:
+    """A motion prior (Engine.match_batch(prior_information=...)) from an earlier alignment of the same motion:
+    scale * Result.information / 0.008^2, in the units of the normal equations, made exactly symmetric (the photometric
+    mode's Schur complement is symmetric only to rounding).  scale < 1 trusts the earlier alignment less."""
+    lam = np.asarray(result.information, dtype=np.float64).reshape(6, 6) * (scale / 0.008 ** 2)
+    return 0.5 * (lam + lam.T)
+
+
 _lib = None
 
 
@@ -295,6 +303,8 @@ def load_library():
     L.dvo_b200_linearize.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, i32, fp, C.POINTER(i64), fp, fp, dp, dp]
     L.dvo_b200_match_batch_photometric.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), dp, dp, C.POINTER(CResult),
                                                    dp, C.POINTER(IterationStats), i32]
+    L.dvo_b200_match_batch_prior.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), dp, dp, dp, dp, C.POINTER(CResult),
+                                             C.POINTER(IterationStats), i32]
     L.dvo_b200_residual_image_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, fp, C.POINTER(i64)]
     L.dvo_b200_linearize_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, i32, fp, C.POINTER(i64), fp, fp, dp, dp]
     L.dvo_b200_set_estimator.argtypes = [vp, i32]
@@ -728,18 +738,23 @@ class Engine:
     def match(self, ref: Pyramid, cur: Pyramid, cfg: Config, T_init=None, with_iterations: bool = False) -> Result:
         return self.match_batch([ref], [cur], cfg, None if T_init is None else [T_init], with_iterations)[0]
 
-    def match_batch_photometric(self, refs, curs, cfg: Config, T_init=None, photometric_init=None, with_iterations: bool = False):
+    def match_batch_photometric(self, refs, curs, cfg: Config, T_init=None, photometric_init=None, with_iterations: bool = False,
+                                prior_information=None):
         """match_batch in the photometric mode (include/dvo_b200.h): the pose and an intensity gain and bias per pair.
-        photometric_init: [n, 2] (alpha, beta) or None = (1, 0).  Returns (results, [n, 2] float64 final (alpha, beta))."""
+        photometric_init: [n, 2] (alpha, beta) or None = (1, 0).  prior_information as in match_batch.  Returns (results,
+        [n, 2] float64 final (alpha, beta))."""
         n = len(refs)
         ab0 = None
         if photometric_init is not None:
             ab0 = np.ascontiguousarray(np.asarray(photometric_init, dtype=np.float64).reshape(n, 2))
         ab = np.zeros((n, 2), dtype=np.float64)
-        out = self.match_batch(refs, curs, cfg, T_init, with_iterations, _photometric=(ab0, ab))
+        out = self.match_batch(refs, curs, cfg, T_init, with_iterations, _photometric=(ab0, ab), prior_information=prior_information)
         return out, ab
 
-    def match_batch(self, refs, curs, cfg: Config, T_init=None, with_iterations: bool = False, raw: bool = False, _photometric=None):
+    def match_batch(self, refs, curs, cfg: Config, T_init=None, with_iterations: bool = False, raw: bool = False, _photometric=None,
+                    prior_information=None):
+        """prior_information: [n, 6, 6] float64, a motion prior per pair in place of cfg.mu I (dvo_b200_match_batch_prior,
+        which requires cfg.mu == 0); prior_from_result builds one from an earlier Result."""
         n = len(refs)
         assert n == len(curs) and n > 0
         rh = (C.c_void_p * n)(*[p.handle for p in refs])
@@ -753,14 +768,23 @@ class Engine:
         if with_iterations:
             max_log = (cfg.first_level - cfg.last_level + 1) * (cfg.max_iterations_per_level + 1)
             log = (IterationStats * (n * max_log))()
-        Tp = T.ctypes.data_as(C.POINTER(C.c_double)) if T is not None else None
-        if _photometric is None:
+        dp = C.POINTER(C.c_double)
+        Tp = T.ctypes.data_as(dp) if T is not None else None
+        ab0, ab = _photometric if _photometric is not None else (None, None)
+        ab0p = ab0.ctypes.data_as(dp) if ab0 is not None else None
+        if prior_information is not None:
+            lam = np.asarray(prior_information, dtype=np.float64)
+            if lam.size != 36 * n:
+                raise ValueError(f"prior_information {lam.shape}: want [{n}, 6, 6]")
+            lam = np.ascontiguousarray(lam.reshape(n, 36))
+            self._check(self.lib.dvo_b200_match_batch_prior(
+                self.ctx, C.byref(cfg), n, rh, ch, Tp, lam.ctypes.data_as(dp), ab0p, ab.ctypes.data_as(dp) if ab is not None else None,
+                res, log, max_log))
+        elif _photometric is None:
             self._check(self.lib.dvo_b200_match_batch(self.ctx, C.byref(cfg), n, rh, ch, Tp, res, log, max_log))
         else:
-            ab0, ab = _photometric
-            self._check(self.lib.dvo_b200_match_batch_photometric(
-                self.ctx, C.byref(cfg), n, rh, ch, Tp, ab0.ctypes.data_as(C.POINTER(C.c_double)) if ab0 is not None else None, res,
-                ab.ctypes.data_as(C.POINTER(C.c_double)), log, max_log))
+            self._check(self.lib.dvo_b200_match_batch_photometric(self.ctx, C.byref(cfg), n, rh, ch, Tp, ab0p, res, ab.ctypes.data_as(dp),
+                                                                  log, max_log))
         if raw:
             return res
         out = []

@@ -8,6 +8,7 @@
 #include <stdexcept>
 
 #include "dvo/dense_tracking.h"
+#include "../csrc/prior_args.h"   // the prior checks of dvo_b200_match_batch_prior, run here so that a refusal returns false
 
 namespace dvo {
 namespace core {
@@ -361,8 +362,43 @@ static void fill_result(const dvo_b200_result& r, const dvo_b200_iteration_stats
 
 bool DenseTracker::matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
                               std::vector<Result>& results) {
+  return matchBatch(references, currents, static_cast<const double*>(0), results);
+}
+
+bool DenseTracker::matchWithPrior(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current,
+                                  const core::Matrix6d& prior_information, Result& result) {
+  std::vector<core::RgbdImagePyramid*> refs(1, &reference), curs(1, &current);
+  std::vector<core::Matrix6d> priors(1, prior_information);
+  std::vector<Result> results(1, result);
+  const bool ok = matchBatch(refs, curs, priors, results);
+  if (ok) result = results[0];
+  return ok;
+}
+
+bool DenseTracker::matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
+                              const std::vector<core::Matrix6d>& prior_information, std::vector<Result>& results) {
+  const size_t n = references.size();
+  if (prior_information.size() != n) return false;
+  std::vector<double> L(36 * n);
+  for (size_t i = 0; i < n; ++i)
+    for (int a = 0; a < 6; ++a)
+      for (int b = 0; b < 6; ++b) L[36 * i + a * 6 + b] = prior_information[i](a, b);
+  std::vector<Result> out(results);
+  out.resize(n);
+  if (!matchBatch(references, currents, n ? L.data() : 0, out)) return false;
+  results = out;
+  return true;
+}
+
+bool DenseTracker::matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
+                              const double* prior_information, std::vector<Result>& results) {
   const size_t n = references.size();
   if (n == 0 || currents.size() != n) return false;
+  if (prior_information) {   // refused before any upload
+    dvo_b200_config pc;
+    pc.mu = cfg.Mu;
+    if (!dvo_b200::prior_args_error(&pc, int(n), prior_information, 0, 0).empty()) return false;
+  }
   results.resize(n);
   dvo_b200_ctx* ctx = context();
   dvo_b200_config c;
@@ -387,8 +423,11 @@ bool DenseTracker::matchBatch(const std::vector<core::RgbdImagePyramid*>& refere
   std::vector<dvo_b200_result> raw(n);
   const int max_log = collect_iterations_ ? (cfg.FirstLevel - cfg.LastLevel + 1) * (cfg.MaxIterationsPerLevel + 1) : 0;
   std::vector<dvo_b200_iteration_stats> log(size_t(max_log) * n);
-  int rc = dvo_b200_match_batch(ctx, &c, int(n), r.data(), q.data(), cfg.UseInitialEstimate ? T.data() : 0, raw.data(),
-                                max_log ? log.data() : 0, max_log);
+  const double* T0 = cfg.UseInitialEstimate ? T.data() : 0;
+  int rc = prior_information
+               ? dvo_b200_match_batch_prior(ctx, &c, int(n), r.data(), q.data(), T0, prior_information, 0, 0, raw.data(),
+                                            max_log ? log.data() : 0, max_log)
+               : dvo_b200_match_batch(ctx, &c, int(n), r.data(), q.data(), T0, raw.data(), max_log ? log.data() : 0, max_log);
   if (rc != 0) throw std::runtime_error(std::string("dvo_b200_match_batch: ") + dvo_b200_last_error(ctx));
   for (size_t i = 0; i < n; ++i) fill_result(raw[i], max_log ? &log[size_t(max_log) * i] : 0, results[i]);
   return true;   // the reference's match() always returns true (dense_tracking.cpp:135,375)

@@ -104,6 +104,14 @@ class DenseTracker {
   bool matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
                   std::vector<Result>& results);
 
+  // --- extension: a motion prior, a 6 x 6 prior information per pair in place of Mu I (dvo_b200_match_batch_prior; units and
+  // coordinates in include/dvo_b200.h).  Returns false, without aligning, when Mu != 0 or a prior is refused (not finite, not
+  // exactly symmetric, not positive semi-definite). ---
+  bool matchWithPrior(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current, const core::Matrix6d& prior_information,
+                      Result& result);
+  bool matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
+                  const std::vector<core::Matrix6d>& prior_information, std::vector<Result>& results);
+
   // per-iteration statistics are copied back only when requested (they are optional in the C ABI)
   void collectIterationStatistics(bool on) { collect_iterations_ = on; }
   // Extension: the corrected estimator of dvo_b200_estimator (exact scale sum, log-likelihood over all points, the odd last
@@ -112,6 +120,8 @@ class DenseTracker {
 
  private:
   dvo_b200_ctx* context();
+  bool matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
+                  const double* prior_information, std::vector<Result>& results);   // prior_information: n * 36 or NULL
   Config cfg;
   dvo_b200_ctx* ctx_;
   bool collect_iterations_;

@@ -530,6 +530,46 @@ int dvo_b200_linearize_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg
                                    int32_t use_weights, const float* prev_precision, int64_t* count, float* precision_out,
                                    float* ll_out, double A_out[64], double b_out[8]);
 
+/* ---- motion prior: a full 6 x 6 prior information per pair on the pose, in place of mu I -----------------------------
+ * What a caller knows about the motion -- a constant-velocity prediction with the previous alignment's information, an
+ * IMU or wheel-odometry preintegration with its covariance, the relative pose of a keyframe-graph edge -- enters each
+ * alignment as a symmetric positive semi-definite Lambda_p (row-major, fp64), one per pair.  Definitions:
+ *   T0       the initial estimate as the kernel reads it: T_init of the pair when cfg->use_initial_estimate is set and T_init
+ *            is given, else the identity.
+ *   initial  the reference's Revertable "initial" (dense_tracking.cpp:147-149, 259-261), T0 estimate^-1 at every iteration.
+ *   li       log(initial) in the twist order of the engine, [v; omega].
+ * Where the default path uses mu, this one uses Lambda_p:
+ *   normal equations         A + Lambda_p          (default A + mu I)
+ *   right-hand side          b + Lambda_p li       (default b + mu li)
+ *   prior log-likelihood     li^T Lambda_p li      (default mu sum li^2)
+ *   iteration information    A + Lambda_p          (default A + mu I)
+ *   result information       (A_last + Lambda_p) 0.008^2
+ * Result.log_likelihood keeps its meaning, with this prior term.  The accept test ignores the prior, as by default
+ * (SURVEY Q18); termination, the Revertable handling and the levels are unchanged.  In the photometric mode Lambda_p acts on
+ * the pose block of the 8 x 8 system, exactly where mu does (A_ij, b_i for i, j < 6, and the system whose Schur complement
+ * is the information); there is no prior on (alpha, beta).
+ * Units and coordinates: Lambda has the units of A, not of Result.information.  The prior is on eps where
+ * estimate = exp(eps) T0; equivalently Result.transformation = T0^-1 exp(-eps), a right perturbation of the returned
+ * transformation.  An IMU covariance Sigma in those coordinates gives Lambda = Sigma^-1; a previous alignment of the same
+ * motion gives Lambda = Result.information / 0.008^2, because its A is in the same coordinates.
+ * Arithmetic: b_i + sum_j Lambda_ij li_j is an in-order FMA chain over j and A_ij + Lambda_ij one addition, so Lambda = mu I
+ * returns the bits of dvo_b200_match_batch[_photometric] with cfg->mu = mu in everything but the prior log-likelihood (and
+ * with it log_likelihood), which may differ in the last bits; Lambda = 0 returns the bits of mu = 0 in everything.
+ * Not provided in this mode: match_batch_device and the sharded forms. */
+
+/* dvo_b200_match_batch with a prior information per pair.  prior_information: n * 36 doubles, pair p's Lambda at p * 36.
+ * photometric NULL: the default 6-unknown mode; non-NULL: the photometric mode, photometric_init and photometric as in
+ * dvo_b200_match_batch_photometric.  Refused with DVO_B200_ERR_INVALID_ARGUMENT before anything is staged, uploaded or
+ * launched: a NULL prior_information; photometric_init without photometric; cfg->mu != 0 (the prior replaces mu I rather
+ * than adding to it); a Lambda_p with a non-finite entry, with Lambda_ij != Lambda_ji (exact comparison) or with an
+ * eigenvalue below -1e-9 max(1, max |Lambda_ij|); and everything dvo_b200_match_batch[_photometric] refuses.  A zero row
+ * means no prior in that direction. */
+int dvo_b200_match_batch_prior(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n,
+                               dvo_b200_pyramid* const* references, dvo_b200_pyramid* const* currents,
+                               const double* T_init, const double* prior_information, const double* photometric_init,
+                               double* photometric, dvo_b200_result* results, dvo_b200_iteration_stats* iteration_stats,
+                               int32_t max_iteration_stats);
+
 /* ---- profiling hooks (bench.py roofline): per-kernel-class accumulated device time measured with
  *      CUDA events on the ctx stream.  classes: 0 residual/scale stage, 1 normal-equation stage,
  *      2 per-pair step kernels, 3 pyramid build, 4 selection. -------------------------------- */
