@@ -529,13 +529,17 @@ float compute_ll(const std::vector<ErrPoint>& e, const float P[4], const orc_mod
   for (size_t k = 0; k < n; ++k, ++c) {
     float x = e[k].e[0], y = e[k].e[1];
     float d = (x * P[0] + y * P[2]) * x + (x * P[1] + y * P[3]) * y;  // r^T P r in float
+    if (!mode.ll_group_product) {   // the per-point logs summed; ll_drop_tail still drops the last n % 50
+      if (!mode.ll_drop_tail || k < n - n % 50) error_sum += std::log(1.0 + 0.2 * double(d));
+      continue;
+    }
     error_acc *= (1.0 + 0.2 * double(d));
     if ((c % 50) == 0) {
       error_sum += std::log(error_acc);
       error_acc = 1.0;
     }
   }
-  if (!mode.ll_drop_tail) error_sum += std::log(error_acc);
+  if (mode.ll_group_product && !mode.ll_drop_tail) error_sum += std::log(error_acc);
   float det = P[0] * P[3] - P[1] * P[2];
   return float(0.5 * double(n) * double(std::log(det)) - 0.5 * (5.0 + 2.0) * error_sum);
 }
@@ -643,9 +647,9 @@ int64_t max_points(const orc_pyramid* p, int level) {  // point_selection.cpp:68
 // ==========================================================================================
 extern "C" {
 
-orc_mode orc_mode_faithful(void) { return orc_mode{1, 1, 1, 1, 1, 1, 0}; }
-orc_mode orc_mode_exact(void) { return orc_mode{0, 0, 0, 0, 0, 0, 0}; }
-orc_mode orc_mode_mirror(void) { return orc_mode{0, 0, 1, 1, 1, 0, 1}; }
+orc_mode orc_mode_faithful(void) { return orc_mode{1, 1, 1, 1, 1, 1, 0, 1}; }
+orc_mode orc_mode_exact(void) { return orc_mode{0, 0, 0, 0, 0, 0, 0, 0}; }
+orc_mode orc_mode_mirror(void) { return orc_mode{0, 0, 1, 1, 1, 0, 1, 1}; }
 
 orc_config orc_config_default(void) {  // dense_tracking_config.cpp:27-42
   orc_config c;

@@ -32,10 +32,15 @@
  *   fused_pixel_math  per-pixel arithmetic written with explicit fmaf() in the order the
  *                     CUDA kernels use (bit-mirror of the GPU residual record); off = the
  *                     reference's unfused mul/add order.
+ *   ll_group_product  log-likelihood sum as the log of fp64 products of (1 + 0.2 d) over groups of 50 points
+ *                     (dense_tracking_impl.cpp:406-425): a group whose product overflows makes it -inf, and the
+ *                     iteration is rejected; off = the sum of the per-point logs, finite wherever every d is.
  * Presets: FAITHFUL = all reference quirks on, fused off.   (timed CPU baseline, parity target)
  *          EXACT    = everything off (exact division, nearest rounding, fp64 sums).
- *          MIRROR   = structural quirks on (drop_odd_point, scale_pair_bug, ll_drop_tail),
+ *          MIRROR   = structural quirks on (drop_odd_point, scale_pair_bug, ll_drop_tail, ll_group_product),
  *                     numerical noise off, fused_pixel_math on: what the GPU path computes.
+ *          The corrected estimator's definition (tests/helpers.py corrected_mode) is MIRROR with the four structural
+ *          quirks off.
  */
 #ifndef DVO_ORACLE_H_
 #define DVO_ORACLE_H_
@@ -56,6 +61,7 @@ typedef struct orc_mode {
   int ll_drop_tail;
   int f32_serial_accum;
   int fused_pixel_math;
+  int ll_group_product;
 } orc_mode;
 
 /* mirrors dvo::DenseTracker::Config fields that influence match() (dense_tracking.h:42-69) */

@@ -22,7 +22,7 @@ TERMINATION_NAMES = ["IterationsExceeded", "IncrementTooSmall", "LogLikelihoodDe
 
 class Mode(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("rcp_approx", "rtz_residuals", "drop_odd_point", "scale_pair_bug",
-                                       "ll_drop_tail", "f32_serial_accum", "fused_pixel_math")]
+                                       "ll_drop_tail", "f32_serial_accum", "fused_pixel_math", "ll_group_product")]
 
 
 class Config(C.Structure):

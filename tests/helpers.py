@@ -41,6 +41,19 @@ def nan_equal(a, b):
     return np.array_equal(np.isnan(a), np.isnan(b)) and np.array_equal(a[~np.isnan(a)], b[~np.isnan(b)])
 
 
+def corrected_mode(orc, fused=1):
+    """the corrected estimator's oracle definition: MIRROR with the reference's four structural quirks off -- the scale's
+    pair bug, the dropped log-likelihood tail, the dropped odd point, and the log-likelihood as logs of 50-point products
+    (which overflow to -inf where the per-point sum the kernel computes is finite)"""
+    m = orc.mode("mirror")
+    m.scale_pair_bug = 0
+    m.ll_drop_tail = 0
+    m.drop_odd_point = 0
+    m.ll_group_product = 0
+    m.fused_pixel_math = fused
+    return m
+
+
 # TerminationCriteria (dense_tracking.h:62-78), as dvo_b200_termination and the oracle number them
 TERM_ITERATIONS_EXCEEDED, TERM_INCREMENT_TOO_SMALL, TERM_LOG_LIKELIHOOD_DECREASED, TERM_TOO_FEW_CONSTRAINTS = 0, 1, 2, 3
 
@@ -68,6 +81,69 @@ def level_fields(iterations, termination):
         out["last_increment_valid_constraints"] = e["n"]
         out["last_increment_log_likelihood"] = e["nll"]
     return out
+
+
+# ---- the named alignment cases of tests/test_gpu_statistics.py and tests/test_step_replay_host.py -------------------
+# Every termination path is reached by one of them (asserted from the oracle in test_gpu_statistics.py): IncrementTooSmall,
+# IterationsExceeded (max_iterations_per_level 1 and 0), LogLikelihoodDecreased, TooFewConstraints on the first iteration of
+# the last level, TooFewConstraints on the first iteration turned into IncrementTooSmall by the post-loop check, and
+# TooFewConstraints after an accepted iteration on the last level.  All 160x120, 3 levels.
+STATISTICS_CFG = dict(first_level=2, last_level=0, max_iterations_per_level=50, precision=1e-4)
+STATISTICS_CASES = ["golden11", "golden12", "golden13", "iterations_1", "iterations_0", "increment_too_small", "initial_estimate",
+                    "tfc_first_iteration", "tfc_overridden", "tfc_after_accept"]
+
+
+def golden_case(seed, **cfg):
+    """a golden pair as a case dict (images, K, levels, cfg, T_init), STATISTICS_CFG updated by cfg"""
+    from oracle import oracle_py as orc
+    g = load_golden(seed)
+    im = golden_images(g, orc)
+    c = dict(STATISTICS_CFG)
+    c.update(cfg)
+    return dict(I_ref=im["I_ref"], Z_ref=im["Z_ref"], I_cur=im["I_cur"], Z_cur=im["Z_cur"], K=g["K"], levels=GOLDEN_LEVELS,
+                cfg=c, T_init=None)
+
+
+def statistics_case(name):
+    """(images, intrinsics, levels, config, T_init) of a named case of STATISTICS_CASES"""
+    if name.startswith("golden"):
+        return golden_case(int(name[6:]))
+    if name == "iterations_1":
+        return golden_case(12, max_iterations_per_level=1)
+    if name == "iterations_0":
+        return golden_case(12, max_iterations_per_level=0)
+    if name == "increment_too_small":
+        return golden_case(13, precision=2e-3)
+    if name == "initial_estimate":
+        c = golden_case(11, use_initial_estimate=1, mu=0.05)
+        c["T_init"] = load_golden(11)["kat_T"]
+        return c
+    if name == "tfc_first_iteration":
+        # level-0 depth of the current frame NaN on every odd row and column: no 2x2 bilinear footprint is valid there, the
+        # coarser levels (which subsample the even pixels) keep their depth -> TooFewConstraints on the first iteration of
+        # the last level, with the increment of level 1 still large
+        c = golden_case(11)
+        Z = c["Z_cur"].copy()
+        Z[1::2, :] = np.nan
+        Z[:, 1::2] = np.nan
+        c["Z_cur"] = Z
+        return c
+    if name == "tfc_overridden":
+        # no valid current depth: TooFewConstraints on the first iteration of every level, with the initial increment 0 ->
+        # the post-loop check makes it IncrementTooSmall, and LastIterationWithIncrement() is that one entry
+        c = golden_case(12)
+        c["Z_cur"] = np.full_like(c["Z_cur"], np.nan)
+        return c
+    if name == "tfc_after_accept":
+        # found by a seeded search over large-motion 160x120 scenes: the one accepted iteration of level 0 moves the camera
+        # off the overlap and the next finds no constraint; FAITHFUL and MIRROR agree on every level's flow
+        from dvo_slam_b200 import synth
+        scfg = synth.SceneConfig(width=160, height=120, intrinsics=tuple(v / 4 for v in synth.FR1_INTRINSICS),
+                                 max_translation=0.3, max_rotation=0.2)
+        p = synth.make_pair(26, scfg)
+        return dict(I_ref=p["I_ref"].numpy(), Z_ref=p["Z_ref"].numpy(), I_cur=p["I_cur"].numpy(), Z_cur=p["Z_cur"].numpy(),
+                    K=p["intrinsics"], levels=3, cfg=dict(STATISTICS_CFG), T_init=None)
+    raise KeyError(name)
 
 
 # ---- the pin against the original project's object code (tests/test_reference_pin.py, tests/golden/make_reference_pin.py) ----

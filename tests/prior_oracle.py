@@ -31,6 +31,9 @@ def lib():
         L.orc_pyramid_create.restype = vp
         L.orc_pyramid_create.argtypes = [fp, fp, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int]
         L.orc_pyramid_destroy.argtypes = [vp]
+        L.orc_pyramid_plane.restype = fp
+        L.orc_pyramid_plane.argtypes = [vp, C.c_int, C.c_int]
+        L.orc_pyramid_level_info.argtypes = [vp, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), fp]
         L.orc_match.restype = C.c_int
         L.orc_match.argtypes = [vp, vp, C.POINTER(orc.Config), dp, C.POINTER(orc.Mode), C.POINTER(orc.Result),
                                 C.POINTER(orc.IterationStats), C.c_int, C.POINTER(C.c_int)]
@@ -49,12 +52,20 @@ def _d(a):
 
 
 class Pyramid:
-    def __init__(self, intensity, depth, intrinsics, levels):
+    def __init__(self, intensity, depth, intrinsics, levels, mask=None):
+        """mask: as photometric_oracle.Pyramid's (NaN depth at every unusable pixel of every level, both roles)"""
         I = np.ascontiguousarray(intensity, dtype=np.float32)
         Z = np.ascontiguousarray(depth, dtype=np.float32)
         h, w = I.shape
         fp = C.POINTER(C.c_float)
         self.h = lib().orc_pyramid_create(I.ctypes.data_as(fp), Z.ctypes.data_as(fp), w, h, *intrinsics, levels)
+        if mask is not None:
+            from masked_oracle import usable_by_footprint
+            for l, usable in enumerate(usable_by_footprint(mask, levels)):
+                lw, lh, K = C.c_int(), C.c_int(), (C.c_float * 4)()
+                lib().orc_pyramid_level_info(self.h, l, C.byref(lw), C.byref(lh), K)
+                z = np.ctypeslib.as_array(lib().orc_pyramid_plane(self.h, l, 1), shape=(lh.value, lw.value))
+                z[~usable] = np.nan
 
     def __del__(self):
         if getattr(self, "h", None) and _lib is not None:

@@ -1,7 +1,7 @@
 """The corrected estimator without a GPU: its C ABI entry points, and the oracle definition the GPU kernel is checked against.
 
-"corrected" = the oracle's MIRROR mode with the three structural quirks of the reference off (scale_pair_bug, ll_drop_tail,
-drop_odd_point): scale = sum_i w_i r_i r_i^T / (n - 3), log-likelihood over all n points, the odd last point kept."""
+"corrected" = the oracle's MIRROR mode with the four structural quirks of the reference off (helpers.corrected_mode):
+scale = sum_i w_i r_i r_i^T / (n - 3), log-likelihood over all n points as the sum of their logs, the odd last point kept."""
 import ctypes as C
 import os
 import re
@@ -9,18 +9,9 @@ import re
 import numpy as np
 import pytest
 
-from helpers import GOLDEN_SEEDS, golden_images, load_golden, odd_point_margin
+from helpers import GOLDEN_SEEDS, corrected_mode, golden_images, load_golden, odd_point_margin  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def corrected_mode(orc, fused=1):
-    m = orc.mode("mirror")
-    m.scale_pair_bug = 0
-    m.ll_drop_tail = 0
-    m.drop_odd_point = 0
-    m.fused_pixel_math = fused
-    return m
 
 
 @pytest.fixture(scope="module")
@@ -105,3 +96,38 @@ def test_oracle_corrected_keeps_the_odd_point(oracle):
     other = np.ones(pm[0].size, bool)
     other[last] = False
     assert np.array_equal(np.isnan(pm[0].reshape(-1)[other]), np.isnan(pc[0].reshape(-1)[other]))
+
+
+def overflow_state(orc):
+    """golden pair 11, level 0, a small offset, weights from a previous precision of 1e10 I: the weighted scale is tiny, so
+    r^T P r is ~1e9 and a 50-point product of (1 + 0.2 d) passes DBL_MAX -- (pyramids, T, prev_precision)"""
+    g = load_golden(11)
+    im = golden_images(g, orc)
+    oref = orc.Pyramid(im["I_ref"], im["Z_ref"], g["K"], 3)
+    ocur = orc.Pyramid(im["I_cur"], im["Z_cur"], g["K"], 3)
+    T = np.eye(4)
+    T[:3, 3] = [0.01, -0.005, 0.02]
+    return im, g["K"], oref, ocur, T, np.array([[1e10, 0.0], [0.0, 1e10]], dtype=np.float32)
+
+
+def test_oracle_corrected_log_likelihood_past_the_products_overflow(oracle):
+    """The reference takes the log of fp64 products of (1 + 0.2 d) over groups of 50 points; where one overflows its
+    log-likelihood is -inf and the iteration is rejected.  The corrected estimator sums the per-point logs (as the kernel
+    does): finite, and equal to that sum computed here from the residual image and the returned P."""
+    _, _, oref, ocur, T, pp = overflow_state(oracle)
+    assert oracle.linearize(oref, ocur, 0, T, oracle.mode("mirror"), True, pp)["ll"] == -np.inf
+    grouped = corrected_mode(oracle)
+    grouped.ll_group_product = 1
+    assert oracle.linearize(oref, ocur, 0, T, grouped, True, pp)["ll"] == -np.inf
+    m = corrected_mode(oracle)
+    lin = oracle.linearize(oref, ocur, 0, T, m, True, pp)
+    n_img, planes = oracle.residual_image(oref, ocur, 0, T, m)
+    E = planes[0:2].reshape(2, -1).T
+    E = E[~np.isnan(E[:, 0])]
+    assert E.shape[0] == n_img == lin["n"]
+    Pk = lin["precision"].astype(np.float32)
+    x, y = E[:, 0], E[:, 1]
+    d = (x * Pk[0, 0] + y * Pk[1, 0]) * x + (x * Pk[0, 1] + y * Pk[1, 1]) * y
+    detP = np.float32(Pk[0, 0] * Pk[1, 1] - Pk[0, 1] * Pk[1, 0])
+    ll = 0.5 * n_img * float(np.log(detP)) - 3.5 * float(np.sum(np.log1p(0.2 * d.astype(np.float64))))
+    assert np.isfinite(lin["ll"]) and abs(lin["ll"] - ll) <= 1e-5 * abs(ll), (lin["ll"], ll)

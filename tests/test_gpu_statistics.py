@@ -14,73 +14,14 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from helpers import (GOLDEN_LEVELS, TERM_INCREMENT_TOO_SMALL, TERM_ITERATIONS_EXCEEDED,
-                     TERM_LOG_LIKELIHOOD_DECREASED, TERM_TOO_FEW_CONSTRAINTS, golden_images, level_fields, load_golden,
-                     split_levels)
+from helpers import STATISTICS_CASES as CASES
+from helpers import STATISTICS_CFG as CFG
+from helpers import (TERM_INCREMENT_TOO_SMALL, TERM_ITERATIONS_EXCEEDED, TERM_LOG_LIKELIHOOD_DECREASED,
+                     TERM_TOO_FEW_CONSTRAINTS, level_fields, split_levels)
+from helpers import statistics_case as _case
 
-CFG = dict(first_level=2, last_level=0, max_iterations_per_level=50, precision=1e-4)
 FIELDS = ("has_iteration_with_increment", "last_valid_constraints", "last_increment_valid_constraints",
           "last_increment_log_likelihood")
-
-
-def _golden(seed, **cfg):
-    g = load_golden(seed)
-    im = golden_images(g, _orc())
-    c = dict(CFG)
-    c.update(cfg)
-    return dict(I_ref=im["I_ref"], Z_ref=im["Z_ref"], I_cur=im["I_cur"], Z_cur=im["Z_cur"], K=g["K"], levels=GOLDEN_LEVELS,
-                cfg=c, T_init=None)
-
-
-def _orc():
-    from oracle import oracle_py as orc
-    return orc
-
-
-def _case(name):
-    """(images, intrinsics, levels, config, T_init) of a named case"""
-    if name.startswith("golden"):
-        return _golden(int(name[6:]))
-    if name == "iterations_1":
-        return _golden(12, max_iterations_per_level=1)
-    if name == "iterations_0":
-        return _golden(12, max_iterations_per_level=0)
-    if name == "increment_too_small":
-        return _golden(13, precision=2e-3)
-    if name == "initial_estimate":
-        c = _golden(11, use_initial_estimate=1, mu=0.05)
-        c["T_init"] = load_golden(11)["kat_T"]
-        return c
-    if name == "tfc_first_iteration":
-        # level-0 depth of the current frame NaN on every odd row and column: no 2x2 bilinear footprint is valid there, the
-        # coarser levels (which subsample the even pixels) keep their depth -> TooFewConstraints on the first iteration of
-        # the last level, with the increment of level 1 still large
-        c = _golden(11)
-        Z = c["Z_cur"].copy()
-        Z[1::2, :] = np.nan
-        Z[:, 1::2] = np.nan
-        c["Z_cur"] = Z
-        return c
-    if name == "tfc_overridden":
-        # no valid current depth: TooFewConstraints on the first iteration of every level, with the initial increment 0 ->
-        # the post-loop check makes it IncrementTooSmall, and LastIterationWithIncrement() is that one entry
-        c = _golden(12)
-        c["Z_cur"] = np.full_like(c["Z_cur"], np.nan)
-        return c
-    if name == "tfc_after_accept":
-        # found by a seeded search over large-motion 160x120 scenes: the one accepted iteration of level 0 moves the camera
-        # off the overlap and the next finds no constraint; FAITHFUL and MIRROR agree on every level's flow
-        from dvo_slam_b200 import synth
-        scfg = synth.SceneConfig(width=160, height=120, intrinsics=tuple(v / 4 for v in synth.FR1_INTRINSICS),
-                                 max_translation=0.3, max_rotation=0.2)
-        p = synth.make_pair(26, scfg)
-        return dict(I_ref=p["I_ref"].numpy(), Z_ref=p["Z_ref"].numpy(), I_cur=p["I_cur"].numpy(), Z_cur=p["Z_cur"].numpy(),
-                    K=p["intrinsics"], levels=3, cfg=dict(CFG), T_init=None)
-    raise KeyError(name)
-
-
-CASES = ["golden11", "golden12", "golden13", "iterations_1", "iterations_0", "increment_too_small", "initial_estimate",
-         "tfc_first_iteration", "tfc_overridden", "tfc_after_accept"]
 
 
 def _oracle_match(orc, c, mode="mirror"):
