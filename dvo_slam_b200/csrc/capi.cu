@@ -1,7 +1,9 @@
 // capi.cu -- the extern "C" surface declared in include/dvo_b200.h.
 #include "common.cuh"
+#include "maps_args.h"
 #include "prior_args.h"
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -273,7 +275,7 @@ int dvo_b200_destroy(dvo_b200_ctx* ctx) {
   for (cudaEvent_t e : ctx->event_pool) cudaEventDestroy(e);
   Workspace& ws = ctx->ws;
   cudaFree(ws.d_pair_level); cudaFree(ws.d_state); cudaFree(ws.d_scratch); cudaFree(ws.d_dump); cudaFree(ws.d_tinit);
-  cudaFree(ws.d_iter_log); cudaFree(ws.d_csat); cudaFree(ws.d_prior);
+  cudaFree(ws.d_iter_log); cudaFree(ws.d_csat); cudaFree(ws.d_prior); cudaFree(ws.d_maps);
   if (ws.h_active) cudaFreeHost(ws.h_active);
   pool_close(ctx);
   cudaFree(ctx->d_stage);
@@ -742,6 +744,44 @@ int dvo_b200_match_batch_prior(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, in
   cudaSetDevice(ctx->device);
   return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
                              iteration_stats ? max_iteration_stats : 0, photometric_init, photometric, prior_information);
+}
+
+// ---- weight maps ----
+int dvo_b200_match_batch_maps(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,
+                              dvo_b200_pyramid* const* currents, const double* T_init, const double* prior_information,
+                              const double* photometric_init, double* photometric, dvo_b200_result* results,
+                              dvo_b200_iteration_stats* iteration_stats, int32_t max_iteration_stats, const dvo_b200_weight_maps* maps) {
+  if (!ctx || !results) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_maps: null argument");
+  // the refusals of the entry point without maps that come before its batch checks
+  if (prior_information) {
+    const std::string why = prior_args_error(cfg, n, prior_information, photometric_init, photometric);
+    if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
+  } else if (photometric_init && !photometric) {
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_maps: photometric_init without photometric");
+  }
+  if (photometric_init && n > 0 && !all_finite(photometric_init, 2 * (size_t)n))
+    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_maps: photometric_init is not finite");
+  cudaSetDevice(ctx->device);
+  // the largest extents of the batch; a batch the match would refuse is left to its checks (n = 0 here)
+  MapsExtent ext{0, 0, 0, 0};
+  bool sane = cfg && n > 0 && references && cfg->last_level >= 0 && cfg->last_level < kMaxLevels;
+  for (int32_t i = 0; sane && i < n; ++i) {
+    const dvo_b200_pyramid* r = references[i];
+    if (!r || r->levels <= cfg->last_level) { sane = false; break; }
+    ext.w = std::max(ext.w, r->L[cfg->last_level].w); ext.h = std::max(ext.h, r->L[cfg->last_level].h);
+    ext.w0 = std::max(ext.w0, r->L[0].w); ext.h0 = std::max(ext.h0, r->L[0].h);
+  }
+  const int device = ctx->device;
+  const std::string why = maps_args_error(maps, sane ? n : 0, ext, device, [](const void* p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return PtrWhere{kPtrHost, -1}; }
+    if (a.type == cudaMemoryTypeDevice) return PtrWhere{kPtrDevice, a.device};
+    if (a.type == cudaMemoryTypeManaged) return PtrWhere{kPtrManaged, a.device};
+    return PtrWhere{kPtrHost, -1};
+  });
+  if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
+  return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
+                             iteration_stats ? max_iteration_stats : 0, photometric_init, photometric, prior_information, maps);
 }
 
 int dvo_b200_residual_image_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,

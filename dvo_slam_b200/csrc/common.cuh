@@ -168,8 +168,10 @@ struct Workspace {              // per-ctx scratch of the level kernel
   dvo_b200_iteration_stats* d_iter_log = nullptr;
   AffineState* d_affine = nullptr;   // per pair of a photometric alignment
   double* d_prior = nullptr;         // per pair of an alignment with a motion prior: the 6 x 6 information, row-major
+  char* d_maps = nullptr;            // weight maps copied back to the host (DVO_B200_MAPS_HOST): the kernel's packed output
   int* h_active = nullptr;           // pinned: per launch of a call, the kernel's error flag
   size_t cap_pairs = 0, cap_scratch = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0, cap_affine = 0, cap_prior = 0;
+  size_t cap_maps = 0;
 };
 
 }  // namespace dvo_b200
@@ -258,11 +260,22 @@ int ensure_stage(dvo_b200_ctx* ctx, size_t dev_bytes, size_t host_bytes);
 int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                         dvo_b200_pyramid* const* curs, const double* T_init, dvo_b200_result* h_results,
                         void* d_results, dvo_b200_iteration_stats* iter_stats, int max_iter_stats,
-                        const double* ab_init = nullptr, double* ab_out = nullptr, const double* prior = nullptr);
+                        const double* ab_init = nullptr, double* ab_out = nullptr, const double* prior = nullptr,
+                        const dvo_b200_weight_maps* maps = nullptr);   // maps != NULL: also the weight maps (weight_maps.cu)
 int check_level_flags(dvo_b200_ctx* ctx);   // after a stream synchronisation: did a level kernel report a timeout?
 int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* ref, dvo_b200_pyramid* cur,
                       int level, const double* T, int use_weights, const float* prev_precision, int64_t* count,
                       float* precision_out, float* ll_out, double* A_out, double* b_out, float* planes7,
                       const double* ab = nullptr);   // ab != NULL: photometric mode at (alpha, beta); A_out 8 x 8, b_out 8
+
+// weight_maps.cu, the weight maps of a match (maps checked by maps_args.h).  prepare: before the match's first launch, the
+// device scratch of DVO_B200_MAPS_HOST.  launch: k_weight_maps on the batch's final pair states, after the level kernels and
+// k_finalize (level = cfg->last_level; d_pls: the batch's descriptors of that level; d_affine: the photometric mode's
+// brightness states, or NULL); a launch error surfaces at the caller's next cudaGetLastError.  copy_back: with
+// DVO_B200_MAPS_HOST, the copies into the caller's host layout, before the call's synchronisation.
+int weight_maps_prepare(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int n, const dvo_b200_pyramid* ref0, int level);
+void weight_maps_launch(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int n, const dvo_b200_pyramid* ref0, int level,
+                        const PairLevel* d_pls, const AffineState* d_affine);
+int weight_maps_copy_back(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int n, const dvo_b200_pyramid* ref0, int level);
 
 }  // namespace dvo_b200

@@ -1098,6 +1098,9 @@ struct RecordDump {
   float* planes;   // nullptr: off
   int n;
 };
+// Defined in the level kernel's translation unit only: a second one (weight_maps.cu, DVO_B200_STAGES_NO_DUMP) never dumps, and
+// a second definition of this external function would not link.
+#ifndef DVO_B200_STAGES_NO_DUMP
 __device__ __noinline__ void dump_record(const RecordDump& dump, size_t i, bool valid, f2 E, f2 G, f2 H, float z) {
   const float nanv = __int_as_float(0x7fc00000);
   float* p = dump.planes + i;
@@ -1107,6 +1110,9 @@ __device__ __noinline__ void dump_record(const RecordDump& dump, size_t i, bool 
   p[4 * n] = valid ? lo(H) : nanv; p[5 * n] = valid ? hi(H) : nanv;
   p[6 * n] = valid ? z : nanv;
 }
+#else
+__device__ void dump_record(const RecordDump& dump, size_t i, bool valid, f2 E, f2 G, f2 H, float z);
+#endif
 
 // Stage B rounds of one tile row (kExact, kFirst: see stage_a_rounds).  The exact loop also leaves out the rank count of the
 // dropped log-likelihood tail: strips that reach past n_keep (cta_has_tail, at most a few per level) take the generic loop.

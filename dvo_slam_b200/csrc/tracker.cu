@@ -1218,7 +1218,7 @@ int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo
 int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                         dvo_b200_pyramid* const* curs, const double* T_init, dvo_b200_result* h_results,
                         void* d_results_user, dvo_b200_iteration_stats* iter_stats, int max_iter_stats, const double* ab_init,
-                        double* ab_out, const double* prior) {
+                        double* ab_out, const double* prior, const dvo_b200_weight_maps* maps) {
   int rc = check_batch(ctx, cfg, n, refs, curs);
   if (rc) return rc;
   cudaStream_t st = ctx->stream;
@@ -1233,6 +1233,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   rc = ensure_workspace(ctx, n * nlev, plan, n, 0, max_log, affine);     // d_pair_level holds the descriptors of every level
   if (rc) return rc;
   if (with_prior && (rc = grow(ctx, ws.d_prior, ws.cap_prior, (size_t)36 * n))) return rc;
+  if (maps && (rc = weight_maps_prepare(ctx, *maps, n, refs[0], last))) return rc;
 
   // selection masks for non-default thresholds (PointSelection caches per pyramid, point_selection.cpp:100-113)
   for (int i = 0; i < n; ++i)
@@ -1307,6 +1308,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
     k_finalize<<<(n + 63) / 64, 64, 0, st>>>(ws.d_state, d_res, n);
     ctx->launches++;
   }
+  if (maps) weight_maps_launch(ctx, *maps, n, refs[0], last, ws.d_pair_level + (size_t)(nlev - 1) * n, affine ? ws.d_affine : nullptr);
   DVO_CUDA(ctx, cudaGetLastError());
   if ((rc = note_foreign_uses(ctx, n, refs, curs))) return rc;   // the caller may release the pyramids once this returns
   ctx->pending_level_flags = plan.nlaunch;   // checked at the next synchronisation point (device-results variant)
@@ -1325,6 +1327,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
                                       2 * sizeof(double), (size_t)n, cudaMemcpyDeviceToHost, st));
       ctx->d2h_bytes += sizeof(double) * 2 * (size_t)n;
     }
+    if (maps && (rc = weight_maps_copy_back(ctx, *maps, n, refs[0], last))) return rc;
     if (iter_stats) {
       DVO_CUDA(ctx, cudaMemcpyAsync(iter_stats, ws.d_iter_log, sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log,
                                     cudaMemcpyDeviceToHost, st));

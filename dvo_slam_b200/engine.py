@@ -36,7 +36,7 @@ ABI_SYMBOLS = [
     "dvo_b200_undistort_map", "dvo_b200_rectifier_create", "dvo_b200_rectifier_release", "dvo_b200_pyramid_create_rectified_batch",
     "dvo_b200_pyramid_create_rectified_device_batch", "dvo_b200_depth_rays", "dvo_b200_depth_registration_create",
     "dvo_b200_depth_registration_release", "dvo_b200_pyramid_create_registered_batch",
-    "dvo_b200_pyramid_create_registered_device_batch", "dvo_b200_match_batch_prior",
+    "dvo_b200_pyramid_create_registered_device_batch", "dvo_b200_match_batch_prior", "dvo_b200_match_batch_maps",
 ]
 
 # dvo_b200_estimator
@@ -44,6 +44,9 @@ ESTIMATORS = {"reference": 0, "corrected": 1}
 
 # dvo_b200_input_format (dvo_b200_pyramid_create_masked_batch)
 INPUT_FORMATS = {"float32": 0, "grey8_depth16": 1, "bgr8_depth16": 2}
+
+# dvo_b200_weight_maps.memory
+MAPS_MEMORY = {"device": 0, "host": 1}
 
 # role sets of a mask (DVO_B200_MASK_ROLE_*): "reference" = the selection only, "both" = also the current image's taps
 MASK_ROLES = {"reference": 1, "both": 3}
@@ -187,6 +190,17 @@ class LevelStats(C.Structure):
                 ("last_increment_log_likelihood", C.c_double)]
 
 
+class MapPlane(C.Structure):
+    """dvo_b200_map_plane: one output plane of dvo_b200_match_batch_maps (data NULL: not written)"""
+    _fields_ = [("data", C.c_void_p), ("row_bytes", C.c_int64), ("image_bytes", C.c_int64)]
+
+
+class WeightMaps(C.Structure):
+    """dvo_b200_weight_maps: where dvo_b200_match_batch_maps writes each pair's maps"""
+    _fields_ = [("memory", C.c_int32), ("weight", MapPlane), ("residual_i", MapPlane), ("residual_z", MapPlane), ("mask", MapPlane),
+                ("mask_weight", C.c_float), ("estimate", C.POINTER(C.c_double)), ("precision", C.POINTER(C.c_float))]
+
+
 class CResult(C.Structure):
     _fields_ = [("transformation", C.c_double * 16), ("information", C.c_double * 36), ("log_likelihood", C.c_double),
                 ("num_levels", C.c_int32), ("num_iterations_total", C.c_int32), ("levels", LevelStats * MAX_LEVELS)]
@@ -305,6 +319,8 @@ def load_library():
                                                    dp, C.POINTER(IterationStats), i32]
     L.dvo_b200_match_batch_prior.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), dp, dp, dp, dp, C.POINTER(CResult),
                                              C.POINTER(IterationStats), i32]
+    L.dvo_b200_match_batch_maps.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), dp, dp, dp, dp, C.POINTER(CResult),
+                                            C.POINTER(IterationStats), i32, C.POINTER(WeightMaps)]
     L.dvo_b200_residual_image_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, fp, C.POINTER(i64)]
     L.dvo_b200_linearize_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, i32, fp, C.POINTER(i64), fp, fp, dp, dp]
     L.dvo_b200_set_estimator.argtypes = [vp, i32]
@@ -751,8 +767,53 @@ class Engine:
         out = self.match_batch(refs, curs, cfg, T_init, with_iterations, _photometric=(ab0, ab), prior_information=prior_information)
         return out, ab
 
+    def match_batch_maps(self, refs, curs, cfg: Config, T_init=None, prior_information=None, photometric_init=None,
+                         photometric: bool = False, mask_weight=None, with_iterations: bool = False):
+        """An alignment and each pair's weight maps at its returned pose (dvo_b200_match_batch_maps; "weight maps" in
+        include/dvo_b200.h).  The results (and (alpha, beta)) are those of match_batch / match_batch_photometric with the same
+        arguments.  Returns (results, maps), or (results, maps, [n, 2] (alpha, beta)) when photometric.  maps holds torch CUDA
+        tensors on the engine's device: "weight", "residual_i", "residual_z" [n, h_L, w_L] float32 at L = cfg.last_level (NaN
+        where a pixel is not a constraint), "estimate" [n, 4, 4] float64 (the pose the maps are at, reference -> current),
+        "precision" [n, 2, 2] float32 and, with mask_weight, "mask" [n, h, w] uint8 at level 0: 0 where the pixel's level-L
+        parent is a constraint with weight < mask_weight, 1 elsewhere -- the masks= of pyramid_batch_device.  The pyramids of
+        one call must share their size (ValueError otherwise)."""
+        import torch
+        n = len(refs)
+        L = cfg.last_level
+        sizes = {tuple(r.level_info(L)[:2]) + tuple(r.level_info(0)[:2]) for r in refs}
+        if len(sizes) != 1:
+            raise ValueError(f"references of {len(sizes)} different sizes: match_batch_maps takes one size per call")
+        w, h, w0, h0 = sizes.pop()
+        dev = torch.device("cuda", self.device)
+        maps = {k: torch.empty((n, h, w), dtype=torch.float32, device=dev) for k in ("weight", "residual_i", "residual_z")}
+        maps["estimate"] = torch.empty((n, 4, 4), dtype=torch.float64, device=dev)
+        maps["precision"] = torch.empty((n, 2, 2), dtype=torch.float32, device=dev)
+        wm = WeightMaps()
+        wm.memory = MAPS_MEMORY["device"]
+        for k in ("weight", "residual_i", "residual_z"):
+            setattr(wm, k, MapPlane(maps[k].data_ptr(), 4 * w, 4 * w * h))
+        if mask_weight is not None:
+            maps["mask"] = torch.empty((n, h0, w0), dtype=torch.uint8, device=dev)
+            wm.mask = MapPlane(maps["mask"].data_ptr(), w0, w0 * h0)
+            wm.mask_weight = float(mask_weight)
+        wm.estimate = C.cast(maps["estimate"].data_ptr(), C.POINTER(C.c_double))
+        wm.precision = C.cast(maps["precision"].data_ptr(), C.POINTER(C.c_float))
+        ab0 = ab = None
+        if photometric:
+            if photometric_init is not None:
+                ab0 = np.ascontiguousarray(np.asarray(photometric_init, dtype=np.float64).reshape(n, 2))
+            ab = np.zeros((n, 2), dtype=np.float64)
+        elif photometric_init is not None:
+            raise ValueError("photometric_init without photometric=True")
+        # the engine's stream writes memory that torch's current stream allocated; the call synchronises its stream
+        current = torch.cuda.current_stream(dev)
+        torch.cuda.ExternalStream(self.stream, device=dev).wait_stream(current)
+        res = self.match_batch(refs, curs, cfg, T_init, with_iterations, _photometric=(ab0, ab) if photometric else None,
+                               prior_information=prior_information, _maps=wm)
+        return (res, maps, ab) if photometric else (res, maps)
+
     def match_batch(self, refs, curs, cfg: Config, T_init=None, with_iterations: bool = False, raw: bool = False, _photometric=None,
-                    prior_information=None):
+                    prior_information=None, _maps=None):
         """prior_information: [n, 6, 6] float64, a motion prior per pair in place of cfg.mu I (dvo_b200_match_batch_prior,
         which requires cfg.mu == 0); prior_from_result builds one from an earlier Result."""
         n = len(refs)
@@ -772,11 +833,17 @@ class Engine:
         Tp = T.ctypes.data_as(dp) if T is not None else None
         ab0, ab = _photometric if _photometric is not None else (None, None)
         ab0p = ab0.ctypes.data_as(dp) if ab0 is not None else None
+        lam = None
         if prior_information is not None:
             lam = np.asarray(prior_information, dtype=np.float64)
             if lam.size != 36 * n:
                 raise ValueError(f"prior_information {lam.shape}: want [{n}, 6, 6]")
             lam = np.ascontiguousarray(lam.reshape(n, 36))
+        if _maps is not None:
+            self._check(self.lib.dvo_b200_match_batch_maps(
+                self.ctx, C.byref(cfg), n, rh, ch, Tp, lam.ctypes.data_as(dp) if lam is not None else None, ab0p,
+                ab.ctypes.data_as(dp) if ab is not None else None, res, log, max_log, C.byref(_maps)))
+        elif lam is not None:
             self._check(self.lib.dvo_b200_match_batch_prior(
                 self.ctx, C.byref(cfg), n, rh, ch, Tp, lam.ctypes.data_as(dp), ab0p, ab.ctypes.data_as(dp) if ab is not None else None,
                 res, log, max_log))

@@ -390,8 +390,17 @@ bool DenseTracker::matchBatch(const std::vector<core::RgbdImagePyramid*>& refere
   return true;
 }
 
+bool DenseTracker::matchWithWeights(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current, Result& result,
+                                    cv::Mat& weights) {
+  std::vector<core::RgbdImagePyramid*> refs(1, &reference), curs(1, &current);
+  std::vector<Result> results(1, result);
+  const bool ok = matchBatch(refs, curs, static_cast<const double*>(0), results, &weights);
+  if (ok) result = results[0];
+  return ok;
+}
+
 bool DenseTracker::matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
-                              const double* prior_information, std::vector<Result>& results) {
+                              const double* prior_information, std::vector<Result>& results, cv::Mat* weights) {
   const size_t n = references.size();
   if (n == 0 || currents.size() != n) return false;
   if (prior_information) {   // refused before any upload
@@ -424,10 +433,25 @@ bool DenseTracker::matchBatch(const std::vector<core::RgbdImagePyramid*>& refere
   const int max_log = collect_iterations_ ? (cfg.FirstLevel - cfg.LastLevel + 1) * (cfg.MaxIterationsPerLevel + 1) : 0;
   std::vector<dvo_b200_iteration_stats> log(size_t(max_log) * n);
   const double* T0 = cfg.UseInitialEstimate ? T.data() : 0;
-  int rc = prior_information
-               ? dvo_b200_match_batch_prior(ctx, &c, int(n), r.data(), q.data(), T0, prior_information, 0, 0, raw.data(),
-                                            max_log ? log.data() : 0, max_log)
-               : dvo_b200_match_batch(ctx, &c, int(n), r.data(), q.data(), T0, raw.data(), max_log ? log.data() : 0, max_log);
+  int rc;
+  if (weights) {   // the weight map of the one pair, at LastLevel, straight into the cv::Mat
+    int w = 0, h = 0;
+    dvo_b200_pyramid_level_info(r[0], c.last_level, &w, &h, 0);
+    weights->create(h, w, CV_32FC1);
+    dvo_b200_weight_maps maps;
+    std::memset(&maps, 0, sizeof(maps));
+    maps.memory = DVO_B200_MAPS_HOST;
+    maps.weight.data = weights->ptr<float>();
+    maps.weight.row_bytes = int64_t(sizeof(float)) * w;
+    maps.weight.image_bytes = maps.weight.row_bytes * h;
+    rc = dvo_b200_match_batch_maps(ctx, &c, int(n), r.data(), q.data(), T0, 0, 0, 0, raw.data(), max_log ? log.data() : 0, max_log,
+                                   &maps);
+  } else if (prior_information) {
+    rc = dvo_b200_match_batch_prior(ctx, &c, int(n), r.data(), q.data(), T0, prior_information, 0, 0, raw.data(),
+                                    max_log ? log.data() : 0, max_log);
+  } else {
+    rc = dvo_b200_match_batch(ctx, &c, int(n), r.data(), q.data(), T0, raw.data(), max_log ? log.data() : 0, max_log);
+  }
   if (rc != 0) throw std::runtime_error(std::string("dvo_b200_match_batch: ") + dvo_b200_last_error(ctx));
   for (size_t i = 0; i < n; ++i) fill_result(raw[i], max_log ? &log[size_t(max_log) * i] : 0, results[i]);
   return true;   // the reference's match() always returns true (dense_tracking.cpp:135,375)

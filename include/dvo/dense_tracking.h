@@ -112,6 +112,11 @@ class DenseTracker {
   bool matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
                   const std::vector<core::Matrix6d>& prior_information, std::vector<Result>& results);
 
+  // --- extension: the alignment's Student-t weight map (dvo_b200_match_batch_maps): weights becomes a CV_32FC1 image of the
+  // reference at LastLevel, in host memory, with w = 7 / (5 + r^T P r) at every constraint of the returned pose and NaN at
+  // every other pixel.  Small weights mark the pixels the estimator treated as outliers (moving objects, occlusions). ---
+  bool matchWithWeights(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current, Result& result, cv::Mat& weights);
+
   // per-iteration statistics are copied back only when requested (they are optional in the C ABI)
   void collectIterationStatistics(bool on) { collect_iterations_ = on; }
   // Extension: the corrected estimator of dvo_b200_estimator (exact scale sum, log-likelihood over all points, the odd last
@@ -121,7 +126,8 @@ class DenseTracker {
  private:
   dvo_b200_ctx* context();
   bool matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
-                  const double* prior_information, std::vector<Result>& results);   // prior_information: n * 36 or NULL
+                  const double* prior_information, std::vector<Result>& results,    // prior_information: n * 36 or NULL
+                  cv::Mat* weights = 0);                                             // n == 1 only: matchWithWeights
   Config cfg;
   dvo_b200_ctx* ctx_;
   bool collect_iterations_;

@@ -570,6 +570,71 @@ int dvo_b200_match_batch_prior(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, in
                                double* photometric, dvo_b200_result* results, dvo_b200_iteration_stats* iteration_stats,
                                int32_t max_iteration_stats);
 
+/* ---- weight maps: each alignment's per-pixel Student-t weights and residuals at its returned pose, and an outlier mask --
+ * The estimator down-weights every constraint by w = 7 / (5 + r^T P r); at convergence the pixels of a moving object, a
+ * specularity or a depth edge are the ones with small w.  dvo_b200_match_batch_maps runs an alignment exactly as the
+ * entry point without maps would, then one more kernel that writes these maps for every pair.  Definitions, with
+ * L = cfg->last_level:
+ *   kept iteration  the last iteration on level L whose pose was not reverted.  It supplies T^ (the estimate that
+ *              Result.transformation inverts: T^ = Result.transformation^-1 up to rounding), P^ (the precision that
+ *              iteration estimated, which is the iteration log's tdist_precision of that entry), n^ (its constraint
+ *              count, levels[L].last_increment_valid_constraints) and, in the photometric mode, (alpha, beta) as returned.
+ *   K T        K_cur,L * float(T^)[0:3, :] in float, in the operation order of the level kernel (the current image's
+ *              level-L intrinsics).
+ *   residuals  the residual record of every reference pixel of level L at K T, with the projection, bilinear blend,
+ *              NaN test and occlusion test of the level kernel, and the current-role mask rejection where the current
+ *              pyramid has one: residual_i = c_i I_cur(w) - c_i I_ref (photometric mode: c_i fmaf(alpha, I_ref, beta) with
+ *              alpha, beta rounded to float), residual_z = Z_cur(w) - Z'(x).  Bit for bit planes 0 and 1 of
+ *              dvo_b200_residual_image[_photometric] at the 4 x 4 se3 matrix of T^ (and (alpha, beta)).
+ *   weight     w = 7 rcp(5 + d), d = r^T P^ r, with the operation sequence of the level kernel (rcp.approx: within a few
+ *              ulp of 7 / (5 + d) in fp64).
+ *   not a constraint   a pixel that is not selected, or is out of bounds, NaN or occluded at T^: NaN in all three
+ *              maps.  With DVO_B200_ESTIMATOR_REFERENCE the odd last selected point is not a constraint either; with
+ *              DVO_B200_ESTIMATOR_CORRECTED it is.  So exactly n^ weights are finite.
+ *   NaN result a pair whose Result has NaN information (no accepted iteration on level L, or TooFewConstraints) gets NaN
+ *              maps, a NaN P^ and an all-1 mask; its estimate is still written.
+ *   mask       one byte per level-0 pixel of the reference: 0 iff its level-L parent (x >> L, y >> L) is a constraint with
+ *              w < mask_weight, 1 otherwise (level-0 pixels without a parent, past an odd size, are 1).  It is the masks
+ *              plane dvo_b200_pyramid_create_device_batch takes (nonzero = usable), so the outliers of one alignment can
+ *              be kept out of the next alignment against the same keyframe without a host round trip.  No dilation.
+ * Outputs, per requested plane: pair p's map starts at data + p * image_bytes, row y at + y * row_bytes.  The weight and
+ * residual planes are float32 of level L's size, the mask uint8 of level 0's size. */
+#define DVO_B200_MAPS_DEVICE 0   /* every pointer of the dvo_b200_weight_maps is device or managed memory of the ctx's device */
+#define DVO_B200_MAPS_HOST 1     /* every pointer is host memory (pageable or pinned); the maps are copied back */
+typedef struct dvo_b200_map_plane {
+  void* data;            /* NULL: not written */
+  int64_t row_bytes;     /* >= width * element size, a multiple of the element size */
+  int64_t image_bytes;   /* >= height * row_bytes, a multiple of the element size */
+} dvo_b200_map_plane;
+typedef struct dvo_b200_weight_maps {
+  int32_t memory;                 /* DVO_B200_MAPS_DEVICE or DVO_B200_MAPS_HOST: where every pointer below lies */
+  dvo_b200_map_plane weight;      /* float32, level-L size of pair p's reference */
+  dvo_b200_map_plane residual_i;  /* float32, residual_i */
+  dvo_b200_map_plane residual_z;  /* float32, residual_z */
+  dvo_b200_map_plane mask;        /* uint8, level-0 size */
+  float mask_weight;              /* finite and > 0; read iff mask.data */
+  double* estimate;               /* n * 16, the se3 matrix of T^ row-major (reference -> current), or NULL */
+  float* precision;               /* n * 4, P^ row-major, or NULL */
+} dvo_b200_weight_maps;
+
+/* An alignment and its weight maps.  The arguments before maps are those of dvo_b200_match_batch_prior, with
+ * prior_information NULL for the plain cfg->mu path and photometric NULL for the 6-unknown mode; results, photometric and
+ * the iteration statistics are bit for bit those of dvo_b200_match_batch, _photometric or _prior with the same arguments,
+ * for every estimator, current-role mask and launch plan.  One kernel launch more than that call (k_weight_maps, which
+ * writes the mask in the same pass).  Synchronises as dvo_b200_match_batch does; with DVO_B200_MAPS_HOST the maps have been
+ * copied back when it returns.  Refused with DVO_B200_ERR_INVALID_ARGUMENT before anything is staged, uploaded or launched:
+ * a NULL maps; an unknown memory; no output requested; a row_bytes below the largest width of the batch times the element
+ * size or not a multiple of it; an image_bytes below the largest height times row_bytes or not a multiple of the element
+ * size; a misaligned pointer; under DVO_B200_MAPS_DEVICE a first or last byte of an output that cudaPointerGetAttributes
+ * does not report as device or managed memory of the ctx's device, and under DVO_B200_MAPS_HOST one in device memory; a
+ * non-finite or non-positive mask_weight with a mask; and everything the matching entry point refuses (a batch of mixed
+ * sizes included: DVO_B200_ERR_SHAPE_MISMATCH). */
+int dvo_b200_match_batch_maps(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n,
+                              dvo_b200_pyramid* const* references, dvo_b200_pyramid* const* currents,
+                              const double* T_init, const double* prior_information, const double* photometric_init,
+                              double* photometric, dvo_b200_result* results, dvo_b200_iteration_stats* iteration_stats,
+                              int32_t max_iteration_stats, const dvo_b200_weight_maps* maps);
+
 /* ---- profiling hooks (bench.py roofline): per-kernel-class accumulated device time measured with
  *      CUDA events on the ctx stream.  classes: 0 residual/scale stage, 1 normal-equation stage,
  *      2 per-pair step kernels, 3 pyramid build, 4 selection. -------------------------------- */
