@@ -147,7 +147,23 @@ struct PairState {
   int iter_log_count;
   int pad_;
   LevelSummary levels[kMaxLevels];
+
+  // the Result is defined (not NaN): the last level has an accepted iteration (SURVEY Q24)
+  __host__ __device__ bool result_defined() const {
+    return have_done == 1 && termination != DVO_B200_TERM_TOO_FEW_CONSTRAINTS;
+  }
 };
+
+// K * float(T)[0:3,:] in float, in the reference's operation order (dense_tracking_impl.cpp:142-152): every copy of K T must
+// round alike (the weight maps recompute the level kernel's, DESIGN §4.10).
+__device__ __forceinline__ void kt_of(const double T[16], const PairLevel& pl, float kt[12]) {
+  for (int j = 0; j < 4; ++j) {
+    const float t0 = (float)T[j], t1 = (float)T[4 + j], t2 = (float)T[8 + j];
+    kt[j] = __fadd_rn(__fmul_rn(pl.cfx, t0), __fmul_rn(pl.cox, t2));
+    kt[4 + j] = __fadd_rn(__fmul_rn(pl.cfy, t1), __fmul_rn(pl.coy, t2));
+    kt[8 + j] = t2;
+  }
+}
 
 // The affine brightness model of one pair (photometric alignments only: an array of its own, so that PairState and the
 // default instances of the level kernel stay as they are).  (alpha, beta) is what the current iteration's residuals use
@@ -159,7 +175,7 @@ struct AffineState {
 };
 
 struct Workspace {              // per-ctx scratch of the level kernel
-  PairLevel* d_pair_level = nullptr;
+  PairLevel* d_pair_level = nullptr; // one descriptor of slack past the last: k_stage_words copies whole 16-byte words
   const int** d_csat = nullptr;      // per descriptor of d_pair_level: CurPairLevel::csat (only written for kCurMask launches)
   PairState* d_state = nullptr;
   char* d_scratch = nullptr;         // the level kernel's per-launch scratch (tracker.cu: ScratchLayout)
@@ -170,8 +186,8 @@ struct Workspace {              // per-ctx scratch of the level kernel
   double* d_prior = nullptr;         // per pair of an alignment with a motion prior: the 6 x 6 information, row-major
   char* d_maps = nullptr;            // weight maps copied back to the host (DVO_B200_MAPS_HOST): the kernel's packed output
   int* h_active = nullptr;           // pinned: per launch of a call, the kernel's error flag
-  size_t cap_pairs = 0, cap_scratch = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0, cap_affine = 0, cap_prior = 0;
-  size_t cap_maps = 0;
+  size_t cap_pair_level = 0, cap_state = 0, cap_scratch = 0, cap_iter_log = 0, cap_dump = 0, cap_tinit = 0, cap_csat = 0,
+         cap_affine = 0, cap_prior = 0, cap_maps = 0;   // in elements (see grow)
 };
 
 }  // namespace dvo_b200
@@ -179,9 +195,8 @@ struct Workspace {              // per-ctx scratch of the level kernel
 struct dvo_b200_ctx {
   int device = 0;
   uint64_t uid = 0;                   // unique over the process lifetime (a context's address may be reused after destroy)
-  int num_sms = 0, ctas_per_sm = 0;   // persistent-kernel grid geometry (queried once)
-  int ctas_per_sm_affine = 0;         // the same for the instances of the photometric mode
-  int ctas_per_sm_prior[2] = {0, 0};  // the same for the instances with a motion prior: [0] default, [1] photometric mode
+  int num_sms = 0;                        // persistent-kernel grid geometry (queried once)
+  int ctas_per_sm[2][2] = {{0, 0}, {0, 0}};   // [photometric][motion prior]: resident CTAs of those level kernel instances, 0 = not queried yet
   int estimator = DVO_B200_ESTIMATOR_REFERENCE;   // dvo_b200_estimator of every later alignment / test hook on this context
   unsigned long long* d_dbg = nullptr;   // DVO_B200_TIMING=1: per-level phase timers of the persistent kernel (64 slots)
   cudaStream_t stream = nullptr;
@@ -215,6 +230,17 @@ int check_cuda(dvo_b200_ctx* ctx, cudaError_t e, const char* what);
     int rc__ = ::dvo_b200::check_cuda((ctx), (call), #call);             \
     if (rc__ != 0) return rc__;                                          \
   } while (0)
+
+// A workspace buffer of at least `need` elements: a smaller one is freed once the stream has drained, and the new one is
+// uninitialised.
+template <typename T>
+int grow(dvo_b200_ctx* ctx, T*& ptr, size_t& cap, size_t need) {
+  if (need <= cap) return 0;
+  if (ptr) { cudaStreamSynchronize(ctx->stream); cudaFree(ptr); ptr = nullptr; cap = 0; }
+  DVO_CUDA(ctx, cudaMalloc((void**)&ptr, need * sizeof(T)));
+  cap = need;
+  return 0;
+}
 
 // profiling scope: records start/stop events around a kernel class when enabled
 struct ProfScope {

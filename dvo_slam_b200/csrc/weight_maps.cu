@@ -55,21 +55,13 @@ k_weight_maps(const PairState* __restrict__ states, const AffineState* __restric
   const float nanv = __int_as_float(0x7fc00000);
   if (threadIdx.x == 0 && threadIdx.y == 0) {
     const PairState& st = states[pair];
-    // a Result is defined iff k_finalize finds an accepted iteration on the last level (its `ok`)
-    const bool ok = st.have_done == 1 && st.termination != DVO_B200_TERM_TOO_FEW_CONSTRAINTS;
+    const bool ok = st.result_defined();
     // P^: after a rejected last iteration (LogLikelihoodDecreased) pair_mid_warp has moved the kept iteration's precision to
     // precision_prev; after an accepted one it is still `precision`
     const float* Pk = st.termination == DVO_B200_TERM_LOG_LIKELIHOOD_DECREASED ? st.precision_prev : st.precision;
     double T[16];
     se3_matrix(st.estimate, T);
-    // K T from T^ in the operation order of prepare_iteration / pair_end_cta (tracker.cu): PairState::kt may belong to a
-    // rejected iteration
-    for (int j = 0; j < 4; ++j) {
-      const float t0 = (float)T[j], t1 = (float)T[4 + j], t2 = (float)T[8 + j];
-      pc.kt[j] = __fadd_rn(__fmul_rn(pl.cfx, t0), __fmul_rn(pl.cox, t2));
-      pc.kt[4 + j] = __fadd_rn(__fmul_rn(pl.cfy, t1), __fmul_rn(pl.coy, t2));
-      pc.kt[8 + j] = t2;
-    }
+    kt_of(T, pl, pc.kt);   // K T from T^: PairState::kt may belong to a rejected iteration
     for (int i = 0; i < 4; ++i) pc.P[i] = Pk[i];
     pc.alpha = affine ? (float)affine[pair].ab[0] : 1.f;
     pc.beta = affine ? (float)affine[pair].ab[1] : 0.f;
@@ -170,15 +162,8 @@ size_t host_scratch_layout(const dvo_b200_weight_maps& maps, int n, const dvo_b2
 
 int weight_maps_prepare(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int n, const dvo_b200_pyramid* ref0, int level) {
   if (maps.memory != DVO_B200_MAPS_HOST) return 0;
-  Workspace& ws = ctx->ws;
   size_t off[6];
-  const size_t need = host_scratch_layout(maps, n, ref0, level, off);
-  if (need > ws.cap_maps) {
-    if (ws.d_maps) { cudaStreamSynchronize(ctx->stream); cudaFree(ws.d_maps); ws.d_maps = nullptr; ws.cap_maps = 0; }
-    DVO_CUDA(ctx, cudaMalloc((void**)&ws.d_maps, need));
-    ws.cap_maps = need;
-  }
-  return 0;
+  return grow(ctx, ctx->ws.d_maps, ctx->ws.cap_maps, host_scratch_layout(maps, n, ref0, level, off));
 }
 
 void weight_maps_launch(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int n, const dvo_b200_pyramid* ref0, int level,
