@@ -31,7 +31,9 @@ __host__ __device__ __forceinline__ int sat_rows(int h) { return (h + kSatBlock 
 // Cells outside the image hold (0, NaN) / 0 / (0, 0).
 constexpr int kRecTx = kTileH * kTileW;              // float2 offset of tx[]
 constexpr int kRecP1 = kRecTx + kTileW / 2;          // float2 offset of the gradient rows
-constexpr int kRecF2 = kRecP1 + kTileH * kTileW;     // float2 elements per record (14 848 bytes)
+constexpr int kRecF2 = kRecP1 + kTileH * kTileW;     // float2 elements per record (18 560 bytes)
+// the bulk copies of a record (whole, or up to kRecP1 in stage A) need 16-byte multiples, and so do record offsets in HBM
+static_assert(kTileW % 32 == 0 && (kRecP1 * 8) % 16 == 0 && (kRecF2 * 8) % 16 == 0, "tile records must stay 16-byte granular");
 __host__ __device__ __forceinline__ size_t rec_cell(int x, int y, int nbands) {   // (I, Zsel) of pixel (x, y) relative to the level's records
   return (size_t)((y / kTileH) * nbands + x / kTileW) * kRecF2 + (size_t)(y % kTileH) * kTileW + (x % kTileW);
 }

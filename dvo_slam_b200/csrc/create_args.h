@@ -31,7 +31,7 @@ namespace dvo_b200 {
 constexpr int kMaxLevels = DVO_B200_MAX_LEVELS;
 
 // tile geometry of the level kernel (tracker.cu) and of the per-tile depth ranges (pyramid.cu)
-constexpr int kTileW = 128;    // reference pixels per tile row: 4 warp rounds
+constexpr int kTileW = 160;    // reference pixels per tile row: 5 warp rounds; 640, 320 and 160 columns are whole bands
 #ifndef DVO_TILE_H
 #define DVO_TILE_H 7
 #endif

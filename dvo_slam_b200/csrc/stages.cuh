@@ -48,17 +48,21 @@ constexpr unsigned kFullMask = 0xffffffffu;
 constexpr int kConsumerWarps = kTileH;                    // warp q walks row q of every tile
 constexpr int kCtaThreads = (kConsumerWarps + 1) * 32;    // + one producer warp
 #ifndef DVO_WIN_COLS
-#define DVO_WIN_COLS 152
+#define DVO_WIN_COLS (kTileW + 24)
 #endif
+// 19 rows: the most that keeps two CTAs of every level-kernel instance inside the 196 KB shared-memory carveout (tracker.cu),
+// and so 60 KB of L1 for the pixel loops' spill reloads and the producer's __ldg reads.  24 rows need the 228 KB carveout;
+// the 28 KB of L1 it leaves made the level kernel slower on an H100 than the extra exact tiles made it faster.
 #ifndef DVO_WIN_ROWS
-#define DVO_WIN_ROWS 24
+#define DVO_WIN_ROWS 19
 #endif
 #ifndef DVO_STAGES
 #define DVO_STAGES 2
 #endif
 constexpr int kWinCols = DVO_WIN_COLS;                    // window capacity: kTileW + 24 columns
-constexpr int kWinRows = DVO_WIN_ROWS;                    //                  kTileH + 17 rows
+constexpr int kWinRows = DVO_WIN_ROWS;                    //                  kTileH + 12 rows
 constexpr int kStages = DVO_STAGES;
+static_assert(kWinCols % 2 == 0 && kWinCols < 256, "produce_tiles packs an even window width into 8 bits");
 
 // ---- mbarrier / bulk-copy primitives (PTX ISA 8.6, sm_90a) ------------------------------------------
 __device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -861,13 +865,15 @@ __device__ __forceinline__ float ref_intensity(float Ir, const Brightness& br) {
 }
 
 // Stage A rounds of one tile row: two rounds per trip, whose projection / tap / blend chains are independent and interleave.
+// The exact loop takes the whole pairs of a full band's rounds, and an odd last round after the loop.
 // kCorrected: plain scale sums; the generic loop also re-admits the odd last point at tile column odd_col (-1: none).
 template <bool kCorrected, bool kExact, bool kFirst, bool kAffine = false>
 __device__ __forceinline__ void stage_a_rounds(const WinView& wv, int bw, unsigned refa, unsigned txa, float ty, const StageConsts& c,
                                                typename ScaleOf<kCorrected>::type& ss, int lane, unsigned lt_mask, int odd_col,
                                                float odd_z, const Brightness& br = {1.f, 0.f}) {
-  static_assert(kTileW % 64 == 0, "the exact loop takes whole pairs of rounds");
-  const int nr = kExact ? kTileW / 32 : (bw + 31) >> 5;
+  static_assert(kTileW % 32 == 0, "a band is whole rounds");
+  constexpr int kBandRounds = kTileW / 32;
+  const int nr = kExact ? kBandRounds & ~1 : (bw + 31) >> 5;
   const int xlim = bw - lane;        // lane's column r*32+lane is inside the band iff r*32 < xlim
   const bool first = kExact ? kFirst : c.first_iteration != 0;
 #pragma unroll 1
@@ -893,6 +899,14 @@ __device__ __forceinline__ void stage_a_rounds(const WinView& wv, int bw, unsign
     const float w0 = student_weight(c, first, ei0, ez0), w1 = student_weight(c, first, ei1, ez1);
     scale_add(ss, lane, lt_mask, v0, w0, ei0, ez0);
     scale_add(ss, lane, lt_mask, v1, w1, ei1, ez1);
+  }
+  if constexpr (kExact && (kBandRounds & 1)) {   // the odd last round of a full band (refa / txa point at it)
+    const f2 rz = lds_f2_at(refa);
+    const float tx = lds_f32(txa), z = hi(rz);
+    const PixelProjection p = project_pixel(tx, ty, z, c);
+    float ei, ez;
+    const bool v = residual_pixel<kExact>(p, wv, ref_intensity<kAffine>(lo(rz), br), z, c, ei, ez);
+    scale_add(ss, lane, lt_mask, v, student_weight(c, first, ei, ez), ei, ez);
   }
 }
 // Stage A over this CTA's strips: warp q walks image row strip*kTileH + q band by band, carries the pairwise

@@ -449,7 +449,7 @@ __device__ __noinline__ void pair_end_cta(PairState& st, const PairLevel& pl, in
 // ------------------------------------------------------------------------------------------------
 // The persistent cooperative level kernel.
 //
-// The grid is num_sms x C CTAs (C = resident CTAs per SM, 2 with ~93 KB of shared memory each) of 8 warps.  CTAs are
+// The grid is num_sms x C CTAs (C = resident CTAs per SM, 2 with 95-97 KB of shared memory each) of 8 warps.  CTAs are
 // grouped into squads of g CTAs; a squad owns ONE frame pair at a time, CTA r of the squad the strips r, r+g, r+2g, ...
 // (kTileH image rows each), and runs all its Gauss-Newton iterations on the segment's levels inside the kernel:
 //   stage A over the CTA's tiles -> per-row scale summaries -> per-strip summaries (fp64) -> squad barrier, the last
@@ -475,6 +475,9 @@ struct LevelTailOf {    // shared memory after the tile pipeline
 };
 template <bool kAffine, bool kPrior = false>
 constexpr size_t kLevelSmemBytesOf = sizeof(TilePipe) + sizeof(LevelTailOf<kAffine, kPrior>);
+// Two resident CTAs per SM: an H100 SM has up to 228 KB of shared memory and reserves 1 KB of it per resident CTA.  (With
+// the default window, kWinRows of stages.cuh, two CTAs take at most 196 KB, the carveout that leaves 60 KB of L1.)
+constexpr size_t kSmemPerSm = 228 * 1024, kSmemReservedPerCta = 1024;
 
 // One segment of a launch: a group of consecutive pyramid levels that a squad of g CTAs walks a pair through.  A launch
 // has one segment, or two (the coarse levels with one CTA per pair, then the fine levels with squads of g CTAs) that the
@@ -923,6 +926,7 @@ struct LevelInstance {
 };
 template <bool kAffine, bool kPrior>
 LevelInstance level_instance_of(const LevelVariant& v) {
+  static_assert(2 * (kLevelSmemBytesOf<kAffine, kPrior> + kSmemReservedPerCta) <= kSmemPerSm, "two CTAs of the level kernel must fit on an SM");
   const void* const k[2][2] = {
       {(const void*)k_level_persistent<false, false, kAffine, kPrior>, (const void*)k_level_persistent<false, true, kAffine, kPrior>},
       {(const void*)k_level_persistent<true, false, kAffine, kPrior>, (const void*)k_level_persistent<true, true, kAffine, kPrior>}};
