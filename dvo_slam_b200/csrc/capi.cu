@@ -1,5 +1,6 @@
 // capi.cu -- the extern "C" surface declared in include/dvo_b200.h.
 #include "common.cuh"
+#include "hypotheses_args.h"
 #include "maps_args.h"
 #include "prior_args.h"
 
@@ -782,6 +783,21 @@ int dvo_b200_match_batch_maps(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int
   if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
   return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
                              iteration_stats ? max_iteration_stats : 0, photometric_init, photometric, prior_information, maps);
+}
+
+// ---- multi-hypothesis alignment ----
+int dvo_b200_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,
+                                    dvo_b200_pyramid* const* currents, int32_t k, const double* hypotheses, int32_t screen_level,
+                                    double min_constraint_ratio, dvo_b200_result* results, int32_t* best, double* scores,
+                                    dvo_b200_result* screen_results, dvo_b200_iteration_stats* iteration_stats,
+                                    int32_t max_iteration_stats) {
+  if (!ctx) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_hypotheses: null argument");
+  const std::string why = hypotheses_args_error(cfg, n, k, hypotheses, screen_level, min_constraint_ratio, results, best);
+  if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
+  cudaSetDevice(ctx->device);
+  return tracker_match_batch_hypotheses(ctx, cfg, n, references, currents, k, hypotheses, screen_level, min_constraint_ratio,
+                                        results, best, scores, screen_results, iteration_stats,
+                                        iteration_stats ? max_iteration_stats : 0);
 }
 
 int dvo_b200_residual_image_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,

@@ -291,6 +291,13 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
                         const double* ab_init = nullptr, double* ab_out = nullptr, const double* prior = nullptr,
                         const dvo_b200_weight_maps* maps = nullptr);   // maps != NULL: also the weight maps (weight_maps.cu)
 int check_level_flags(dvo_b200_ctx* ctx);   // after a stream synchronisation: did a level kernel report a timeout?
+// dvo_b200_match_batch_hypotheses after its argument checks (hypotheses_args.h): the screening of n * k virtual pairs on levels
+// first .. screen_level, k_pick_hypotheses, and the continuation of the n chosen ones on the levels below.  scores and
+// screen_results (host, n * k) may be NULL.
+int tracker_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
+                                   dvo_b200_pyramid* const* curs, int k, const double* hypotheses, int screen_level,
+                                   double min_ratio, dvo_b200_result* h_results, int32_t* h_best, double* h_scores,
+                                   dvo_b200_result* h_screen, dvo_b200_iteration_stats* iter_stats, int max_iter_stats);
 int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* ref, dvo_b200_pyramid* cur,
                       int level, const double* T, int use_weights, const float* prev_precision, int64_t* count,
                       float* precision_out, float* ll_out, double* A_out, double* b_out, float* planes7,

@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "stages.cuh"
 #include "launch_plan.h"
+#include "hypotheses_args.h"
 
 #include <cstdio>
 #include <cstring>
@@ -909,6 +910,40 @@ __global__ void k_affine_init(AffineState* s, const double* ab, int n) {
   s[p].ab[0] = a; s[p].ab[1] = b; s[p].ab_old[0] = a; s[p].ab_old[1] = b;
 }
 
+// Multi-hypothesis alignment, between the screening and the continuation: one warp per pair p.  The scores of its k screened
+// hypotheses (states p k .. p k + k - 1, their statistics of the screening level at level index ls) go to scores[p k + j]
+// (hypothesis_score), the choice to best[p] (pick_hypothesis), and the chosen hypothesis's state and first
+// min(iter_log_count, max_log) iteration-log entries to slot p of the continuation, which picks up from there.
+__global__ void k_pick_hypotheses(const PairState* __restrict__ screened, const dvo_b200_iteration_stats* __restrict__ screened_log,
+                                  PairState* __restrict__ chosen, dvo_b200_iteration_stats* __restrict__ chosen_log, int max_log, int n,
+                                  int k, int ls, double min_ratio, double* __restrict__ scores, int* __restrict__ best) {
+  const int p = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (p >= n) return;
+  double* const sc = scores + (size_t)p * k;
+  for (int j = lane; j < k; j += 32) {
+    const LevelSummary& L = screened[(size_t)p * k + j].levels[ls];
+    sc[j] = hypothesis_score(L.has_inc, L.last_inc_n, L.valid_pixels, L.last_inc_nll, min_ratio);
+  }
+  __syncwarp();
+  int b = 0;
+  if (lane == 0) {
+    b = pick_hypothesis(sc, k);
+    best[p] = b;
+  }
+  b = __shfl_sync(kFull, b, 0);
+  static_assert(sizeof(PairState) % 8 == 0 && sizeof(dvo_b200_iteration_stats) % 8 == 0, "copied as 8-byte words");
+  const PairState& src = screened[(size_t)p * k + b];
+  const unsigned long long* s = reinterpret_cast<const unsigned long long*>(&src);
+  unsigned long long* d = reinterpret_cast<unsigned long long*>(chosen + p);
+  for (int i = lane; i < (int)(sizeof(PairState) / 8); i += 32) d[i] = s[i];
+  if (max_log > 0) {
+    const size_t words = (size_t)min(src.iter_log_count, max_log) * (sizeof(dvo_b200_iteration_stats) / 8);
+    const unsigned long long* ls8 = reinterpret_cast<const unsigned long long*>(screened_log + ((size_t)p * k + b) * max_log);
+    unsigned long long* ld8 = reinterpret_cast<unsigned long long*>(chosen_log + (size_t)p * max_log);
+    for (size_t i = lane; i < words; i += 32) ld8[i] = ls8[i];
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
@@ -1100,20 +1135,34 @@ LevelLaunch make_level_launch(const LevelInfo& L, const dvo_b200_config* cfg, in
   return lp;
 }
 
-// Enqueue launch `index` of a plan whose level li is pyramid level first - li of `levels`.  Squad states, queues, the ready
-// ring and the error flag are zeroed first; the error flag is copied to ws.h_active[index] after the launch.
+// Where the npairs pairs of a launch live: their states, the descriptors of the plan's levels ([level][pair], inside
+// ws.d_pair_level, whose index CurPairLevel::csat shares), their iteration log (max_log entries per pair), and li0, the
+// position of the plan's first level in Result.Statistics.Levels.  A match that runs from its first level has li0 = 0 (that
+// level starts the pairs from T_init); li0 > 0 continues pairs whose earlier levels another plan ran.
+struct LaunchTarget {
+  PairState* states;
+  const PairLevel* pls;
+  dvo_b200_iteration_stats* ilog;
+  int li0;
+};
+LaunchTarget whole_workspace(const Workspace& ws) { return {ws.d_state, ws.d_pair_level, ws.d_iter_log, 0}; }
+
+// Enqueue launch `index` of a plan whose level li is pyramid level first - li of `levels`, and level li0 + li of the match.
+// Squad states, queues, the ready ring and the error flag are zeroed first; the error flag is copied to ws.h_active[index]
+// after the launch.
 int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo_b200_config* cfg, const LevelInfo* levels,
-                    int first, const double* d_Tinit, int npairs, int max_log, float* dump, int skip_begin, const LevelVariant& v) {
+                    int first, const double* d_Tinit, int npairs, int max_log, float* dump, int skip_begin, const LevelVariant& v,
+                    const LaunchTarget& t) {
   Workspace& ws = ctx->ws;
   cudaStream_t st = ctx->stream;
   const ScratchLayout o = scratch_layout(L, npairs, v.affine ? kNormalValuesAffine : kNormalValues);
   char* const base = ws.d_scratch;
   DVO_CUDA(ctx, cudaMemsetAsync(base + o.squads[0], 0, o.bytes - o.squads[0], st));
   PersistentArgs pa;
-  pa.states = ws.d_state;
+  pa.states = t.states;
   int* counters = reinterpret_cast<int*>(base + o.counters);
   pa.error_flag = counters + 3 * kMaxSeg;
-  pa.ilog = ws.d_iter_log; pa.max_log = max_log;
+  pa.ilog = t.ilog; pa.max_log = max_log;
   pa.T_init = d_Tinit; pa.skip_begin = skip_begin;
   pa.dump = dump;
   pa.npairs = npairs; pa.nseg = L.nseg;
@@ -1123,7 +1172,7 @@ int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo
   for (int s = 0; s < L.nseg; ++s) {
     const PlanSegment& P = L.seg[s];
     Segment& S = pa.seg[s];
-    S.pls = ws.d_pair_level + (size_t)P.first_li * npairs;
+    S.pls = t.pls + (size_t)P.first_li * npairs;
     S.row_exports = reinterpret_cast<float*>(base + o.row_exports[s]);
     S.row_base = reinterpret_cast<int*>(base + o.row_base[s]);
     S.strip_exports = reinterpret_cast<double*>(base + o.strip_exports[s]);
@@ -1140,7 +1189,7 @@ int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo
     for (int k = 0; k < kMaxLevels; ++k) S.strips_per_cta[k] = P.strips_per_cta[k];
     for (int k = 0; k < P.nlev; ++k) {
       const int li = P.first_li + k;
-      S.lp[k] = make_level_launch(levels[first - li], cfg, li, first - li);
+      S.lp[k] = make_level_launch(levels[first - li], cfg, t.li0 + li, first - li);
     }
   }
   {
@@ -1155,24 +1204,25 @@ int launch_segments(dvo_b200_ctx* ctx, const PlanLaunch& L, int index, const dvo
   return 0;
 }
 
-// The pinned stage of a match, in 16-byte aligned sections: the pair descriptors of every level ([level][pair]), the initial
-// estimates, the current-mask summaries (CurPairLevel::csat, same index), (alpha, beta) and the prior informations.  A section
-// the call does not need has 0 bytes.  `bytes` is what crosses PCIe: whole 16-byte words for the sections k_stage_words
-// copies, and the doubles themselves for (alpha, beta), which k_affine_init reads in place.
+// The pinned stage of a match, in 16-byte aligned sections: ndesc pair descriptors (those of every level, [level][pair]), the
+// initial estimates of n pairs, the current-mask summaries (CurPairLevel::csat, same index as the descriptors), (alpha, beta)
+// and the prior informations of n pairs.  A section the call does not need has 0 bytes.  `bytes` is what crosses PCIe: whole
+// 16-byte words for the sections k_stage_words copies, and the doubles themselves for (alpha, beta), which k_affine_init
+// reads in place.
 struct MatchStageLayout {
   struct Section { size_t at, bytes; };
   Section desc, tinit, csat, ab, prior;
   size_t total;
 };
 
-MatchStageLayout match_stage_layout(int n, int nlev, bool have_init, bool have_ab, const LevelVariant& v) {
+MatchStageLayout match_stage_layout(size_t ndesc, int n, bool have_init, bool have_ab, const LevelVariant& v) {
   auto words = [](size_t bytes) { return (bytes + 15) / 16 * 16; };
   MatchStageLayout s;
   size_t at = 0;
   auto take = [&](size_t bytes) { const MatchStageLayout::Section o{at, bytes}; at += words(bytes); return o; };
-  s.desc = take(words(sizeof(PairLevel) * (size_t)n * nlev));
+  s.desc = take(words(sizeof(PairLevel) * ndesc));
   s.tinit = take(have_init ? sizeof(double) * 16 * (size_t)n : 0);
-  s.csat = take(v.cur_mask ? words(sizeof(const int*) * (size_t)n * nlev) : 0);
+  s.csat = take(v.cur_mask ? words(sizeof(const int*) * ndesc) : 0);
   s.ab = take(have_ab ? sizeof(double) * 2 * (size_t)n : 0);
   s.prior = take(v.prior ? sizeof(double) * 36 * (size_t)n : 0);
   s.total = at;
@@ -1184,6 +1234,17 @@ void stage_words(dvo_b200_ctx* ctx, const void* src, void* dst, size_t bytes) {
   const size_t n16 = bytes / 16;
   k_stage_words<<<(unsigned)((n16 + 255) / 256), 256, 0, ctx->stream>>>((const uint4*)src, (uint4*)dst, n16);
   ctx->launches++;
+}
+
+// ctx->h_results of at least `bytes`: the pinned buffer the results of a call are copied back through
+int ensure_pinned_results(dvo_b200_ctx* ctx, size_t bytes) {
+  if (bytes > ctx->h_results_bytes) {
+    if (ctx->h_results) cudaFreeHost(ctx->h_results);
+    ctx->h_results = nullptr; ctx->h_results_bytes = 0;
+    DVO_CUDA(ctx, cudaMallocHost(&ctx->h_results, bytes));
+    ctx->h_results_bytes = bytes;
+  }
+  return 0;
 }
 
 }  // namespace
@@ -1214,7 +1275,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   // Pair descriptors of every level and the initial estimates go into the pinned stage once; one small kernel copies
   // them to device memory (reads over PCIe: no H2D copy-engine work, no host round trip between the launches below).
   const bool have_init = cfg->use_initial_estimate && T_init;
-  const MatchStageLayout s = match_stage_layout(n, nlev, have_init, v.affine && ab_init, v);
+  const MatchStageLayout s = match_stage_layout((size_t)n * nlev, n, have_init, v.affine && ab_init, v);
   if ((rc = ensure_stage(ctx, 0, s.total))) return rc;
   if (v.cur_mask && (rc = grow(ctx, ws.d_csat, ws.cap_csat, s.csat.bytes / sizeof(const int*)))) return rc;
   if ((rc = grow(ctx, ws.d_tinit, ws.cap_tinit, (size_t)16 * n))) return rc;
@@ -1246,7 +1307,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   if (max_log > 0) DVO_CUDA(ctx, cudaMemsetAsync(ws.d_iter_log, 0, sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log, st));
   for (int i = 0; i < plan.nlaunch; ++i)
     if ((rc = launch_segments(ctx, plan.launch[i], i, cfg, refs[0]->L, first, have_init ? ws.d_tinit : nullptr, n, max_log,
-                              nullptr, 0, v)))
+                              nullptr, 0, v, whole_workspace(ws))))
       return rc;
   // results
   dvo_b200_result* d_res = (dvo_b200_result*)d_results_user;
@@ -1267,12 +1328,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
   if (h_results) {
     size_t bytes = sizeof(dvo_b200_result) * n;
     const size_t pinned = bytes + (v.affine ? sizeof(double) * 2 * (size_t)n : 0);   // the results, then (alpha, beta) of each pair
-    if (pinned > ctx->h_results_bytes) {
-      if (ctx->h_results) cudaFreeHost(ctx->h_results);
-      ctx->h_results = nullptr; ctx->h_results_bytes = 0;
-      DVO_CUDA(ctx, cudaMallocHost(&ctx->h_results, pinned));
-      ctx->h_results_bytes = pinned;
-    }
+    if ((rc = ensure_pinned_results(ctx, pinned))) return rc;
     DVO_CUDA(ctx, cudaMemcpyAsync(ctx->h_results, d_res, bytes, cudaMemcpyDeviceToHost, st));
     if (v.affine) {
       DVO_CUDA(ctx, cudaMemcpy2DAsync((char*)ctx->h_results + bytes, 2 * sizeof(double), ws.d_affine[0].ab, sizeof(AffineState),
@@ -1360,7 +1416,8 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
     ctx->launches += 1;
   }
   ws.h_active[0] = 0;
-  if ((rc = launch_segments(ctx, plan.launch[0], 0, &c, ref->L, level, nullptr, 1, 0, planes7 ? ws.d_dump : nullptr, 1, v)))
+  if ((rc = launch_segments(ctx, plan.launch[0], 0, &c, ref->L, level, nullptr, 1, 0, planes7 ? ws.d_dump : nullptr, 1, v,
+                            whole_workspace(ws))))
     return rc;
   DVO_CUDA(ctx, cudaGetLastError());
   if ((rc = note_foreign_uses(ctx, 1, refs, curs))) return rc;
@@ -1384,6 +1441,120 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
     ctx->d2h_bytes += sizeof(float) * 7 * (size_t)L.n;
   }
   return 0;
+}
+
+
+// dvo_b200_match_batch_hypotheses (include/dvo_b200.h).  Stage 1 screens n k virtual pairs, pair p k + j being (refs[p],
+// curs[p]) from H[p][j], on levels first .. s with the plan of n k pairs; k_pick_hypotheses scores them and copies each pair's
+// chosen state (and log) into one of n continuation slots; stage 2 runs levels s-1 .. last on those n slots with the plan of
+// n pairs, its level indices continuing at first - s + 1.  Both stages are launches of the level kernel like any other match,
+// so plan independence gives each pair the bits of one dvo_b200_match_batch.
+// Workspace: descriptors [stage 1: level][virtual pair] then [stage 2: level][pair]; states and iteration log: the n k
+// screened pairs, then the n continued ones; the device stage: results (n), screen results (n k, if requested), scores
+// (n k), best (n), copied back through the pinned results buffer in that layout.
+int tracker_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
+                                   dvo_b200_pyramid* const* curs, int k, const double* hypotheses, int screen_level,
+                                   double min_ratio, dvo_b200_result* h_results, int32_t* h_best, double* h_scores,
+                                   dvo_b200_result* h_screen, dvo_b200_iteration_stats* iter_stats, int max_iter_stats) {
+  int rc = check_batch(ctx, cfg, n, refs, curs);
+  if (rc) return rc;
+  cudaStream_t st = ctx->stream;
+  Workspace& ws = ctx->ws;
+  const int first = cfg->first_level, last = cfg->last_level, s = screen_level;
+  const int nk = n * k, nlev1 = first - s + 1, nlev2 = s - last;
+  const int max_log = iter_stats ? max_iter_stats : 0;
+  const LevelVariant v{ctx->estimator == DVO_B200_ESTIMATOR_CORRECTED, any_current_mask(n, curs), false, false};
+  if ((rc = ensure_geometry(ctx, v))) return rc;
+  const LaunchPlan plan1 = plan_launches(ctx, refs[0], first, s, nk, v);
+  LaunchPlan plan2{};
+  if (nlev2 > 0) plan2 = plan_launches(ctx, refs[0], s - 1, last, n, v);
+  const size_t ndesc1 = (size_t)nk * nlev1, ndesc = ndesc1 + (size_t)n * nlev2;
+  const int slots = (int)std::max(ndesc, (size_t)nk + n);   // descriptors, and states and logs of both stages
+  if ((rc = ensure_workspace(ctx, slots, plan1, nk, 0, max_log, v))) return rc;
+  if (nlev2 > 0 && (rc = ensure_workspace(ctx, slots, plan2, n, 0, max_log, v))) return rc;
+  for (int i = 0; i < n; ++i)
+    if ((rc = pyramid_reselect(ctx, refs[i], cfg->intensity_derivative_threshold, cfg->depth_derivative_threshold))) return rc;
+
+  const size_t res_bytes = sizeof(dvo_b200_result) * (size_t)n, screen_bytes = h_screen ? sizeof(dvo_b200_result) * (size_t)nk : 0;
+  const size_t score_bytes = sizeof(double) * (size_t)nk, out_bytes = res_bytes + screen_bytes + score_bytes + sizeof(int) * (size_t)n;
+  if ((rc = ensure_stage(ctx, out_bytes, 0))) return rc;
+  if ((rc = ensure_pinned_results(ctx, out_bytes))) return rc;
+  const MatchStageLayout sl = match_stage_layout(ndesc, nk, true, false, v);
+  if ((rc = ensure_stage(ctx, 0, sl.total))) return rc;
+  if (v.cur_mask && (rc = grow(ctx, ws.d_csat, ws.cap_csat, sl.csat.bytes / sizeof(const int*)))) return rc;
+  if ((rc = grow(ctx, ws.d_tinit, ws.cap_tinit, (size_t)16 * nk))) return rc;
+  DVO_CUDA(ctx, cudaStreamSynchronize(st));   // previous use of the pinned stage has drained
+  char* const h = (char*)ctx->h_stage;
+  PairLevel* const h_desc = (PairLevel*)(h + sl.desc.at);
+  const int** h_csat = (const int**)(h + sl.csat.at);
+  std::vector<dvo_b200_pyramid*> vrefs((size_t)nk), vcurs((size_t)nk);
+  for (int q = 0; q < nk; ++q) { vrefs[q] = refs[q / k]; vcurs[q] = curs[q / k]; }
+  for (int level = first, li = 0; level >= s; --level, ++li) {
+    fill_pair_levels(h_desc + (size_t)li * nk, nk, vrefs.data(), vcurs.data(), level);
+    if (v.cur_mask) fill_pair_csat(h_csat + (size_t)li * nk, nk, vcurs.data(), level);
+  }
+  for (int level = s - 1, li = 0; level >= last; --level, ++li) {
+    fill_pair_levels(h_desc + ndesc1 + (size_t)li * n, n, refs, curs, level);
+    if (v.cur_mask) fill_pair_csat(h_csat + ndesc1 + (size_t)li * n, n, curs, level);
+  }
+  std::memcpy(h + sl.tinit.at, hypotheses, sl.tinit.bytes);
+  ctx->h2d_bytes += sl.desc.bytes + sl.tinit.bytes + sl.csat.bytes;
+  {
+    ProfScope prof(ctx, 2);
+    stage_words(ctx, h_desc, ws.d_pair_level, sl.desc.bytes);
+    stage_words(ctx, h + sl.tinit.at, ws.d_tinit, sl.tinit.bytes);
+    if (v.cur_mask) stage_words(ctx, h_csat, ws.d_csat, sl.csat.bytes);
+  }
+
+  for (int i = 0; i < 8; ++i) ws.h_active[i] = 0;
+  if (max_log > 0)
+    DVO_CUDA(ctx, cudaMemsetAsync(ws.d_iter_log, 0, sizeof(dvo_b200_iteration_stats) * (size_t)(nk + n) * max_log, st));
+  const LaunchTarget screen{ws.d_state, ws.d_pair_level, ws.d_iter_log, 0};
+  const LaunchTarget chosen{ws.d_state + nk, ws.d_pair_level + ndesc1, ws.d_iter_log + (size_t)nk * max_log, nlev1};
+  for (int i = 0; i < plan1.nlaunch; ++i)
+    if ((rc = launch_segments(ctx, plan1.launch[i], i, cfg, refs[0]->L, first, ws.d_tinit, nk, max_log, nullptr, 0, v, screen)))
+      return rc;
+  char* const d_out = (char*)ctx->d_stage;
+  dvo_b200_result* const d_res = (dvo_b200_result*)d_out;
+  double* const d_scores = (double*)(d_out + res_bytes + screen_bytes);
+  int* const d_best = (int*)(d_out + res_bytes + screen_bytes + score_bytes);
+  {
+    ProfScope prof(ctx, 2);
+    if (h_screen) {
+      k_finalize<<<(nk + 63) / 64, 64, 0, st>>>(ws.d_state, (dvo_b200_result*)(d_out + res_bytes), nk);
+      ctx->launches++;
+    }
+    k_pick_hypotheses<<<(n + 3) / 4, 128, 0, st>>>(screen.states, screen.ilog, chosen.states, chosen.ilog, max_log, n, k, nlev1 - 1,
+                                                   min_ratio, d_scores, d_best);
+    ctx->launches++;
+  }
+  for (int i = 0; i < plan2.nlaunch; ++i)
+    if ((rc = launch_segments(ctx, plan2.launch[i], plan1.nlaunch + i, cfg, refs[0]->L, s - 1, nullptr, n, max_log, nullptr, 0, v,
+                              chosen)))
+      return rc;
+  {
+    ProfScope prof(ctx, 2);
+    k_finalize<<<(n + 63) / 64, 64, 0, st>>>(chosen.states, d_res, n);
+    ctx->launches++;
+  }
+  DVO_CUDA(ctx, cudaGetLastError());
+  if ((rc = note_foreign_uses(ctx, n, refs, curs))) return rc;   // the caller may release the pyramids once this returns
+  ctx->pending_level_flags = plan1.nlaunch + plan2.nlaunch;
+
+  DVO_CUDA(ctx, cudaMemcpyAsync(ctx->h_results, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+  ctx->d2h_bytes += out_bytes;
+  if (iter_stats) {
+    DVO_CUDA(ctx, cudaMemcpyAsync(iter_stats, chosen.ilog, sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log,
+                                  cudaMemcpyDeviceToHost, st));
+    ctx->d2h_bytes += sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log;
+  }
+  DVO_CUDA(ctx, cudaStreamSynchronize(st));
+  const char* const hr = (const char*)ctx->h_results;
+  std::memcpy(h_results, hr, res_bytes);
+  if (h_screen) std::memcpy(h_screen, hr + res_bytes, screen_bytes);
+  if (h_scores) std::memcpy(h_scores, hr + res_bytes + screen_bytes, score_bytes);
+  std::memcpy(h_best, hr + res_bytes + screen_bytes + score_bytes, sizeof(int) * (size_t)n);
+  return check_level_flags(ctx);
 }
 
 }  // namespace dvo_b200

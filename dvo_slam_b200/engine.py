@@ -15,6 +15,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("DVO_B200_LIB", os.path.join(_HERE, "libdvo_b200.so"))   # env override: developer A/B builds
 MAX_LEVELS = 8
+MAX_HYPOTHESES = 64   # DVO_B200_MAX_HYPOTHESES
 
 TERMINATION_NAMES = ["IterationsExceeded", "IncrementTooSmall", "LogLikelihoodDecreased", "TooFewConstraints"]
 
@@ -37,6 +38,7 @@ ABI_SYMBOLS = [
     "dvo_b200_pyramid_create_rectified_device_batch", "dvo_b200_depth_rays", "dvo_b200_depth_registration_create",
     "dvo_b200_depth_registration_release", "dvo_b200_pyramid_create_registered_batch",
     "dvo_b200_pyramid_create_registered_device_batch", "dvo_b200_match_batch_prior", "dvo_b200_match_batch_maps",
+    "dvo_b200_match_batch_hypotheses",
 ]
 
 # dvo_b200_estimator
@@ -237,6 +239,21 @@ def prior_from_result(result: Result, scale: float = 1.0) -> np.ndarray:
     return 0.5 * (lam + lam.T)
 
 
+def _results(res, n, log=None, max_log=0) -> list[Result]:
+    """Result views of n dvo_b200_result, with each pair's iterations when a log of max_log entries per pair is given"""
+    out = []
+    for i in range(n):
+        its = []
+        if log is not None:
+            for k in range(res[i].num_iterations_total):
+                s = log[i * max_log + k]
+                its.append({"level": s.level, "id": s.id, "n": s.valid_constraints, "nll": s.tdist_log_likelihood,
+                            "precision": np.array(s.tdist_precision).reshape(2, 2), "prior": s.prior_log_likelihood,
+                            "x": np.array(s.increment), "A": np.array(s.information).reshape(6, 6)})
+        out.append(Result(res[i], its))
+    return out
+
+
 _lib = None
 
 
@@ -321,6 +338,8 @@ def load_library():
                                              C.POINTER(IterationStats), i32]
     L.dvo_b200_match_batch_maps.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), dp, dp, dp, dp, C.POINTER(CResult),
                                             C.POINTER(IterationStats), i32, C.POINTER(WeightMaps)]
+    L.dvo_b200_match_batch_hypotheses.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), i32, dp, i32, C.c_double,
+                                                   C.POINTER(CResult), C.POINTER(i32), dp, C.POINTER(CResult), C.POINTER(IterationStats), i32]
     L.dvo_b200_residual_image_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, fp, C.POINTER(i64)]
     L.dvo_b200_linearize_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, i32, fp, C.POINTER(i64), fp, fp, dp, dp]
     L.dvo_b200_set_estimator.argtypes = [vp, i32]
@@ -854,16 +873,42 @@ class Engine:
                                                                   log, max_log))
         if raw:
             return res
-        out = []
-        for i in range(n):
-            its = []
-            if with_iterations:
-                for k in range(res[i].num_iterations_total):
-                    s = log[i * max_log + k]
-                    its.append({"level": s.level, "id": s.id, "n": s.valid_constraints, "nll": s.tdist_log_likelihood,
-                                "precision": np.array(s.tdist_precision).reshape(2, 2), "prior": s.prior_log_likelihood,
-                                "x": np.array(s.increment), "A": np.array(s.information).reshape(6, 6)})
-            out.append(Result(res[i], its))
+        return _results(res, n, log, max_log)
+
+    def match_batch_hypotheses(self, refs, curs, hypotheses, screen_level: int, min_constraint_ratio: float = 0.0,
+                               cfg: Config | None = None, with_iterations: bool = False, screen_results: bool = False):
+        """Multi-hypothesis alignment (dvo_b200_match_batch_hypotheses): pair i starts from each of the k poses
+        hypotheses[i] ([n, k, 4, 4], read as T_init) on levels cfg.first_level .. screen_level, and the one with the lowest
+        per-constraint negative log-likelihood among those with a large enough constraint ratio continues to cfg.last_level.
+        cfg: default Config(use_initial_estimate=1).  Returns (results, best [n] int32, scores [n, k] float64, NaN where a
+        hypothesis was not eligible), and with screen_results=True also the screening results, a list of n lists of k."""
+        if cfg is None:
+            cfg = Config(use_initial_estimate=1)
+        n = len(refs)
+        assert n == len(curs) and n > 0
+        H = np.asarray(hypotheses, dtype=np.float64)
+        if H.ndim != 4 or H.shape[0] != n or H.shape[2:] != (4, 4):
+            raise ValueError(f"hypotheses {H.shape}: want [{n}, k, 4, 4]")
+        k = H.shape[1]
+        H = np.ascontiguousarray(H.reshape(n * k, 16))
+        rh = (C.c_void_p * n)(*[p.handle for p in refs])
+        ch = (C.c_void_p * n)(*[p.handle for p in curs])
+        res = (CResult * n)()
+        best = np.zeros(n, dtype=np.int32)
+        scores = np.zeros((n, k), dtype=np.float64)
+        screen = (CResult * (n * k))() if screen_results else None
+        max_log, log = 0, None
+        if with_iterations:
+            max_log = (cfg.first_level - cfg.last_level + 1) * (cfg.max_iterations_per_level + 1)
+            log = (IterationStats * (n * max_log))()
+        dp = C.POINTER(C.c_double)
+        self._check(self.lib.dvo_b200_match_batch_hypotheses(
+            self.ctx, C.byref(cfg), n, rh, ch, k, H.ctypes.data_as(dp), int(screen_level), float(min_constraint_ratio), res,
+            best.ctypes.data_as(C.POINTER(C.c_int32)), scores.ctypes.data_as(dp), screen, log, max_log))
+        out = (_results(res, n, log, max_log), best, scores)
+        if screen_results:
+            flat = [Result(screen[i]) for i in range(n * k)]
+            out += ([flat[i * k:(i + 1) * k] for i in range(n)],)
         return out
 
     def match_batch_device(self, refs, curs, cfg: Config, d_results_ptr: int, T_init=None):

@@ -8,6 +8,7 @@
 #include <stdexcept>
 
 #include "dvo/dense_tracking.h"
+#include "../csrc/hypotheses_args.h"   // the checks of dvo_b200_match_batch_hypotheses, run here so that a refusal returns false
 #include "../csrc/prior_args.h"   // the prior checks of dvo_b200_match_batch_prior, run here so that a refusal returns false
 
 namespace dvo {
@@ -397,6 +398,43 @@ bool DenseTracker::matchWithWeights(core::RgbdImagePyramid& reference, core::Rgb
   const bool ok = matchBatch(refs, curs, static_cast<const double*>(0), results, &weights);
   if (ok) result = results[0];
   return ok;
+}
+
+bool DenseTracker::matchWithHypotheses(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current,
+                                       const std::vector<core::AffineTransformd>& initial, int screen_level, Result& result, int* best,
+                                       double min_constraint_ratio) {
+  dvo_b200_config c;
+  dvo_b200_config_default(&c);
+  c.first_level = cfg.FirstLevel; c.last_level = cfg.LastLevel; c.max_iterations_per_level = cfg.MaxIterationsPerLevel;
+  c.use_initial_estimate = 1; c.precision = cfg.Precision; c.mu = cfg.Mu;
+  c.intensity_derivative_threshold = cfg.IntensityDerivativeThreshold; c.depth_derivative_threshold = cfg.DepthDerivativeThreshold;
+  const int k = int(initial.size());
+  std::vector<double> H(16 * initial.size());
+  for (int j = 0; j < k; ++j)
+    for (int a = 0; a < 4; ++a) for (int b = 0; b < 4; ++b) H[16 * j + a * 4 + b] = initial[j].matrix()(a, b);
+  dvo_b200_result raw;
+  int32_t chosen = 0;
+  if (!dvo_b200::hypotheses_args_error(&c, 1, k, H.data(), screen_level, min_constraint_ratio, &raw, &chosen).empty()) return false;
+  dvo_b200_ctx* ctx = context();
+  dvo_b200_pyramid *r, *q;
+  {
+    std::vector<core::RgbdImagePyramid*> all(1, &reference);
+    all.push_back(&current);
+    for (size_t i = 0; i < all.size(); ++i) all[i]->compute(cfg.getNumLevels());
+    std::vector<dvo_b200_pyramid*> dev;
+    core::RgbdImagePyramid::deviceBatch(ctx, all, cfg.getNumLevels(), dev);
+    r = dev[0]; q = dev[1];
+  }
+  const int max_log = collect_iterations_ ? (cfg.FirstLevel - cfg.LastLevel + 1) * (cfg.MaxIterationsPerLevel + 1) : 0;
+  std::vector<dvo_b200_iteration_stats> its((size_t)max_log);
+  if (dvo_b200_match_batch_hypotheses(ctx, &c, 1, &r, &q, k, H.data(), screen_level, min_constraint_ratio, &raw, &chosen, 0, 0,
+                                      max_log ? its.data() : 0, max_log) != 0)
+    throw std::runtime_error(std::string("dvo_b200_match_batch_hypotheses: ") + dvo_b200_last_error(ctx));
+  Result out;
+  fill_result(raw, max_log ? its.data() : 0, out);
+  result = out;
+  if (best) *best = chosen;
+  return true;
 }
 
 bool DenseTracker::matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,

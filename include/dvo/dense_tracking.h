@@ -117,6 +117,17 @@ class DenseTracker {
   // every other pixel.  Small weights mark the pixels the estimator treated as outliers (moving objects, occlusions). ---
   bool matchWithWeights(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current, Result& result, cv::Mat& weights);
 
+  // --- extension: multi-hypothesis alignment (dvo_b200_match_batch_hypotheses; include/dvo_b200.h).  Aligns from each pose of
+  // `initial` (1 .. DVO_B200_MAX_HYPOTHESES initial estimates, UseInitialEstimate implied) on the levels FirstLevel ..
+  // screen_level, and continues the one with the lowest per-constraint negative log-likelihood among those whose constraint
+  // ratio is at least min_constraint_ratio (dvo_slam's ConstraintRatioVoter) to LastLevel.  result is then what match()
+  // returns from that hypothesis; *best (if given) its index.  Returns false, without aligning, when the arguments are
+  // refused (no or too many hypotheses, a non-finite or non-rigid 4 x 4, screen_level outside [LastLevel, FirstLevel], a
+  // ratio outside [0, 1]). ---
+  bool matchWithHypotheses(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current,
+                           const std::vector<core::AffineTransformd>& initial, int screen_level, Result& result, int* best = 0,
+                           double min_constraint_ratio = 0.0);
+
   // per-iteration statistics are copied back only when requested (they are optional in the C ABI)
   void collectIterationStatistics(bool on) { collect_iterations_ = on; }
   // Extension: the corrected estimator of dvo_b200_estimator (exact scale sum, log-likelihood over all points, the odd last

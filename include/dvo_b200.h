@@ -635,6 +635,45 @@ int dvo_b200_match_batch_maps(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int
                               double* photometric, dvo_b200_result* results, dvo_b200_iteration_stats* iteration_stats,
                               int32_t max_iteration_stats, const dvo_b200_weight_maps* maps);
 
+/* ---- multi-hypothesis alignment: screen several initial poses per pair on the coarse levels, continue the best one -------
+ * Dense Gauss-Newton has a small basin of convergence: after a fast rotation, a dropped frame or a loop-closure candidate
+ * whose relative pose comes from a drifted graph, one initial estimate can end in a confident, wrong pose.  This call
+ * starts pair p from k hypotheses H[p][0..k-1] (row-major 4 x 4, read as T_init), runs each of them on the coarse levels
+ * first_level .. s only (s = screen_level), keeps one, and continues that one, from where its screening run ended, through
+ * levels s-1 .. last_level.  With cfg->first_level = s the screening is dvo_slam's proposal validation on one level
+ * (ConstraintProposalValidator with FirstLevel = LastLevel = 3), and the continuation its second stage.
+ *   screening  hypothesis j runs levels first_level .. s exactly as dvo_b200_match_batch does with T_init = H[p][j], the
+ *              same cfg except last_level = s.  Let L be that run's dvo_b200_level_stats of level s.
+ *   score      j is eligible iff L.has_iteration_with_increment, ratio = L.last_increment_valid_constraints / L.valid_pixels
+ *              >= min_constraint_ratio (fp64, as dvo_slam's ConstraintRatioVoter), and score =
+ *              L.last_increment_log_likelihood / L.last_increment_valid_constraints, the per-constraint negative
+ *              log-likelihood, is finite.  Lower is better.
+ *   choice     best[p] is the eligible j with the smallest score, the lowest j on a tie; 0 if none is eligible (then every
+ *              score of the pair is NaN).
+ * Results, bit for bit, for every estimator, mask, batch size and launch plan:
+ *   results[p] and pair p's iteration log are those of dvo_b200_match_batch of that pair alone with T_init = H[p][best[p]]
+ *              (every field, the statistics of the screening levels included);
+ *   screen_results[p * k + j] (optional) are those of dvo_b200_match_batch with last_level = s and T_init = H[p][j];
+ *   scores[p * k + j] (optional) are the scores above, NaN where j is not eligible.
+ * Cost: the screening aligns n * k pairs on the coarse levels, the continuation n pairs on the fine ones; a coarse level has a
+ * quarter of the pixels of the next finer one.  Reference-role and both-role masks, cfg->mu and mixed intrinsics are
+ * supported as by dvo_b200_match_batch.
+ * Not provided in this mode: the photometric mode, motion priors, weight maps, match_batch_device and the sharded forms. */
+#define DVO_B200_MAX_HYPOTHESES 64
+
+/* hypotheses: n * k * 16 doubles, H[p][j] at (p * k + j) * 16.  results, best: n each.  scores: n * k or NULL.
+ * screen_results: n * k or NULL.  iteration_stats / max_iteration_stats as in dvo_b200_match_batch (the continued alignment's
+ * log).  Refused with DVO_B200_ERR_INVALID_ARGUMENT, and dvo_b200_last_error set, before anything is staged, uploaded or
+ * launched: a NULL hypotheses, results or best; k outside [1, DVO_B200_MAX_HYPOTHESES]; cfg->use_initial_estimate == 0 (the
+ * hypotheses are the initial estimates); screen_level outside [cfg->last_level, cfg->first_level]; a min_constraint_ratio
+ * that is not finite or lies outside [0, 1]; a hypothesis with a non-finite entry or a bottom row other than (0, 0, 0, 1);
+ * and everything dvo_b200_match_batch refuses for the same n pairs.  Synchronises as dvo_b200_match_batch does. */
+int dvo_b200_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n,
+                                    dvo_b200_pyramid* const* references, dvo_b200_pyramid* const* currents, int32_t k,
+                                    const double* hypotheses, int32_t screen_level, double min_constraint_ratio,
+                                    dvo_b200_result* results, int32_t* best, double* scores, dvo_b200_result* screen_results,
+                                    dvo_b200_iteration_stats* iteration_stats, int32_t max_iteration_stats);
+
 /* ---- profiling hooks (bench.py roofline): per-kernel-class accumulated device time measured with
  *      CUDA events on the ctx stream.  classes: 0 residual/scale stage, 1 normal-equation stage,
  *      2 per-pair step kernels, 3 pyramid build, 4 selection. -------------------------------- */
