@@ -281,7 +281,9 @@ void pyramid_free(dvo_b200_pyramid* p);
 void pool_close(dvo_b200_ctx* ctx);
 int ensure_stage(dvo_b200_ctx* ctx, size_t dev_bytes, size_t host_bytes);
 
-// tracker.cu
+// tracker.cu.  The three calls below run the level kernel in legs (tracker.cu: Leg), each one run over a range of pyramid
+// levels of a batch of pairs, through one path: check_batch and begin_call, ensure_workspace, stage_inputs, launch_segments,
+// end_call.  A match is one leg, the hypotheses call two, and a test hook one leg of one pair at one level.
 // ab_out != NULL: the photometric mode (8 unknowns: pose, gain, bias), from ab_init (2n doubles, NULL = (1, 0) each); the
 // final (alpha, beta) of each pair go to ab_out (host, 2n doubles).  Needs h_results.
 // prior != NULL: a motion prior, n row-major 6 x 6 informations (host) in place of cfg->mu I (which must then be 0).
@@ -291,13 +293,14 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
                         const double* ab_init = nullptr, double* ab_out = nullptr, const double* prior = nullptr,
                         const dvo_b200_weight_maps* maps = nullptr);   // maps != NULL: also the weight maps (weight_maps.cu)
 int check_level_flags(dvo_b200_ctx* ctx);   // after a stream synchronisation: did a level kernel report a timeout?
-// dvo_b200_match_batch_hypotheses after its argument checks (hypotheses_args.h): the screening of n * k virtual pairs on levels
-// first .. screen_level, k_pick_hypotheses, and the continuation of the n chosen ones on the levels below.  scores and
+// dvo_b200_match_batch_hypotheses after its argument checks (hypotheses_args.h): a leg screening n * k virtual pairs on levels
+// first .. screen_level, k_pick_hypotheses, and a leg continuing the n chosen ones on the levels below.  scores and
 // screen_results (host, n * k) may be NULL.
 int tracker_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                                    dvo_b200_pyramid* const* curs, int k, const double* hypotheses, int screen_level,
                                    double min_ratio, dvo_b200_result* h_results, int32_t* h_best, double* h_scores,
                                    dvo_b200_result* h_screen, dvo_b200_iteration_stats* iter_stats, int max_iter_stats);
+// The test hooks: one iteration at T (staged as the leg's initial estimate and placed into the state by k_set_state).
 int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* ref, dvo_b200_pyramid* cur,
                       int level, const double* T, int use_weights, const float* prev_precision, int64_t* count,
                       float* precision_out, float* ll_out, double* A_out, double* b_out, float* planes7,
