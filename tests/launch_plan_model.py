@@ -4,9 +4,10 @@ The plan is chosen on the host from the batch size, the grid (SMs x resident CTA
 launch per level with squads of up to 69 CTAs for small batches; for batches of at least grid/4 pairs a coarse segment
 with one CTA per pair, fused with up to three slices of the fine levels with squads of g, 2g and 4g CTAs; and the developer
 overrides DVO_B200_* on top.  test_launch_plan_host.py checks the C++ against this restatement segment for segment;
-test_gpu_launch_plans.py uses it to pick batch sizes and to count the persistent launches of a call on the device.
+test_gpu_launch_plans.py uses it to pick batch sizes and to count the persistent launches of a call on the device.  The
+tile geometry is the kernel's (tests/tile_geometry.py).
 """
-TILE_W, TILE_H = 128, 7
+from tile_geometry import TILE_H, TILE_W
 OVERHEAD_TILES = 45.0      # level_squad_size's per-stage overhead, in tile-times
 COARSE_TILES = 110         # levels of at most this many tiles take one CTA per pair in a walking plan
 KNOBS = ("DVO_B200_NO_WALK", "DVO_B200_NO_FUSE", "DVO_B200_CONTIGUOUS", "DVO_B200_COARSE_TILES", "DVO_B200_TAIL",

@@ -5,9 +5,9 @@ their tiles take the exact pixel loops (which end with an odd fifth stage-A roun
 is not a multiple of 160: 400 x 300 has bands of 160, 160 and 80 columns at level 0 and of 160 and 40 at level 1, so each
 level has both full bands (exact loops) and a partial band (generic loop).  That case is checked here as the other
 generic-loop cases are: residual records bit-exact against the oracle's MIRROR mode (and the corrected estimator's
-definition), and a batch returning the bits of single alignments, for both estimators.  On the host: the shared-memory
-layout still leaves room for two CTAs per SM, and every geometry the launch-plan tests run keeps the launch count that
-their 128-column restatement of the plan predicts.
+definition), and a batch returning the bits of single alignments, for both estimators.  On the host: the compiled tile
+geometry is the one the suite computes with (tests/tile_geometry.py), and the shared-memory layout still leaves room for
+two CTAs per SM.
 """
 import os
 import shutil
@@ -17,16 +17,13 @@ import numpy as np
 import pytest
 
 import launch_plan_model as lpm
+import tile_geometry as tg
+from tile_geometry import TILE_H, TILE_W, assert_partial_band, bands
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-TILE_W, TILE_H = 160, 7
 W, H, LEVELS = 400, 300, 4
 CARVEOUT, SMEM_RESERVED_PER_CTA = 196 * 1024, 1024     # of an H100 SM's 256 KB: 60 KB stay L1; 1 KB per resident CTA
 LARGEST_TAIL = 5696      # sizeof(LevelTailOf<true, true>) (photometric, motion prior) in tracker.cu under nvcc 12.9
-
-
-def _bands(w):
-    return [min(TILE_W, w - x0) for x0 in range(0, w, TILE_W)]
 
 
 # ---- host ----
@@ -47,15 +44,43 @@ def layout(tmp_path_factory):
 
 def test_tile_geometry(layout):
     """160 x 7 tiles; the window holds the tile's columns plus 24, in 19 rows; the record is 2 320 float2, of which stage A
-    copies the first 1 200; every bulk copy is a multiple of 16 bytes"""
+    copies the first 1 200; every bulk copy is a multiple of 16 bytes.  The suite's geometry (tests/tile_geometry.py) is the
+    compiled one."""
     L = layout
-    assert (L["tile_w"], L["tile_h"], L["win_cols"], L["win_rows"], L["stages"]) == (TILE_W, TILE_H, TILE_W + 24, 19, 2)
+    assert (L["tile_w"], L["tile_h"], L["win_cols"], L["win_rows"]) == (tg.TILE_W, tg.TILE_H, tg.WIN_COLS, tg.WIN_ROWS)
+    assert (L["tile_w"], L["tile_h"], L["win_cols"], L["win_rows"], L["stages"]) == (160, 7, 160 + 24, 19, 2)
+    assert lpm.TILE_W == tg.TILE_W and lpm.TILE_H == tg.TILE_H
     assert L["rec_bytes"] == 8 * (2 * TILE_H * TILE_W + TILE_W // 2) == 18560
     assert L["rec_stage_a_bytes"] == 8 * (TILE_H * TILE_W + TILE_W // 2) == 9600
     assert L["rec_bytes"] % 16 == 0 and L["rec_stage_a_bytes"] % 16 == 0 and (8 * L["win_cols"]) % 16 == 0
     assert L["win_cols"] < 256                                  # produce_tiles packs the window width into 8 bits
-    assert _bands(640) == [160] * 4 and _bands(320) == [160] * 2 and _bands(160) == [160]
-    assert _bands(W) == [160, 160, 80] and _bands(W // 2) == [160, 40]
+    assert bands(640) == [160] * 4 and bands(320) == [160] * 2 and bands(160) == [160]
+    assert bands(W) == [160, 160, 80] and bands(W // 2) == [160, 40]
+
+
+def test_partial_band_helper():
+    """the helper the partial-band cases assert their geometry with: full bands followed by a partial one, nothing else"""
+    assert assert_partial_band(W) == [160, 160, 80] and assert_partial_band(W // 2) == [160, 40]
+    assert assert_partial_band(161) == [160, 1] and assert_partial_band(319) == [160, 159]
+    for w in (640, 320, 160, 80, 40, 128, 1280):
+        with pytest.raises(AssertionError):
+            assert_partial_band(w)
+    assert tg.in_partial_band(160, 161) and not tg.in_partial_band(159, 161) and not tg.in_partial_band(319, 320)
+    assert tg.level_shapes(640, 480, 5) == [(640, 480), (320, 240), (160, 120), (80, 60), (40, 30)]
+    assert tg.strips(480) == [7] * 68 + [4] and tg.strips(14) == [7, 7]
+
+
+def test_tile_edge_sizes_state_their_case():
+    """every size of test_gpu_geometry reaches the case it states on 160-column bands; the sizes chosen for 128-column
+    bands (a 1-, 33- and 63-column band at 129, 161 and 191, whole bands at 256) are refused"""
+    from test_gpu_geometry import SIZES, _assert_reason
+    for w, h, levels in SIZES:
+        _assert_reason(w, h, levels)
+    partial = sorted(bands(w)[-1] for w, _, _ in SIZES if len(bands(w)) >= 2 and bands(w)[-1] < TILE_W)
+    assert {1, 33, 63, 128, 159} <= set(partial), partial
+    for w, h, levels in ((129, 50, 3), (161, 55, 3), (191, 49, 3), (256, 96, 3)):
+        with pytest.raises(AssertionError):
+            _assert_reason(w, h, levels)
 
 
 def test_shared_memory_leaves_two_ctas_per_sm(layout):
@@ -67,23 +92,6 @@ def test_shared_memory_leaves_two_ctas_per_sm(layout):
     assert L["tile_pipe"] == 93312
     assert L["seg_combine"] < LARGEST_TAIL           # the tail holds the strip combine's scratch and the end step's state
     assert 2 * (L["tile_pipe"] + LARGEST_TAIL + SMEM_RESERVED_PER_CTA) <= CARVEOUT
-
-
-@pytest.mark.parametrize("geom,first,last", [((640, 480, 5), 4, 0), ((640, 480, 5), 3, 1), ((640, 480, 5), 0, 0),
-                                             ((1280, 960, 6), 5, 0)], ids=["640-4..0", "640-3..1", "640-0..0", "1280-5..0"])
-def test_launch_counts_do_not_depend_on_the_band_width(monkeypatch, geom, first, last):
-    """The ranges test_gpu_launch_plans.py runs, at every batch size up to 1077 and with every override: 160-column bands
-    give the same coarse / fine split and the same number of persistent launches as the 128-column restatement."""
-    grid = 264
-    envs = [{}] + [{f"DVO_B200_{k}": v} for k, v in lpm.OVERRIDES]
-
-    def plans(tile_w):
-        monkeypatch.setattr(lpm, "TILE_W", tile_w)
-        g = lpm.level_geometry(*geom)
-        return [(p["launches"], p["fused"], [(G["first_li"], G["nlev"]) for G in p["groups"]])
-                for env in envs for n in range(1, 1078) for p in [lpm.plan(g, first, last, grid, n, env)]]
-
-    assert plans(128) == plans(TILE_W)
 
 
 # ---- GPU ----
@@ -130,7 +138,7 @@ def _pose(name):
 def test_records_reference_estimator(engine, oracle, pair400, lvl, pose):
     """full bands and a partial band in every strip: records bit-exact against MIRROR, counts exact, P / LL / A / b to 2e-6"""
     from test_gpu_generic_tiles import _check_level
-    assert len(_bands(W >> lvl)) >= 2 and _bands(W >> lvl)[-1] < TILE_W
+    assert_partial_band(W >> lvl)
     _check_level(engine, oracle, pair400, lvl, _pose(pose))
 
 
@@ -162,7 +170,7 @@ def test_batch_equals_single_alignments(engine, corrected, batch400, est):
     """a 72-pair batch (fused walking launch) returns, pair for pair, the bits of the pair's single alignment"""
     from dvo_slam_b200.engine import Config
     from test_gpu_mixed_batch import _same
-    assert (H // TILE_H + 1) * len(_bands(W)) > lpm.COARSE_TILES >= (H // 2 // TILE_H + 1) * len(_bands(W // 2))
+    assert (H // TILE_H + 1) * len(bands(W)) > lpm.COARSE_TILES >= (H // 2 // TILE_H + 1) * len(bands(W // 2))
     eng = engine if est == "reference" else corrected
     cfg = Config(first_level=LEVELS - 1, last_level=0, max_iterations_per_level=50, precision=1e-4)
     pairs = batch400[est]

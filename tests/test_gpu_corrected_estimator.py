@@ -12,7 +12,8 @@ import pytest
 
 from helpers import nan_equal, odd_point_margin, pose_delta
 from test_corrected_estimator import corrected_mode
-from test_gpu_generic_tiles import TILE_H, TILE_W, WIN_ROWS, _rot_z, _shift_z
+from test_gpu_generic_tiles import partial_pair, partial_pose, _rot_z, _shift_z
+from tile_geometry import TILE_H, TILE_W, WIN_ROWS, assert_partial_band
 
 pytestmark = pytest.mark.gpu
 
@@ -34,6 +35,17 @@ def pair(engine, oracle):
     p = synth.make_pair(0)
     a = {k: p[k].numpy() for k in ("I_ref", "Z_ref", "I_cur", "Z_cur")}
     a["K"] = p["intrinsics"]
+    a["gref"] = engine.pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
+    a["gcur"] = engine.pyramid(a["I_cur"], a["Z_cur"], a["K"], 5)
+    a["oref"] = oracle.Pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
+    a["ocur"] = oracle.Pyramid(a["I_cur"], a["Z_cur"], a["K"], 5)
+    return a
+
+
+@pytest.fixture(scope="module")
+def pair720(engine, oracle):
+    """the partial-band scene of test_gpu_generic_tiles"""
+    a = partial_pair(0)
     a["gref"] = engine.pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
     a["gcur"] = engine.pyramid(a["I_cur"], a["Z_cur"], a["K"], 5)
     a["oref"] = oracle.Pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
@@ -147,9 +159,9 @@ def test_corner_behind_camera(corrected, oracle, pair):
 
 
 @pytest.mark.parametrize("lvl", [1, 2])
-def test_partial_band(corrected, oracle, pair, lvl):
-    assert (pair["I_ref"].shape[1] >> lvl) % TILE_W != 0
-    _check_level(corrected, oracle, pair, lvl, _rot_z(3.0) @ _shift_z(0.02))
+def test_partial_band(corrected, oracle, pair720, lvl):
+    assert_partial_band(pair720["oref"].level_info(lvl)[0])
+    _check_level(corrected, oracle, pair720, lvl, partial_pose())
 
 
 # ---- whole alignments ----

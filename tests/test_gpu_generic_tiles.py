@@ -4,16 +4,41 @@ Almost every tile of an alignment takes the exact loop (window holds all taps, f
 rest: windows the taps do not fit, tiles with a corner behind the camera (no window at all: every tap is gathered), and
 partial bands at the right edge.  Each case is forced here by the pose or the level, shown from the geometry, and checked
 as test_gpu_parity checks the exact loop: residual records bit-exact, counts exact, P / LL / A / b to 2e-6.
+
+The partial bands come from a 720 x 540 scene (PARTIAL): levels 0, 1 and 2 are 720, 360 and 180 columns wide, so each has
+full 160-column bands and a partial last band of 80, 40 and 20 columns.  The other modules that force the generic loop
+take their partial-band case from here.
 """
 import numpy as np
 import pytest
 
 from helpers import nan_equal
+from tile_geometry import TILE_H, TILE_W, WIN_ROWS, assert_partial_band
 
 pytestmark = pytest.mark.gpu
 
-TILE_W, TILE_H = 128, 7
-WIN_ROWS = 24           # window capacity in rows (kWinRows of csrc/stages.cuh)
+PARTIAL_W, PARTIAL_H = 720, 540
+
+
+def partial_scene():
+    """the scene config of the partial-band cases: fr1 intrinsics scaled to 720 x 540"""
+    from dvo_slam_b200 import synth
+    s = PARTIAL_W / 640
+    return synth.SceneConfig(width=PARTIAL_W, height=PARTIAL_H, intrinsics=tuple(v * s for v in synth.FR1_INTRINSICS))
+
+
+def partial_pair(seed=0):
+    """images and intrinsics of one pair of the partial-band scene"""
+    from dvo_slam_b200 import synth
+    p = synth.make_pair(seed, partial_scene())
+    a = {k: p[k].numpy() for k in ("I_ref", "Z_ref", "I_cur", "Z_cur")}
+    a["K"] = p["intrinsics"]
+    return a
+
+
+def partial_pose():
+    """a small motion under which most tiles of levels 1 and 2 keep a window"""
+    return _rot_z(3.0) @ _shift_z(0.02)
 
 
 def _rot_z(deg):
@@ -42,6 +67,16 @@ def pair(engine, oracle):
     return a
 
 
+@pytest.fixture(scope="module")
+def pair720(engine, oracle):
+    a = partial_pair(0)
+    a["gref"] = engine.pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
+    a["gcur"] = engine.pyramid(a["I_cur"], a["Z_cur"], a["K"], 5)
+    a["oref"] = oracle.Pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
+    a["ocur"] = oracle.Pyramid(a["I_cur"], a["Z_cur"], a["K"], 5)
+    return a
+
+
 def _check_level(engine, oracle, a, lvl, T):
     mir = oracle.mode("mirror")
     n_g, img_g = engine.residual_image(a["gref"], a["gcur"], lvl, T)
@@ -59,7 +94,7 @@ def _check_level(engine, oracle, a, lvl, T):
 
 
 def test_window_too_small(engine, oracle, pair):
-    """A rotation about the optical axis tilts every tile row: a 128-pixel row then spans more image rows than the window
+    """A rotation about the optical axis tilts every tile row: a 160-pixel row then spans more image rows than the window
     holds.  A pure rotation maps pixels independently of depth, so the span is exact geometry."""
     fx, fy, ox, oy = pair["K"]
     T = _rot_z(20.0)
@@ -92,8 +127,7 @@ def test_corner_behind_camera(engine, oracle, pair):
 
 
 @pytest.mark.parametrize("lvl", [1, 2])
-def test_partial_band(engine, oracle, pair, lvl):
-    """640 / 2 and 640 / 4 columns are not multiples of the 128-column band: the last band of every strip is partial."""
-    w = pair["I_ref"].shape[1] >> lvl
-    assert w % TILE_W != 0
-    _check_level(engine, oracle, pair, lvl, _rot_z(3.0) @ _shift_z(0.02))
+def test_partial_band(engine, oracle, pair720, lvl):
+    """720 / 2 and 720 / 4 columns are full 160-column bands followed by a partial one in every strip."""
+    assert_partial_band(pair720["oref"].level_info(lvl)[0])
+    _check_level(engine, oracle, pair720, lvl, partial_pose())

@@ -1,10 +1,10 @@
 """The pyramid and the level kernel across image sizes chosen for the tile edges, against the oracle.
 
-The level kernel cuts every level into 128 x 7 tiles; the pyramid pads odd widths to an even pitch and ends the selection
-mask on a partial word when w * h is not a multiple of 32.  Each size below reaches a case the 640 x 480 family never does
-(a 1-, 33- or 63-column band, strips of 5 or 6 rows, odd widths below an even level 0, one band per level, very tall or
-very wide levels, the smallest legal sizes), and each test asserts that case from the geometry first, so that a later
-change of the sizes cannot make it vacuous.  Per size, level and selection: the pyramid bit for bit, the residual records
+The level kernel cuts every level into 160 x 7 tiles (tests/tile_geometry.py); the pyramid pads odd widths to an even pitch
+and ends the selection mask on a partial word when w * h is not a multiple of 32.  Each size below reaches a case the
+640 x 480 family never does (a partial band of 1, 33, 63, 128 or 159 columns, whole bands only, strips of 5 or 6 rows, odd
+widths below an even level 0, one band per level, very tall or very wide levels, the smallest legal sizes), and each test
+asserts that case from the geometry first, so that a later change of the sizes or of the tiles cannot make it vacuous.  Per size, level and selection: the pyramid bit for bit, the residual records
 and the intensity error image bit for bit against MIRROR, P / LL / A / b to 2e-6, the same in the corrected estimator,
 whole alignments, the three input paths, the argument bounds and a pyramid built into a recycled slab.
 """
@@ -15,12 +15,14 @@ import pytest
 
 from helpers import nan_equal, pose_delta
 from test_corrected_estimator import corrected_mode
-from test_gpu_generic_tiles import TILE_H, TILE_W, _rot_z, _shift_z
+from test_gpu_generic_tiles import _rot_z, _shift_z
+from tile_geometry import TILE_H, TILE_W, bands, in_partial_band, level_shapes, strips
 
 pytestmark = pytest.mark.gpu
 
 # (level-0 width, height, levels)
-SIZES = [(129, 50, 3), (161, 55, 3), (191, 49, 3), (256, 96, 3), (250, 188, 4), (40, 300, 3), (700, 9, 3), (32, 8, 3)]
+SIZES = [(161, 50, 3), (193, 55, 3), (223, 49, 3), (288, 62, 3), (319, 41, 3), (320, 96, 3), (250, 188, 4), (40, 300, 3),
+         (700, 9, 3), (32, 8, 3)]
 IDS = [f"{w}x{h}" for w, h, _ in SIZES]
 SELECTIONS = [(0.0, 0.0), (4.0, 0.02)]      # the default thresholds, and one non-default (intensity, depth) pair
 PP = np.array([[2000.0, -30.0], [-30.0, 9000.0]], dtype=np.float32)
@@ -33,37 +35,28 @@ def _intrinsics(w, h):
     return (0.81 * s, 0.81 * s + 0.5, 0.47 * w + 0.3, 0.52 * h - 0.2)
 
 
-def _level_sizes(w, h, levels):
-    out = [(w, h)]
-    for _ in range(1, levels):
-        w, h = w // 2, h // 2
-        out.append((w, h))
-    return out
-
-
-def _bands(w):
-    """widths of the 128-column bands of a level, left to right"""
-    return [min(TILE_W, w - x0) for x0 in range(0, w, TILE_W)]
-
-
 def _assert_reason(w, h, levels):
     """the case each size exists for, from the geometry alone"""
-    ls = _level_sizes(w, h, levels)
+    ls = level_shapes(w, h, levels)
     ws, hs = [s[0] for s in ls], [s[1] for s in ls]
-    if (w, h) == (129, 50):
-        assert _bands(129) == [128, 1] and h % TILE_H == 1 and w % 2 == 1 and (w * h) % 32 != 0 and hs[2] % TILE_H == 5
-    elif (w, h) == (161, 55):
-        assert _bands(161) == [128, 33] and all(v % TILE_H == 6 for v in hs)
-    elif (w, h) == (191, 49):
-        assert _bands(191) == [128, 63] and h % TILE_H == 0 and ws[1] % 2 == 1 and ws[2] % 2 == 1
-    elif (w, h) == (256, 96):
-        assert _bands(ws[0]) == [128, 128] and _bands(ws[1]) == [128] and h % TILE_H == 5
+    if (w, h) == (161, 50):        # a 1-column band; an odd width and a mask tail at level 0; a last strip of 1 and of 5 rows
+        assert bands(w) == [160, 1] and h % TILE_H == 1 and w % 2 == 1 and (w * h) % 32 != 0 and hs[2] % TILE_H == 5
+    elif (w, h) == (193, 55):      # a 33-column band: one round and one pixel; a last strip of 6 rows at every level
+        assert bands(w) == [160, 33] and all(v % TILE_H == 6 for v in hs)
+    elif (w, h) == (223, 49):      # a 63-column band: two rounds less one pixel; whole strips; odd widths below an even level 0
+        assert bands(w) == [160, 63] and h % TILE_H == 0 and ws[0] % 2 == 1 and ws[1] % 2 == 1 and ws[2] % 2 == 1
+    elif (w, h) == (288, 62):      # a partial band of whole rounds: the generic loop with no pixel masked off in its last round
+        assert bands(w) == [160, 128] and bands(w)[-1] % 32 == 0 and h % TILE_H == 6
+    elif (w, h) == (319, 41):      # a band one column short of full, then a level of one such band
+        assert bands(w) == [160, 159] and bands(ws[1]) == [159] and h % TILE_H == 6
+    elif (w, h) == (320, 96):      # whole bands only at levels 0 and 1, with a last strip of 5 rows
+        assert bands(ws[0]) == [160, 160] and bands(ws[1]) == [160] and h % TILE_H == 5 and len(strips(h)) == 14
     elif (w, h) == (250, 188):
         assert ws == [250, 125, 62, 31] and [v % 2 for v in ws] == [0, 1, 0, 1]
     elif (w, h) == (40, 300):
-        assert all(len(_bands(v)) == 1 and v < TILE_W for v in ws) and -(-h // TILE_H) == 43
+        assert all(len(bands(v)) == 1 and v < TILE_W for v in ws) and len(strips(h)) == 43
     elif (w, h) == (700, 9):
-        assert len(_bands(w)) == 6 and _bands(w)[-1] < TILE_W and -(-h // TILE_H) == 2 and hs[-1] == 2
+        assert len(bands(w)) == 5 and bands(w)[-1] < TILE_W and len(strips(h)) == 2 and hs[-1] == 2
     elif (w, h) == (32, 8):
         assert ls == [(32, 8), (16, 4), (8, 2)]
     else:
@@ -239,8 +232,8 @@ def test_pyramid(gpu_pyramids, w, h, levels):
 
 
 def test_some_level_has_a_mask_tail_and_an_odd_pitch():
-    tails = [(w, h, l) for w, h, n in SIZES for l, (lw, lh) in enumerate(_level_sizes(w, h, n)) if (lw * lh) % 32]
-    odd = [(w, h, l) for w, h, n in SIZES for l, (lw, _) in enumerate(_level_sizes(w, h, n)) if lw % 2]
+    tails = [(w, h, l) for w, h, n in SIZES for l, (lw, lh) in enumerate(level_shapes(w, h, n)) if (lw * lh) % 32]
+    odd = [(w, h, l) for w, h, n in SIZES for l, (lw, _) in enumerate(level_shapes(w, h, n)) if lw % 2]
     assert any(l == 0 for _, _, l in tails) and len(tails) >= 8 and len(odd) >= 8, (tails, odd)
 
 
@@ -278,9 +271,8 @@ def test_an_odd_selection_ends_in_a_partial_band_or_the_last_strip(oracle):
                     continue
                 last = int(np.flatnonzero(mask.reshape(-1))[-1])
                 y, x = divmod(last, lw)
-                in_partial_band = x >= (lw // TILE_W) * TILE_W
                 in_last_strip = y >= ((lh - 1) // TILE_H) * TILE_H
-                if in_partial_band or in_last_strip:
+                if in_partial_band(x, lw) or in_last_strip:
                     hits.append((w, h, lvl, sel, S, x, y))
     assert hits
     print("odd selections ending in a partial band or the last strip:", hits)
@@ -361,13 +353,13 @@ def test_argument_bounds_are_status_codes(engine):
         Z = rng.uniform(0.5, 3.0, (h, w)).astype(np.float32)
         return engine.pyramid(I, Z, _intrinsics(w, h), levels)
 
-    assert [s[0] for s in _level_sizes(40, 300, 4)][-1] < 8 and [s[1] for s in _level_sizes(700, 9, 4)][-1] < 2
+    assert [s[0] for s in level_shapes(40, 300, 4)][-1] < 8 and [s[1] for s in level_shapes(700, 9, 4)][-1] < 2
     for w, h, levels in ((31, 8, 1), (32, 1, 1), (40, 300, 4), (700, 9, 4), (32, 8, 4)):
         with pytest.raises(RuntimeError):
             build(w, h, levels)
     for w, h, levels in ((40, 300, 3), (700, 9, 3), (32, 8, 3), (32, 2, 1)):     # the largest legal level counts
         p = build(w, h, levels)
-        assert p.num_levels == levels and p.level_info(levels - 1)[:2] == _level_sizes(w, h, levels)[-1]
+        assert p.num_levels == levels and p.level_info(levels - 1)[:2] == level_shapes(w, h, levels)[-1]
         p.release()
 
 
@@ -415,14 +407,14 @@ def _identical(a, b):
             assert x == y, k
 
 
-@pytest.mark.parametrize("w,h,levels", [(129, 50, 3), (40, 300, 3)], ids=["129x50", "40x300"])
+@pytest.mark.parametrize("w,h,levels", [(161, 50, 3), (40, 300, 3)], ids=["161x50", "40x300"])
 def test_recycled_slab(oracle, w, h, levels):
     """Pyramid memory comes from a per-context pool keyed by byte size and is never cleared.  A pyramid built into a slab
     that held garbage of the same size must compute exactly what the same pyramid on a fresh context computes."""
     from dvo_slam_b200.engine import Engine
     _assert_reason(w, h, levels)
-    ls = _level_sizes(w, h, levels)
-    assert any(lw % 2 for lw, _ in ls) or all(len(_bands(lw)) == 1 and lw < TILE_W for lw, _ in ls)
+    ls = level_shapes(w, h, levels)
+    assert any(lw % 2 for lw, _ in ls) or all(len(bands(lw)) == 1 and lw < TILE_W for lw, _ in ls)
     tails = [l for l, (lw, lh) in enumerate(ls) if (lw * lh) % 32]
     assert tails
     a = _scene(w, h)

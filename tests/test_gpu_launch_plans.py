@@ -33,7 +33,7 @@ def special_positions(n, p):
 
 GEOM_640 = level_geometry(640, 480, 5)
 GEOM_1280 = level_geometry(1280, 960, 6)
-SIZES_264 = [1, 2, 65, 66, 67, 88, 89, 132, 133, 264, 265, 294, 295, 475, 476, 512]
+SIZES_264 = [1, 2, 65, 66, 67, 88, 89, 132, 133, 264, 265, 294, 295, 370, 371, 382, 383, 441, 442, 512]
 
 
 def test_restated_plan_at_264_ctas():
@@ -49,8 +49,11 @@ def test_restated_plan_at_264_ctas():
             continue
         assert p["walk"] and p["fused"] and p["launches"] == 1, n
         assert [(G["first_li"], G["nlev"], G["g"]) for G in p["groups"]][0] == (0, 4, 1), n   # levels 4..1, one CTA per pair
+        # from 371 pairs on, the fine level takes squads of 2: one slice until the first keeps two pairs per squad beside
+        # the second (383), two until it does so beside the third as well (442)
         want = ((4,) if n == 66 else (3,) if n <= 88 else (2,) if n <= 132 else (1,) if n <= 264 else (3, 6) if n <= 294
-                else (3, 6, 12) if n <= 475 else (2, 4, 8))
+                else (3, 6, 12) if n <= 370 else (2,) if n <= 382 else (2, 4) if n <= 441 else (2, 4, 8) if n <= 879
+                else (1, 2) if n <= 884 else (1, 2, 4))
         assert tuple(s[0] for s in p["slices"]) == want, (n, p["slices"])
         if n in (265, 294):
             assert [s[2] for s in p["slices"]] == [n - 79, 79]
@@ -58,12 +61,17 @@ def test_restated_plan_at_264_ctas():
     assert all(a >= b for a, b in zip(g0, g0[1:]))
     assert plan(GEOM_640, 4, 0, grid, 265)["slices"] == [(3, 0, 186), (6, 186, 79)]
     assert plan(GEOM_640, 4, 0, grid, 512)["slices"] == [(2, 0, 334), (4, 334, 119), (8, 453, 59)]   # DESIGN 4.1
+    assert plan(GEOM_640, 4, 0, grid, 371)["slices"] == [(2, 0, 371)]
+    assert plan(GEOM_640, 4, 0, grid, 383)["slices"] == [(2, 0, 264), (4, 264, 119)]
+    assert plan(GEOM_640, 4, 0, grid, 442)["slices"] == [(2, 0, 264), (4, 264, 119), (8, 383, 59)]
     assert boundary_sizes(GEOM_640, 4, 0, grid) == SIZES_264
-    # 1280x960, levels 5..0: a fine group of two levels (1 and 0) behind the coarse walk; three slices of 6 / 12 / 24 at 148..175
-    for n in range(148, 176):
+    # 1280x960, levels 5..0: a fine group of two levels (1 and 0) behind the coarse walk; three slices of 6 / 12 / 24 at 148..167
+    for n in range(148, 168):
         p = plan(GEOM_1280, 5, 0, grid, n)
         assert p["fused"] and p["groups"][1]["nlev"] == 2 and [s[0] for s in p["slices"]] == [6, 12, 24], n
+    assert [s[0] for s in plan(GEOM_1280, 5, 0, grid, 168)["slices"]] == [1]
     assert size_of_shape(GEOM_1280, 5, 0, grid, ("fused", 6, 12, 24), pick="first") == 148
+    assert size_of_shape(GEOM_1280, 5, 0, grid, ("fused", 6, 12, 24), pick="last") == 167
     # levels 3..1: a coarse-only walk (one launch instead of three); level 0 alone: a walk without fusion
     for n in (66, 100, 512):
         p = plan(GEOM_640, 3, 1, grid, n)
@@ -304,7 +312,7 @@ def test_grid_is_two_ctas_per_sm(ctx):
 def test_every_plan_shape_equals_single_alignments(ctx, k, est):
     """640x480, levels 4..0: the first and last batch size of every plan shape (the sizes in the id are those of 132 SMs)"""
     sizes = boundary_sizes(ctx.p640.geom, 4, 0, ctx.grid)
-    assert len(sizes) == len(SIZES_264), f"grid {ctx.grid}: plan shapes give the sizes {sizes}, this file expects 16"
+    assert len(sizes) == len(SIZES_264), f"grid {ctx.grid}: plan shapes give the sizes {sizes}, this file expects {len(SIZES_264)}"
     if ctx.grid == 264:
         assert sizes == SIZES_264
     ctx.run(est, "4..0", ctx.p640, sizes[k], 4, 0, what="640x480 4..0")
@@ -374,8 +382,8 @@ def test_match_batch_device_three_slices(ctx):
     import torch
     from dvo_slam_b200.engine import CResult
     pool = ctx.p640
-    want_shape = shape(plan(pool.geom, 4, 0, ctx.grid, 400))
-    assert len(want_shape) == 4, f"no three-slice plan at 400 pairs on grid {ctx.grid}: {want_shape}"
+    want_shape = shape(plan(pool.geom, 4, 0, ctx.grid, 512))
+    assert len(want_shape) == 4, f"no three-slice plan at 512 pairs on grid {ctx.grid}: {want_shape}"
     n = size_of_shape(pool.geom, 4, 0, ctx.grid, want_shape)
     p = plan(pool.geom, 4, 0, ctx.grid, n)
     slots = pool.compose(n, special_positions(n, p))

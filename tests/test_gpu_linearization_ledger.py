@@ -14,8 +14,9 @@ import numpy as np
 import pytest
 
 import linearization_ledger as L
-from test_gpu_generic_tiles import _rot_z, _shift_z
-from test_gpu_geometry import SIZES, _level_sizes, _scene, _small_motion
+from test_gpu_generic_tiles import _rot_z, _shift_z, partial_pair, partial_pose
+from test_gpu_geometry import SIZES, _scene, _small_motion
+from tile_geometry import assert_partial_band, level_shapes
 
 pytestmark = pytest.mark.gpu
 
@@ -96,13 +97,13 @@ def test_640x480(engines, maxima, bench640, level, estimator):
 @pytest.mark.parametrize("estimator", ["reference", "corrected"])
 @pytest.mark.parametrize("level", [0, 5])
 def test_1280x960(engine, engines, maxima, level, estimator):
-    """bench.py --config 5: level 0 has 10 bands, the longest lane chains"""
+    """bench.py --config 5: level 0 has 8 bands and 40 rounds of 32 pixels per row, the longest lane chains"""
     from dvo_slam_b200 import synth
     p = synth.make_pair(41, synth.SceneConfig().scaled(2))
     K = p["intrinsics"]
     gref = engine.pyramid(p["I_ref"].numpy(), p["Z_ref"].numpy(), K, 6)
     gcur = engine.pyramid(p["I_cur"].numpy(), p["Z_cur"].numpy(), K, 6)
-    assert L.nbands(gref.level_info(0)[0]) == 10
+    assert L.nbands(gref.level_info(0)[0]) == 8 and L.rounds(gref.level_info(0)[0]) == 40
     for T in (p["T_true"], synth.se3_exp(p["xi"] * 0.9)):
         _check(engines, maxima, "1280x960", estimator, gref, gcur, level, T, K)
 
@@ -113,15 +114,15 @@ def test_tile_edge_sizes(engine, engines, maxima, w, h, levels, estimator):
     a = _scene(w, h)
     gref = engine.pyramid(a["I_ref"], a["Z_ref"], a["K"], levels)
     gcur = engine.pyramid(a["I_cur"], a["Z_cur"], a["K"], levels)
-    for lvl in range(len(_level_sizes(w, h, levels))):
+    for lvl in range(len(level_shapes(w, h, levels))):
         _check(engines, maxima, "sizes", estimator, gref, gcur, lvl, _small_motion(), a["K"])
 
 
 # ---- tile paths, masks, selection ------------------------------------------------------------------------------------------
 GENERIC = {"roll20": (0, lambda a: _rot_z(20.0)),
            "corner_behind": (0, lambda a: _shift_z(-float(np.nanmedian(a["Z_ref"])))),
-           "partial_band_l1": (1, lambda a: _rot_z(3.0) @ _shift_z(0.02)),
-           "partial_band_l2": (2, lambda a: _rot_z(3.0) @ _shift_z(0.02))}
+           "partial_band_l1": (1, lambda a: partial_pose()),        # on the 720 x 540 scene of test_gpu_generic_tiles
+           "partial_band_l2": (2, lambda a: partial_pose())}
 
 
 @pytest.fixture(scope="module")
@@ -136,11 +137,23 @@ def pair0(engine):
     return a
 
 
+@pytest.fixture(scope="module")
+def pair720(engine):
+    """the partial-band scene of test_gpu_generic_tiles"""
+    a = partial_pair(0)
+    a["gref"] = engine.pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
+    a["gcur"] = engine.pyramid(a["I_cur"], a["Z_cur"], a["K"], 5)
+    return a
+
+
 @pytest.mark.parametrize("estimator", ["reference", "corrected"])
 @pytest.mark.parametrize("case", list(GENERIC))
-def test_generic_tile_paths(engines, maxima, pair0, case, estimator):
+def test_generic_tile_paths(engines, maxima, pair0, pair720, case, estimator):
     level, pose = GENERIC[case]
-    _check(engines, maxima, "generic", estimator, pair0["gref"], pair0["gcur"], level, pose(pair0), pair0["K"])
+    a = pair720 if case.startswith("partial_band") else pair0
+    if a is pair720:
+        assert_partial_band(a["gref"].level_info(level)[0])
+    _check(engines, maxima, "generic", estimator, a["gref"], a["gcur"], level, pose(a), a["K"])
 
 
 @pytest.fixture(scope="module")

@@ -19,6 +19,7 @@ from masked_oracle import masked_pyramid, usable_by_footprint
 from test_corrected_estimator import corrected_mode
 from test_mask_roles_accuracy import CFG as OVERLAY_CFG
 from test_mask_roles_accuracy import SEEDS as OVERLAY_SEEDS
+from tile_geometry import TILE_W, assert_partial_band
 
 pytestmark = pytest.mark.gpu
 
@@ -141,9 +142,11 @@ def pair0(engine, oracle):
 def test_forced_tile_paths(engine, corrected, oracle, pair0, case):
     """clean_exact: a mask in one corner, a small motion -- most tiles have an exact window that misses it, a few (near the
     corner) a dirty one; dirty_exact: many small blobs, every exact window touches one; inexact: a 20 degree roll (no
-    128-pixel tile row fits the window); no_window: the camera moved past the median depth (tile corners behind it);
-    partial_band: levels 1 and 2 (640 / 2 and 640 / 4 columns are not multiples of 128)."""
-    a = pair0
+    160-pixel tile row fits the window); no_window: the camera moved past the median depth (tile corners behind it);
+    partial_band: levels 1 and 2 of the 720 x 540 scene of test_gpu_generic_tiles (full 160-column bands and a partial one),
+    with the mask inside the partial band."""
+    from test_gpu_generic_tiles import partial_pair, partial_pose
+    a = partial_pair(0) if case == "partial_band" else pair0
     h, w = a["I_ref"].shape
     if case == "clean_exact":
         m, T, lvls = _blob_at(h, w, 40, 40, 25), _rot_z(0.5) @ _shift_z(0.01), [0]
@@ -156,7 +159,11 @@ def test_forced_tile_paths(engine, corrected, oracle, pair0, case):
     elif case == "no_window":
         m, T, lvls = _blob_at(h, w, 320, 240, 60), _shift_z(-float(np.nanmedian(a["Z_ref"]))), [0]
     else:
-        m, T, lvls = _blob_at(h, w, 600, 240, 50), _rot_z(3.0) @ _shift_z(0.02), [1, 2]
+        m, T, lvls = _blob_at(h, w, 680, 270, 30), partial_pose(), [1, 2]
+        for lvl in lvls:
+            assert_partial_band(w >> lvl)
+            x0 = ((w >> lvl) // TILE_W * TILE_W) << lvl         # the level-0 column where the level's partial band starts
+            assert (m[:, x0:] == 0).any() and (m[:, :x0] != 0).all()
     gref, oref = _pyrs(engine, oracle, a["I_ref"], a["Z_ref"], a["K"], None, "both", 5)
     gcur, ocur = _pyrs(engine, oracle, a["I_cur"], a["Z_cur"], a["K"], m, "both", 5)
     for lvl in lvls:

@@ -13,7 +13,8 @@ import numpy as np
 import pytest
 
 from helpers import nan_equal, pose_delta
-from test_gpu_generic_tiles import TILE_H, TILE_W, _rot_z, _shift_z
+from test_gpu_generic_tiles import _rot_z, _shift_z
+from tile_geometry import TILE_H, TILE_W
 
 pytestmark = pytest.mark.gpu
 

@@ -205,9 +205,12 @@ def _check_records_both_estimators(engine, oracle, gref, gcur, pref, pcur, lvl, 
 def test_records_on_the_generic_loops(engine, oracle, pair0, case):
     """The cases of test_gpu_generic_tiles.py / test_gpu_mask_roles.py at (alpha, beta) != (1, 0): inexact = a 20 degree roll
     (no tile row fits the window), no_window = the camera past the median depth (tile corners behind it), partial_band =
-    levels 1 and 2, cur_mask_* = a mask in the current role (the per-tap test of the masked stage-B loop), on exact-window
-    tiles that touch it and on inexact ones."""
-    a = pair0
+    levels 1 and 2 of the 720 x 540 scene of test_gpu_generic_tiles (full 160-column bands and a partial one), cur_mask_* =
+    a mask in the current role (the per-tap test of the masked stage-B loop), on exact-window tiles that touch it and on
+    inexact ones."""
+    from test_gpu_generic_tiles import partial_pair, partial_pose
+    from tile_geometry import assert_partial_band
+    a = partial_pair(0) if case == "partial_band" else pair0
     h, w = a["I_ref"].shape
     m, lvls = None, [0]
     if case == "inexact":
@@ -215,7 +218,9 @@ def test_records_on_the_generic_loops(engine, oracle, pair0, case):
     elif case == "no_window":
         T = _shift_z(-float(np.nanmedian(a["Z_ref"])))
     elif case == "partial_band":
-        T, lvls = _rot_z(3.0) @ _shift_z(0.02), [1, 2]
+        T, lvls = partial_pose(), [1, 2]
+        for lvl in lvls:
+            assert_partial_band(w >> lvl)
     elif case == "cur_mask_dirty":
         m = np.ones((h, w), np.uint8)
         m[4::32, 4::32] = 0

@@ -12,6 +12,8 @@ from dvo_slam_b200.engine import CResult, Config
 
 pytestmark = pytest.mark.gpu
 SCENE = synth.SceneConfig(width=320, height=240, intrinsics=tuple(v / 2 for v in synth.FR1_INTRINSICS))
+# levels 0 and 1 of 400 x 300 have full 160-column bands and a partial one (160, 160, 80 and 160, 40 columns)
+SCENE400 = synth.SceneConfig(width=400, height=300, intrinsics=tuple(v * 400 / 640 for v in synth.FR1_INTRINSICS))
 MUS = (0.05, 1.0, 25.0)
 DELTA = np.array([4e-3, -3e-3, 2e-3, -2e-3, 3e-3, 1e-3])
 PLANS = ((None, None), ("DVO_B200_FINE_G", "2"), ("DVO_B200_FINE_G", "4"), ("DVO_B200_TAIL", "6,6"), ("DVO_B200_COARSE_TILES", "0"),
@@ -24,23 +26,36 @@ def _cfg(mu=0.0):
     return Config(first_level=2, last_level=0, max_iterations_per_level=50, precision=1e-4, mu=mu, use_initial_estimate=1)
 
 
-def _mask(k):
-    m = np.ones((240, 320), np.uint8)
+def _mask(k, h=240, w=320):
+    m = np.ones((h, w), np.uint8)
     m[40 + 10 * k:110 + 10 * k, 60:150] = 0
     return m
+
+
+def _batch(engine, scene, seed0):
+    out = []
+    for k in range(6):
+        p = synth.make_pair(seed0 + k, scene)
+        kw = {"mask": _mask(k, scene.height, scene.width), "mask_roles": "both"} if k in (1, 4) else {}
+        out.append({"ref": engine.pyramid(p["I_ref"].numpy(), p["Z_ref"].numpy(), scene.intrinsics, 3, **kw),
+                    "cur": engine.pyramid(p["I_cur"].numpy(), p["Z_cur"].numpy(), scene.intrinsics, 3, **kw),
+                    "T0": synth.se3_exp(DELTA * (1 + 0.3 * k)) @ p["T_true"], "pair": p})
+    return out
 
 
 @pytest.fixture(scope="module")
 def batch(engine):
     """six pairs with their initial estimates; pairs 1 and 4 have a mask in both roles (the kCurMask instances)"""
-    out = []
-    for k in range(6):
-        p = synth.make_pair(60 + k, SCENE)
-        kw = {"mask": _mask(k), "mask_roles": "both"} if k in (1, 4) else {}
-        out.append({"ref": engine.pyramid(p["I_ref"].numpy(), p["Z_ref"].numpy(), SCENE.intrinsics, 3, **kw),
-                    "cur": engine.pyramid(p["I_cur"].numpy(), p["Z_cur"].numpy(), SCENE.intrinsics, 3, **kw),
-                    "T0": synth.se3_exp(DELTA * (1 + 0.3 * k)) @ p["T_true"], "pair": p})
-    return out
+    return _batch(engine, SCENE, 60)
+
+
+@pytest.fixture(scope="module")
+def batch400(engine):
+    """the same at 400 x 300: the prior instances' generic loop in partial bands, which no hook reaches"""
+    from tile_geometry import assert_partial_band
+    assert_partial_band(SCENE400.width)
+    assert_partial_band(SCENE400.width // 2)
+    return _batch(engine, SCENE400, 160)
 
 
 def _spd(rng, scale):
@@ -82,7 +97,12 @@ def _same(r0, r1, ll_tol=None):
 
 @pytest.mark.parametrize("photometric", [False, True])
 @pytest.mark.parametrize("estimator", ["reference", "corrected"])
-def test_scalar_prior_equals_the_mu_path_under_every_plan(engine, batch, estimator, photometric, monkeypatch):
+def test_scalar_prior_equals_the_mu_path_under_every_plan(engine, batch, batch400, estimator, photometric, monkeypatch):
+    for b in (batch, batch400):
+        _scalar_prior_equals_the_mu_path_under_every_plan(engine, b, estimator, photometric, monkeypatch)
+
+
+def _scalar_prior_equals_the_mu_path_under_every_plan(engine, batch, estimator, photometric, monkeypatch):
     refs, curs, T0 = [q["ref"] for q in batch], [q["cur"] for q in batch], [q["T0"] for q in batch]
     n = len(refs)
     mus = [MUS[i % 3] for i in range(n)]

@@ -16,7 +16,8 @@ import pytest
 from helpers import (GOLDEN_LEVELS, GOLDEN_SEEDS, POSE_TOL_R, POSE_TOL_T, golden_images, load_golden, nan_equal,
                      odd_point_margin, pose_delta)
 from test_corrected_estimator import corrected_mode
-from test_gpu_generic_tiles import WIN_ROWS, _rot_z, _shift_z
+from test_gpu_generic_tiles import _rot_z, _shift_z, partial_pair
+from tile_geometry import WIN_ROWS, assert_partial_band, in_partial_band
 
 pytestmark = pytest.mark.gpu
 
@@ -70,6 +71,12 @@ def full(engine, oracle):
 
 
 @pytest.fixture(scope="module")
+def wide(engine, oracle):
+    """the 720 x 540 scene of test_gpu_generic_tiles: every level to 2 has full bands and a partial one"""
+    return _planes(partial_pair(0), oracle, 5, engine)
+
+
+@pytest.fixture(scope="module")
 def odd_size(engine, oracle):
     from dvo_slam_b200 import synth
     scfg = synth.SceneConfig(width=203, height=155, intrinsics=(164.0, 163.5, 101.3, 77.2))
@@ -116,14 +123,18 @@ def _check(eng, m, oracle, c, lvl, T, ti, td):
     return n_o, S
 
 
-def _odd_thresholds(oracle, c, lvl, T):
+def _odd_thresholds(oracle, c, lvl, T, partial_band=False):
     """the first thresholds (1.0, 0.02), (1.25, 0.02), ... that select an odd number S of points at this level whose last
-    point has a valid residual by itself (EXACT mode keeps the odd point): the point the reference's SSE loop never visits"""
+    point has a valid residual by itself (EXACT mode keeps the odd point): the point the reference's SSE loop never visits;
+    partial_band: and that point lies in the level's partial band"""
+    lw = c["oref"].level_info(lvl)[0]
     for ti in np.arange(1.0, 40.0, 0.25):
         S, mask = oracle.select(c["oref"], lvl, float(ti), 0.02)
         if S % 2 == 0 or S < 50:
             continue
         last = np.flatnonzero(mask.reshape(-1))[-1]
+        if partial_band and not in_partial_band(int(last) % lw, lw):
+            continue
         _, exact = oracle.residual_image(c["oref"], c["ocur"], lvl, T, oracle.mode("exact"), float(ti), 0.02)
         if not np.isnan(exact[0].reshape(-1)[last]):
             return float(ti), 0.02, last
@@ -152,20 +163,24 @@ def test_thresholds_change_what_is_selected(oracle, full):
 
 
 @pytest.mark.parametrize("estimator", ["reference", "corrected"])
-def test_odd_selection_with_a_valid_last_point(engine, corrected, oracle, full, estimator):
-    """An odd selection count S whose last point is valid: reference mode drops it (as MIRROR does), corrected mode keeps it."""
+def test_odd_selection_with_a_valid_last_point(engine, corrected, oracle, wide, estimator):
+    """An odd selection count S whose last point is valid: reference mode drops it (as MIRROR does), corrected mode keeps it.
+    Level 1 of the 720 x 540 scene (bands of 160, 160 and 40 columns), with the last point in the partial band: the
+    corrected kernel re-admits it in the generic loop of a partial-band tile."""
     eng, m = _engines(engine, corrected, oracle)[estimator]
     T = _pose()
-    ti, td, last = _odd_thresholds(oracle, full, 1, T)      # level 1: 320x240, partial bands
-    n, S = _check(eng, m, oracle, full, 1, T, ti, td)
-    assert S % 2 == 1 and S < oracle.select(full["oref"], 1)[0]
-    _, img = eng.residual_image(full["gref"], full["gcur"], 1, T, _cfg(ti, td))
+    c = wide
+    assert_partial_band(c["oref"].level_info(1)[0])
+    ti, td, last = _odd_thresholds(oracle, c, 1, T, partial_band=True)
+    n, S = _check(eng, m, oracle, c, 1, T, ti, td)
+    assert S % 2 == 1 and S < oracle.select(c["oref"], 1)[0]
+    _, img = eng.residual_image(c["gref"], c["gcur"], 1, T, _cfg(ti, td))
     assert np.isnan(img[0].reshape(-1)[last]) == (estimator == "reference")
     if estimator == "corrected":
-        n_r, _ = engine.residual_image(full["gref"], full["gcur"], 1, T, _cfg(ti, td))
+        n_r, _ = engine.residual_image(c["gref"], c["gcur"], 1, T, _cfg(ti, td))
         assert n == n_r + 1
-        ne, err = eng.intensity_error_image(full["gref"], full["gcur"], 1, T, _cfg(ti, td))
-        ne_o, err_o = oracle.intensity_error_image(full["oref"], full["ocur"], 1, T, m, ti, td)
+        ne, err = eng.intensity_error_image(c["gref"], c["gcur"], 1, T, _cfg(ti, td))
+        ne_o, err_o = oracle.intensity_error_image(c["oref"], c["ocur"], 1, T, m, ti, td)
         assert ne == ne_o == n and np.array_equal(err, err_o) and err.reshape(-1)[last] > 0
 
 
@@ -195,7 +210,7 @@ def test_generic_loop_with_thresholds(engine, corrected, oracle, full, estimator
     """thresholds together with the poses that force the generic pixel loop (test_gpu_generic_tiles.py): a 20 degree roll
     (tile rows span more rows than the window holds) and a camera moved past the median depth (corners behind it)"""
     eng, m = _engines(engine, corrected, oracle)[estimator]
-    assert WIN_ROWS < 640 * np.tan(np.deg2rad(20.0))
+    assert WIN_ROWS < 160 * np.tan(np.deg2rad(20.0))          # a tile row spans more rows than the window holds
     dz = float(np.nanmedian(full["Z_ref"]))
     for T in (_rot_z(20.0), _shift_z(-dz)):
         n, _ = _check(eng, m, oracle, full, 0, T, *THRESHOLDS["moderate"])

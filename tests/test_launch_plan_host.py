@@ -36,6 +36,7 @@ def test_launch_plan_equals_the_restatement(tmp_path):
                         "-o", exe, os.path.join(ROOT, "tests", "native", "launch_plan.cpp")],
                        capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr[-2000:]
+    assert [nb for _, nb, _ in level_geometry(640, 480, 5)] == [4, 2, 1, 1, 1]      # the kernel's 160-column bands
     cases = _cases()
     lines = []
     for geom, first, last, grid, n, env in cases:

@@ -133,7 +133,7 @@ def test_ledger_holds_photometric_mirror(oracle, photometric_scene, estimator, a
 # ---- the kernel's summation order in fp32 ------------------------------------------------------------------------------
 @pytest.mark.parametrize("width", [320, 640])
 def test_fp32_row_order_stays_inside_the_bound(oracle, scenes, width):
-    """MIRROR's per-point terms, split as the kernel splits them and summed in fp32 lane chains of 4 nbands pixels (two
+    """MIRROR's per-point terms, split as the kernel splits them and summed in fp32 lane chains of ceil(w/32) pixels (two
     rank-1 updates each), the halving exchange and fp64 rows, against the ledger: inside the bound, and not exact"""
     a = scenes[width]
     rec, out = _mirror(oracle, a, 0, a["T_true"], "reference", 1)
@@ -256,3 +256,13 @@ def test_mutation_odd_point_counted_in_reference_mode(oracle):
     assert bad["n"] == out["n"] + 1
     rep = L.compare(led, bad)
     assert {"n", "A"} <= rep.failed, rep.failures
+
+
+def test_lane_chains_follow_the_rounds_of_32():
+    """A lane adds one pixel per round of 32 columns: 5 per full 160-column band, ceil(bw / 32) in a partial band of bw.  k
+    is the same at 640 and 1280 columns as when bands were 128 wide (DESIGN 5), and shorter where a partial band is narrow."""
+    assert [L.rounds(w) for w in (640, 1280, 400, 161, 288, 319, 32)] == [20, 40, 13, 6, 9, 10, 1]
+    assert [L.k_counts(w, "reference")["A"] for w in (640, 1280)] == [79, 119]
+    assert [L.k_counts(w, "reference")["b"] for w in (640, 1280)] == [68, 108]
+    assert L.k_counts(161, "reference") == {"A": 51, "b": 40, "ll": 13, "scale": 20}
+    assert L.k_counts(161, "corrected")["scale"] == 12
