@@ -748,6 +748,29 @@ int dvo_b200_match_batch_prior(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, in
 }
 
 // ---- weight maps ----
+// The largest extents of a batch's references at cfg->last_level and level 0, or false for a batch the match would refuse
+// (the maps are then checked as for n = 0 and the batch checks refuse it)
+static bool maps_extent(const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references, MapsExtent* ext) {
+  *ext = MapsExtent{0, 0, 0, 0};
+  if (!(cfg && n > 0 && references && cfg->last_level >= 0 && cfg->last_level < kMaxLevels)) return false;
+  for (int32_t i = 0; i < n; ++i) {
+    const dvo_b200_pyramid* r = references[i];
+    if (!r || r->levels <= cfg->last_level) return false;
+    ext->w = std::max(ext->w, r->L[cfg->last_level].w); ext->h = std::max(ext->h, r->L[cfg->last_level].h);
+    ext->w0 = std::max(ext->w0, r->L[0].w); ext->h0 = std::max(ext->h0, r->L[0].h);
+  }
+  return true;
+}
+
+// where one byte of a maps output lies (maps_args.h)
+static PtrWhere pointer_where(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return PtrWhere{kPtrHost, -1}; }
+  if (a.type == cudaMemoryTypeDevice) return PtrWhere{kPtrDevice, a.device};
+  if (a.type == cudaMemoryTypeManaged) return PtrWhere{kPtrManaged, a.device};
+  return PtrWhere{kPtrHost, -1};
+}
+
 int dvo_b200_match_batch_maps(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,
                               dvo_b200_pyramid* const* currents, const double* T_init, const double* prior_information,
                               const double* photometric_init, double* photometric, dvo_b200_result* results,
@@ -763,41 +786,43 @@ int dvo_b200_match_batch_maps(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int
   if (photometric_init && n > 0 && !all_finite(photometric_init, 2 * (size_t)n))
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_maps: photometric_init is not finite");
   cudaSetDevice(ctx->device);
-  // the largest extents of the batch; a batch the match would refuse is left to its checks (n = 0 here)
-  MapsExtent ext{0, 0, 0, 0};
-  bool sane = cfg && n > 0 && references && cfg->last_level >= 0 && cfg->last_level < kMaxLevels;
-  for (int32_t i = 0; sane && i < n; ++i) {
-    const dvo_b200_pyramid* r = references[i];
-    if (!r || r->levels <= cfg->last_level) { sane = false; break; }
-    ext.w = std::max(ext.w, r->L[cfg->last_level].w); ext.h = std::max(ext.h, r->L[cfg->last_level].h);
-    ext.w0 = std::max(ext.w0, r->L[0].w); ext.h0 = std::max(ext.h0, r->L[0].h);
-  }
-  const int device = ctx->device;
-  const std::string why = maps_args_error(maps, sane ? n : 0, ext, device, [](const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return PtrWhere{kPtrHost, -1}; }
-    if (a.type == cudaMemoryTypeDevice) return PtrWhere{kPtrDevice, a.device};
-    if (a.type == cudaMemoryTypeManaged) return PtrWhere{kPtrManaged, a.device};
-    return PtrWhere{kPtrHost, -1};
-  });
+  MapsExtent ext;
+  const bool sane = maps_extent(cfg, n, references, &ext);
+  const std::string why = maps_args_error(maps, sane ? n : 0, ext, ctx->device, pointer_where);
   if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
   return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
                              iteration_stats ? max_iteration_stats : 0, photometric_init, photometric, prior_information, maps);
 }
 
 // ---- multi-hypothesis alignment ----
+int dvo_b200_match_batch_hypotheses_modes(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,
+                                          dvo_b200_pyramid* const* currents, int32_t k, const double* hypotheses, int32_t screen_level,
+                                          double min_constraint_ratio, const double* prior_information, const double* photometric_init,
+                                          double* photometric, double* screen_photometric, dvo_b200_result* results, int32_t* best,
+                                          double* scores, dvo_b200_result* screen_results, dvo_b200_iteration_stats* iteration_stats,
+                                          int32_t max_iteration_stats, const dvo_b200_weight_maps* maps) {
+  if (!ctx) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_hypotheses: null argument");
+  MapsExtent ext;
+  const bool sane = maps && maps_extent(cfg, n, references, &ext);
+  const std::string why = hypotheses_modes_args_error(cfg, n, k, hypotheses, screen_level, min_constraint_ratio, results, best,
+                                                      prior_information, photometric_init, photometric, screen_photometric, maps,
+                                                      sane ? &ext : nullptr, ctx->device, pointer_where);
+  if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
+  cudaSetDevice(ctx->device);
+  return tracker_match_batch_hypotheses(ctx, cfg, n, references, currents, k, hypotheses, screen_level, min_constraint_ratio,
+                                        results, best, scores, screen_results, iteration_stats,
+                                        iteration_stats ? max_iteration_stats : 0, prior_information, photometric_init, photometric,
+                                        screen_photometric, maps);
+}
+
 int dvo_b200_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,
                                     dvo_b200_pyramid* const* currents, int32_t k, const double* hypotheses, int32_t screen_level,
                                     double min_constraint_ratio, dvo_b200_result* results, int32_t* best, double* scores,
                                     dvo_b200_result* screen_results, dvo_b200_iteration_stats* iteration_stats,
                                     int32_t max_iteration_stats) {
-  if (!ctx) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_hypotheses: null argument");
-  const std::string why = hypotheses_args_error(cfg, n, k, hypotheses, screen_level, min_constraint_ratio, results, best);
-  if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
-  cudaSetDevice(ctx->device);
-  return tracker_match_batch_hypotheses(ctx, cfg, n, references, currents, k, hypotheses, screen_level, min_constraint_ratio,
-                                        results, best, scores, screen_results, iteration_stats,
-                                        iteration_stats ? max_iteration_stats : 0);
+  return dvo_b200_match_batch_hypotheses_modes(ctx, cfg, n, references, currents, k, hypotheses, screen_level, min_constraint_ratio,
+                                               nullptr, nullptr, nullptr, nullptr, results, best, scores, screen_results,
+                                               iteration_stats, max_iteration_stats, nullptr);
 }
 
 int dvo_b200_residual_image_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,

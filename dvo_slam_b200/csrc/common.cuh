@@ -293,13 +293,17 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
                         const double* ab_init = nullptr, double* ab_out = nullptr, const double* prior = nullptr,
                         const dvo_b200_weight_maps* maps = nullptr);   // maps != NULL: also the weight maps (weight_maps.cu)
 int check_level_flags(dvo_b200_ctx* ctx);   // after a stream synchronisation: did a level kernel report a timeout?
-// dvo_b200_match_batch_hypotheses after its argument checks (hypotheses_args.h): a leg screening n * k virtual pairs on levels
-// first .. screen_level, k_pick_hypotheses, and a leg continuing the n chosen ones on the levels below.  scores and
-// screen_results (host, n * k) may be NULL.
+// dvo_b200_match_batch_hypotheses[_modes] after its argument checks (hypotheses_args.h): a leg screening n * k virtual pairs on
+// levels first .. screen_level, k_pick_hypotheses, and a leg continuing the n chosen ones on the levels below.  scores and
+// screen_results (host, n * k) may be NULL.  The modes as in tracker_match_batch, per hypothesis: prior (n * k * 36) and
+// ab_init (n * k * 2) per virtual pair, ab_out (n * 2) per pair, screen_ab (n * k * 2, or NULL) where each screening run
+// ended; maps of the continued alignments.
 int tracker_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                                    dvo_b200_pyramid* const* curs, int k, const double* hypotheses, int screen_level,
                                    double min_ratio, dvo_b200_result* h_results, int32_t* h_best, double* h_scores,
-                                   dvo_b200_result* h_screen, dvo_b200_iteration_stats* iter_stats, int max_iter_stats);
+                                   dvo_b200_result* h_screen, dvo_b200_iteration_stats* iter_stats, int max_iter_stats,
+                                   const double* prior = nullptr, const double* ab_init = nullptr, double* ab_out = nullptr,
+                                   double* screen_ab = nullptr, const dvo_b200_weight_maps* maps = nullptr);
 // The test hooks: one iteration at T (staged as the leg's initial estimate and placed into the state by k_set_state).
 int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* ref, dvo_b200_pyramid* cur,
                       int level, const double* T, int use_weights, const float* prev_precision, int64_t* count,
@@ -307,13 +311,13 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
                       const double* ab = nullptr);   // ab != NULL: photometric mode at (alpha, beta); A_out 8 x 8, b_out 8
 
 // weight_maps.cu, the weight maps of a match (maps checked by maps_args.h).  prepare: before the match's first launch, the
-// device scratch of DVO_B200_MAPS_HOST.  launch: k_weight_maps on the batch's final pair states, after the level kernels and
-// k_finalize (level = cfg->last_level; d_pls: the batch's descriptors of that level; d_affine: the photometric mode's
-// brightness states, or NULL); a launch error surfaces at the caller's next cudaGetLastError.  copy_back: with
+// device scratch of DVO_B200_MAPS_HOST.  launch: k_weight_maps on the batch's final pair states d_states, after the level kernels
+// and k_finalize (level = cfg->last_level; d_pls: the batch's descriptors of that level; d_affine: the photometric mode's
+// brightness states, or NULL; all three in the pair slots of the leg the results come from); a launch error surfaces at the caller's next cudaGetLastError.  copy_back: with
 // DVO_B200_MAPS_HOST, the copies into the caller's host layout, before the call's synchronisation.
 int weight_maps_prepare(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int n, const dvo_b200_pyramid* ref0, int level);
 void weight_maps_launch(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int n, const dvo_b200_pyramid* ref0, int level,
-                        const PairLevel* d_pls, const AffineState* d_affine);
+                        const PairState* d_states, const PairLevel* d_pls, const AffineState* d_affine);
 int weight_maps_copy_back(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int n, const dvo_b200_pyramid* ref0, int level);
 
 }  // namespace dvo_b200

@@ -1,7 +1,7 @@
-// hypotheses_args.h -- multi-hypothesis alignment (dvo_b200_match_batch_hypotheses): the checks of its arguments that need no
-// CUDA call, and the rule that picks one screened hypothesis per pair.  Plain C++ that nvcc also compiles for the device, so
-// that both run on the host alone (tests/native/hypotheses_args.cpp); capi.cu runs the checks before anything is staged,
-// uploaded or launched, and k_pick_hypotheses (tracker.cu) runs the rule.
+// hypotheses_args.h -- multi-hypothesis alignment (dvo_b200_match_batch_hypotheses[_modes]): the checks of its arguments that
+// need no CUDA call, and the rule that picks one screened hypothesis per pair.  Plain C++ that nvcc also compiles for the
+// device, so that both run on the host alone (tests/native/hypotheses_args.cpp, tests/native/hypotheses_modes_args.cpp);
+// capi.cu runs the checks before anything is staged, uploaded or launched, and k_pick_hypotheses (tracker.cu) runs the rule.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -9,6 +9,8 @@
 #include <string>
 
 #include "../../include/dvo_b200.h"
+#include "maps_args.h"
+#include "prior_args.h"
 
 #ifndef DVO_HD
 #ifdef __CUDACC__
@@ -74,6 +76,43 @@ inline std::string hypotheses_args_error(const dvo_b200_config* cfg, int32_t n, 
     for (int i = 0; i < 16; ++i)
       if (!finite_fp64(T[i])) return fn + which + " is not finite";
     if (T[12] != 0.0 || T[13] != 0.0 || T[14] != 0.0 || T[15] != 1.0) return fn + which + " has a bottom row other than (0, 0, 0, 1)";
+  }
+  return "";
+}
+
+// The checks of dvo_b200_match_batch_hypotheses_modes, in this order: those of hypotheses_args_error; photometric_init without
+// photometric; screen_photometric without photometric; with a prior, cfg->mu != 0, then each hypothesis's Lambda
+// (prior_matrix_error; skipped with a NULL cfg); each hypothesis's (alpha, beta)_0 not finite; with maps, everything maps_args_error refuses, at the
+// batch's largest extents `extent` (NULL: the batch checks that follow will refuse the batch, so the maps are checked as
+// for n = 0).  A NULL cfg or n <= 0 is left to the batch checks.  Every message is prefixed with "match_batch_hypotheses: ",
+// and the per-hypothesis ones name the hypothesis as hypotheses_args_error does.
+template <typename Where>
+std::string hypotheses_modes_args_error(const dvo_b200_config* cfg, int32_t n, int32_t k, const double* hypotheses, int32_t screen_level,
+                                        double min_constraint_ratio, const void* results, const int32_t* best,
+                                        const double* prior_information, const double* photometric_init, const double* photometric,
+                                        const double* screen_photometric, const dvo_b200_weight_maps* maps, const MapsExtent* extent,
+                                        int device, Where where) {
+  const std::string why = hypotheses_args_error(cfg, n, k, hypotheses, screen_level, min_constraint_ratio, results, best);
+  if (!why.empty()) return why;
+  const std::string fn = "match_batch_hypotheses: ";
+  if (photometric_init && !photometric) return fn + "photometric_init without photometric";
+  if (screen_photometric && !photometric) return fn + "screen_photometric without photometric";
+  auto which = [&](int64_t h) { return "hypothesis " + std::to_string(h % k) + " of pair " + std::to_string(h / k); };
+  if (prior_information && cfg) {
+    if (cfg->mu != 0.0) return fn + "cfg->mu must be 0: the prior replaces mu I";
+    for (int64_t h = 0; h < (int64_t)n * k; ++h) {
+      const std::string bad = prior_matrix_error(prior_information + (size_t)h * 36);
+      if (!bad.empty()) return fn + "prior_information of " + which(h) + " " + bad;
+    }
+  }
+  if (photometric_init)
+    for (int64_t h = 0; h < (int64_t)n * k; ++h)
+      if (!finite_fp64(photometric_init[2 * h]) || !finite_fp64(photometric_init[2 * h + 1]))
+        return fn + "photometric_init of " + which(h) + " is not finite";
+  if (maps) {
+    const std::string bad = maps_args_error(maps, extent ? n : 0, extent ? *extent : MapsExtent{0, 0, 0, 0}, device, where);
+    const std::string maps_fn = "match_batch_maps: ";
+    if (!bad.empty()) return fn + bad.substr(maps_fn.size());
   }
   return "";
 }

@@ -913,10 +913,15 @@ __global__ void k_affine_init(AffineState* s, const double* ab, int n) {
 // Multi-hypothesis alignment, between the screening and the continuation: one warp per pair p.  The scores of its k screened
 // hypotheses (states p k .. p k + k - 1, their statistics of the screening level at level index ls) go to scores[p k + j]
 // (hypothesis_score), the choice to best[p] (pick_hypothesis), and the chosen hypothesis's state and first
-// min(iter_log_count, max_log) iteration-log entries to slot p of the continuation, which picks up from there.
+// min(iter_log_count, max_log) iteration-log entries to slot p of the continuation, which picks up from there.  kAffine: the
+// chosen hypothesis's AffineState follows its state (screened_aff -> chosen_aff); kPrior: its 36 doubles of Lambda
+// (screened_prior -> chosen_prior).  The <false, false> instance ignores those four arguments.
+template <bool kAffine, bool kPrior>
 __global__ void k_pick_hypotheses(const PairState* __restrict__ screened, const dvo_b200_iteration_stats* __restrict__ screened_log,
                                   PairState* __restrict__ chosen, dvo_b200_iteration_stats* __restrict__ chosen_log, int max_log, int n,
-                                  int k, int ls, double min_ratio, double* __restrict__ scores, int* __restrict__ best) {
+                                  int k, int ls, double min_ratio, double* __restrict__ scores, int* __restrict__ best,
+                                  const AffineState* __restrict__ screened_aff, AffineState* __restrict__ chosen_aff,
+                                  const double* __restrict__ screened_prior, double* __restrict__ chosen_prior) {
   const int p = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (p >= n) return;
   double* const sc = scores + (size_t)p * k;
@@ -941,6 +946,16 @@ __global__ void k_pick_hypotheses(const PairState* __restrict__ screened, const 
     const unsigned long long* ls8 = reinterpret_cast<const unsigned long long*>(screened_log + ((size_t)p * k + b) * max_log);
     unsigned long long* ld8 = reinterpret_cast<unsigned long long*>(chosen_log + (size_t)p * max_log);
     for (size_t i = lane; i < words; i += 32) ld8[i] = ls8[i];
+  }
+  if constexpr (kAffine) {
+    static_assert(sizeof(AffineState) % 8 == 0, "copied as 8-byte words");
+    const unsigned long long* a = reinterpret_cast<const unsigned long long*>(screened_aff + (size_t)p * k + b);
+    unsigned long long* ad = reinterpret_cast<unsigned long long*>(chosen_aff + p);
+    for (int i = lane; i < (int)(sizeof(AffineState) / 8); i += 32) ad[i] = a[i];
+  }
+  if constexpr (kPrior) {
+    const double* lam = screened_prior + ((size_t)p * k + b) * 36;
+    for (int i = lane; i < 36; i += 32) chosen_prior[(size_t)p * 36 + i] = lam[i];
   }
 }
 
@@ -1042,7 +1057,8 @@ LaunchPlan plan_launches(const dvo_b200_ctx* ctx, const dvo_b200_pyramid* ref, i
 // (states, iteration logs), descriptors ([level][pair], inside ws.d_pair_level, whose index CurPairLevel::csat shares) and
 // level-flag slots after those of the leg before it.  li0 is the position of its first level in Result.Statistics.Levels: a
 // leg that starts the pairs from T_init has li0 = 0, a later one continues the pairs the leg before it chose.  A leg with
-// first < last runs no level; it only holds the pair slots of a continuation.
+// first < last runs no level; it only holds the pair slots of a continuation, and with maps_desc the descriptors of level
+// `last` of its pairs, which the weight maps read.
 struct Leg {
   int first, last, npairs;
   dvo_b200_pyramid* const* refs;
@@ -1053,8 +1069,8 @@ struct Leg {
 };
 
 Leg make_leg(const dvo_b200_ctx* ctx, const Leg* before, int first, int last, int npairs, dvo_b200_pyramid* const* refs,
-             dvo_b200_pyramid* const* curs, const LevelVariant& v) {
-  Leg g{first, last, npairs, refs, curs, {}, 0, 0, (size_t)npairs * std::max(first - last + 1, 0), 0, 0};
+             dvo_b200_pyramid* const* curs, const LevelVariant& v, bool maps_desc = false) {
+  Leg g{first, last, npairs, refs, curs, {}, 0, 0, (size_t)npairs * std::max(first - last + 1, maps_desc ? 1 : 0), 0, 0};
   if (first >= last) g.plan = plan_launches(ctx, refs[0], first, last, npairs, v);
   if (before) {
     g.pair0 = before->pair0 + before->npairs; g.desc0 = before->desc0 + before->ndesc;
@@ -1202,8 +1218,8 @@ int launch_segments(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, const Leg& g,
   pa.dump = dump;
   pa.npairs = npairs; pa.nseg = L.nseg;
   pa.pls0 = ws.d_pair_level; pa.csat = ws.d_csat;
-  pa.affine = v.affine ? ws.d_affine : nullptr;
-  pa.prior = v.prior ? ws.d_prior : nullptr;
+  pa.affine = v.affine ? ws.d_affine + g.pair0 : nullptr;      // the per-pair mode state, in the leg's pair slots like the states
+  pa.prior = v.prior ? ws.d_prior + 36 * g.pair0 : nullptr;
   for (int s = 0; s < L.nseg; ++s) {
     const PlanSegment& P = L.seg[s];
     Segment& S = pa.seg[s];
@@ -1290,7 +1306,9 @@ int stage_inputs(dvo_b200_ctx* ctx, const Leg* legs, int nlegs, const double* T,
   const int** h_csat = (const int**)(h + s.csat.at);
   for (int j = 0; j < nlegs; ++j) {
     const Leg& g = legs[j];
-    for (int level = g.first, li = 0; level >= g.last; --level, ++li) {
+    // a leg that runs no level and has descriptors (make_leg's maps_desc) holds those of level g.last
+    const int top = g.first < g.last && g.ndesc ? g.last : g.first;
+    for (int level = top, li = 0; level >= g.last; --level, ++li) {
       const size_t at = g.desc0 + (size_t)li * g.npairs;
       fill_pair_levels(h_desc + at, v.cur_mask ? h_csat + at : nullptr, g.npairs, g.refs, g.curs, level);
     }
@@ -1334,6 +1352,15 @@ int ensure_pinned_results(dvo_b200_ctx* ctx, size_t bytes) {
   return 0;
 }
 
+// Enqueue the copy of (alpha, beta) of the n brightness states at src (the pair slots of the leg the results come from)
+// to dst, 2 n doubles of the pinned results buffer
+int copy_back_photometric(dvo_b200_ctx* ctx, void* dst, const AffineState* src, size_t n) {
+  DVO_CUDA(ctx, cudaMemcpy2DAsync(dst, 2 * sizeof(double), src->ab, sizeof(AffineState), 2 * sizeof(double), n,
+                                  cudaMemcpyDeviceToHost, ctx->stream));
+  ctx->d2h_bytes += sizeof(double) * 2 * n;
+  return 0;
+}
+
 }  // namespace
 
 int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
@@ -1363,7 +1390,9 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
     d_res = (dvo_b200_result*)ctx->d_stage;
   }
   finalize(ctx, ws.d_state, d_res, n);
-  if (maps) weight_maps_launch(ctx, *maps, n, refs[0], last, ws.d_pair_level + leg.ndesc - n, v.affine ? ws.d_affine : nullptr);
+  if (maps)
+    weight_maps_launch(ctx, *maps, n, refs[0], last, ws.d_state + leg.pair0, ws.d_pair_level + leg.desc0 + leg.ndesc - n,
+                       v.affine ? ws.d_affine + leg.pair0 : nullptr);
   // a device-results call leaves its level flags to dvo_b200_synchronize
   if ((rc = end_call(ctx, n, refs, curs, leg.plan.nlaunch))) return rc;
   if (h_results) {
@@ -1371,11 +1400,7 @@ int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dv
     const size_t pinned = bytes + (v.affine ? sizeof(double) * 2 * (size_t)n : 0);   // the results, then (alpha, beta) of each pair
     if ((rc = ensure_pinned_results(ctx, pinned))) return rc;
     DVO_CUDA(ctx, cudaMemcpyAsync(ctx->h_results, d_res, bytes, cudaMemcpyDeviceToHost, st));
-    if (v.affine) {
-      DVO_CUDA(ctx, cudaMemcpy2DAsync((char*)ctx->h_results + bytes, 2 * sizeof(double), ws.d_affine[0].ab, sizeof(AffineState),
-                                      2 * sizeof(double), (size_t)n, cudaMemcpyDeviceToHost, st));
-      ctx->d2h_bytes += sizeof(double) * 2 * (size_t)n;
-    }
+    if (v.affine && (rc = copy_back_photometric(ctx, (char*)ctx->h_results + bytes, ws.d_affine + leg.pair0, (size_t)n))) return rc;
     if (maps && (rc = weight_maps_copy_back(ctx, *maps, n, refs[0], last))) return rc;
     if (iter_stats) {
       DVO_CUDA(ctx, cudaMemcpyAsync(iter_stats, ws.d_iter_log, sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log,
@@ -1460,37 +1485,46 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
 }
 
 
-// dvo_b200_match_batch_hypotheses (include/dvo_b200.h), as two legs.  The screening leg runs n k virtual pairs, pair p k + j
-// being (refs[p], curs[p]) from H[p][j], on levels first .. s; k_pick_hypotheses scores them and copies each pair's chosen
-// state (and log) into its slot of the continuation leg, which runs levels s-1 .. last (none if s = last) on the n chosen
-// pairs, its level indices continuing at first - s + 1.  Both legs launch the level kernel like any other match, so plan
-// independence gives each pair the bits of one dvo_b200_match_batch.  The device stage holds the results (n), screen
-// results (n k, if requested), scores (n k) and best (n), copied back through the pinned results buffer in that layout.
+// dvo_b200_match_batch_hypotheses[_modes] (include/dvo_b200.h), as two legs.  The screening leg runs n k virtual pairs, pair
+// p k + j being (refs[p], curs[p]) from H[p][j] (and Lambda[p][j], (alpha, beta)_0[p][j]), on levels first .. s;
+// k_pick_hypotheses scores them and copies each pair's chosen state (log, AffineState, Lambda) into its slot of the
+// continuation leg, which runs levels s-1 .. last (none if s = last) on the n chosen pairs, its level indices continuing at
+// first - s + 1.  Both legs launch the level kernel like any other match, so plan independence gives each pair the bits of
+// one dvo_b200_match_batch[_photometric, _prior].  With maps the continuation leg also holds the level-last descriptors of
+// its pairs when it runs no level (s = last), so that k_weight_maps reads the descriptors, states and AffineStates of one
+// leg as after a match.  The device stage holds the results (n), screen results (n k, if requested), scores (n k) and best
+// (n), copied back through the pinned results buffer in that layout, followed there by (alpha, beta) of the n continued
+// pairs and of the n k screening runs (if requested).
 int tracker_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                                    dvo_b200_pyramid* const* curs, int k, const double* hypotheses, int screen_level,
                                    double min_ratio, dvo_b200_result* h_results, int32_t* h_best, double* h_scores,
-                                   dvo_b200_result* h_screen, dvo_b200_iteration_stats* iter_stats, int max_iter_stats) {
+                                   dvo_b200_result* h_screen, dvo_b200_iteration_stats* iter_stats, int max_iter_stats,
+                                   const double* prior, const double* ab_init, double* ab_out, double* screen_ab,
+                                   const dvo_b200_weight_maps* maps) {
   int rc = check_batch(ctx, cfg, n, refs, curs);
   if (rc) return rc;
   LevelVariant v;
-  if ((rc = begin_call(ctx, cfg, n, refs, curs, false, false, v))) return rc;
+  if ((rc = begin_call(ctx, cfg, n, refs, curs, ab_out != nullptr, prior != nullptr, v))) return rc;
   cudaStream_t st = ctx->stream;
   Workspace& ws = ctx->ws;
-  const int s = screen_level, nk = n * k;
+  const int s = screen_level, nk = n * k, last = cfg->last_level;
   const int max_log = iter_stats ? max_iter_stats : 0;
   std::vector<dvo_b200_pyramid*> vrefs((size_t)nk), vcurs((size_t)nk);
   for (int q = 0; q < nk; ++q) { vrefs[q] = refs[q / k]; vcurs[q] = curs[q / k]; }
   Leg legs[2];
   legs[0] = make_leg(ctx, nullptr, cfg->first_level, s, nk, vrefs.data(), vcurs.data(), v);
-  legs[1] = make_leg(ctx, &legs[0], s - 1, cfg->last_level, n, refs, curs, v);
+  legs[1] = make_leg(ctx, &legs[0], s - 1, last, n, refs, curs, v, maps != nullptr);
   const Leg &screen = legs[0], &chosen = legs[1];
   if ((rc = ensure_workspace(ctx, legs, 2, 0, max_log, v))) return rc;
+  if (maps && (rc = weight_maps_prepare(ctx, *maps, n, refs[0], last))) return rc;
 
   const size_t res_bytes = sizeof(dvo_b200_result) * (size_t)n, screen_bytes = h_screen ? sizeof(dvo_b200_result) * (size_t)nk : 0;
   const size_t score_bytes = sizeof(double) * (size_t)nk, out_bytes = res_bytes + screen_bytes + score_bytes + sizeof(int) * (size_t)n;
+  const size_t ab_at = (out_bytes + 15) / 16 * 16, ab_bytes = v.affine ? sizeof(double) * 2 * (size_t)n : 0;
+  const size_t screen_ab_bytes = screen_ab ? sizeof(double) * 2 * (size_t)nk : 0;
   if ((rc = ensure_stage(ctx, out_bytes, 0))) return rc;
-  if ((rc = ensure_pinned_results(ctx, out_bytes))) return rc;
-  if ((rc = stage_inputs(ctx, legs, 2, hypotheses, nullptr, nullptr, max_log, v))) return rc;
+  if ((rc = ensure_pinned_results(ctx, ab_at + ab_bytes + screen_ab_bytes))) return rc;
+  if ((rc = stage_inputs(ctx, legs, 2, hypotheses, ab_init, prior, max_log, v))) return rc;
   for (int i = 0; i < screen.plan.nlaunch; ++i)
     if ((rc = launch_segments(ctx, cfg, screen, i, ws.d_tinit, max_log, nullptr, 0, v))) return rc;
   char* const d_out = (char*)ctx->d_stage;
@@ -1500,29 +1534,40 @@ int tracker_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg
   if (h_screen) finalize(ctx, ws.d_state, (dvo_b200_result*)(d_out + res_bytes), nk);
   {
     ProfScope prof(ctx, 2);
-    k_pick_hypotheses<<<(n + 3) / 4, 128, 0, st>>>(ws.d_state, ws.d_iter_log, ws.d_state + chosen.pair0,
-                                                   ws.d_iter_log + chosen.pair0 * max_log, max_log, n, k,
-                                                   screen.first - screen.last, min_ratio, d_scores, d_best);
+    auto pick = v.affine ? (v.prior ? k_pick_hypotheses<true, true> : k_pick_hypotheses<true, false>)
+                         : (v.prior ? k_pick_hypotheses<false, true> : k_pick_hypotheses<false, false>);
+    pick<<<(n + 3) / 4, 128, 0, st>>>(ws.d_state, ws.d_iter_log, ws.d_state + chosen.pair0, ws.d_iter_log + chosen.pair0 * max_log,
+                                      max_log, n, k, screen.first - screen.last, min_ratio, d_scores, d_best,
+                                      v.affine ? ws.d_affine : nullptr, v.affine ? ws.d_affine + chosen.pair0 : nullptr,
+                                      v.prior ? ws.d_prior : nullptr, v.prior ? ws.d_prior + 36 * chosen.pair0 : nullptr);
     ctx->launches++;
   }
   for (int i = 0; i < chosen.plan.nlaunch; ++i)
     if ((rc = launch_segments(ctx, cfg, chosen, i, nullptr, max_log, nullptr, 0, v))) return rc;
   finalize(ctx, ws.d_state + chosen.pair0, d_res, n);
+  if (maps)
+    weight_maps_launch(ctx, *maps, n, refs[0], last, ws.d_state + chosen.pair0, ws.d_pair_level + chosen.desc0 + chosen.ndesc - n,
+                       v.affine ? ws.d_affine + chosen.pair0 : nullptr);
   if ((rc = end_call(ctx, n, refs, curs, screen.plan.nlaunch + chosen.plan.nlaunch))) return rc;
 
-  DVO_CUDA(ctx, cudaMemcpyAsync(ctx->h_results, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+  char* const hr = (char*)ctx->h_results;
+  DVO_CUDA(ctx, cudaMemcpyAsync(hr, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
   ctx->d2h_bytes += out_bytes;
+  if (v.affine && (rc = copy_back_photometric(ctx, hr + ab_at, ws.d_affine + chosen.pair0, (size_t)n))) return rc;
+  if (screen_ab && (rc = copy_back_photometric(ctx, hr + ab_at + ab_bytes, ws.d_affine + screen.pair0, (size_t)nk))) return rc;
+  if (maps && (rc = weight_maps_copy_back(ctx, *maps, n, refs[0], last))) return rc;
   if (iter_stats) {
     DVO_CUDA(ctx, cudaMemcpyAsync(iter_stats, ws.d_iter_log + chosen.pair0 * max_log,
                                   sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log, cudaMemcpyDeviceToHost, st));
     ctx->d2h_bytes += sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log;
   }
   DVO_CUDA(ctx, cudaStreamSynchronize(st));
-  const char* const hr = (const char*)ctx->h_results;
   std::memcpy(h_results, hr, res_bytes);
   if (h_screen) std::memcpy(h_screen, hr + res_bytes, screen_bytes);
   if (h_scores) std::memcpy(h_scores, hr + res_bytes + screen_bytes, score_bytes);
   std::memcpy(h_best, hr + res_bytes + screen_bytes + score_bytes, sizeof(int) * (size_t)n);
+  if (v.affine) std::memcpy(ab_out, hr + ab_at, ab_bytes);
+  if (screen_ab) std::memcpy(screen_ab, hr + ab_at + ab_bytes, screen_ab_bytes);
   return check_level_flags(ctx);
 }
 

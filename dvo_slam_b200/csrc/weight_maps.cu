@@ -167,7 +167,7 @@ int weight_maps_prepare(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int
 }
 
 void weight_maps_launch(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int n, const dvo_b200_pyramid* ref0, int level,
-                        const PairLevel* d_pls, const AffineState* d_affine) {
+                        const PairState* d_states, const PairLevel* d_pls, const AffineState* d_affine) {
   Workspace& ws = ctx->ws;
   const LevelInfo& L = ref0->L[level];
   MapsLaunch m;
@@ -191,7 +191,7 @@ void weight_maps_launch(dvo_b200_ctx* ctx, const dvo_b200_weight_maps& maps, int
   const int sc = 1 << level;
   const int gx = std::max(L.w, (m.w0 + sc - 1) / sc), gy = std::max(L.h, (m.h0 + sc - 1) / sc);
   const dim3 grid((gx + kMapsBlockX - 1) / kMapsBlockX, (gy + kMapsBlockY - 1) / kMapsBlockY, n);
-  k_weight_maps<<<grid, dim3(kMapsBlockX, kMapsBlockY), 0, ctx->stream>>>(ws.d_state, d_affine, d_pls, m);
+  k_weight_maps<<<grid, dim3(kMapsBlockX, kMapsBlockY), 0, ctx->stream>>>(d_states, d_affine, d_pls, m);
   ctx->launches++;
 }
 

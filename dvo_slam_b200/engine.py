@@ -38,7 +38,7 @@ ABI_SYMBOLS = [
     "dvo_b200_pyramid_create_rectified_device_batch", "dvo_b200_depth_rays", "dvo_b200_depth_registration_create",
     "dvo_b200_depth_registration_release", "dvo_b200_pyramid_create_registered_batch",
     "dvo_b200_pyramid_create_registered_device_batch", "dvo_b200_match_batch_prior", "dvo_b200_match_batch_maps",
-    "dvo_b200_match_batch_hypotheses",
+    "dvo_b200_match_batch_hypotheses", "dvo_b200_match_batch_hypotheses_modes",
 ]
 
 # dvo_b200_estimator
@@ -340,6 +340,9 @@ def load_library():
                                             C.POINTER(IterationStats), i32, C.POINTER(WeightMaps)]
     L.dvo_b200_match_batch_hypotheses.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), i32, dp, i32, C.c_double,
                                                    C.POINTER(CResult), C.POINTER(i32), dp, C.POINTER(CResult), C.POINTER(IterationStats), i32]
+    L.dvo_b200_match_batch_hypotheses_modes.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), i32, dp, i32, C.c_double,
+                                                         dp, dp, dp, dp, C.POINTER(CResult), C.POINTER(i32), dp, C.POINTER(CResult),
+                                                         C.POINTER(IterationStats), i32, C.POINTER(WeightMaps)]
     L.dvo_b200_residual_image_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, fp, C.POINTER(i64)]
     L.dvo_b200_linearize_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, i32, fp, C.POINTER(i64), fp, fp, dp, dp]
     L.dvo_b200_set_estimator.argtypes = [vp, i32]
@@ -786,16 +789,9 @@ class Engine:
         out = self.match_batch(refs, curs, cfg, T_init, with_iterations, _photometric=(ab0, ab), prior_information=prior_information)
         return out, ab
 
-    def match_batch_maps(self, refs, curs, cfg: Config, T_init=None, prior_information=None, photometric_init=None,
-                         photometric: bool = False, mask_weight=None, with_iterations: bool = False):
-        """An alignment and each pair's weight maps at its returned pose (dvo_b200_match_batch_maps; "weight maps" in
-        include/dvo_b200.h).  The results (and (alpha, beta)) are those of match_batch / match_batch_photometric with the same
-        arguments.  Returns (results, maps), or (results, maps, [n, 2] (alpha, beta)) when photometric.  maps holds torch CUDA
-        tensors on the engine's device: "weight", "residual_i", "residual_z" [n, h_L, w_L] float32 at L = cfg.last_level (NaN
-        where a pixel is not a constraint), "estimate" [n, 4, 4] float64 (the pose the maps are at, reference -> current),
-        "precision" [n, 2, 2] float32 and, with mask_weight, "mask" [n, h, w] uint8 at level 0: 0 where the pixel's level-L
-        parent is a constraint with weight < mask_weight, 1 elsewhere -- the masks= of pyramid_batch_device.  The pyramids of
-        one call must share their size (ValueError otherwise)."""
+    def _device_maps(self, refs, cfg: Config, mask_weight):
+        """The torch CUDA tensors of match_batch_maps and the WeightMaps that points at them, with the engine's stream ordered
+        after torch's current stream (the engine's stream writes memory that stream allocated; the call synchronises)."""
         import torch
         n = len(refs)
         L = cfg.last_level
@@ -817,6 +813,22 @@ class Engine:
             wm.mask_weight = float(mask_weight)
         wm.estimate = C.cast(maps["estimate"].data_ptr(), C.POINTER(C.c_double))
         wm.precision = C.cast(maps["precision"].data_ptr(), C.POINTER(C.c_float))
+        current = torch.cuda.current_stream(dev)
+        torch.cuda.ExternalStream(self.stream, device=dev).wait_stream(current)
+        return maps, wm
+
+    def match_batch_maps(self, refs, curs, cfg: Config, T_init=None, prior_information=None, photometric_init=None,
+                         photometric: bool = False, mask_weight=None, with_iterations: bool = False):
+        """An alignment and each pair's weight maps at its returned pose (dvo_b200_match_batch_maps; "weight maps" in
+        include/dvo_b200.h).  The results (and (alpha, beta)) are those of match_batch / match_batch_photometric with the same
+        arguments.  Returns (results, maps), or (results, maps, [n, 2] (alpha, beta)) when photometric.  maps holds torch CUDA
+        tensors on the engine's device: "weight", "residual_i", "residual_z" [n, h_L, w_L] float32 at L = cfg.last_level (NaN
+        where a pixel is not a constraint), "estimate" [n, 4, 4] float64 (the pose the maps are at, reference -> current),
+        "precision" [n, 2, 2] float32 and, with mask_weight, "mask" [n, h, w] uint8 at level 0: 0 where the pixel's level-L
+        parent is a constraint with weight < mask_weight, 1 elsewhere -- the masks= of pyramid_batch_device.  The pyramids of
+        one call must share their size (ValueError otherwise)."""
+        n = len(refs)
+        maps, wm = self._device_maps(refs, cfg, mask_weight)
         ab0 = ab = None
         if photometric:
             if photometric_init is not None:
@@ -824,9 +836,6 @@ class Engine:
             ab = np.zeros((n, 2), dtype=np.float64)
         elif photometric_init is not None:
             raise ValueError("photometric_init without photometric=True")
-        # the engine's stream writes memory that torch's current stream allocated; the call synchronises its stream
-        current = torch.cuda.current_stream(dev)
-        torch.cuda.ExternalStream(self.stream, device=dev).wait_stream(current)
         res = self.match_batch(refs, curs, cfg, T_init, with_iterations, _photometric=(ab0, ab) if photometric else None,
                                prior_information=prior_information, _maps=wm)
         return (res, maps, ab) if photometric else (res, maps)
@@ -876,12 +885,22 @@ class Engine:
         return _results(res, n, log, max_log)
 
     def match_batch_hypotheses(self, refs, curs, hypotheses, screen_level: int, min_constraint_ratio: float = 0.0,
-                               cfg: Config | None = None, with_iterations: bool = False, screen_results: bool = False):
-        """Multi-hypothesis alignment (dvo_b200_match_batch_hypotheses): pair i starts from each of the k poses
+                               cfg: Config | None = None, with_iterations: bool = False, screen_results: bool = False,
+                               prior_information=None, photometric_init=None, photometric: bool = False, maps: bool = False,
+                               mask_weight=None):
+        """Multi-hypothesis alignment (dvo_b200_match_batch_hypotheses[_modes]): pair i starts from each of the k poses
         hypotheses[i] ([n, k, 4, 4], read as T_init) on levels cfg.first_level .. screen_level, and the one with the lowest
         per-constraint negative log-likelihood among those with a large enough constraint ratio continues to cfg.last_level.
         cfg: default Config(use_initial_estimate=1).  Returns (results, best [n] int32, scores [n, k] float64, NaN where a
-        hypothesis was not eligible), and with screen_results=True also the screening results, a list of n lists of k."""
+        hypothesis was not eligible), and with screen_results=True also the screening results, a list of n lists of k.
+        The modes, per hypothesis (include/dvo_b200.h, dvo_b200_match_batch_hypotheses_modes):
+          prior_information  [n, k, 6, 6] float64: Lambda of each hypothesis, anchored at that hypothesis (cfg.mu must be 0).
+          photometric        True: the photometric mode; photometric_init [n, k, 2] (alpha, beta)_0 per hypothesis, or None
+                             = (1, 0).  Appends the final (alpha, beta) [n, 2] and, with screen_results, where each screening
+                             run ended [n, k, 2].
+          maps, mask_weight  True / a mask weight: the weight maps of the continued alignments, the dict of match_batch_maps
+                             (mask only with mask_weight), appended last.
+        The score is that of the data term alone whatever the mode."""
         if cfg is None:
             cfg = Config(use_initial_estimate=1)
         n = len(refs)
@@ -891,6 +910,26 @@ class Engine:
             raise ValueError(f"hypotheses {H.shape}: want [{n}, k, 4, 4]")
         k = H.shape[1]
         H = np.ascontiguousarray(H.reshape(n * k, 16))
+        lam = ab0 = ab = screen_ab = None
+        if prior_information is not None:
+            lam = np.asarray(prior_information, dtype=np.float64)
+            if lam.size != 36 * n * k:
+                raise ValueError(f"prior_information {lam.shape}: want [{n}, {k}, 6, 6]")
+            lam = np.ascontiguousarray(lam.reshape(n * k, 36))
+        if photometric:
+            if photometric_init is not None:
+                ab0 = np.asarray(photometric_init, dtype=np.float64)
+                if ab0.size != 2 * n * k:
+                    raise ValueError(f"photometric_init {ab0.shape}: want [{n}, {k}, 2]")
+                ab0 = np.ascontiguousarray(ab0.reshape(n * k, 2))
+            ab = np.zeros((n, 2), dtype=np.float64)
+            if screen_results:
+                screen_ab = np.zeros((n, k, 2), dtype=np.float64)
+        elif photometric_init is not None:
+            raise ValueError("photometric_init without photometric=True")
+        dmaps = wm = None
+        if maps or mask_weight is not None:
+            dmaps, wm = self._device_maps(refs, cfg, mask_weight)
         rh = (C.c_void_p * n)(*[p.handle for p in refs])
         ch = (C.c_void_p * n)(*[p.handle for p in curs])
         res = (CResult * n)()
@@ -902,13 +941,19 @@ class Engine:
             max_log = (cfg.first_level - cfg.last_level + 1) * (cfg.max_iterations_per_level + 1)
             log = (IterationStats * (n * max_log))()
         dp = C.POINTER(C.c_double)
-        self._check(self.lib.dvo_b200_match_batch_hypotheses(
-            self.ctx, C.byref(cfg), n, rh, ch, k, H.ctypes.data_as(dp), int(screen_level), float(min_constraint_ratio), res,
-            best.ctypes.data_as(C.POINTER(C.c_int32)), scores.ctypes.data_as(dp), screen, log, max_log))
+        ptr = lambda a: a.ctypes.data_as(dp) if a is not None else None
+        self._check(self.lib.dvo_b200_match_batch_hypotheses_modes(
+            self.ctx, C.byref(cfg), n, rh, ch, k, H.ctypes.data_as(dp), int(screen_level), float(min_constraint_ratio), ptr(lam),
+            ptr(ab0), ptr(ab), ptr(screen_ab), res, best.ctypes.data_as(C.POINTER(C.c_int32)), scores.ctypes.data_as(dp), screen,
+            log, max_log, C.byref(wm) if wm is not None else None))
         out = (_results(res, n, log, max_log), best, scores)
         if screen_results:
             flat = [Result(screen[i]) for i in range(n * k)]
             out += ([flat[i * k:(i + 1) * k] for i in range(n)],)
+        if photometric:
+            out += (ab,) + ((screen_ab,) if screen_results else ())
+        if dmaps is not None:
+            out += (dmaps,)
         return out
 
     def match_batch_device(self, refs, curs, cfg: Config, d_results_ptr: int, T_init=None):

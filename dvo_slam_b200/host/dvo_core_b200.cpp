@@ -8,7 +8,7 @@
 #include <stdexcept>
 
 #include "dvo/dense_tracking.h"
-#include "../csrc/hypotheses_args.h"   // the checks of dvo_b200_match_batch_hypotheses, run here so that a refusal returns false
+#include "../csrc/hypotheses_args.h"   // the checks of dvo_b200_match_batch_hypotheses[_modes], run here so that a refusal returns false
 #include "../csrc/prior_args.h"   // the prior checks of dvo_b200_match_batch_prior, run here so that a refusal returns false
 
 namespace dvo {
@@ -403,6 +403,25 @@ bool DenseTracker::matchWithWeights(core::RgbdImagePyramid& reference, core::Rgb
 bool DenseTracker::matchWithHypotheses(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current,
                                        const std::vector<core::AffineTransformd>& initial, int screen_level, Result& result, int* best,
                                        double min_constraint_ratio) {
+  return matchWithHypotheses(reference, current, initial, static_cast<const double*>(0), screen_level, result, best, min_constraint_ratio, 0);
+}
+
+bool DenseTracker::matchWithHypotheses(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current,
+                                       const std::vector<core::AffineTransformd>& initial, const std::vector<core::Matrix6d>& prior_information,
+                                       int screen_level, Result& result, int* best, double min_constraint_ratio, cv::Mat* weights) {
+  if (prior_information.size() != initial.size()) return false;
+  std::vector<double> L(36 * prior_information.size());
+  for (size_t j = 0; j < prior_information.size(); ++j)
+    for (int a = 0; a < 6; ++a)
+      for (int b = 0; b < 6; ++b) L[36 * j + a * 6 + b] = prior_information[j](a, b);
+  return matchWithHypotheses(reference, current, initial, L.data(), screen_level, result, best, min_constraint_ratio, weights);
+}
+
+// Both public forms: prior (k * 36, Lambda of hypothesis j at 36 j) or NULL, and the weight map of the continued alignment at
+// LastLevel, in host memory, if weights is given.
+bool DenseTracker::matchWithHypotheses(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current,
+                                       const std::vector<core::AffineTransformd>& initial, const double* prior, int screen_level,
+                                       Result& result, int* best, double min_constraint_ratio, cv::Mat* weights) {
   dvo_b200_config c;
   dvo_b200_config_default(&c);
   c.first_level = cfg.FirstLevel; c.last_level = cfg.LastLevel; c.max_iterations_per_level = cfg.MaxIterationsPerLevel;
@@ -415,6 +434,11 @@ bool DenseTracker::matchWithHypotheses(core::RgbdImagePyramid& reference, core::
   dvo_b200_result raw;
   int32_t chosen = 0;
   if (!dvo_b200::hypotheses_args_error(&c, 1, k, H.data(), screen_level, min_constraint_ratio, &raw, &chosen).empty()) return false;
+  if (prior) {   // the prior checks of dvo_b200_match_batch_hypotheses_modes, refused before any upload
+    if (c.mu != 0.0) return false;
+    for (int j = 0; j < k; ++j)
+      if (!dvo_b200::prior_matrix_error(prior + 36 * (size_t)j).empty()) return false;
+  }
   dvo_b200_ctx* ctx = context();
   dvo_b200_pyramid *r, *q;
   {
@@ -427,9 +451,20 @@ bool DenseTracker::matchWithHypotheses(core::RgbdImagePyramid& reference, core::
   }
   const int max_log = collect_iterations_ ? (cfg.FirstLevel - cfg.LastLevel + 1) * (cfg.MaxIterationsPerLevel + 1) : 0;
   std::vector<dvo_b200_iteration_stats> its((size_t)max_log);
-  if (dvo_b200_match_batch_hypotheses(ctx, &c, 1, &r, &q, k, H.data(), screen_level, min_constraint_ratio, &raw, &chosen, 0, 0,
-                                      max_log ? its.data() : 0, max_log) != 0)
-    throw std::runtime_error(std::string("dvo_b200_match_batch_hypotheses: ") + dvo_b200_last_error(ctx));
+  dvo_b200_weight_maps maps;
+  if (weights) {   // the weight map of the continued alignment, at LastLevel, straight into the cv::Mat
+    int w = 0, h = 0;
+    dvo_b200_pyramid_level_info(r, c.last_level, &w, &h, 0);
+    weights->create(h, w, CV_32FC1);
+    std::memset(&maps, 0, sizeof(maps));
+    maps.memory = DVO_B200_MAPS_HOST;
+    maps.weight.data = weights->ptr<float>();
+    maps.weight.row_bytes = int64_t(sizeof(float)) * w;
+    maps.weight.image_bytes = maps.weight.row_bytes * h;
+  }
+  if (dvo_b200_match_batch_hypotheses_modes(ctx, &c, 1, &r, &q, k, H.data(), screen_level, min_constraint_ratio, prior, 0, 0, 0, &raw,
+                                            &chosen, 0, 0, max_log ? its.data() : 0, max_log, weights ? &maps : 0) != 0)
+    throw std::runtime_error(std::string("dvo_b200_match_batch_hypotheses_modes: ") + dvo_b200_last_error(ctx));
   Result out;
   fill_result(raw, max_log ? its.data() : 0, out);
   result = out;

@@ -123,10 +123,18 @@ class DenseTracker {
   // ratio is at least min_constraint_ratio (dvo_slam's ConstraintRatioVoter) to LastLevel.  result is then what match()
   // returns from that hypothesis; *best (if given) its index.  Returns false, without aligning, when the arguments are
   // refused (no or too many hypotheses, a non-finite or non-rigid 4 x 4, screen_level outside [LastLevel, FirstLevel], a
-  // ratio outside [0, 1]). ---
+  // ratio outside [0, 1]).
   bool matchWithHypotheses(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current,
                            const std::vector<core::AffineTransformd>& initial, int screen_level, Result& result, int* best = 0,
                            double min_constraint_ratio = 0.0);
+  // The same with a motion prior per hypothesis (dvo_b200_match_batch_hypotheses_modes): prior_information[j], the 6 x 6
+  // prior information of initial[j], anchored at initial[j] (an IMU start its Sigma^-1, a zero-motion start 0; Mu must be 0),
+  // and with weights (if given) the continued alignment's weight map as matchWithWeights returns it.  The prior is not part
+  // of the score.  Returns false, without aligning, on the refusals above, a prior_information of another size than
+  // initial, Mu != 0, or a prior that matchWithPrior would refuse. ---
+  bool matchWithHypotheses(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current,
+                           const std::vector<core::AffineTransformd>& initial, const std::vector<core::Matrix6d>& prior_information,
+                           int screen_level, Result& result, int* best = 0, double min_constraint_ratio = 0.0, cv::Mat* weights = 0);
 
   // per-iteration statistics are copied back only when requested (they are optional in the C ABI)
   void collectIterationStatistics(bool on) { collect_iterations_ = on; }
@@ -139,6 +147,9 @@ class DenseTracker {
   bool matchBatch(const std::vector<core::RgbdImagePyramid*>& references, const std::vector<core::RgbdImagePyramid*>& currents,
                   const double* prior_information, std::vector<Result>& results,    // prior_information: n * 36 or NULL
                   cv::Mat* weights = 0);                                             // n == 1 only: matchWithWeights
+  bool matchWithHypotheses(core::RgbdImagePyramid& reference, core::RgbdImagePyramid& current,   // prior: k * 36 or NULL
+                           const std::vector<core::AffineTransformd>& initial, const double* prior, int screen_level, Result& result,
+                           int* best, double min_constraint_ratio, cv::Mat* weights);
   Config cfg;
   dvo_b200_ctx* ctx_;
   bool collect_iterations_;

@@ -657,8 +657,9 @@ int dvo_b200_match_batch_maps(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int
  *   scores[p * k + j] (optional) are the scores above, NaN where j is not eligible.
  * Cost: the screening aligns n * k pairs on the coarse levels, the continuation n pairs on the fine ones; a coarse level has a
  * quarter of the pixels of the next finer one.  Reference-role and both-role masks, cfg->mu and mixed intrinsics are
- * supported as by dvo_b200_match_batch.
- * Not provided in this mode: the photometric mode, motion priors, weight maps, match_batch_device and the sharded forms. */
+ * supported as by dvo_b200_match_batch; the photometric mode, motion priors and weight maps through
+ * dvo_b200_match_batch_hypotheses_modes below.
+ * Not provided in this mode: match_batch_device and the sharded forms. */
 #define DVO_B200_MAX_HYPOTHESES 64
 
 /* hypotheses: n * k * 16 doubles, H[p][j] at (p * k + j) * 16.  results, best: n each.  scores: n * k or NULL.
@@ -673,6 +674,43 @@ int dvo_b200_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cf
                                     const double* hypotheses, int32_t screen_level, double min_constraint_ratio,
                                     dvo_b200_result* results, int32_t* best, double* scores, dvo_b200_result* screen_results,
                                     dvo_b200_iteration_stats* iteration_stats, int32_t max_iteration_stats);
+
+/* Multi-hypothesis alignment in the photometric mode, with motion priors and with weight maps.  The arguments of
+ * dvo_b200_match_batch_hypotheses, plus, each optional:
+ *   prior_information   n * k * 36 doubles or NULL: Lambda[p][j], the prior information of hypothesis j of pair p, at
+ *                       (p * k + j) * 36.  Requires cfg->mu == 0.
+ *   photometric_init    n * k * 2 doubles or NULL (= (1, 0) each): (alpha, beta)_0[p][j].  Only with photometric.
+ *   photometric         n * 2 doubles out, or NULL: non-NULL selects the photometric mode; the final (alpha, beta) of pair p.
+ *   screen_photometric  n * k * 2 doubles out, or NULL: (alpha, beta) where screening run (p, j) ended.  Only with photometric.
+ *   maps                NULL (no maps) or the weight maps of the continued alignments, as dvo_b200_match_batch_maps writes them.
+ * Let E be the single-pair entry point of the mode: dvo_b200_match_batch_prior with a prior (photometric as given),
+ * otherwise dvo_b200_match_batch_photometric or dvo_b200_match_batch.  Bit for bit, for both estimators, every mask role
+ * set, mixed intrinsics, every batch size and position and every launch plan:
+ *   screening     run (p, j) is E of that pair with last_level = s from T_init = H[p][j], Lambda[p][j] and
+ *                 (alpha, beta)_0[p][j]; screen_results[p * k + j] and screen_photometric[p * k + j] are what that call returns.
+ *   score, choice exactly as above: the per-constraint negative log-likelihood of the data term alone.  The prior term is
+ *                 not part of the score, so a hypothesis cannot win by its own prior: a tight Lambda about a wrong start
+ *                 does not make that start look better.
+ *   continuation  results[p], photometric[p] and pair p's iteration log are what E returns for pair p alone from the chosen
+ *                 triple (H, Lambda, (alpha, beta)_0)[p][best[p]] with the call's last_level.
+ *   maps          the maps, estimate and precision are what dvo_b200_match_batch_maps returns for that same single call, also
+ *                 when s = last_level.
+ * The prior of run (p, j) is anchored where dvo_b200_match_batch_prior anchors it, at the run's own initial estimate
+ * T0 = H[p][j]; that is why Lambda is given per hypothesis.  An IMU prediction carries its Sigma^-1, a constant-velocity
+ * prediction the information of the alignment it extrapolates, a zero-motion or relocalisation start 0.
+ * Refused with DVO_B200_ERR_INVALID_ARGUMENT, and dvo_b200_last_error set, before anything is staged, uploaded or launched:
+ * everything dvo_b200_match_batch_hypotheses refuses (checked first); photometric_init or screen_photometric without
+ * photometric; with a prior, cfg->mu != 0 and a Lambda[p][j] that dvo_b200_match_batch_prior would refuse; a non-finite
+ * photometric_init; with maps, everything dvo_b200_match_batch_maps refuses of its maps.  The messages name the hypothesis
+ * ("hypothesis j of pair p").  dvo_b200_match_batch_hypotheses is this call with every new argument NULL.  One kernel
+ * launch more with maps (k_weight_maps); synchronises once, as dvo_b200_match_batch does. */
+int dvo_b200_match_batch_hypotheses_modes(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n,
+                                          dvo_b200_pyramid* const* references, dvo_b200_pyramid* const* currents, int32_t k,
+                                          const double* hypotheses, int32_t screen_level, double min_constraint_ratio,
+                                          const double* prior_information, const double* photometric_init, double* photometric,
+                                          double* screen_photometric, dvo_b200_result* results, int32_t* best, double* scores,
+                                          dvo_b200_result* screen_results, dvo_b200_iteration_stats* iteration_stats,
+                                          int32_t max_iteration_stats, const dvo_b200_weight_maps* maps);
 
 /* ---- profiling hooks (bench.py roofline): per-kernel-class accumulated device time measured with
  *      CUDA events on the ctx stream.  classes: 0 residual/scale stage, 1 normal-equation stage,
