@@ -662,8 +662,10 @@ int dvo_b200_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t 
                          dvo_b200_iteration_stats* iteration_stats, int32_t max_iteration_stats) {
   if (!ctx || !results) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch: null argument");
   cudaSetDevice(ctx->device);
-  return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
-                             iteration_stats ? max_iteration_stats : 0);
+  MatchCall c;
+  c.cfg = cfg; c.n = n; c.refs = references; c.curs = currents; c.T_init = T_init;
+  c.results = results; c.iter_stats = iteration_stats; c.max_log = max_iteration_stats;
+  return tracker_match(ctx, c);
 }
 
 int dvo_b200_match(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference, dvo_b200_pyramid* current,
@@ -678,7 +680,10 @@ int dvo_b200_match_batch_device(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, i
                                 const double* T_init, void* d_results) {
   if (!ctx || !d_results) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_device: null argument");
   cudaSetDevice(ctx->device);
-  return tracker_match_batch(ctx, cfg, n, references, currents, T_init, nullptr, d_results, nullptr, 0);
+  MatchCall c;
+  c.cfg = cfg; c.n = n; c.refs = references; c.curs = currents; c.T_init = T_init;
+  c.d_results = d_results;
+  return tracker_match(ctx, c);
 }
 
 int dvo_b200_residual_image(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,
@@ -728,8 +733,11 @@ int dvo_b200_match_batch_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* c
   if (photometric_init && n > 0 && !all_finite(photometric_init, 2 * (size_t)n))
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_photometric: photometric_init is not finite");
   cudaSetDevice(ctx->device);
-  return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
-                             iteration_stats ? max_iteration_stats : 0, photometric_init, photometric);
+  MatchCall c;
+  c.cfg = cfg; c.n = n; c.refs = references; c.curs = currents; c.T_init = T_init;
+  c.ab_init = photometric_init;
+  c.results = results; c.ab_out = photometric; c.iter_stats = iteration_stats; c.max_log = max_iteration_stats;
+  return tracker_match(ctx, c);
 }
 
 // ---- motion prior ----
@@ -743,8 +751,11 @@ int dvo_b200_match_batch_prior(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, in
   if (photometric_init && n > 0 && !all_finite(photometric_init, 2 * (size_t)n))
     return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_prior: photometric_init is not finite");
   cudaSetDevice(ctx->device);
-  return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
-                             iteration_stats ? max_iteration_stats : 0, photometric_init, photometric, prior_information);
+  MatchCall c;
+  c.cfg = cfg; c.n = n; c.refs = references; c.curs = currents; c.T_init = T_init;
+  c.prior = prior_information; c.ab_init = photometric_init;
+  c.results = results; c.ab_out = photometric; c.iter_stats = iteration_stats; c.max_log = max_iteration_stats;
+  return tracker_match(ctx, c);
 }
 
 // ---- weight maps ----
@@ -790,8 +801,11 @@ int dvo_b200_match_batch_maps(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int
   const bool sane = maps_extent(cfg, n, references, &ext);
   const std::string why = maps_args_error(maps, sane ? n : 0, ext, ctx->device, pointer_where);
   if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
-  return tracker_match_batch(ctx, cfg, n, references, currents, T_init, results, nullptr, iteration_stats,
-                             iteration_stats ? max_iteration_stats : 0, photometric_init, photometric, prior_information, maps);
+  MatchCall c;
+  c.cfg = cfg; c.n = n; c.refs = references; c.curs = currents; c.T_init = T_init;
+  c.prior = prior_information; c.ab_init = photometric_init;
+  c.results = results; c.ab_out = photometric; c.iter_stats = iteration_stats; c.max_log = max_iteration_stats; c.maps = maps;
+  return tracker_match(ctx, c);
 }
 
 // ---- multi-hypothesis alignment ----
@@ -809,10 +823,14 @@ int dvo_b200_match_batch_hypotheses_modes(dvo_b200_ctx* ctx, const dvo_b200_conf
                                                       sane ? &ext : nullptr, ctx->device, pointer_where);
   if (!why.empty()) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, why);
   cudaSetDevice(ctx->device);
-  return tracker_match_batch_hypotheses(ctx, cfg, n, references, currents, k, hypotheses, screen_level, min_constraint_ratio,
-                                        results, best, scores, screen_results, iteration_stats,
-                                        iteration_stats ? max_iteration_stats : 0, prior_information, photometric_init, photometric,
-                                        screen_photometric, maps);
+  MatchCall c;
+  c.cfg = cfg; c.n = n; c.refs = references; c.curs = currents; c.T_init = hypotheses;
+  c.k = k; c.screen_level = screen_level; c.min_ratio = min_constraint_ratio;
+  c.prior = prior_information; c.ab_init = photometric_init;
+  c.results = results; c.ab_out = photometric; c.screen_ab = screen_photometric;
+  c.best = best; c.scores = scores; c.screen_results = screen_results;
+  c.iter_stats = iteration_stats; c.max_log = max_iteration_stats; c.maps = maps;
+  return tracker_match(ctx, c);
 }
 
 int dvo_b200_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,

@@ -281,29 +281,36 @@ void pyramid_free(dvo_b200_pyramid* p);
 void pool_close(dvo_b200_ctx* ctx);
 int ensure_stage(dvo_b200_ctx* ctx, size_t dev_bytes, size_t host_bytes);
 
-// tracker.cu.  The three calls below run the level kernel in legs (tracker.cu: Leg), each one run over a range of pyramid
+// tracker.cu.  The two calls below run the level kernel in legs (tracker.cu: Leg), each one run over a range of pyramid
 // levels of a batch of pairs, through one path: check_batch and begin_call, ensure_workspace, stage_inputs, launch_segments,
-// end_call.  A match is one leg, the hypotheses call two, and a test hook one leg of one pair at one level.
-// ab_out != NULL: the photometric mode (8 unknowns: pose, gain, bias), from ab_init (2n doubles, NULL = (1, 0) each); the
-// final (alpha, beta) of each pair go to ab_out (host, 2n doubles).  Needs h_results.
-// prior != NULL: a motion prior, n row-major 6 x 6 informations (host) in place of cfg->mu I (which must then be 0).
-int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
-                        dvo_b200_pyramid* const* curs, const double* T_init, dvo_b200_result* h_results,
-                        void* d_results, dvo_b200_iteration_stats* iter_stats, int max_iter_stats,
-                        const double* ab_init = nullptr, double* ab_out = nullptr, const double* prior = nullptr,
-                        const dvo_b200_weight_maps* maps = nullptr);   // maps != NULL: also the weight maps (weight_maps.cu)
+// end_call.  A match is one leg, a multi-hypothesis match two, and a test hook one leg of one pair at one level.
+// One match of n pairs (refs[i], curs[i]) after its entry point's argument checks (capi.cu).  k = 0: a plain match; k >= 1:
+// dvo_b200_match_batch_hypotheses[_modes] (checked by hypotheses_args.h), whose per-pair inputs are per hypothesis, n * k.
+// A field left at its default is an input the call does not have or an output it does not want.
+struct MatchCall {
+  const dvo_b200_config* cfg = nullptr;  // levels, iterations, thresholds of every alignment of the call
+  int n = 0;                             // pairs
+  dvo_b200_pyramid* const* refs = nullptr;   // the reference pyramid of each pair
+  dvo_b200_pyramid* const* curs = nullptr;   // the current pyramid of each pair
+  const double* T_init = nullptr;        // row-major 4 x 4 initial estimates (host): n, or with k >= 1 the n * k hypotheses
+  int k = 0;                             // hypotheses per pair, screened on levels first .. screen_level; 0: a plain match
+  int screen_level = 0;                  // k >= 1: the last level of the screening
+  double min_ratio = 0.0;                // k >= 1: hypothesis_score's minimum ratio of constraints to valid pixels
+  const double* prior = nullptr;         // a motion prior: row-major 6 x 6 informations (host) in place of cfg->mu I (then 0)
+  const double* ab_init = nullptr;       // photometric mode: the starting (alpha, beta) (host, 2 doubles each), NULL = (1, 0)
+  dvo_b200_result* results = nullptr;    // host, n; or
+  void* d_results = nullptr;             // device, n: the call enqueues its work and returns (k = 0, no other output)
+  double* ab_out = nullptr;              // != NULL: the photometric mode (pose, gain, bias); final (alpha, beta) (host, 2n)
+  double* screen_ab = nullptr;           // k >= 1, photometric: (alpha, beta) where each screening run ended (host, 2nk)
+  int32_t* best = nullptr;               // k >= 1: the chosen hypothesis of each pair (host, n)
+  double* scores = nullptr;              // k >= 1: the score of each hypothesis (host, nk)
+  dvo_b200_result* screen_results = nullptr;   // k >= 1: the result of each screening run (host, nk)
+  dvo_b200_iteration_stats* iter_stats = nullptr;   // iteration logs (host, max_log per pair)
+  int max_log = 0;                       // entries per pair of iter_stats (ignored without it)
+  const dvo_b200_weight_maps* maps = nullptr;   // also the weight maps (weight_maps.cu) of the returned alignments
+};
+int tracker_match(dvo_b200_ctx* ctx, const MatchCall& c);
 int check_level_flags(dvo_b200_ctx* ctx);   // after a stream synchronisation: did a level kernel report a timeout?
-// dvo_b200_match_batch_hypotheses[_modes] after its argument checks (hypotheses_args.h): a leg screening n * k virtual pairs on
-// levels first .. screen_level, k_pick_hypotheses, and a leg continuing the n chosen ones on the levels below.  scores and
-// screen_results (host, n * k) may be NULL.  The modes as in tracker_match_batch, per hypothesis: prior (n * k * 36) and
-// ab_init (n * k * 2) per virtual pair, ab_out (n * 2) per pair, screen_ab (n * k * 2, or NULL) where each screening run
-// ended; maps of the continued alignments.
-int tracker_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
-                                   dvo_b200_pyramid* const* curs, int k, const double* hypotheses, int screen_level,
-                                   double min_ratio, dvo_b200_result* h_results, int32_t* h_best, double* h_scores,
-                                   dvo_b200_result* h_screen, dvo_b200_iteration_stats* iter_stats, int max_iter_stats,
-                                   const double* prior = nullptr, const double* ab_init = nullptr, double* ab_out = nullptr,
-                                   double* screen_ab = nullptr, const dvo_b200_weight_maps* maps = nullptr);
 // The test hooks: one iteration at T (staged as the leg's initial estimate and placed into the state by k_set_state).
 int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* ref, dvo_b200_pyramid* cur,
                       int level, const double* T, int use_weights, const float* prev_precision, int64_t* count,

@@ -1352,68 +1352,109 @@ int ensure_pinned_results(dvo_b200_ctx* ctx, size_t bytes) {
   return 0;
 }
 
-// Enqueue the copy of (alpha, beta) of the n brightness states at src (the pair slots of the leg the results come from)
-// to dst, 2 n doubles of the pinned results buffer
+// Enqueue the copy of (alpha, beta) of the n brightness states at src to dst, 2 n doubles of the pinned results buffer
 int copy_back_photometric(dvo_b200_ctx* ctx, void* dst, const AffineState* src, size_t n) {
   DVO_CUDA(ctx, cudaMemcpy2DAsync(dst, 2 * sizeof(double), src->ab, sizeof(AffineState), 2 * sizeof(double), n,
                                   cudaMemcpyDeviceToHost, ctx->stream));
-  ctx->d2h_bytes += sizeof(double) * 2 * n;
   return 0;
 }
 
 }  // namespace
 
-int tracker_match_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
-                        dvo_b200_pyramid* const* curs, const double* T_init, dvo_b200_result* h_results,
-                        void* d_results_user, dvo_b200_iteration_stats* iter_stats, int max_iter_stats, const double* ab_init,
-                        double* ab_out, const double* prior, const dvo_b200_weight_maps* maps) {
-  int rc = check_batch(ctx, cfg, n, refs, curs);
+// A match (k = 0) is one leg over levels first .. last of the n pairs.  A multi-hypothesis match (include/dvo_b200.h) is two:
+// the screening leg runs n k virtual pairs, pair p k + j being (refs[p], curs[p]) from H[p][j] (and Lambda[p][j],
+// (alpha, beta)_0[p][j]), on levels first .. s; k_pick_hypotheses scores them and copies each pair's chosen state (log,
+// AffineState, Lambda) into its slot of the continuation leg, which runs levels s-1 .. last (none if s = last) on the n
+// chosen pairs, its level indices continuing at first - s + 1.  Both legs launch the level kernel like any other match, so
+// plan independence gives each pair the bits of one plain match of its mode.  With maps the continuation leg also holds the
+// level-last descriptors of its pairs when it runs no level (s = last), so that k_weight_maps reads the descriptors, states
+// and AffineStates of the last leg whichever the call.  The device stage holds the results (n), screen results (n k, if
+// requested), scores (n k) and best (n; none of the three with k = 0), copied back through the pinned results buffer in
+// that layout, followed there at the next 16-byte boundary by (alpha, beta) of the n pairs and of the n k screening runs
+// (if requested).  A device-results call writes its results to d_results and uses neither.
+int tracker_match(dvo_b200_ctx* ctx, const MatchCall& c) {
+  const dvo_b200_config* const cfg = c.cfg;
+  dvo_b200_pyramid* const* const refs = c.refs;
+  dvo_b200_pyramid* const* const curs = c.curs;
+  int rc = check_batch(ctx, cfg, c.n, refs, curs);
   if (rc) return rc;
   LevelVariant v;
-  if ((rc = begin_call(ctx, cfg, n, refs, curs, ab_out != nullptr, prior != nullptr, v))) return rc;
+  if ((rc = begin_call(ctx, cfg, c.n, refs, curs, c.ab_out != nullptr, c.prior != nullptr, v))) return rc;
   cudaStream_t st = ctx->stream;
   Workspace& ws = ctx->ws;
-  const int last = cfg->last_level;
-  const int max_log = iter_stats ? max_iter_stats : 0;
-  const Leg leg = make_leg(ctx, nullptr, cfg->first_level, last, n, refs, curs, v);
-  if ((rc = ensure_workspace(ctx, &leg, 1, 0, max_log, v))) return rc;
-  if (maps && (rc = weight_maps_prepare(ctx, *maps, n, refs[0], last))) return rc;
-  const double* const tinit = cfg->use_initial_estimate ? T_init : nullptr;
-  if ((rc = stage_inputs(ctx, &leg, 1, tinit, ab_init, prior, max_log, v))) return rc;
-  for (int i = 0; i < leg.plan.nlaunch; ++i)
-    if ((rc = launch_segments(ctx, cfg, leg, i, tinit ? ws.d_tinit : nullptr, max_log, nullptr, 0, v))) return rc;
-  // results
-  dvo_b200_result* d_res = (dvo_b200_result*)d_results_user;
-  if (!d_res) {
-    size_t bytes = sizeof(dvo_b200_result) * n;
-    if ((rc = ensure_stage(ctx, bytes, 0))) return rc;
-    d_res = (dvo_b200_result*)ctx->d_stage;
+  const int n = c.n, k = c.k, nk = n * k, last = cfg->last_level;
+  const int max_log = c.iter_stats ? c.max_log : 0;
+  std::vector<dvo_b200_pyramid*> vrefs((size_t)nk), vcurs((size_t)nk);
+  for (int q = 0; q < nk; ++q) { vrefs[q] = refs[q / k]; vcurs[q] = curs[q / k]; }
+  Leg legs[2];
+  const int nlegs = k ? 2 : 1;
+  if (k) {
+    legs[0] = make_leg(ctx, nullptr, cfg->first_level, c.screen_level, nk, vrefs.data(), vcurs.data(), v);
+    legs[1] = make_leg(ctx, &legs[0], c.screen_level - 1, last, n, refs, curs, v, c.maps != nullptr);
+  } else {
+    legs[0] = make_leg(ctx, nullptr, cfg->first_level, last, n, refs, curs, v);
   }
-  finalize(ctx, ws.d_state, d_res, n);
-  if (maps)
-    weight_maps_launch(ctx, *maps, n, refs[0], last, ws.d_state + leg.pair0, ws.d_pair_level + leg.desc0 + leg.ndesc - n,
-                       v.affine ? ws.d_affine + leg.pair0 : nullptr);
-  // a device-results call leaves its level flags to dvo_b200_synchronize
-  if ((rc = end_call(ctx, n, refs, curs, leg.plan.nlaunch))) return rc;
-  if (h_results) {
-    size_t bytes = sizeof(dvo_b200_result) * n;
-    const size_t pinned = bytes + (v.affine ? sizeof(double) * 2 * (size_t)n : 0);   // the results, then (alpha, beta) of each pair
-    if ((rc = ensure_pinned_results(ctx, pinned))) return rc;
-    DVO_CUDA(ctx, cudaMemcpyAsync(ctx->h_results, d_res, bytes, cudaMemcpyDeviceToHost, st));
-    if (v.affine && (rc = copy_back_photometric(ctx, (char*)ctx->h_results + bytes, ws.d_affine + leg.pair0, (size_t)n))) return rc;
-    if (maps && (rc = weight_maps_copy_back(ctx, *maps, n, refs[0], last))) return rc;
-    if (iter_stats) {
-      DVO_CUDA(ctx, cudaMemcpyAsync(iter_stats, ws.d_iter_log, sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log,
-                                    cudaMemcpyDeviceToHost, st));
-      ctx->d2h_bytes += sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log;
+  const Leg& z = legs[nlegs - 1];   // the leg the results come from
+  if ((rc = ensure_workspace(ctx, legs, nlegs, 0, max_log, v))) return rc;
+  if (c.maps && (rc = weight_maps_prepare(ctx, *c.maps, n, refs[0], last))) return rc;
+
+  const size_t res_bytes = sizeof(dvo_b200_result) * (size_t)n;
+  const size_t screen_bytes = c.screen_results ? sizeof(dvo_b200_result) * (size_t)nk : 0, score_bytes = sizeof(double) * (size_t)nk;
+  const size_t scores_at = res_bytes + screen_bytes, best_at = scores_at + score_bytes;
+  const size_t out_bytes = best_at + (k ? sizeof(int32_t) * (size_t)n : 0);
+  const size_t ab_at = (out_bytes + 15) / 16 * 16, ab_bytes = v.affine ? sizeof(double) * 2 * (size_t)n : 0;
+  const size_t screen_ab_bytes = c.screen_ab ? sizeof(double) * 2 * (size_t)nk : 0;
+  if (!c.d_results) {
+    if ((rc = ensure_stage(ctx, out_bytes, 0))) return rc;
+    if ((rc = ensure_pinned_results(ctx, ab_at + ab_bytes + screen_ab_bytes))) return rc;
+  }
+  const double* const tinit = cfg->use_initial_estimate ? c.T_init : nullptr;
+  if ((rc = stage_inputs(ctx, legs, nlegs, tinit, c.ab_init, c.prior, max_log, v))) return rc;
+  for (int i = 0; i < legs[0].plan.nlaunch; ++i)
+    if ((rc = launch_segments(ctx, cfg, legs[0], i, tinit ? ws.d_tinit : nullptr, max_log, nullptr, 0, v))) return rc;
+  char* const d_out = (char*)ctx->d_stage;
+  dvo_b200_result* const d_res = c.d_results ? (dvo_b200_result*)c.d_results : (dvo_b200_result*)d_out;
+  if (k) {
+    const Leg &screen = legs[0], &chosen = legs[1];
+    if (c.screen_results) finalize(ctx, ws.d_state, (dvo_b200_result*)(d_out + res_bytes), nk);
+    {
+      ProfScope prof(ctx, 2);
+      auto pick = v.affine ? (v.prior ? k_pick_hypotheses<true, true> : k_pick_hypotheses<true, false>)
+                           : (v.prior ? k_pick_hypotheses<false, true> : k_pick_hypotheses<false, false>);
+      pick<<<(n + 3) / 4, 128, 0, st>>>(ws.d_state, ws.d_iter_log, ws.d_state + chosen.pair0, ws.d_iter_log + chosen.pair0 * max_log,
+                                        max_log, n, k, screen.first - screen.last, c.min_ratio, (double*)(d_out + scores_at),
+                                        (int*)(d_out + best_at), v.affine ? ws.d_affine : nullptr,
+                                        v.affine ? ws.d_affine + chosen.pair0 : nullptr, v.prior ? ws.d_prior : nullptr,
+                                        v.prior ? ws.d_prior + 36 * chosen.pair0 : nullptr);
+      ctx->launches++;
     }
-    DVO_CUDA(ctx, cudaStreamSynchronize(st));
-    std::memcpy(h_results, ctx->h_results, bytes);
-    if (v.affine) std::memcpy(ab_out, (char*)ctx->h_results + bytes, sizeof(double) * 2 * (size_t)n);
-    ctx->d2h_bytes += bytes;
-    return check_level_flags(ctx);
+    for (int i = 0; i < chosen.plan.nlaunch; ++i)
+      if ((rc = launch_segments(ctx, cfg, chosen, i, nullptr, max_log, nullptr, 0, v))) return rc;
   }
-  return 0;
+  finalize(ctx, ws.d_state + z.pair0, d_res, n);
+  if (c.maps)
+    weight_maps_launch(ctx, *c.maps, n, refs[0], last, ws.d_state + z.pair0, ws.d_pair_level + z.desc0 + z.ndesc - n,
+                       v.affine ? ws.d_affine + z.pair0 : nullptr);
+  if ((rc = end_call(ctx, n, refs, curs, z.flag0 + z.plan.nlaunch))) return rc;
+  if (c.d_results) return 0;   // a device-results call leaves its level flags to dvo_b200_synchronize
+
+  char* const hr = (char*)ctx->h_results;
+  const size_t log_bytes = sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log;
+  DVO_CUDA(ctx, cudaMemcpyAsync(hr, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
+  if (ab_bytes && (rc = copy_back_photometric(ctx, hr + ab_at, ws.d_affine + z.pair0, (size_t)n))) return rc;
+  if (screen_ab_bytes && (rc = copy_back_photometric(ctx, hr + ab_at + ab_bytes, ws.d_affine, (size_t)nk))) return rc;
+  if (c.maps && (rc = weight_maps_copy_back(ctx, *c.maps, n, refs[0], last))) return rc;
+  if (log_bytes)
+    DVO_CUDA(ctx, cudaMemcpyAsync(c.iter_stats, ws.d_iter_log + z.pair0 * max_log, log_bytes, cudaMemcpyDeviceToHost, st));
+  ctx->d2h_bytes += out_bytes + ab_bytes + screen_ab_bytes + log_bytes;
+  DVO_CUDA(ctx, cudaStreamSynchronize(st));
+  std::memcpy(c.results, hr, res_bytes);
+  if (screen_bytes) std::memcpy(c.screen_results, hr + res_bytes, screen_bytes);
+  if (c.scores) std::memcpy(c.scores, hr + scores_at, score_bytes);
+  if (k) std::memcpy(c.best, hr + best_at, out_bytes - best_at);
+  if (ab_bytes) std::memcpy(c.ab_out, hr + ab_at, ab_bytes);
+  if (screen_ab_bytes) std::memcpy(c.screen_ab, hr + ab_at + ab_bytes, screen_ab_bytes);
+  return check_level_flags(ctx);
 }
 
 // The persistent kernels report a barrier / transaction timeout through a flag copied to pinned memory after every level.
@@ -1482,93 +1523,6 @@ int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_py
     ctx->d2h_bytes += sizeof(float) * 7 * (size_t)L.n;
   }
   return 0;
-}
-
-
-// dvo_b200_match_batch_hypotheses[_modes] (include/dvo_b200.h), as two legs.  The screening leg runs n k virtual pairs, pair
-// p k + j being (refs[p], curs[p]) from H[p][j] (and Lambda[p][j], (alpha, beta)_0[p][j]), on levels first .. s;
-// k_pick_hypotheses scores them and copies each pair's chosen state (log, AffineState, Lambda) into its slot of the
-// continuation leg, which runs levels s-1 .. last (none if s = last) on the n chosen pairs, its level indices continuing at
-// first - s + 1.  Both legs launch the level kernel like any other match, so plan independence gives each pair the bits of
-// one dvo_b200_match_batch[_photometric, _prior].  With maps the continuation leg also holds the level-last descriptors of
-// its pairs when it runs no level (s = last), so that k_weight_maps reads the descriptors, states and AffineStates of one
-// leg as after a match.  The device stage holds the results (n), screen results (n k, if requested), scores (n k) and best
-// (n), copied back through the pinned results buffer in that layout, followed there by (alpha, beta) of the n continued
-// pairs and of the n k screening runs (if requested).
-int tracker_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
-                                   dvo_b200_pyramid* const* curs, int k, const double* hypotheses, int screen_level,
-                                   double min_ratio, dvo_b200_result* h_results, int32_t* h_best, double* h_scores,
-                                   dvo_b200_result* h_screen, dvo_b200_iteration_stats* iter_stats, int max_iter_stats,
-                                   const double* prior, const double* ab_init, double* ab_out, double* screen_ab,
-                                   const dvo_b200_weight_maps* maps) {
-  int rc = check_batch(ctx, cfg, n, refs, curs);
-  if (rc) return rc;
-  LevelVariant v;
-  if ((rc = begin_call(ctx, cfg, n, refs, curs, ab_out != nullptr, prior != nullptr, v))) return rc;
-  cudaStream_t st = ctx->stream;
-  Workspace& ws = ctx->ws;
-  const int s = screen_level, nk = n * k, last = cfg->last_level;
-  const int max_log = iter_stats ? max_iter_stats : 0;
-  std::vector<dvo_b200_pyramid*> vrefs((size_t)nk), vcurs((size_t)nk);
-  for (int q = 0; q < nk; ++q) { vrefs[q] = refs[q / k]; vcurs[q] = curs[q / k]; }
-  Leg legs[2];
-  legs[0] = make_leg(ctx, nullptr, cfg->first_level, s, nk, vrefs.data(), vcurs.data(), v);
-  legs[1] = make_leg(ctx, &legs[0], s - 1, last, n, refs, curs, v, maps != nullptr);
-  const Leg &screen = legs[0], &chosen = legs[1];
-  if ((rc = ensure_workspace(ctx, legs, 2, 0, max_log, v))) return rc;
-  if (maps && (rc = weight_maps_prepare(ctx, *maps, n, refs[0], last))) return rc;
-
-  const size_t res_bytes = sizeof(dvo_b200_result) * (size_t)n, screen_bytes = h_screen ? sizeof(dvo_b200_result) * (size_t)nk : 0;
-  const size_t score_bytes = sizeof(double) * (size_t)nk, out_bytes = res_bytes + screen_bytes + score_bytes + sizeof(int) * (size_t)n;
-  const size_t ab_at = (out_bytes + 15) / 16 * 16, ab_bytes = v.affine ? sizeof(double) * 2 * (size_t)n : 0;
-  const size_t screen_ab_bytes = screen_ab ? sizeof(double) * 2 * (size_t)nk : 0;
-  if ((rc = ensure_stage(ctx, out_bytes, 0))) return rc;
-  if ((rc = ensure_pinned_results(ctx, ab_at + ab_bytes + screen_ab_bytes))) return rc;
-  if ((rc = stage_inputs(ctx, legs, 2, hypotheses, ab_init, prior, max_log, v))) return rc;
-  for (int i = 0; i < screen.plan.nlaunch; ++i)
-    if ((rc = launch_segments(ctx, cfg, screen, i, ws.d_tinit, max_log, nullptr, 0, v))) return rc;
-  char* const d_out = (char*)ctx->d_stage;
-  dvo_b200_result* const d_res = (dvo_b200_result*)d_out;
-  double* const d_scores = (double*)(d_out + res_bytes + screen_bytes);
-  int* const d_best = (int*)(d_out + res_bytes + screen_bytes + score_bytes);
-  if (h_screen) finalize(ctx, ws.d_state, (dvo_b200_result*)(d_out + res_bytes), nk);
-  {
-    ProfScope prof(ctx, 2);
-    auto pick = v.affine ? (v.prior ? k_pick_hypotheses<true, true> : k_pick_hypotheses<true, false>)
-                         : (v.prior ? k_pick_hypotheses<false, true> : k_pick_hypotheses<false, false>);
-    pick<<<(n + 3) / 4, 128, 0, st>>>(ws.d_state, ws.d_iter_log, ws.d_state + chosen.pair0, ws.d_iter_log + chosen.pair0 * max_log,
-                                      max_log, n, k, screen.first - screen.last, min_ratio, d_scores, d_best,
-                                      v.affine ? ws.d_affine : nullptr, v.affine ? ws.d_affine + chosen.pair0 : nullptr,
-                                      v.prior ? ws.d_prior : nullptr, v.prior ? ws.d_prior + 36 * chosen.pair0 : nullptr);
-    ctx->launches++;
-  }
-  for (int i = 0; i < chosen.plan.nlaunch; ++i)
-    if ((rc = launch_segments(ctx, cfg, chosen, i, nullptr, max_log, nullptr, 0, v))) return rc;
-  finalize(ctx, ws.d_state + chosen.pair0, d_res, n);
-  if (maps)
-    weight_maps_launch(ctx, *maps, n, refs[0], last, ws.d_state + chosen.pair0, ws.d_pair_level + chosen.desc0 + chosen.ndesc - n,
-                       v.affine ? ws.d_affine + chosen.pair0 : nullptr);
-  if ((rc = end_call(ctx, n, refs, curs, screen.plan.nlaunch + chosen.plan.nlaunch))) return rc;
-
-  char* const hr = (char*)ctx->h_results;
-  DVO_CUDA(ctx, cudaMemcpyAsync(hr, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
-  ctx->d2h_bytes += out_bytes;
-  if (v.affine && (rc = copy_back_photometric(ctx, hr + ab_at, ws.d_affine + chosen.pair0, (size_t)n))) return rc;
-  if (screen_ab && (rc = copy_back_photometric(ctx, hr + ab_at + ab_bytes, ws.d_affine + screen.pair0, (size_t)nk))) return rc;
-  if (maps && (rc = weight_maps_copy_back(ctx, *maps, n, refs[0], last))) return rc;
-  if (iter_stats) {
-    DVO_CUDA(ctx, cudaMemcpyAsync(iter_stats, ws.d_iter_log + chosen.pair0 * max_log,
-                                  sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log, cudaMemcpyDeviceToHost, st));
-    ctx->d2h_bytes += sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log;
-  }
-  DVO_CUDA(ctx, cudaStreamSynchronize(st));
-  std::memcpy(h_results, hr, res_bytes);
-  if (h_screen) std::memcpy(h_screen, hr + res_bytes, screen_bytes);
-  if (h_scores) std::memcpy(h_scores, hr + res_bytes + screen_bytes, score_bytes);
-  std::memcpy(h_best, hr + res_bytes + screen_bytes + score_bytes, sizeof(int) * (size_t)n);
-  if (v.affine) std::memcpy(ab_out, hr + ab_at, ab_bytes);
-  if (screen_ab) std::memcpy(screen_ab, hr + ab_at + ab_bytes, screen_ab_bytes);
-  return check_level_flags(ctx);
 }
 
 }  // namespace dvo_b200
