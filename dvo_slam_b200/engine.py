@@ -7,6 +7,7 @@ CUDA device is present, construction raises.
 from __future__ import annotations
 
 import ctypes as C
+import operator
 import os
 import weakref
 
@@ -177,6 +178,45 @@ def _mask_roles(mask_roles) -> int:
     if mask_roles not in MASK_ROLES:
         raise ValueError(f"unknown mask_roles {mask_roles!r}: one of {sorted(MASK_ROLES)}")
     return MASK_ROLES[mask_roles]
+
+
+_DP = C.POINTER(C.c_double)
+
+
+def _ptr(a, ptype=_DP):
+    """a numpy array as a C pointer, None as NULL"""
+    return a.ctypes.data_as(ptype) if a is not None else None
+
+
+def _rows(a, name, want, width):
+    """An optional float64 input of shape want (per pair or per hypothesis) as C-contiguous rows of width values; None
+    stays None.  Any other number of values raises ValueError."""
+    if a is None:
+        return None
+    A = np.asarray(a, dtype=np.float64)
+    if A.size != int(np.prod(want)):
+        raise ValueError(f"{name} {A.shape}: want {list(want)}")
+    return np.ascontiguousarray(A.reshape(-1, width))
+
+
+def _photometric_init(photometric, photometric_init, want):
+    """the (alpha, beta)_0 rows of the photometric mode, None = (1, 0); refused without the mode"""
+    if photometric_init is not None and not photometric:
+        raise ValueError("photometric_init without photometric=True")
+    return _rows(photometric_init, "photometric_init", want, 2)
+
+
+def _handles(pyramids, attr="handle"):
+    """the C array of n pyramid handles: Pyramid.handle, or attr="value" for ShardedEngine's c_void_p handles"""
+    return (C.c_void_p * len(pyramids))(*map(operator.attrgetter(attr), pyramids))
+
+
+def _iteration_log(cfg, n, with_iterations):
+    """(log, max_log): room for every iteration of levels cfg.first_level .. cfg.last_level per pair, or (None, 0)"""
+    if not with_iterations:
+        return None, 0
+    max_log = (cfg.first_level - cfg.last_level + 1) * (cfg.max_iterations_per_level + 1)
+    return (IterationStats * (n * max_log))(), max_log
 
 
 class IterationStats(C.Structure):
@@ -549,80 +589,70 @@ class Engine:
     # pointer (int) to n*h*w bytes.
     # mask_roles="reference" (default): the mask keeps its pixels out of the point selection; "both": also out of the
     # bilinear taps when the pyramid is the current image of an alignment (dvo_b200_pyramid_create_masked_batch_roles).
-    def _create_masked(self, n, fmt, pI, pZ, depth_scale, masks, w, h, intrinsics, levels, mask_roles="reference") -> list[Pyramid]:
-        roles = _mask_roles(mask_roles)
-        pM, M = _host_masks(masks, n, h, w)
-        fx, fy, ox, oy = intrinsics
+    def _create_host(self, fmt, n, h, w, pI, pZ, depth_scale, masks, mask_roles, levels, intrinsics=None, remap=None, single=False,
+                     sync=False) -> list[Pyramid]:
+        """Every create from host memory: n images of h x w in format fmt at pI / pZ.  remap = (rectifier, registration):
+        dvo_b200_pyramid_create_rectified_batch (registration None) or _registered_batch, which take the masks themselves.
+        Otherwise masks -> dvo_b200_pyramid_create_masked_batch_roles, without masks the plain entry point of the format
+        (single: the one-image form).  Synchronises when the masks were converted (except a remapped create) and, with
+        sync, when the caller's staged arrays die with the call."""
+        roles = _mask_roles(mask_roles) if masks is not None or remap is not None else None
+        pM, M = _host_masks(masks, n, h, w) if masks is not None else (None, None)   # M: kept until the upload is done
+        f = INPUT_FORMATS[fmt]
         out = (C.c_void_p * n)()
-        self._check(self.lib.dvo_b200_pyramid_create_masked_batch_roles(self.ctx, n, INPUT_FORMATS[fmt], pI, pZ, depth_scale, pM,
-                                                                        roles, w, h, fx, fy, ox, oy, levels, out))
-        if M is not None and M is not masks:
-            self.synchronize()   # the converted copy dies with this call
+        if remap is not None:
+            rect, reg = remap
+            rh = rect.handle if rect is not None else None
+            args = (n, f, pI, pZ, depth_scale, pM, roles, w, h, levels, out)
+            if reg is None:
+                rc = self.lib.dvo_b200_pyramid_create_rectified_batch(self.ctx, rh, *args)
+            else:
+                rc = self.lib.dvo_b200_pyramid_create_registered_batch(self.ctx, reg.handle, rh, *args)
+        else:
+            fx, fy, ox, oy = intrinsics
+            if masks is not None:
+                rc = self.lib.dvo_b200_pyramid_create_masked_batch_roles(self.ctx, n, f, pI, pZ, depth_scale, pM, roles, w, h, fx, fy,
+                                                                         ox, oy, levels, out)
+            else:
+                entry = {("float32", True): "create", ("float32", False): "create_batch", ("grey8_depth16", True): "create_raw",
+                         ("grey8_depth16", False): "create_raw_batch", ("bgr8_depth16", False): "create_bgr_batch"}[fmt, single]
+                args = (() if single else (n,)) + (pI, pZ) + (() if fmt == "float32" else (depth_scale,))
+                rc = getattr(self.lib, "dvo_b200_pyramid_" + entry)(self.ctx, *args, w, h, fx, fy, ox, oy, levels, out)
+        self._check(rc)
+        if M is not None and M is not masks and remap is None:
+            self.synchronize()   # the converted masks die with this call
+        if sync:
+            self.synchronize()   # so may the caller's staged arrays
         return [Pyramid(self, out[i]) for i in range(n)]
 
     def pyramid(self, intensity, depth, intrinsics, levels: int, mask=None, mask_roles="reference") -> Pyramid:
         I = np.ascontiguousarray(intensity, dtype=np.float32)
         Z = np.ascontiguousarray(depth, dtype=np.float32)
         assert I.ndim == 2 and I.shape == Z.shape
-        h, w = I.shape
-        if mask is not None:
-            p = self._create_masked(1, "float32", I.ctypes.data, Z.ctypes.data, 0.0, mask, w, h, intrinsics, levels, mask_roles)[0]
-            self.synchronize()
-            return p
-        fx, fy, ox, oy = intrinsics
-        out = C.c_void_p()
-        self._check(self.lib.dvo_b200_pyramid_create(self.ctx, I.ctypes.data, Z.ctypes.data, w, h, fx, fy, ox, oy, levels, C.byref(out)))
-        self.synchronize()  # numpy temporaries may die
-        return Pyramid(self, out.value)
+        return self._create_host("float32", 1, *I.shape, I.ctypes.data, Z.ctypes.data, 0.0, mask, mask_roles, levels, intrinsics,
+                                 single=True, sync=True)[0]
 
     def pyramid_batch(self, intensity, depth, intrinsics, levels: int, host_ptrs=None, masks=None, mask_roles="reference") -> list[Pyramid]:
         """intensity/depth: [n,h,w] float32 arrays, or (ptr_I, ptr_Z, n, h, w) raw host pointers via host_ptrs."""
-        if masks is not None:
-            if host_ptrs is not None:
-                pI, pZ, n, h, w = host_ptrs
-                return self._create_masked(n, "float32", pI, pZ, 0.0, masks, w, h, intrinsics, levels, mask_roles)
-            I = np.ascontiguousarray(intensity, dtype=np.float32)
-            Z = np.ascontiguousarray(depth, dtype=np.float32)
-            assert I.ndim == 3 and I.shape == Z.shape
-            n, h, w = I.shape
-            out = self._create_masked(n, "float32", I.ctypes.data, Z.ctypes.data, 0.0, masks, w, h, intrinsics, levels, mask_roles)
-            self.synchronize()
-            return out
         if host_ptrs is not None:
             pI, pZ, n, h, w = host_ptrs
         else:
             I = np.ascontiguousarray(intensity, dtype=np.float32)
             Z = np.ascontiguousarray(depth, dtype=np.float32)
             assert I.ndim == 3 and I.shape == Z.shape
-            n, h, w = I.shape
-            pI, pZ = I.ctypes.data, Z.ctypes.data
-        fx, fy, ox, oy = intrinsics
-        out = (C.c_void_p * n)()
-        self._check(self.lib.dvo_b200_pyramid_create_batch(self.ctx, n, pI, pZ, w, h, fx, fy, ox, oy, levels, out))
-        if host_ptrs is None:
-            self.synchronize()
-        return [Pyramid(self, out[i]) for i in range(n)]
+            (n, h, w), pI, pZ = I.shape, I.ctypes.data, Z.ctypes.data
+        return self._create_host("float32", n, h, w, pI, pZ, 0.0, masks, mask_roles, levels, intrinsics, sync=host_ptrs is None)
 
     def pyramid_raw_batch(self, host_ptrs, depth_scale, intrinsics, levels: int, masks=None, mask_roles="reference") -> list[Pyramid]:
         """host_ptrs = (ptr_grey_u8, ptr_depth_u16, n, h, w): n consecutive raw images in (pinned) host memory."""
         pG, pD, n, h, w = host_ptrs
-        if masks is not None:
-            return self._create_masked(n, "grey8_depth16", pG, pD, depth_scale, masks, w, h, intrinsics, levels, mask_roles)
-        fx, fy, ox, oy = intrinsics
-        out = (C.c_void_p * n)()
-        self._check(self.lib.dvo_b200_pyramid_create_raw_batch(self.ctx, n, pG, pD, depth_scale, w, h, fx, fy, ox, oy, levels, out))
-        return [Pyramid(self, out[i]) for i in range(n)]
+        return self._create_host("grey8_depth16", n, h, w, pG, pD, depth_scale, masks, mask_roles, levels, intrinsics)
 
     def pyramid_bgr_batch(self, host_ptrs, depth_scale, intrinsics, levels: int, masks=None, mask_roles="reference") -> list[Pyramid]:
         """host_ptrs = (ptr_bgr_u8x3, ptr_depth_u16, n, h, w): n consecutive interleaved-BGR images and raw depth images
         in (pinned) host memory; grey conversion (OpenCV BGR2GRAY) and depth scaling run on the device."""
         pC, pD, n, h, w = host_ptrs
-        if masks is not None:
-            return self._create_masked(n, "bgr8_depth16", pC, pD, depth_scale, masks, w, h, intrinsics, levels, mask_roles)
-        fx, fy, ox, oy = intrinsics
-        out = (C.c_void_p * n)()
-        self._check(self.lib.dvo_b200_pyramid_create_bgr_batch(self.ctx, n, pC, pD, depth_scale, w, h, fx, fy, ox, oy, levels, out))
-        return [Pyramid(self, out[i]) for i in range(n)]
+        return self._create_host("bgr8_depth16", n, h, w, pC, pD, depth_scale, masks, mask_roles, levels, intrinsics)
 
     def pyramid_batch_device(self, image, depth, intrinsics, levels: int, depth_scale=None, masks=None,
                              mask_roles="reference") -> list[Pyramid]:
@@ -709,16 +739,8 @@ class Engine:
                     self.ctx, reg.handle, rh, n, fmt, I, Z, scale, M, roles, w, h, levels, out)
             return self._create_device(image, depth, masks, depth_scale, depth_size, create)
         fmt, (n, h, w), I, Z = _host_frames(image, depth, depth_size)
-        scale = _depth_scale(fmt, depth_scale)
-        pM, M = _host_masks(masks, n, h, w) if masks is not None else (None, None)   # M: kept until the upload is done
-        args = (n, INPUT_FORMATS[fmt], I.ctypes.data, Z.ctypes.data, scale, pM, roles, w, h, levels)
-        out = (C.c_void_p * n)()
-        if reg is None:
-            self._check(self.lib.dvo_b200_pyramid_create_rectified_batch(self.ctx, rh, *args, out))
-        else:
-            self._check(self.lib.dvo_b200_pyramid_create_registered_batch(self.ctx, reg.handle, rh, *args, out))
-        self.synchronize()   # the staged host arrays may die with this call
-        return [Pyramid(self, out[i]) for i in range(n)]
+        return self._create_host(fmt, n, h, w, I.ctypes.data, Z.ctypes.data, _depth_scale(fmt, depth_scale), masks, mask_roles, levels,
+                                 remap=(rect, reg), sync=True)
 
     # ---- unregistered depth ----
     depth_rays = staticmethod(depth_rays)
@@ -759,18 +781,8 @@ class Engine:
         G = np.ascontiguousarray(grey_u8, dtype=np.uint8)
         D = np.ascontiguousarray(depth_u16, dtype=np.uint16)
         assert G.ndim == 2 and G.shape == D.shape
-        h, w = G.shape
-        if mask is not None:
-            p = self._create_masked(1, "grey8_depth16", G.ctypes.data, D.ctypes.data, depth_scale, mask, w, h, intrinsics, levels,
-                                    mask_roles)[0]
-            self.synchronize()
-            return p
-        fx, fy, ox, oy = intrinsics
-        out = C.c_void_p()
-        self._check(self.lib.dvo_b200_pyramid_create_raw(self.ctx, G.ctypes.data, D.ctypes.data, depth_scale, w, h, fx, fy, ox, oy,
-                                                         levels, C.byref(out)))
-        self.synchronize()
-        return Pyramid(self, out.value)
+        return self._create_host("grey8_depth16", 1, *G.shape, G.ctypes.data, D.ctypes.data, depth_scale, mask, mask_roles, levels,
+                                 intrinsics, single=True, sync=True)[0]
 
     # ---- alignment ----
     def match(self, ref: Pyramid, cur: Pyramid, cfg: Config, T_init=None, with_iterations: bool = False) -> Result:
@@ -781,13 +793,7 @@ class Engine:
         """match_batch in the photometric mode (include/dvo_b200.h): the pose and an intensity gain and bias per pair.
         photometric_init: [n, 2] (alpha, beta) or None = (1, 0).  prior_information as in match_batch.  Returns (results,
         [n, 2] float64 final (alpha, beta))."""
-        n = len(refs)
-        ab0 = None
-        if photometric_init is not None:
-            ab0 = np.ascontiguousarray(np.asarray(photometric_init, dtype=np.float64).reshape(n, 2))
-        ab = np.zeros((n, 2), dtype=np.float64)
-        out = self.match_batch(refs, curs, cfg, T_init, with_iterations, _photometric=(ab0, ab), prior_information=prior_information)
-        return out, ab
+        return self._match(refs, curs, cfg, T_init, with_iterations, prior_information, True, photometric_init)
 
     def _device_maps(self, refs, cfg: Config, mask_weight):
         """The torch CUDA tensors of match_batch_maps and the WeightMaps that points at them, with the engine's stream ordered
@@ -827,62 +833,39 @@ class Engine:
         "precision" [n, 2, 2] float32 and, with mask_weight, "mask" [n, h, w] uint8 at level 0: 0 where the pixel's level-L
         parent is a constraint with weight < mask_weight, 1 elsewhere -- the masks= of pyramid_batch_device.  The pyramids of
         one call must share their size (ValueError otherwise)."""
-        n = len(refs)
         maps, wm = self._device_maps(refs, cfg, mask_weight)
-        ab0 = ab = None
-        if photometric:
-            if photometric_init is not None:
-                ab0 = np.ascontiguousarray(np.asarray(photometric_init, dtype=np.float64).reshape(n, 2))
-            ab = np.zeros((n, 2), dtype=np.float64)
-        elif photometric_init is not None:
-            raise ValueError("photometric_init without photometric=True")
-        res = self.match_batch(refs, curs, cfg, T_init, with_iterations, _photometric=(ab0, ab) if photometric else None,
-                               prior_information=prior_information, _maps=wm)
+        res, ab = self._match(refs, curs, cfg, T_init, with_iterations, prior_information, photometric, photometric_init, wm)
         return (res, maps, ab) if photometric else (res, maps)
 
-    def match_batch(self, refs, curs, cfg: Config, T_init=None, with_iterations: bool = False, raw: bool = False, _photometric=None,
-                    prior_information=None, _maps=None):
+    def match_batch(self, refs, curs, cfg: Config, T_init=None, with_iterations: bool = False, raw: bool = False, prior_information=None):
         """prior_information: [n, 6, 6] float64, a motion prior per pair in place of cfg.mu I (dvo_b200_match_batch_prior,
         which requires cfg.mu == 0); prior_from_result builds one from an earlier Result."""
+        return self._match(refs, curs, cfg, T_init, with_iterations, prior_information, raw=raw)[0]
+
+    def _match(self, refs, curs, cfg: Config, T_init, with_iterations, prior_information=None, photometric=False,
+               photometric_init=None, maps=None, raw=False):
+        """One n-pair alignment through dvo_b200_match_batch_maps (maps: a WeightMaps), _prior (prior_information),
+        _photometric or dvo_b200_match_batch -> (results, or the CResult array with raw, and [n, 2] (alpha, beta) or None)"""
         n = len(refs)
         assert n == len(curs) and n > 0
-        rh = (C.c_void_p * n)(*[p.handle for p in refs])
-        ch = (C.c_void_p * n)(*[p.handle for p in curs])
-        T = None
-        if T_init is not None:
-            T = np.ascontiguousarray(np.asarray(T_init, dtype=np.float64).reshape(n, 16))
+        rh, ch = _handles(refs), _handles(curs)
+        T = _rows(T_init, "T_init", (n, 4, 4), 16)
+        ab0 = _photometric_init(photometric, photometric_init, (n, 2))
+        ab = np.zeros((n, 2), dtype=np.float64) if photometric else None
+        lam = _rows(prior_information, "prior_information", (n, 6, 6), 36)
         res = (CResult * n)()
-        max_log = 0
-        log = None
-        if with_iterations:
-            max_log = (cfg.first_level - cfg.last_level + 1) * (cfg.max_iterations_per_level + 1)
-            log = (IterationStats * (n * max_log))()
-        dp = C.POINTER(C.c_double)
-        Tp = T.ctypes.data_as(dp) if T is not None else None
-        ab0, ab = _photometric if _photometric is not None else (None, None)
-        ab0p = ab0.ctypes.data_as(dp) if ab0 is not None else None
-        lam = None
-        if prior_information is not None:
-            lam = np.asarray(prior_information, dtype=np.float64)
-            if lam.size != 36 * n:
-                raise ValueError(f"prior_information {lam.shape}: want [{n}, 6, 6]")
-            lam = np.ascontiguousarray(lam.reshape(n, 36))
-        if _maps is not None:
-            self._check(self.lib.dvo_b200_match_batch_maps(
-                self.ctx, C.byref(cfg), n, rh, ch, Tp, lam.ctypes.data_as(dp) if lam is not None else None, ab0p,
-                ab.ctypes.data_as(dp) if ab is not None else None, res, log, max_log, C.byref(_maps)))
+        log, max_log = _iteration_log(cfg, n, with_iterations)
+        head = (self.ctx, C.byref(cfg), n, rh, ch, _ptr(T))
+        if maps is not None:
+            rc = self.lib.dvo_b200_match_batch_maps(*head, _ptr(lam), _ptr(ab0), _ptr(ab), res, log, max_log, C.byref(maps))
         elif lam is not None:
-            self._check(self.lib.dvo_b200_match_batch_prior(
-                self.ctx, C.byref(cfg), n, rh, ch, Tp, lam.ctypes.data_as(dp), ab0p, ab.ctypes.data_as(dp) if ab is not None else None,
-                res, log, max_log))
-        elif _photometric is None:
-            self._check(self.lib.dvo_b200_match_batch(self.ctx, C.byref(cfg), n, rh, ch, Tp, res, log, max_log))
+            rc = self.lib.dvo_b200_match_batch_prior(*head, _ptr(lam), _ptr(ab0), _ptr(ab), res, log, max_log)
+        elif photometric:
+            rc = self.lib.dvo_b200_match_batch_photometric(*head, _ptr(ab0), res, _ptr(ab), log, max_log)
         else:
-            self._check(self.lib.dvo_b200_match_batch_photometric(self.ctx, C.byref(cfg), n, rh, ch, Tp, ab0p, res, ab.ctypes.data_as(dp),
-                                                                  log, max_log))
-        if raw:
-            return res
-        return _results(res, n, log, max_log)
+            rc = self.lib.dvo_b200_match_batch(*head, res, log, max_log)
+        self._check(rc)
+        return (res if raw else _results(res, n, log, max_log)), ab
 
     def match_batch_hypotheses(self, refs, curs, hypotheses, screen_level: int, min_constraint_ratio: float = 0.0,
                                cfg: Config | None = None, with_iterations: bool = False, screen_results: bool = False,
@@ -909,43 +892,23 @@ class Engine:
         if H.ndim != 4 or H.shape[0] != n or H.shape[2:] != (4, 4):
             raise ValueError(f"hypotheses {H.shape}: want [{n}, k, 4, 4]")
         k = H.shape[1]
-        H = np.ascontiguousarray(H.reshape(n * k, 16))
-        lam = ab0 = ab = screen_ab = None
-        if prior_information is not None:
-            lam = np.asarray(prior_information, dtype=np.float64)
-            if lam.size != 36 * n * k:
-                raise ValueError(f"prior_information {lam.shape}: want [{n}, {k}, 6, 6]")
-            lam = np.ascontiguousarray(lam.reshape(n * k, 36))
-        if photometric:
-            if photometric_init is not None:
-                ab0 = np.asarray(photometric_init, dtype=np.float64)
-                if ab0.size != 2 * n * k:
-                    raise ValueError(f"photometric_init {ab0.shape}: want [{n}, {k}, 2]")
-                ab0 = np.ascontiguousarray(ab0.reshape(n * k, 2))
-            ab = np.zeros((n, 2), dtype=np.float64)
-            if screen_results:
-                screen_ab = np.zeros((n, k, 2), dtype=np.float64)
-        elif photometric_init is not None:
-            raise ValueError("photometric_init without photometric=True")
+        H = _rows(H, "hypotheses", H.shape, 16)
+        lam = _rows(prior_information, "prior_information", (n, k, 6, 6), 36)
+        ab0 = _photometric_init(photometric, photometric_init, (n, k, 2))
+        ab = np.zeros((n, 2), dtype=np.float64) if photometric else None
+        screen_ab = np.zeros((n, k, 2), dtype=np.float64) if photometric and screen_results else None
         dmaps = wm = None
         if maps or mask_weight is not None:
             dmaps, wm = self._device_maps(refs, cfg, mask_weight)
-        rh = (C.c_void_p * n)(*[p.handle for p in refs])
-        ch = (C.c_void_p * n)(*[p.handle for p in curs])
         res = (CResult * n)()
         best = np.zeros(n, dtype=np.int32)
         scores = np.zeros((n, k), dtype=np.float64)
         screen = (CResult * (n * k))() if screen_results else None
-        max_log, log = 0, None
-        if with_iterations:
-            max_log = (cfg.first_level - cfg.last_level + 1) * (cfg.max_iterations_per_level + 1)
-            log = (IterationStats * (n * max_log))()
-        dp = C.POINTER(C.c_double)
-        ptr = lambda a: a.ctypes.data_as(dp) if a is not None else None
+        log, max_log = _iteration_log(cfg, n, with_iterations)
         self._check(self.lib.dvo_b200_match_batch_hypotheses_modes(
-            self.ctx, C.byref(cfg), n, rh, ch, k, H.ctypes.data_as(dp), int(screen_level), float(min_constraint_ratio), ptr(lam),
-            ptr(ab0), ptr(ab), ptr(screen_ab), res, best.ctypes.data_as(C.POINTER(C.c_int32)), scores.ctypes.data_as(dp), screen,
-            log, max_log, C.byref(wm) if wm is not None else None))
+            self.ctx, C.byref(cfg), n, _handles(refs), _handles(curs), k, _ptr(H), int(screen_level), float(min_constraint_ratio),
+            _ptr(lam), _ptr(ab0), _ptr(ab), _ptr(screen_ab), res, _ptr(best, C.POINTER(C.c_int32)), _ptr(scores), screen, log, max_log,
+            C.byref(wm) if wm is not None else None))
         out = (_results(res, n, log, max_log), best, scores)
         if screen_results:
             flat = [Result(screen[i]) for i in range(n * k)]
@@ -958,29 +921,21 @@ class Engine:
 
     def match_batch_device(self, refs, curs, cfg: Config, d_results_ptr: int, T_init=None):
         n = len(refs)
-        rh = (C.c_void_p * n)(*[p.handle for p in refs])
-        ch = (C.c_void_p * n)(*[p.handle for p in curs])
-        T = None
-        if T_init is not None:
-            T = np.ascontiguousarray(np.asarray(T_init, dtype=np.float64).reshape(n, 16))
-        self._check(self.lib.dvo_b200_match_batch_device(self.ctx, C.byref(cfg), n, rh, ch,
-                                                         T.ctypes.data_as(C.POINTER(C.c_double)) if T is not None else None,
-                                                         C.c_void_p(d_results_ptr)))
+        self._check(self.lib.dvo_b200_match_batch_device(self.ctx, C.byref(cfg), n, _handles(refs), _handles(curs),
+                                                         _ptr(_rows(T_init, "T_init", (n, 4, 4), 16)), C.c_void_p(d_results_ptr)))
 
     def residual_image(self, ref: Pyramid, cur: Pyramid, level: int, T, cfg: Config | None = None, ab=None):
         """ab = (alpha, beta): the photometric mode's hook at that brightness model (dvo_b200_residual_image_photometric)."""
         cfg = cfg or Config()
         w, h, _ = ref.level_info(level)
         out = np.empty((7, h, w), dtype=np.float32)
-        T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(16))
         cnt = C.c_int64()
-        Tp, op = T.ctypes.data_as(C.POINTER(C.c_double)), out.ctypes.data_as(C.POINTER(C.c_float))
+        head = (self.ctx, C.byref(cfg), ref.handle, cur.handle, level, _ptr(_rows(T, "T", (4, 4), 16)))
+        tail = (_ptr(out, C.POINTER(C.c_float)), C.byref(cnt))
         if ab is None:
-            self._check(self.lib.dvo_b200_residual_image(self.ctx, C.byref(cfg), ref.handle, cur.handle, level, Tp, op, C.byref(cnt)))
+            self._check(self.lib.dvo_b200_residual_image(*head, *tail))
         else:
-            ab = np.ascontiguousarray(np.asarray(ab, dtype=np.float64).reshape(2))
-            self._check(self.lib.dvo_b200_residual_image_photometric(self.ctx, C.byref(cfg), ref.handle, cur.handle, level, Tp,
-                                                                     ab.ctypes.data_as(C.POINTER(C.c_double)), op, C.byref(cnt)))
+            self._check(self.lib.dvo_b200_residual_image_photometric(*head, _ptr(_rows(ab, "ab", (2,), 2)), *tail))
         return cnt.value, out
 
     def intensity_error_image(self, ref: Pyramid, cur: Pyramid, level: int, T, cfg: Config | None = None):
@@ -988,18 +943,16 @@ class Engine:
         cfg = cfg or Config()
         w, h, _ = ref.level_info(level)
         out = np.empty((h, w), dtype=np.float32)
-        T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(16))
         cnt = C.c_int64()
         self._check(self.lib.dvo_b200_intensity_error_image(self.ctx, C.byref(cfg), ref.handle, cur.handle, level,
-                                                            T.ctypes.data_as(C.POINTER(C.c_double)),
-                                                            out.ctypes.data_as(C.POINTER(C.c_float)), C.byref(cnt)))
+                                                            _ptr(_rows(T, "T", (4, 4), 16)), _ptr(out, C.POINTER(C.c_float)),
+                                                            C.byref(cnt)))
         return int(cnt.value), out
 
     def linearize(self, ref: Pyramid, cur: Pyramid, level: int, T, use_weights=False, prev_precision=None, cfg: Config | None = None,
                   ab=None):
         """ab = (alpha, beta): the photometric mode's hook (dvo_b200_linearize_photometric); A is then 8 x 8 and b 8."""
         cfg = cfg or Config()
-        T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(16))
         pp = np.ascontiguousarray(np.asarray(prev_precision if prev_precision is not None else np.zeros(4), dtype=np.float32).reshape(4))
         P = np.zeros(4, dtype=np.float32)
         ll = C.c_float()
@@ -1007,16 +960,13 @@ class Engine:
         A = np.zeros(k * k)
         b = np.zeros(k)
         cnt = C.c_int64()
-        Tp, ppp = T.ctypes.data_as(C.POINTER(C.c_double)), pp.ctypes.data_as(C.POINTER(C.c_float))
-        Pp, Ap, bp = P.ctypes.data_as(C.POINTER(C.c_float)), A.ctypes.data_as(C.POINTER(C.c_double)), b.ctypes.data_as(C.POINTER(C.c_double))
+        fp = C.POINTER(C.c_float)
+        head = (self.ctx, C.byref(cfg), ref.handle, cur.handle, level, _ptr(_rows(T, "T", (4, 4), 16)))
+        tail = (int(use_weights), _ptr(pp, fp), C.byref(cnt), _ptr(P, fp), C.byref(ll), _ptr(A), _ptr(b))
         if ab is None:
-            self._check(self.lib.dvo_b200_linearize(self.ctx, C.byref(cfg), ref.handle, cur.handle, level, Tp, int(use_weights), ppp,
-                                                    C.byref(cnt), Pp, C.byref(ll), Ap, bp))
+            self._check(self.lib.dvo_b200_linearize(*head, *tail))
         else:
-            ab = np.ascontiguousarray(np.asarray(ab, dtype=np.float64).reshape(2))
-            self._check(self.lib.dvo_b200_linearize_photometric(self.ctx, C.byref(cfg), ref.handle, cur.handle, level, Tp,
-                                                                ab.ctypes.data_as(C.POINTER(C.c_double)), int(use_weights), ppp,
-                                                                C.byref(cnt), Pp, C.byref(ll), Ap, bp))
+            self._check(self.lib.dvo_b200_linearize_photometric(*head, _ptr(_rows(ab, "ab", (2,), 2)), *tail))
         return {"n": cnt.value, "precision": P.reshape(2, 2), "ll": ll.value, "A": A.reshape(k, k), "b": b}
 
     # ---- profiling ----
@@ -1090,13 +1040,7 @@ class ShardedEngine:
 
     def match_batch(self, refs, curs, cfg: Config, T_init=None):
         n = len(refs)
-        rh = (C.c_void_p * n)(*[p.value for p in refs])
-        ch = (C.c_void_p * n)(*[p.value for p in curs])
-        T = None
-        if T_init is not None:
-            T = np.ascontiguousarray(np.asarray(T_init, dtype=np.float64).reshape(n, 16))
         res = (CResult * n)()
-        self._check(self.lib.dvo_b200_match_batch_sharded(self.h, C.byref(cfg), n, rh, ch,
-                                                          T.ctypes.data_as(C.POINTER(C.c_double)) if T is not None else None,
-                                                          res, None, 0))
+        self._check(self.lib.dvo_b200_match_batch_sharded(self.h, C.byref(cfg), n, _handles(refs, "value"), _handles(curs, "value"),
+                                                          _ptr(_rows(T_init, "T_init", (n, 4, 4), 16)), res, None, 0))
         return res

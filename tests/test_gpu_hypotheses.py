@@ -239,7 +239,10 @@ def test_refusals_move_no_counters(engine, batch):
 
 
 def test_cpp_adapter(engine, tmp_path):
-    """DenseTracker::matchWithHypotheses: the pose and index of Engine.match_batch_hypotheses, and false on a refusal"""
+    """DenseTracker::matchWithHypotheses: the pose and index of Engine.match_batch_hypotheses, and false on a refusal; the
+    overload with one prior per start and a weight map: the pose, index and weight map of the same call with
+    prior_information and maps"""
+    from helpers import nan_equal
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     lib = os.path.join(root, "dvo_slam_b200")
     exe = str(tmp_path / "hypotheses_adapter")
@@ -256,14 +259,25 @@ def test_cpp_adapter(engine, tmp_path):
     H = _hypotheses(pair, 4, 0)
     hpath = tmp_path / "hypotheses.bin"
     np.ascontiguousarray(H, dtype=np.float64).tofile(hpath)
-    r = subprocess.run([exe, str(path), "640", "480"] + [repr(float(v)) for v in K] + [str(hpath), "4"], capture_output=True, text=True,
-                       timeout=300)
+    rng = np.random.default_rng(11)
+    lam = np.stack([0.5 * (S + S.T) for S in ((M @ M.T + 0.5 * np.eye(6)) * 10.0 ** rng.uniform(6, 9)
+                                              for M in rng.standard_normal((4, 6, 6)))])
+    lpath, wpath = tmp_path / "priors.bin", str(tmp_path / "weights.bin")
+    lam.tofile(lpath)
+    r = subprocess.run([exe, str(path), "640", "480"] + [repr(float(v)) for v in K] + [str(hpath), "4", str(lpath), wpath],
+                       capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr
     out = json.loads(r.stdout.strip().splitlines()[-1])
     assert out["ok"] == 1 and out["refused_ok"] == 0 and out["refused_best"] == -1 and out["levels"] == 3
     refs = [engine.pyramid(pair["I_ref"].numpy(), pair["Z_ref"].numpy(), K, 4)]
     curs = [engine.pyramid(pair["I_cur"].numpy(), pair["Z_cur"].numpy(), K, 4)]
-    res, best, _ = engine.match_batch_hypotheses(refs, curs, H[None], 2, 0.0, Config(first_level=3, last_level=1, max_iterations_per_level=50,
-                                                                                      precision=1e-4, use_initial_estimate=1))
+    cfg = Config(first_level=3, last_level=1, max_iterations_per_level=50, precision=1e-4, use_initial_estimate=1)
+    res, best, _ = engine.match_batch_hypotheses(refs, curs, H[None], 2, 0.0, cfg)
     assert out["best"] == best[0]
     assert np.array_equal(np.array(out["T"]).reshape(4, 4), res[0].transformation)
+    res, best, _, maps = engine.match_batch_hypotheses(refs, curs, H[None], 2, 0.0, cfg, prior_information=lam[None], maps=True)
+    assert out["prior_ok"] == 1 and out["prior_best"] == best[0]
+    assert np.array_equal(np.array(out["prior_T"]).reshape(4, 4), res[0].transformation)
+    assert (out["rows"], out["cols"]) == (240, 320)
+    weights = np.fromfile(wpath, dtype=np.float32).reshape(240, 320)
+    assert nan_equal(weights, maps["weight"][0].cpu().numpy()) and np.isfinite(weights).sum() > 10000

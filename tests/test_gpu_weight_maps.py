@@ -357,7 +357,8 @@ def test_moving_object(engine, oracle):
 
 
 def test_adapter_match_with_weights(engine, tmp_path):
-    """DenseTracker::matchWithWeights (C++ adapter): the Result of match(), and the weight map of match_batch_maps"""
+    """DenseTracker::matchWithWeights (C++ adapter): the Result of match(), and the weight map of match_batch_maps;
+    matchWithPrior and the prior overload of matchBatch: the poses of match_batch with prior_information"""
     import os
     import subprocess
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -373,7 +374,12 @@ def test_adapter_match_with_weights(engine, tmp_path):
         for k in ("I_ref", "Z_ref", "I_cur", "Z_cur"):
             f.write(np.ascontiguousarray(pair[k].numpy(), dtype=np.float32).tobytes())
     out_bin = str(tmp_path / "weights.bin")
-    r = subprocess.run([exe, str(path), "640", "480"] + [repr(float(v)) for v in K] + [out_bin], capture_output=True, text=True, timeout=300)
+    rng = np.random.default_rng(12)
+    lam = np.stack([0.5 * (S + S.T) for S in ((M @ M.T + 0.5 * np.eye(6)) * 10.0 ** rng.uniform(6, 9)
+                                              for M in rng.standard_normal((2, 6, 6)))])
+    lam.tofile(tmp_path / "priors.bin")
+    r = subprocess.run([exe, str(path), "640", "480"] + [repr(float(v)) for v in K] + [out_bin, str(tmp_path / "priors.bin")],
+                       capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr
     import json
     out = json.loads(r.stdout.strip().splitlines()[-1])
@@ -381,6 +387,13 @@ def test_adapter_match_with_weights(engine, tmp_path):
     weights = np.fromfile(out_bin, dtype=np.float32).reshape(240, 320)
     refs = [engine.pyramid(pair["I_ref"].numpy(), pair["Z_ref"].numpy(), K, 4)]
     curs = [engine.pyramid(pair["I_cur"].numpy(), pair["Z_cur"].numpy(), K, 4)]
-    res, maps = engine.match_batch_maps(refs, curs, Config(first_level=3, last_level=1, max_iterations_per_level=50, precision=1e-4))
+    cfg = Config(first_level=3, last_level=1, max_iterations_per_level=50, precision=1e-4)
+    res, maps = engine.match_batch_maps(refs, curs, cfg)
     assert np.array_equal(np.array(out["T"]).reshape(4, 4), res[0].transformation)
     assert nan_equal(weights, maps["weight"][0].cpu().numpy()) and np.isfinite(weights).sum() > 10000
+    assert out["prior_ok"] == 1 and out["batch_ok"] == 1
+    res = engine.match_batch(refs, curs, cfg, prior_information=lam[:1])
+    assert np.array_equal(np.array(out["prior_T"]).reshape(4, 4), res[0].transformation)
+    res = engine.match_batch(refs * 2, curs * 2, cfg, prior_information=lam)
+    assert np.array_equal(np.array(out["batch_T"]).reshape(2, 4, 4), np.stack([r.transformation for r in res]))
+    assert not np.array_equal(res[0].transformation, res[1].transformation)
