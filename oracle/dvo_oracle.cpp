@@ -264,14 +264,13 @@ struct Revertable {
 };
 
 // ------------------------------------------------------------------------------------------
-// 6x6 LDLT (Eigen::LDLT restated: diagonal pivoting, in-place, then solve with the tolerance
-// rule for D).  dense_tracking.cpp:347  x = A.ldlt().solve(b)
+// n x n LDLT, n <= 8 (Eigen::LDLT restated: diagonal pivoting, in-place, then solve with the
+// tolerance rule for D).  dense_tracking.cpp:347  x = A.ldlt().solve(b); n = 8 in the photometric mode.
 // ------------------------------------------------------------------------------------------
-void ldlt_solve6(const double Ain[36], const double bin[6], double x[6]) {
-  const int n = 6;
-  double A[36];
-  std::memcpy(A, Ain, sizeof(A));
-  int perm[6];
+void ldlt_solve(const double* Ain, const double* bin, double* x, int n) {
+  double A[64];
+  std::memcpy(A, Ain, sizeof(double) * n * n);
+  int perm[8];
   for (int k = 0; k < n; ++k) {
     int piv = k;
     double best = std::fabs(A[k * n + k]);
@@ -291,7 +290,7 @@ void ldlt_solve6(const double Ain[36], const double bin[6], double x[6]) {
       A[i * n + k] = (d != 0.0) ? s / d : 0.0;
     }
   }
-  double y[6];
+  double y[8];
   for (int i = 0; i < n; ++i) y[i] = bin[i];
   for (int k = 0; k < n; ++k) std::swap(y[k], y[perm[k]]);  // P b
   for (int i = 0; i < n; ++i)
@@ -304,6 +303,38 @@ void ldlt_solve6(const double Ain[36], const double bin[6], double x[6]) {
     for (int j = i + 1; j < n; ++j) y[i] -= A[j * n + i] * y[j];  // L^-T
   for (int k = n - 1; k >= 0; --k) std::swap(y[k], y[perm[k]]);  // P^T
   for (int i = 0; i < n; ++i) x[i] = y[i];
+}
+void ldlt_solve6(const double A[36], const double b[6], double x[6]) { ldlt_solve(A, b, x, 6); }
+
+// A_xx - A_xp A_pp^-1 A_px of an 8 x 8 onto its first 6 unknowns, fp64, the 2 x 2 inverse written out
+void schur_onto_pose(const double A[64], double S[36]) {
+  const double a = A[6 * 8 + 6], c = A[6 * 8 + 7], d = A[7 * 8 + 7];
+  const double rdet = 1.0 / (a * d - c * c);
+  const double i00 = d * rdet, i01 = -c * rdet, i11 = a * rdet;
+  for (int i = 0; i < 6; ++i) {
+    const double g0 = i00 * A[i * 8 + 6] + i01 * A[i * 8 + 7], g1 = i01 * A[i * 8 + 6] + i11 * A[i * 8 + 7];
+    for (int j = 0; j < 6; ++j) S[i * 6 + j] = A[i * 8 + j] - (g0 * A[j * 8 + 6] + g1 * A[j * 8 + 7]);
+  }
+}
+
+// The motion prior Lambda (6 x 6, row-major) in place of mu I: s_i = sum_j Lambda_ij li_j in order j = 0..5 from 0, and the
+// prior log-likelihood sum_i li_i s_i.  With -ffp-contract=off and Lambda = mu I every term but mu li_i is an exact zero, so
+// b_i + s_i is the mu path's b_i + mu li_i; the log-likelihood rounds differently from mu |li|^2.
+struct MotionPriorTerms {
+  double s[6];   // Lambda li
+  double ll;     // li^T Lambda li
+};
+
+MotionPriorTerms motion_prior_terms(const double L[36], const double li[6]) {
+  MotionPriorTerms t;
+  t.ll = 0.0;
+  for (int i = 0; i < 6; ++i) {
+    double s = 0.0;
+    for (int j = 0; j < 6; ++j) s += L[i * 6 + j] * li[j];
+    t.s[i] = s;
+  }
+  for (int i = 0; i < 6; ++i) t.ll += li[i] * t.s[i];
+  return t;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -336,6 +367,13 @@ void select_points(const Level& L, float ti, float td, std::vector<RefPoint>& pt
       r.pix = int(p);
       pts.push_back(r);
     }
+}
+
+// The photometric mode (include/dvo_b200.h): the reference intensity of every selected point becomes alpha I_ref + beta
+// before the residual loop, rounded to nearest, with (alpha, beta) as float.  At (1, 0) that is I_ref exactly.
+void brighten_selection(std::vector<RefPoint>& pts, const double ab[2], const orc_mode& mode) {
+  const float a = float(ab[0]), b = float(ab[1]);
+  for (RefPoint& p : pts) p.i = mode.fused_pixel_math ? std::fmaf(a, p.i, b) : a * p.i + b;
 }
 
 struct ErrPoint {  // points_error entry: untransformed point + residual record (dense_tracking_impl.cpp:265-281)
@@ -625,6 +663,46 @@ void normal_equations(const std::vector<ErrPoint>& e, const std::vector<float>& 
   }
 }
 
+// The photometric mode's 8 x 8: the per-entry arithmetic of normal_equations over the Jacobian rows extended by
+// de_i/dalpha = -I_ref/255, de_i/dbeta = -1/255 (intensity row) and zeros (depth row), I_ref read from the reference level
+// R; f32_serial_accum: fp32 in point order (the pose block equals the default FAITHFUL A and b bit for bit), else fp64.
+void normal_equations_photometric(const std::vector<ErrPoint>& e, const std::vector<float>& w, const float P[4], const Level& R,
+                       const orc_mode& mode, double A[64], double b[8]) {
+  const float wref0 = -1.0f / 255.0f;
+  const size_t n = e.size();
+  float Af[64] = {0}, bf[8] = {0};
+  double Ad[64] = {0}, bd[8] = {0};
+  for (size_t k = 0; k < n; ++k) {
+    float J0[8], J1[8];
+    jacobian_rows<float>(e[k].x, e[k].y, e[k].z, e[k].e[2], e[k].e[3], e[k].e[4], e[k].e[5], J0, J1);
+    J0[6] = wref0 * R.ch[0][size_t(e[k].pix)]; J0[7] = wref0;
+    J1[6] = 0.0f; J1[7] = 0.0f;
+    if (mode.f32_serial_accum) {
+      const float W[4] = {w[k] * P[0], w[k] * P[1], w[k] * P[2], w[k] * P[3]};
+      const float r0 = e[k].e[0], r1 = e[k].e[1];
+      for (int i = 0; i < 8; ++i) {
+        const float ua = J0[i] * W[0] + J1[i] * W[2], ub = J0[i] * W[1] + J1[i] * W[3];
+        for (int j = i; j < 8; ++j) Af[i * 8 + j] += ua * J0[j] + ub * J1[j];
+        bf[i] -= ua * r0 + ub * r1;
+      }
+    } else {
+      const double W[4] = {double(w[k]) * P[0], double(w[k]) * P[1], double(w[k]) * P[2], double(w[k]) * P[3]};
+      const double r0 = e[k].e[0], r1 = e[k].e[1];
+      for (int i = 0; i < 8; ++i) {
+        const double ua = J0[i] * W[0] + J1[i] * W[2], ub = J0[i] * W[1] + J1[i] * W[3];
+        for (int j = i; j < 8; ++j) Ad[i * 8 + j] += ua * J0[j] + ub * J1[j];
+        bd[i] -= ua * r0 + ub * r1;
+      }
+    }
+  }
+  for (int i = 0; i < 8; ++i)
+    for (int j = 0; j < 8; ++j) {
+      const int u = i <= j ? i * 8 + j : j * 8 + i;
+      A[i * 8 + j] = mode.f32_serial_accum ? double(Af[u]) : Ad[u];
+    }
+  for (int i = 0; i < 8; ++i) b[i] = mode.f32_serial_accum ? double(bf[i]) : bd[i];
+}
+
 double linf6(const double x[6]) {
   double m = 0;
   for (int i = 0; i < 6; ++i) m = std::fmax(m, std::fabs(x[i]));
@@ -703,11 +781,12 @@ int64_t orc_select(const orc_pyramid* ref, int level, float ti, float td, const 
 }
 
 int64_t orc_residual_image(const orc_pyramid* ref, const orc_pyramid* cur, int level, const double T[16],
-                           float ti, float td, const orc_mode* mode, float* planes7) {
+                           const double ab[2], float ti, float td, const orc_mode* mode, float* planes7) {
   const Level& R = ref->levels[level];
   const Level& C = cur->levels[level];
   std::vector<RefPoint> pts;
   select_points(R, ti, td, pts);
+  if (ab) brighten_selection(pts, ab, *mode);
   LevelConsts c;
   make_level_consts(C, T, c);
   std::vector<ErrPoint> e;
@@ -758,13 +837,14 @@ int64_t orc_intensity_error_image(const orc_pyramid* ref, const orc_pyramid* cur
   return int64_t(res_it);
 }
 
-int64_t orc_linearize(const orc_pyramid* ref, const orc_pyramid* cur, int level, const double T[16], float ti,
-                      float td, int use_weights, const float prev_precision[4], const orc_mode* mode,
-                      float precision_out[4], float* ll_out, double A_out[36], double b_out[6]) {
+int64_t orc_linearize(const orc_pyramid* ref, const orc_pyramid* cur, int level, const double T[16], const double ab[2],
+                      float ti, float td, int use_weights, const float prev_precision[4], const orc_mode* mode,
+                      float precision_out[4], float* ll_out, double* A_out, double* b_out) {
   const Level& R = ref->levels[level];
   const Level& C = cur->levels[level];
   std::vector<RefPoint> pts;
   select_points(R, ti, td, pts);
+  if (ab) brighten_selection(pts, ab, *mode);
   LevelConsts c;
   make_level_consts(C, T, c);
   std::vector<ErrPoint> e;
@@ -777,14 +857,17 @@ int64_t orc_linearize(const orc_pyramid* ref, const orc_pyramid* cur, int level,
   compute_scale(e, w, *mode, Cov);
   inverse2(Cov, precision_out);
   *ll_out = compute_ll(e, precision_out, *mode);
-  normal_equations(e, w, precision_out, *mode, A_out, b_out);
+  if (ab) normal_equations_photometric(e, w, precision_out, R, *mode, A_out, b_out);
+  else normal_equations(e, w, precision_out, *mode, A_out, b_out);
   return n;
 }
 
-int orc_match(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const double T_init[16],
-              const orc_mode* mode_p, orc_result* result, orc_iteration_stats* iters, int max_iters,
-              int* num_iters) {
+int orc_match_with(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const double T_init[16], const double prior[36],
+                   const double ab_init[2], const orc_mode* mode_p, orc_result* result, double ab_out[2],
+                   orc_iteration_stats* iters, int max_iters, int* num_iters) {
   const orc_mode mode = *mode_p;
+  const bool photometric = ab_out != nullptr;
+  const int nu = photometric ? 8 : 6;  // unknowns: the pose, then (alpha, beta) in the photometric mode
   int iter_count = 0;
   std::memset(result, 0, sizeof(*result));
 
@@ -793,11 +876,16 @@ int orc_match(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const d
   if (cfg->use_initial_estimate) inc = se3_from_matrix(T_init);
   Revertable<SE3> initial{inc, inc};
   Revertable<SE3> estimate{SE3(), SE3()};
+  // the photometric mode's (alpha, beta): updated and reverted with the pose, carried over between levels
+  struct AB { double v[2]; };
+  Revertable<AB> ab{{{1.0, 0.0}}, {{1.0, 0.0}}};
+  if (ab_init) { ab.value.v[0] = ab.old.v[0] = ab_init[0]; ab.value.v[1] = ab.old.v[1] = ab_init[1]; }
   bool accept = true;
 
   float precision[4] = {0, 0, 0, 0};
   // per-thread scratch (the reference keeps points_error / residuals / weights as DenseTracker members, dense_tracking.cpp:160-165)
-  static thread_local std::vector<RefPoint> pts;
+  // and pts_ab, the selection with the brightness model applied in the photometric mode
+  static thread_local std::vector<RefPoint> pts, pts_ab;
   static thread_local std::vector<ErrPoint> err;
   static thread_local std::vector<float> weights;
 
@@ -820,8 +908,9 @@ int orc_match(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const d
     ls.valid_pixels = int64_t(pts.size());
     ls.termination = -1;
 
-    double A[36], b[6], x[6];
+    double A[64], b[8], x[8];
     se3_log(inc, x);  // line 238
+    double dab[2] = {0.0, 0.0};  // the (alpha, beta) part of the last accepted increment of this level
 
     do {
       orc_iteration_stats it;
@@ -834,17 +923,26 @@ int orc_match(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const d
       inc = se3_exp(x);                                             // line 259
       initial.update() = se3_mul(se3_inverse(inc), initial.value);  // line 260
       estimate.update() = se3_mul(inc, estimate.value);             // line 261
+      if (photometric) {
+        const AB prev = ab.value;
+        ab.update() = AB{{prev.v[0] + dab[0], prev.v[1] + dab[1]}};
+      }
 
       double T[16];
       se3_matrix(estimate.value, T);
       LevelConsts c;
       make_level_consts(C, T, c);
-      int64_t n = compute_residuals(pts, C, c, mode, err);          // line 271
+      if (photometric) {
+        pts_ab = pts;
+        brighten_selection(pts_ab, ab.value.v, mode);
+      }
+      int64_t n = compute_residuals(photometric ? pts_ab : pts, C, c, mode, err);  // line 271
       it.valid_constraints = n;
 
       if (n < 6) {                                                  // lines 276-284
         initial.revert();
         estimate.revert();
+        if (photometric) ab.revert();
         ls.termination = ORC_TERM_TOO_FEW_CONSTRAINTS;
         level_iters.push_back(it);
         break;
@@ -861,9 +959,15 @@ int orc_match(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const d
       for (int i = 0; i < 4; ++i) it.tdist_precision[i] = double(precision[i]);
       double li[6];
       se3_log(initial.value, li);
-      double sq = 0;
-      for (int i = 0; i < 6; ++i) sq += li[i] * li[i];
-      it.prior_log_likelihood = cfg->mu * sq;                       // line 302
+      MotionPriorTerms pt;
+      if (prior) {
+        pt = motion_prior_terms(prior, li);
+        it.prior_log_likelihood = pt.ll;
+      } else {
+        double sq = 0;
+        for (int i = 0; i < 6; ++i) sq += li[i] * li[i];
+        it.prior_log_likelihood = cfg->mu * sq;                     // line 302
+      }
 
       last_error = error;                                           // lines 306-307
       error = -double(ll);
@@ -871,19 +975,31 @@ int orc_match(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const d
       if (!accept) {
         initial.revert();
         estimate.revert();
+        if (photometric) ab.revert();
         ls.termination = ORC_TERM_LOG_LIKELIHOOD_DECREASED;
         level_iters.push_back(it);
         break;
       }
 
-      normal_equations(err, weights, precision, mode, A, b);        // lines 333-343
+      if (photometric) normal_equations_photometric(err, weights, precision, R, mode, A, b);
+      else normal_equations(err, weights, precision, mode, A, b);   // lines 333-343
       for (int i = 0; i < 6; ++i) {
-        A[i * 6 + i] += cfg->mu;                                    // line 345
-        b[i] += cfg->mu * li[i];                                    // line 346 (log of updated initial)
+        if (prior) {
+          for (int j = 0; j < 6; ++j) A[i * nu + j] += prior[i * 6 + j];
+          b[i] += pt.s[i];
+        } else {
+          A[i * nu + i] += cfg->mu;                                 // line 345
+          b[i] += cfg->mu * li[i];                                  // line 346 (log of updated initial)
+        }
       }
-      ldlt_solve6(A, b, x);                                         // line 347
+      ldlt_solve(A, b, x, nu);                                      // line 347
       for (int i = 0; i < 6; ++i) it.increment[i] = x[i];
-      for (int i = 0; i < 36; ++i) it.information[i] = A[i];
+      if (photometric) {
+        dab[0] = x[6]; dab[1] = x[7];
+        schur_onto_pose(A, it.information);
+      } else {
+        for (int i = 0; i < 36; ++i) it.information[i] = A[i];
+      }
       level_iters.push_back(it);
       iteration++;                                                  // line 353
     } while (accept && linf6(x) > cfg->precision && !(iteration >= cfg->max_iterations_per_level));  // line 357
@@ -912,13 +1028,22 @@ int orc_match(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const d
     for (int i = 0; i < 36; ++i) result->information[i] = kNaN;
     result->log_likelihood = kNaN;
   }
+  if (ab_out) { ab_out[0] = ab.value.v[0]; ab_out[1] = ab.value.v[1]; }
   if (num_iters) *num_iters = iter_count;
   return 0;
+}
+
+int orc_match(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const double T_init[16],
+              const orc_mode* mode, orc_result* result, orc_iteration_stats* iters, int max_iters,
+              int* num_iters) {
+  return orc_match_with(ref, cur, cfg, T_init, nullptr, nullptr, mode, result, nullptr, iters, max_iters, num_iters);
 }
 
 void orc_se3_exp(const double xi[6], double T[16]) { se3_matrix(se3_exp(xi), T); }
 void orc_se3_log(const double T[16], double xi[6]) { se3_log(se3_from_matrix(T), xi); }
 void orc_ldlt_solve6(const double A[36], const double b[6], double x[6]) { ldlt_solve6(A, b, x); }
+void orc_ldlt_solve(const double* A, const double* b, double* x, int n) { ldlt_solve(A, b, x, n); }
+void orc_schur_onto_pose(const double A[64], double S[36]) { schur_onto_pose(A, S); }
 
 void orc_convert_raw_depth(const uint16_t* in, float* out, int64_t count, float scale) {
   for (int64_t i = 0; i < count; ++i) out[i] = in[i] == 0 ? kNaNf : float(in[i]) * scale;

@@ -140,10 +140,12 @@ int64_t orc_select(const orc_pyramid* ref, int level, float ti, float td, const 
 /* One evaluation of computeResidualsSse at a given transform (dense_tracking_impl.cpp:133-393)
  * in dense image form: 7 planes of h*w floats {e.i, e.z, e.idx, e.idy, e.zdx, e.zdy, z_ref},
  * NaN in every plane where the reference point is not selected / not valid.  T is the 4x4
- * row-major double "estimate" (cast to float inside, dense_tracking.cpp:263).  Returns n. */
+ * row-major double "estimate" (cast to float inside, dense_tracking.cpp:263).  ab: NULL, or the
+ * photometric mode's (alpha, beta), applied to the reference intensities as alpha I_ref + beta
+ * (float, rounded to nearest; fmaf under fused_pixel_math).  Returns n. */
 int64_t orc_residual_image(const orc_pyramid* ref, const orc_pyramid* cur, int level,
-                           const double T[16], float ti, float td, const orc_mode* mode,
-                           float* planes7);
+                           const double T[16], const double ab[2], float ti, float td,
+                           const orc_mode* mode, float* planes7);
 
 /* DenseTracker::computeIntensityErrorImage (dense_tracking.cpp:378-444): h*w floats, |intensity residual| at
  * every selected pixel whose residual is valid, 0 elsewhere (including the odd last selected point, which the
@@ -154,11 +156,14 @@ int64_t orc_intensity_error_image(const orc_pyramid* ref, const orc_pyramid* cur
 
 /* One full Gauss-Newton linearisation at T with given previous precision (iteration>0 semantics
  * when use_weights!=0, else weights=1): returns n, and fills scale precision P (row-major 2x2
- * float), ll (float), A (36 doubles incl. no mu), b (6 doubles).  Follows dense_tracking.cpp:271-343. */
+ * float), ll (float), A (36 doubles incl. no mu), b (6 doubles).  Follows dense_tracking.cpp:271-343.
+ * ab non-NULL: the photometric mode at (alpha, beta) as in orc_residual_image; A is then 8x8 (64
+ * doubles) and b 8 doubles, the unknowns (pose, alpha, beta), with de_i/dalpha = -I_ref/255 and
+ * de_i/dbeta = -1/255 on the intensity row. */
 int64_t orc_linearize(const orc_pyramid* ref, const orc_pyramid* cur, int level, const double T[16],
-                      float ti, float td, int use_weights, const float prev_precision[4],
+                      const double ab[2], float ti, float td, int use_weights, const float prev_precision[4],
                       const orc_mode* mode, float precision_out[4], float* ll_out,
-                      double A_out[36], double b_out[6]);
+                      double* A_out, double* b_out);
 
 /* DenseTracker::match(reference, current, result) (dense_tracking.cpp:123-376).
  * T_init: row-major 4x4 initial Result.Transformation (used iff cfg.use_initial_estimate).
@@ -168,11 +173,27 @@ int orc_match(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const d
               const orc_mode* mode, orc_result* result, orc_iteration_stats* iters, int max_iters,
               int* num_iters);
 
+/* orc_match with its optional inputs; orc_match is this with prior, ab_init and ab_out NULL.
+ * prior: NULL, or a motion prior information Lambda (36 doubles, row-major) in place of cfg.mu I
+ *   (cfg.mu is then ignored): A += Lambda and b += Lambda li on the pose block, and the prior
+ *   log-likelihood li^T Lambda li, with li = log(initial).
+ * ab_out: NULL, or the photometric mode, which receives the final (alpha, beta).  (alpha, beta) start
+ *   at ab_init (NULL: (1, 0)) and are a Revertable updated with the pose: the top of every iteration
+ *   adds the (alpha, beta) part of the level's last accepted increment, a rejected iteration reverts
+ *   both, and levels carry them over.  The system is orc_linearize's 8x8 and the information its Schur
+ *   complement onto the pose (prior included). */
+int orc_match_with(orc_pyramid* ref, orc_pyramid* cur, const orc_config* cfg, const double T_init[16],
+                   const double prior[36], const double ab_init[2], const orc_mode* mode, orc_result* result,
+                   double ab_out[2], orc_iteration_stats* iters, int max_iters, int* num_iters);
+
 /* SE(3) helpers (restated Sophus se3.hpp algorithm), exposed for tests. */
 void orc_se3_exp(const double xi[6], double T[16]);
 void orc_se3_log(const double T[16], double xi[6]);
-/* Eigen-style pivoted LDLT solve of a 6x6 SPD system (dense_tracking.cpp:347). */
-void orc_ldlt_solve6(const double A[36], const double b[6], double x[6]);
+/* Eigen-style pivoted LDLT solve of an n x n SPD system, n <= 8 (dense_tracking.cpp:347; n = 8 in the photometric mode). */
+void orc_ldlt_solve(const double* A, const double* b, double* x, int n);
+void orc_ldlt_solve6(const double A[36], const double b[6], double x[6]);   /* orc_ldlt_solve with n = 6 */
+/* The Schur complement of an 8x8 onto its first 6 unknowns: the photometric mode's information. */
+void orc_schur_onto_pose(const double A[64], double S[36]);
 
 /* SurfacePyramid::convertRawDepthImageSse (surface_pyramid.cpp:45-105): u16 -> f32*scale, 0 -> NaN */
 void orc_convert_raw_depth(const uint16_t* in, float* out, int64_t count, float scale);

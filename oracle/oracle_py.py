@@ -82,18 +82,19 @@ def lib():
         L.orc_select.restype = C.c_int64
         L.orc_select.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float, C.POINTER(Mode), C.POINTER(C.c_uint8)]
         L.orc_residual_image.restype = C.c_int64
-        L.orc_residual_image.argtypes = [C.c_void_p, C.c_void_p, C.c_int, dp, C.c_float, C.c_float, C.POINTER(Mode), fp]
+        L.orc_residual_image.argtypes = [C.c_void_p, C.c_void_p, C.c_int, dp, dp, C.c_float, C.c_float, C.POINTER(Mode), fp]
         L.orc_intensity_error_image.restype = C.c_int64
         L.orc_intensity_error_image.argtypes = [C.c_void_p, C.c_void_p, C.c_int, dp, C.c_float, C.c_float, C.POINTER(Mode), fp]
         L.orc_linearize.restype = C.c_int64
-        L.orc_linearize.argtypes = [C.c_void_p, C.c_void_p, C.c_int, dp, C.c_float, C.c_float, C.c_int, fp,
+        L.orc_linearize.argtypes = [C.c_void_p, C.c_void_p, C.c_int, dp, dp, C.c_float, C.c_float, C.c_int, fp,
                                     C.POINTER(Mode), fp, fp, dp, dp]
-        L.orc_match.restype = C.c_int
-        L.orc_match.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Config), dp, C.POINTER(Mode), C.POINTER(Result),
-                                C.POINTER(IterationStats), C.c_int, C.POINTER(C.c_int)]
+        L.orc_match_with.restype = C.c_int
+        L.orc_match_with.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(Config), dp, dp, dp, C.POINTER(Mode), C.POINTER(Result),
+                                     dp, C.POINTER(IterationStats), C.c_int, C.POINTER(C.c_int)]
         L.orc_se3_exp.argtypes = [dp, dp]
         L.orc_se3_log.argtypes = [dp, dp]
-        L.orc_ldlt_solve6.argtypes = [dp, dp, dp]
+        L.orc_ldlt_solve.argtypes = [dp, dp, dp, C.c_int]
+        L.orc_schur_onto_pose.argtypes = [dp, dp]
         L.orc_convert_raw_depth.argtypes = [C.POINTER(C.c_uint16), fp, C.c_int64, C.c_float]
         L.orc_bgr_to_grey.argtypes = [C.POINTER(C.c_uint8), fp, C.c_int64]
         _lib = L
@@ -105,7 +106,13 @@ def _fptr(a):
 
 
 def _dptr(a):
-    return a.ctypes.data_as(C.POINTER(C.c_double))
+    """a's data, or NULL for None"""
+    return None if a is None else a.ctypes.data_as(C.POINTER(C.c_double))
+
+
+def _doubles(a, n):
+    """a as n contiguous float64 (kept alive by the caller), or None for None"""
+    return None if a is None else np.ascontiguousarray(np.asarray(a, dtype=np.float64).reshape(n))
 
 
 def mode(name: str) -> Mode:
@@ -165,11 +172,12 @@ def select(ref: Pyramid, level, ti=0.0, td=0.0, m: Mode | None = None):
     return int(S), mask
 
 
-def residual_image(ref: Pyramid, cur: Pyramid, level, T, m: Mode, ti=0.0, td=0.0):
+def residual_image(ref: Pyramid, cur: Pyramid, level, T, m: Mode, ti=0.0, td=0.0, ab=None):
+    """ab: None, or the photometric mode's (alpha, beta)"""
     w, h, _ = ref.level_info(level)
     out = np.empty((7, h, w), dtype=np.float32)
-    T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(16))
-    n = lib().orc_residual_image(ref.h, cur.h, level, _dptr(T), ti, td, C.byref(m), _fptr(out))
+    T, ab = _doubles(T, 16), _doubles(ab, 2)
+    n = lib().orc_residual_image(ref.h, cur.h, level, _dptr(T), _dptr(ab), ti, td, C.byref(m), _fptr(out))
     return int(n), out
 
 
@@ -182,24 +190,32 @@ def intensity_error_image(ref: Pyramid, cur: Pyramid, level, T, m: Mode, ti=0.0,
     return int(n), out
 
 
-def linearize(ref: Pyramid, cur: Pyramid, level, T, m: Mode, use_weights=False, prev_precision=None, ti=0.0, td=0.0):
-    T = np.ascontiguousarray(np.asarray(T, dtype=np.float64).reshape(16))
+def linearize(ref: Pyramid, cur: Pyramid, level, T, m: Mode, use_weights=False, prev_precision=None, ti=0.0, td=0.0, ab=None):
+    """ab: None, or the photometric mode's (alpha, beta), whose A is 8 x 8 and b 8 long"""
+    T, ab = _doubles(T, 16), _doubles(ab, 2)
     pp = np.ascontiguousarray(np.asarray(prev_precision if prev_precision is not None else np.zeros(4), dtype=np.float32).reshape(4))
     P = np.zeros(4, dtype=np.float32)
     ll = C.c_float()
-    A = np.zeros(36, dtype=np.float64)
-    b = np.zeros(6, dtype=np.float64)
-    n = lib().orc_linearize(ref.h, cur.h, level, _dptr(T), ti, td, int(use_weights), _fptr(pp), C.byref(m), _fptr(P),
-                            C.byref(ll), _dptr(A), _dptr(b))
-    return {"n": int(n), "precision": P.reshape(2, 2), "ll": ll.value, "A": A.reshape(6, 6), "b": b}
+    nu = 6 if ab is None else 8
+    A = np.zeros(nu * nu, dtype=np.float64)
+    b = np.zeros(nu, dtype=np.float64)
+    n = lib().orc_linearize(ref.h, cur.h, level, _dptr(T), _dptr(ab), ti, td, int(use_weights), _fptr(pp), C.byref(m),
+                            _fptr(P), C.byref(ll), _dptr(A), _dptr(b))
+    return {"n": int(n), "precision": P.reshape(2, 2), "ll": ll.value, "A": A.reshape(nu, nu), "b": b}
 
 
-def match(ref: Pyramid, cur: Pyramid, cfg: Config, m: Mode, T_init=None, max_iters=1024):
-    T0 = np.ascontiguousarray(np.asarray(T_init if T_init is not None else np.eye(4), dtype=np.float64).reshape(16))
+def match(ref: Pyramid, cur: Pyramid, cfg: Config, m: Mode, T_init=None, max_iters=1024, prior=None, photometric=False,
+          ab_init=None):
+    """prior: None for cfg.mu I, else a 6 x 6 prior information in its place.  photometric: estimate (alpha, beta) with the
+    pose, from ab_init (None: (1, 0)); the result then holds the final ones as "ab"."""
+    T0 = _doubles(T_init if T_init is not None else np.eye(4), 16)
+    prior, ab_init = _doubles(prior, 36), _doubles(ab_init, 2)
+    ab = np.zeros(2) if photometric else None
     res = Result()
     its = (IterationStats * max_iters)()
     n = C.c_int()
-    rc = lib().orc_match(ref.h, cur.h, C.byref(cfg), _dptr(T0), C.byref(m), C.byref(res), its, max_iters, C.byref(n))
+    rc = lib().orc_match_with(ref.h, cur.h, C.byref(cfg), _dptr(T0), _dptr(prior), _dptr(ab_init), C.byref(m),
+                              C.byref(res), _dptr(ab), its, max_iters, C.byref(n))
     assert rc == 0
     levels = []
     for i in range(res.num_levels):
@@ -212,8 +228,11 @@ def match(ref: Pyramid, cur: Pyramid, cfg: Config, m: Mode, T_init=None, max_ite
         iters.append({"level": s.level, "id": s.id, "n": s.valid_constraints, "nll": s.tdist_log_likelihood,
                       "precision": np.array(s.tdist_precision).reshape(2, 2), "prior": s.prior_log_likelihood,
                       "x": np.array(s.increment), "A": np.array(s.information).reshape(6, 6)})
-    return {"T": np.array(res.transformation).reshape(4, 4), "information": np.array(res.information).reshape(6, 6),
-            "log_likelihood": res.log_likelihood, "levels": levels, "iterations": iters}
+    out = {"T": np.array(res.transformation).reshape(4, 4), "information": np.array(res.information).reshape(6, 6),
+           "log_likelihood": res.log_likelihood, "levels": levels, "iterations": iters}
+    if photometric:
+        out["ab"] = ab
+    return out
 
 
 def se3_exp(xi):
@@ -230,12 +249,25 @@ def se3_log(T):
     return xi
 
 
-def ldlt_solve6(A, b):
-    A = np.ascontiguousarray(np.asarray(A, dtype=np.float64).reshape(36))
-    b = np.ascontiguousarray(np.asarray(b, dtype=np.float64))
-    x = np.zeros(6)
-    lib().orc_ldlt_solve6(_dptr(A), _dptr(b), _dptr(x))
+def ldlt_solve(A, b):
+    """x = A^-1 b for an n x n A, n <= 8, by the oracle's pivoted LDL^T"""
+    n = len(b)
+    assert 1 <= n <= 8, n
+    A, b = _doubles(A, n * n), _doubles(b, n)
+    x = np.zeros(n)
+    lib().orc_ldlt_solve(_dptr(A), _dptr(b), _dptr(x), n)
     return x
+
+
+ldlt_solve6 = ldlt_solve   # the 6 x 6 case by its former name
+
+
+def schur_pose(A):
+    """the Schur complement of an 8 x 8 onto its first 6 unknowns (the photometric mode's information)"""
+    A = _doubles(A, 64)
+    S = np.zeros(36)
+    lib().orc_schur_onto_pose(_dptr(A), _dptr(S))
+    return S.reshape(6, 6)
 
 
 def bgr_to_grey(bgr_u8):

@@ -8,8 +8,9 @@ the point selection alone: the depth derivatives were taken at creation, and a p
 sampled as bilinear taps.  So the masked oracle pyramid is the unmasked one with NaN written into the depth plane of every
 unusable pixel after the build.  The gradients of the neighbours and the depth of every selected point stay as they are;
 in every mode and every entry point (select, residual_image, linearize, intensity_error_image, match) the selection is then
-isPointOk AND usable, and S, the odd last point and everything else follow from it.  Such a pyramid must only be used as the
-REFERENCE of an alignment (a mask acts in that role only).
+isPointOk AND usable, and S, the odd last point and everything else follow from it.  In the current role the NaN depth
+makes every bilinear tap that touches an unusable pixel NaN, and the point drops out of the residuals: the engine's rule for a
+mask in both roles (dvo_b200_pyramid_create_masked_batch_roles with both role bits).
 """
 import ctypes as C
 
@@ -29,7 +30,7 @@ def usable_by_footprint(mask, levels):
 
 
 def masked_pyramid(orc, intensity, depth, intrinsics, levels, mask=None):
-    """oracle Pyramid for the REFERENCE role with a reference mask (h, w; nonzero = usable); mask=None: orc.Pyramid"""
+    """oracle Pyramid with a mask (h, w; nonzero = usable), in either role; mask=None: orc.Pyramid"""
     p = orc.Pyramid(intensity, depth, intrinsics, levels)
     if mask is None:
         return p

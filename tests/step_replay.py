@@ -3,20 +3,20 @@ iteration log, in plain numpy / scipy.
 
 Teacher forcing: the log holds every increment x the end step computed.  From those, and from the accept decisions the
 logged log-likelihoods imply, the replay rebuilds in fp64 the pose (and in the photometric mode the brightness (alpha,
-beta)) every iteration linearised at, following DenseTracker::match as oracle/dvo_oracle.cpp:787-912 writes it out:
+beta)) every iteration linearised at, following DenseTracker::match as oracle/dvo_oracle.cpp:865-1034 writes it out:
 
-  inc = T0 (use_initial_estimate, else I); initial = inc; estimate = I           dvo_oracle.cpp:788-791
-  every level: x = log(inc)                                                      :820  (dense_tracking.cpp:238)
-    every iteration: inc = exp(x); initial <- inc^-1 initial; estimate <- inc estimate   :830-832 (259-261)
-      n < 6: revert initial and estimate, TooFewConstraints                      :841-847
-      accept iff nll < the previous entry's nll of the level (first: always)     :864-866
-      rejected: revert, LogLikelihoodDecreased                                   :867-873
-      accepted: x = the logged increment; iteration += 1                         :880-884
-    while accepted, linf(x) > precision and iteration < max_iterations           :885
-    then linf(x) <= precision -> IncrementTooSmall; iteration >= max -> IterationsExceeded   :887-888
+  inc = T0 (use_initial_estimate, else I); initial = inc; estimate = I           dvo_oracle.cpp:875-878
+  every level: x = log(inc)                                                      :912  (dense_tracking.cpp:238)
+    every iteration: inc = exp(x); initial <- inc^-1 initial; estimate <- inc estimate   :923-925 (259-261)
+      n < 6: revert initial and estimate, TooFewConstraints                      :942-948
+      accept iff nll < the previous entry's nll of the level (first: always)     :972-974
+      rejected: revert, LogLikelihoodDecreased                                   :975-981
+      accepted: x = the logged increment; iteration += 1                         :995-1004
+    while accepted, linf(x) > precision and iteration < max_iterations           :1005
+    then linf(x) <= precision -> IncrementTooSmall; iteration >= max -> IterationsExceeded   :1007-1008
 
 So the level start applies again the last `inc` of the previous level, whether that increment was kept or reverted; the last
-increment a level computes is never applied.  The photometric mode (tests/native/photometric_oracle.cpp:199-256) adds
+increment a level computes is never applied.  The photometric mode (dvo_oracle.cpp:879-882, 913-1002) adds
 (alpha, beta) to the Revertable state: the top of an iteration adds the (alpha, beta) part dab of the previous accepted
 solve of the same level (0 at a level start), a revert restores them, and they carry over between levels.  The log does
 not hold dab, so the replay takes it from the reference's own 8 x 8 solve at the replayed pose and brightness.  Each dab
@@ -157,10 +157,9 @@ class Log:
 
 
 def as_log(result, ab=None):
-    """an engine Result (with_iterations=True) with its final (alpha, beta), or an oracle match dict (orc.match,
-    prior_oracle.match)"""
+    """an engine Result (with_iterations=True) with its final (alpha, beta), or an oracle match dict (orc.match)"""
     if isinstance(result, dict):
-        lv = [(l["termination"], l["num_iterations"]) if isinstance(l, dict) else tuple(l) for l in result["levels"]]
+        lv = [(l["termination"], l["num_iterations"]) for l in result["levels"]]
         return Log(result["iterations"], lv, np.asarray(result["T"]), result.get("ab") if ab is None else ab)
     return Log(result.iterations, [(l["termination"], l["num_iterations"]) for l in result.levels], result.transformation, ab)
 
@@ -203,7 +202,7 @@ def replay(log, cfg, linearize, T0=None, mu=0.0, prior=None, photometric=False, 
         return rep
     for li_, (level, (term, count)) in enumerate(zip(level_ids, log.levels)):
         entries = log.iterations[k0:k0 + count]
-        x = np.zeros(6) if (mut == "no_level_start_reapply" and li_ > 0) else se3_log(inc)     # dvo_oracle.cpp:820
+        x = np.zeros(6) if (mut == "no_level_start_reapply" and li_ > 0) else se3_log(inc)     # dvo_oracle.cpp:912
         dab = np.zeros(2)
         prev_nll, prev_P = np.inf, None
         iteration, ended, model_term = 0, False, -1
@@ -214,14 +213,14 @@ def replay(log, cfg, linearize, T0=None, mu=0.0, prior=None, photometric=False, 
                 break
             if e["level"] != level or e["id"] != j:
                 rep.failures.append(("decision", idx, f"entry ({e['level']}, {e['id']}) at ({level}, {j})"))
-            inc = se3_exp(x)                                                                     # :830-832
+            inc = se3_exp(x)                                                                     # :923-925
             saved = (initial, estimate, None if ab is None else ab.copy(), path.copy())
             initial, estimate = se3_inv(inc) @ initial, inc @ estimate
             if photometric:
                 ab, path = ab + dab, path + np.abs(dab)
             r = linearize(level, estimate, ab, j > 0, prev_P)
             rep.note("n", abs(int(e["n"]) - int(r["n"])), bounds.n, idx)
-            if e["n"] < 6:                                                                       # :841-847
+            if e["n"] < 6:                                                                       # :942-948
                 if np.isfinite(e["x"]).any():
                     rep.failures.append(("decision", idx, "an increment on an entry with n < 6"))
                 initial, estimate, sab, spath = saved
@@ -248,12 +247,12 @@ def replay(log, cfg, linearize, T0=None, mu=0.0, prior=None, photometric=False, 
             # The scale has the floor prior_abs / prior_rel, so that the reported value is measured against prior_rel.
             s = max(abs(prior_r) + 2.0 * np.abs(lam @ li).max() * np.abs(li).max(), bounds.prior_abs / bounds.prior_rel)
             rep.note("prior", abs(e["prior"] - prior_r) / s, bounds.prior_rel, idx, f"({e['prior']} vs {prior_r})")
-            accept = e["nll"] < prev_nll                                                         # :864-866
+            accept = e["nll"] < prev_nll                                                         # :972-974
             if mut == "flip_accept" and idx == mutation.entry:
                 accept = not accept
             if np.isfinite(e["x"]).all() != accept or np.isfinite(e["A"]).all() != accept:
                 rep.failures.append(("decision", idx, f"accept = {accept}, increment {e['x']}"))
-            if not accept:                                                                       # :867-873
+            if not accept:                                                                       # :975-981
                 initial, estimate, sab, spath = saved
                 if photometric and mut != "ab_not_reverted":
                     ab, path = sab, spath
@@ -267,19 +266,19 @@ def replay(log, cfg, linearize, T0=None, mu=0.0, prior=None, photometric=False, 
             if np.isfinite(xg).all():
                 eta = np.abs(M @ xg - c).max() / (np.abs(M).sum(axis=1).max() * np.abs(xg).max() + np.abs(c).max())
                 rep.note("x", eta, bounds.tau, idx)
-                x = xg                                                                            # :880-881
+                x = xg                                                                            # :995-996
             if photometric:
                 dab = dab_r
             prev_nll, prev_P = e["nll"], Pg
-            iteration += 1                                                                        # :884
+            iteration += 1                                                                        # :1004
             rep.states.append((estimate, None if ab is None else ab.copy(), path.copy()))
-            if not (np.abs(x).max() > precision and iteration < max_it):                         # :885
+            if not (np.abs(x).max() > precision and iteration < max_it):                         # :1005
                 ended = True
         if not ended:
             rep.failures.append(("decision", k0 + count - 1, f"level {level}: the loop goes on after {count} entries"))
-        if np.abs(x).max() <= precision:                                                         # :887
+        if np.abs(x).max() <= precision:                                                         # :1007
             model_term = TERM_INCREMENT_TOO_SMALL
-        if iteration >= max_it:                                                                  # :888
+        if iteration >= max_it:                                                                  # :1008
             model_term = TERM_ITERATIONS_EXCEEDED
         if model_term != term:
             rep.failures.append(("decision", k0 + count - 1, f"level {level}: termination {term}, replayed {model_term}"))
@@ -411,39 +410,30 @@ def mode_of(c):
     return orc.mode("mirror") if c["estimator"] == "reference" else corrected_mode(orc)
 
 
+def _oracle_pyramids(c):
+    """the oracle's pyramids of case c, its mask (if any) in both roles"""
+    from masked_oracle import masked_pyramid
+    from oracle import oracle_py as orc
+    return (masked_pyramid(orc, c["I_ref"], c["Z_ref"], c["K"], c["levels"], c["mask"]),
+            masked_pyramid(orc, c["I_cur"], c["Z_cur"], c["K"], c["levels"], c["mask"]))
+
+
 def oracle_linearize(c):
-    """the reference linearisation callback of replay() for case c"""
+    """the reference linearisation callback of replay() for case c (ab is None outside the photometric mode)"""
     from oracle import oracle_py as orc
     m = mode_of(c)
     ti = float(c["cfg"].get("intensity_derivative_threshold", 0.0))
     td = float(c["cfg"].get("depth_derivative_threshold", 0.0))
-    if c["photometric"]:
-        import photometric_oracle as pho
-        assert ti == 0.0 and td == 0.0
-        pref = pho.Pyramid(c["I_ref"], c["Z_ref"], c["K"], c["levels"], mask=c["mask"])
-        pcur = pho.Pyramid(c["I_cur"], c["Z_cur"], c["K"], c["levels"], mask=c["mask"])
-        return lambda level, T, ab, uw, pp: pho.linearize(pref, pcur, level, T, ab, m, uw, pp)
-    assert c["mask"] is None
-    oref = orc.Pyramid(c["I_ref"], c["Z_ref"], c["K"], c["levels"])
-    ocur = orc.Pyramid(c["I_cur"], c["Z_cur"], c["K"], c["levels"])
-    return lambda level, T, ab, uw, pp: orc.linearize(oref, ocur, level, T, m, uw, pp, ti, td)
+    oref, ocur = _oracle_pyramids(c)
+    return lambda level, T, ab, uw, pp: orc.linearize(oref, ocur, level, T, m, uw, pp, ti, td, ab=ab)
 
 
 def oracle_log(c):
     """the oracle's own match of case c, with its iteration log"""
     from oracle import oracle_py as orc
-    m = mode_of(c)
-    cfg = orc.config(**c["cfg"])
-    if not c["photometric"] and c["prior"] is None:
-        assert c["mask"] is None
-        oref = orc.Pyramid(c["I_ref"], c["Z_ref"], c["K"], c["levels"])
-        ocur = orc.Pyramid(c["I_cur"], c["Z_cur"], c["K"], c["levels"])
-        return as_log(orc.match(oref, ocur, cfg, m, T_init=c["T_init"]))
-    import prior_oracle as pro
-    pref = pro.Pyramid(c["I_ref"], c["Z_ref"], c["K"], c["levels"], mask=c["mask"])
-    pcur = pro.Pyramid(c["I_cur"], c["Z_cur"], c["K"], c["levels"], mask=c["mask"])
-    return as_log(pro.match(pref, pcur, cfg, m, T_init=c["T_init"], prior=c["prior"], photometric=c["photometric"],
-                            ab_init=c["ab0"]))
+    oref, ocur = _oracle_pyramids(c)
+    return as_log(orc.match(oref, ocur, orc.config(**c["cfg"]), mode_of(c), T_init=c["T_init"], prior=c["prior"],
+                            photometric=c["photometric"], ab_init=c["ab0"]))
 
 
 def replay_case(c, log, bounds=Bounds(), mutation=None, linearize=None):

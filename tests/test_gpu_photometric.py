@@ -1,11 +1,10 @@
-"""The photometric mode on the GPU against its oracle definition (tests/photometric_oracle.py): residual records bit for
+"""The photometric mode on the GPU against its oracle definition (the ab inputs of oracle/dvo_oracle.h): residual records bit for
 bit, the hooks at (1, 0) against the default hooks, whole alignments, batch invariance, accuracy and refusals."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
-import photometric_oracle as pho
 from dvo_slam_b200 import synth
 from dvo_slam_b200.engine import CResult, Config
 
@@ -29,16 +28,16 @@ def _gpu(engine, pair, Ic=None):
 def test_records_match_the_oracle_mirror(engine, oracle, pairs, ab):
     pair = pairs[0]
     ref, cur = _gpu(engine, pair)
-    pref = pho.Pyramid(pair["I_ref"].numpy(), pair["Z_ref"].numpy(), SCENE.intrinsics, 3)
-    pcur = pho.Pyramid(pair["I_cur"].numpy(), pair["Z_cur"].numpy(), SCENE.intrinsics, 3)
+    pref = oracle.Pyramid(pair["I_ref"].numpy(), pair["Z_ref"].numpy(), SCENE.intrinsics, 3)
+    pcur = oracle.Pyramid(pair["I_cur"].numpy(), pair["Z_cur"].numpy(), SCENE.intrinsics, 3)
     T = np.linalg.inv(pair["T_true"])
     m = oracle.mode("mirror")
     for level in (0, 2):
         n, img = engine.residual_image(ref, cur, level, T, ab=ab)
-        no, imgo = pho.residual_image(pref, pcur, level, T, ab, m)
+        no, imgo = oracle.residual_image(pref, pcur, level, T, m, ab=ab)
         assert n == no and np.array_equal(img, imgo, equal_nan=True)
         g = engine.linearize(ref, cur, level, T, ab=ab)
-        o = pho.linearize(pref, pcur, level, T, ab, m)
+        o = oracle.linearize(pref, pcur, level, T, m, ab=ab)
         assert g["n"] == o["n"]
         assert np.allclose(g["precision"], o["precision"], rtol=2e-6)
         assert abs(g["ll"] - o["ll"]) <= 2e-6 * abs(o["ll"])
@@ -80,8 +79,9 @@ def test_alignments_match_the_oracle_and_are_batch_invariant(engine, oracle, pai
         Ic = synth.exposure(pair["I_cur"].numpy(), g, b)
         r, c = _gpu(engine, pair, Ic)
         refs.append(r); curs.append(c)
-        orcs.append(pho.match(pho.Pyramid(pair["I_ref"].numpy(), pair["Z_ref"].numpy(), SCENE.intrinsics, 3),
-                              pho.Pyramid(Ic, pair["Z_cur"].numpy(), SCENE.intrinsics, 3), ocfg, oracle.mode("mirror")))
+        orcs.append(oracle.match(oracle.Pyramid(pair["I_ref"].numpy(), pair["Z_ref"].numpy(), SCENE.intrinsics, 3),
+                                 oracle.Pyramid(Ic, pair["Z_cur"].numpy(), SCENE.intrinsics, 3), ocfg, oracle.mode("mirror"),
+                                 photometric=True))
     res, ab = engine.match_batch_photometric(refs, curs, cfg)
     for i, (r, o) in enumerate(zip(res, orcs)):
         dt, dr = _pose_err(r.transformation, np.linalg.inv(o["T"]))
@@ -145,6 +145,7 @@ def test_refusals_move_no_counters(engine, pairs):
 
 
 # ---- the generic pixel loops, current-role masks, both estimators, every launch plan ----------------------------------
+from masked_oracle import masked_pyramid  # noqa: E402
 from test_corrected_estimator import corrected_mode  # noqa: E402
 
 PP = np.array([[2000.0, -30.0], [-30.0, 9000.0]], dtype=np.float32)
@@ -187,11 +188,11 @@ def _check_records_both_estimators(engine, oracle, gref, gcur, pref, pcur, lvl, 
         engine.set_estimator(est)
         try:
             n, img = engine.residual_image(gref, gcur, lvl, T, ab=ab)
-            no, imgo = pho.residual_image(pref, pcur, lvl, T, ab, mode)
+            no, imgo = oracle.residual_image(pref, pcur, lvl, T, mode, ab=ab)
             assert n == no and n > 0 and np.array_equal(img, imgo, equal_nan=True), (est, lvl, n, no)
             for uw in (False, True):
                 g = engine.linearize(gref, gcur, lvl, T, uw, PP, ab=ab)
-                o = pho.linearize(pref, pcur, lvl, T, ab, mode, uw, PP)
+                o = oracle.linearize(pref, pcur, lvl, T, mode, uw, PP, ab=ab)
                 assert g["n"] == o["n"] == no, (est, lvl, uw)
                 assert np.allclose(g["precision"], o["precision"], rtol=2e-6, atol=2e-6 * np.abs(o["precision"]).max()), (est, lvl, uw)
                 assert abs(g["ll"] - o["ll"]) <= 2e-6 * abs(o["ll"]) + 0.5, (est, lvl, uw)
@@ -230,8 +231,8 @@ def test_records_on_the_generic_loops(engine, oracle, pair0, case):
     gref = engine.pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
     gcur = engine.pyramid(a["I_cur"], a["Z_cur"], a["K"], 5) if m is None else \
         engine.pyramid(a["I_cur"], a["Z_cur"], a["K"], 5, mask=m, mask_roles="both")
-    pref = pho.Pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
-    pcur = pho.Pyramid(a["I_cur"], a["Z_cur"], a["K"], 5, mask=m)
+    pref = oracle.Pyramid(a["I_ref"], a["Z_ref"], a["K"], 5)
+    pcur = masked_pyramid(oracle, a["I_cur"], a["Z_cur"], a["K"], 5, m)
     for lvl in lvls:
         _check_records_both_estimators(engine, oracle, gref, gcur, pref, pcur, lvl, T, AB_FORCED)
 
@@ -245,7 +246,7 @@ def _same(r0, ab0, r1, ab1):
 
 
 @pytest.fixture(scope="module")
-def masked_batch(engine):
+def masked_batch(engine, oracle):
     """six exposure pairs; pairs 1, 3 and 4 have a mask in both roles (the current role selects the kCurMask instances)"""
     exps = [(1.1, 0.0), (0.9, 5.0), (1.2, -15.0), (1.0, 0.0), (0.85, 10.0), (1.05, -8.0)]
     out = []
@@ -256,8 +257,8 @@ def masked_batch(engine):
         kw = {} if m is None else {"mask": m, "mask_roles": "both"}
         out.append({"gref": engine.pyramid(p["I_ref"].numpy(), p["Z_ref"].numpy(), SCENE.intrinsics, 3, **kw),
                     "gcur": engine.pyramid(Ic, p["Z_cur"].numpy(), SCENE.intrinsics, 3, **kw),
-                    "pref": pho.Pyramid(p["I_ref"].numpy(), p["Z_ref"].numpy(), SCENE.intrinsics, 3, mask=m),
-                    "pcur": pho.Pyramid(Ic, p["Z_cur"].numpy(), SCENE.intrinsics, 3, mask=m)})
+                    "pref": masked_pyramid(oracle, p["I_ref"].numpy(), p["Z_ref"].numpy(), SCENE.intrinsics, 3, m),
+                    "pcur": masked_pyramid(oracle, Ic, p["Z_cur"].numpy(), SCENE.intrinsics, 3, m)})
     return out
 
 
@@ -274,7 +275,7 @@ def test_masked_alignments_match_the_oracle_under_every_plan(engine, oracle, mas
     try:
         single = [engine.match_batch_photometric([r], [c], cfg) for r, c in zip(refs, curs)]
         for (res, ab), q in zip(single, masked_batch):
-            o = pho.match(q["pref"], q["pcur"], ocfg, mode)
+            o = oracle.match(q["pref"], q["pcur"], ocfg, mode, photometric=True)
             dt, dr = _pose_err(res[0].transformation, np.linalg.inv(o["T"]))
             assert dt < 1e-4 and dr < 1e-4, (dt, dr)
             assert np.allclose(ab[0], o["ab"], rtol=1e-3, atol=1e-2), (ab[0], o["ab"])

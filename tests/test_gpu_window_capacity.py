@@ -13,7 +13,6 @@ residuals, and the two arithmetic orders give P, A and b up to 4.7e-6 apart.
 import numpy as np
 import pytest
 
-import photometric_oracle as pho
 import window_model as wm
 from test_corrected_estimator import corrected_mode
 from test_gpu_geometry import _check_linearisation, _unfused
@@ -43,7 +42,7 @@ def plane(engine, oracle):
     m = np.ones((wm.H, wm.W), np.uint8)
     m[30:60, 90:140] = 0
     m[90:110, 330:370] = 0
-    out = {"I": I, "Z": Z, "Ic": Ic, "Zc": Zc, "mask": m}
+    out = {"Z": Z}
     out["ref"] = _pyrs(engine, oracle, I, Z, wm.K, None, "both", 1)
     out["cur"] = _pyrs(engine, oracle, Ic, Zc, wm.K, None, "both", 1)
     out["cur_masked"] = _pyrs(engine, oracle, Ic, Zc, wm.K, m, "both", 1)
@@ -61,27 +60,17 @@ def _check(eng, mode, gref, gcur, oref, ocur, T, lin):
         _check_linearisation(lg, lin(oref, ocur, T, mode, uw), lin(oref, ocur, T, _unfused(mode), uw))
 
 
-class _Plain:
-    ab = None
+class _Hooks:
+    """the oracle's records and linearisation at level 0, in the photometric mode at ab, or the default mode for ab None"""
 
-    def __init__(self, oracle):
-        self.o = oracle
+    def __init__(self, oracle, ab=None):
+        self.o, self.ab = oracle, ab
 
     def records(self, oref, ocur, T, mode):
-        return self.o.residual_image(oref, ocur, 0, T, mode)
+        return self.o.residual_image(oref, ocur, 0, T, mode, ab=self.ab)
 
     def __call__(self, oref, ocur, T, mode, uw):
-        return self.o.linearize(oref, ocur, 0, T, mode, uw, PP)
-
-
-class _Photometric:
-    ab = AB_FORCED
-
-    def records(self, pref, pcur, T, mode):
-        return pho.residual_image(pref, pcur, 0, T, self.ab, mode)
-
-    def __call__(self, pref, pcur, T, mode, uw):
-        return pho.linearize(pref, pcur, 0, T, self.ab, mode, uw, PP)
+        return self.o.linearize(oref, ocur, 0, T, mode, uw, PP, ab=self.ab)
 
 
 def _both_estimators(engine, corrected, oracle, gref, gcur, oref, ocur, T, lin):
@@ -95,18 +84,16 @@ def test_records_at_the_window_limits(engine, corrected, oracle, plane, case):
     wins = wm.level_windows(wm.K, T, plane["Z"])
     print(f"\n{case}: {wm.census(wins)}")
     (gref, oref), (gcur, ocur) = plane["ref"], plane["cur"]
-    _both_estimators(engine, corrected, oracle, gref, gcur, oref, ocur, T, _Plain(oracle))
+    _both_estimators(engine, corrected, oracle, gref, gcur, oref, ocur, T, _Hooks(oracle))
     gcm, ocm = plane["cur_masked"]
-    _both_estimators(engine, corrected, oracle, gref, gcm, oref, ocm, T, _Plain(oracle))
+    _both_estimators(engine, corrected, oracle, gref, gcm, oref, ocm, T, _Hooks(oracle))
 
 
 @pytest.mark.parametrize("case", ["edges", "roll2.6", "roll2.9", "forward1.112", "forward1.12", "forward2.5", "right_in",
                                   "bottom_in"])
 def test_photometric_records_at_the_window_limits(engine, corrected, oracle, plane, case):
     T = wm.CASES[case]
-    pref = pho.Pyramid(plane["I"], plane["Z"], wm.K, 1)
-    for masked in (False, True):
-        m = plane["mask"] if masked else None
-        gcur = plane["cur_masked"][0] if masked else plane["cur"][0]
-        pcur = pho.Pyramid(plane["Ic"], plane["Zc"], wm.K, 1, mask=m)
-        _both_estimators(engine, corrected, oracle, plane["ref"][0], gcur, pref, pcur, T, _Photometric())
+    gref, oref = plane["ref"]
+    for key in ("cur", "cur_masked"):
+        gcur, ocur = plane[key]
+        _both_estimators(engine, corrected, oracle, gref, gcur, oref, ocur, T, _Hooks(oracle, AB_FORCED))

@@ -45,13 +45,12 @@ def scenes(oracle):
 
 
 @pytest.fixture(scope="module")
-def photometric_scene():
-    import photometric_oracle as pho
+def photometric_scene(oracle):
     from dvo_slam_b200 import synth
     a = _synth(320)
     a["I_cur"] = synth.exposure(a["I_cur"], *EXPOSURE)
-    a["pref"] = pho.Pyramid(a["I_ref"], a["Z_ref"], a["K"], 3)
-    a["pcur"] = pho.Pyramid(a["I_cur"], a["Z_cur"], a["K"], 3)
+    a["pref"] = oracle.Pyramid(a["I_ref"], a["Z_ref"], a["K"], 3)
+    a["pcur"] = oracle.Pyramid(a["I_cur"], a["Z_cur"], a["K"], 3)
     return a
 
 
@@ -66,17 +65,10 @@ def _mirror(oracle, a, level, T, estimator, uw, pp=PP):
     return rec, oracle.linearize(a["oref"], a["ocur"], level, T, m, uw, pp)
 
 
-def _pho_intensity(p, level):
-    import photometric_oracle as pho
-    w, h = p.level_info(level)
-    return np.ctypeslib.as_array(pho.lib().orc_pyramid_plane(p.h, level, 0), shape=(h, w)).copy()
-
-
 def _pho_mirror(oracle, a, level, T, ab, estimator, uw):
-    import photometric_oracle as pho
     m = _mode(oracle, estimator)
-    _, rec = pho.residual_image(a["pref"], a["pcur"], level, T, ab, m)
-    return rec, pho.linearize(a["pref"], a["pcur"], level, T, ab, m, uw, PP), _pho_intensity(a["pref"], level)
+    _, rec = oracle.residual_image(a["pref"], a["pcur"], level, T, m, ab=ab)
+    return rec, oracle.linearize(a["pref"], a["pcur"], level, T, m, uw, PP, ab=ab), a["pref"].plane(level, 0)
 
 
 def _assert_holds(rep, limit=0.5):

@@ -1,5 +1,5 @@
 """The motion prior without a GPU: the argument checks of csrc/prior_args.h built for the host, and the prior's definition on
-the CPU oracle (tests/native/prior_oracle.cpp) against the oracle's own mu path, in both modes."""
+the CPU oracle (orc_match_with's prior input, oracle/dvo_oracle.h) against the oracle's own mu path, in both modes."""
 import ctypes as C
 import os
 import shutil
@@ -9,7 +9,6 @@ import tempfile
 import numpy as np
 import pytest
 
-import prior_oracle as pro
 from dvo_slam_b200 import synth
 from dvo_slam_b200.engine import prior_from_result
 
@@ -94,12 +93,12 @@ SCENE = synth.SceneConfig(width=160, height=120, intrinsics=tuple(v / 4 for v in
 
 
 @pytest.fixture(scope="module")
-def pyrs():
+def pyrs(oracle):
     out = []
     for seed in (3, 5):
         pair = synth.make_pair(seed, SCENE)
-        out.append((pro.Pyramid(pair["I_ref"].numpy(), pair["Z_ref"].numpy(), SCENE.intrinsics, 3),
-                    pro.Pyramid(pair["I_cur"].numpy(), pair["Z_cur"].numpy(), SCENE.intrinsics, 3), pair))
+        out.append((oracle.Pyramid(pair["I_ref"].numpy(), pair["Z_ref"].numpy(), SCENE.intrinsics, 3),
+                    oracle.Pyramid(pair["I_cur"].numpy(), pair["Z_cur"].numpy(), SCENE.intrinsics, 3), pair))
     return out
 
 
@@ -137,8 +136,8 @@ def test_scalar_prior_is_the_mu_path(oracle, pyrs, mode, photometric, mu):
     m = oracle.mode(mode)
     for ref, cur, pair in pyrs:
         T0 = _T0(pair)
-        d = pro.match(ref, cur, _cfg(oracle, mu), m, T0, photometric=photometric)
-        p = pro.match(ref, cur, _cfg(oracle), m, T0, prior=mu * np.eye(6), photometric=photometric)
+        d = oracle.match(ref, cur, _cfg(oracle, mu), m, T0, photometric=photometric)
+        p = oracle.match(ref, cur, _cfg(oracle), m, T0, prior=mu * np.eye(6), photometric=photometric)
         assert any(it["prior"] != 0.0 for it in d["iterations"])
         _same(p, d, prior_tol=1e-14)
         if photometric:
@@ -151,8 +150,8 @@ def test_zero_prior_is_mu_zero(oracle, pyrs, mode, photometric):
     m = oracle.mode(mode)
     for ref, cur, pair in pyrs:
         T0 = _T0(pair)
-        d = pro.match(ref, cur, _cfg(oracle), m, T0, photometric=photometric)
-        p = pro.match(ref, cur, _cfg(oracle), m, T0, prior=np.zeros((6, 6)), photometric=photometric)
+        d = oracle.match(ref, cur, _cfg(oracle), m, T0, photometric=photometric)
+        p = oracle.match(ref, cur, _cfg(oracle), m, T0, prior=np.zeros((6, 6)), photometric=photometric)
         _same(p, d)
 
 
@@ -166,7 +165,7 @@ def test_stiff_prior_returns_the_initial_estimate(oracle, pyrs, mode, photometri
     m = oracle.mode(mode)
     for ref, cur, pair in pyrs:
         T0 = _T0(pair)
-        p = pro.match(ref, cur, _cfg(oracle), m, T0, prior=STIFF * np.eye(6), photometric=photometric)
+        p = oracle.match(ref, cur, _cfg(oracle), m, T0, prior=STIFF * np.eye(6), photometric=photometric)
         assert np.abs(synth.se3_log(T0 @ p["T"])).max() < 1e-8
 
 
@@ -180,7 +179,7 @@ def test_stiff_rank_one_prior_holds_its_direction(oracle, pyrs, mode, photometri
     for ref, cur, pair in pyrs:
         T0 = _T0(pair)
         e = np.zeros(6); e[k] = 1.0
-        p = pro.match(ref, cur, _cfg(oracle), m, T0, prior=STIFF * np.outer(e, e), photometric=photometric)
+        p = oracle.match(ref, cur, _cfg(oracle), m, T0, prior=STIFF * np.outer(e, e), photometric=photometric)
         d = synth.se3_log(T0 @ p["T"])
         assert abs(d[k]) < 2e-4, d
         assert np.abs(np.delete(d, k)).max() > 4e-3, d
