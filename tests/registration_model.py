@@ -66,9 +66,10 @@ def _row(R, t, r, X, Y, Z):
     return ((R[r, 0] * X + R[r, 1] * Y) + R[r, 2] * Z) + t[r]
 
 
-def register(depth, rays, T, size, K, depth_scale=None):
-    """One depth frame [dh, dw] -> the registered float32 depth plane [h, w] of the colour camera (NaN: uncovered)"""
-    w, h = size
+def footprints(depth, rays, T, K, depth_scale=None):
+    """Per depth pixel [dh, dw]: (ok, zc, x0, x1, y0, y1).  ok: the pixel projects (valid depth, in front of the colour
+    camera at its centre and its four corners, finite corners), before the footprint limit; zc: float32 colour-camera depth
+    of its centre ray; [x0, x1) x [y0, y1): the colour pixel centres inside its footprint, 0 where not ok."""
     R = np.asarray(T, np.float64)[:3, :3].astype(F32)
     t = np.asarray(T, np.float64)[:3, 3].astype(F32)
     fx, fy, cx, cy = (F32(v) for v in K)
@@ -94,6 +95,13 @@ def register(depth, rays, T, size, K, depth_scale=None):
     ys = np.where(ok, np.stack(ys), F32(0))
     x0, x1 = np.ceil(xs.min(0)).astype(np.int64), np.ceil(xs.max(0)).astype(np.int64)
     y0, y1 = np.ceil(ys.min(0)).astype(np.int64), np.ceil(ys.max(0)).astype(np.int64)
+    return ok, zc, x0, x1, y0, y1
+
+
+def register(depth, rays, T, size, K, depth_scale=None):
+    """One depth frame [dh, dw] -> the registered float32 depth plane [h, w] of the colour camera (NaN: uncovered)"""
+    w, h = size
+    ok, zc, x0, x1, y0, y1 = footprints(depth, rays, T, K, depth_scale)
     ok &= (x1 - x0 <= MAX_FOOTPRINT) & (y1 - y0 <= MAX_FOOTPRINT)
     zbuf = np.full(h * w, 0xFFFFFFFF, np.uint32)
     bits = zc.astype(F32).view(np.uint32)
