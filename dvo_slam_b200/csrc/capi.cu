@@ -2,6 +2,7 @@
 #include "common.cuh"
 #include "hypotheses_args.h"
 #include "maps_args.h"
+#include "modes_args.h"
 #include "prior_args.h"
 
 #include <algorithm>
@@ -682,7 +683,7 @@ int dvo_b200_match_batch_device(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, i
   cudaSetDevice(ctx->device);
   MatchCall c;
   c.cfg = cfg; c.n = n; c.refs = references; c.curs = currents; c.T_init = T_init;
-  c.d_results = d_results;
+  c.results = (dvo_b200_result*)d_results; c.device_outputs = true;
   return tracker_match(ctx, c);
 }
 
@@ -762,15 +763,7 @@ int dvo_b200_match_batch_prior(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, in
 // The largest extents of a batch's references at cfg->last_level and level 0, or false for a batch the match would refuse
 // (the maps are then checked as for n = 0 and the batch checks refuse it)
 static bool maps_extent(const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references, MapsExtent* ext) {
-  *ext = MapsExtent{0, 0, 0, 0};
-  if (!(cfg && n > 0 && references && cfg->last_level >= 0 && cfg->last_level < kMaxLevels)) return false;
-  for (int32_t i = 0; i < n; ++i) {
-    const dvo_b200_pyramid* r = references[i];
-    if (!r || r->levels <= cfg->last_level) return false;
-    ext->w = std::max(ext->w, r->L[cfg->last_level].w); ext->h = std::max(ext->h, r->L[cfg->last_level].h);
-    ext->w0 = std::max(ext->w0, r->L[0].w); ext->h0 = std::max(ext->h0, r->L[0].h);
-  }
-  return true;
+  return batch_maps_extent(cfg, n, references, pyramid_view, ext);
 }
 
 // where one byte of a maps output lies (maps_args.h)
@@ -841,6 +834,34 @@ int dvo_b200_match_batch_hypotheses(dvo_b200_ctx* ctx, const dvo_b200_config* cf
   return dvo_b200_match_batch_hypotheses_modes(ctx, cfg, n, references, currents, k, hypotheses, screen_level, min_constraint_ratio,
                                                nullptr, nullptr, nullptr, nullptr, results, best, scores, screen_results,
                                                iteration_stats, max_iteration_stats, nullptr);
+}
+
+// ---- every mode with outputs in device memory ----
+int dvo_b200_match_batch_modes_device(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,
+                                      dvo_b200_pyramid* const* currents, int32_t k, const double* hypotheses, int32_t screen_level,
+                                      double min_constraint_ratio, const double* prior_information, const double* photometric_init,
+                                      double* photometric, double* screen_photometric, dvo_b200_result* results, int32_t* best,
+                                      double* scores, dvo_b200_result* screen_results, dvo_b200_iteration_stats* iteration_stats,
+                                      int32_t max_iteration_stats, const dvo_b200_weight_maps* maps) {
+  if (!ctx) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match_batch_modes_device: null argument");
+  ModesArgs a;
+  a.cfg = cfg; a.n = n; a.refs = references; a.curs = currents; a.k = k; a.hypotheses = hypotheses; a.screen_level = screen_level;
+  a.min_ratio = min_constraint_ratio; a.prior = prior_information; a.ab_init = photometric_init; a.ab = photometric;
+  a.screen_ab = screen_photometric; a.results = results; a.best = best; a.scores = scores; a.screen_results = screen_results;
+  a.iter_stats = iteration_stats; a.max_log = max_iteration_stats; a.maps = maps;
+  int code = 0;
+  const std::string why = modes_args_error(a, kFormDevice, 1, &ctx->device, pyramid_view, pointer_where, &code);
+  if (!why.empty()) return set_error(ctx, code, why);
+  cudaSetDevice(ctx->device);
+  MatchCall c;
+  c.cfg = cfg; c.n = n; c.refs = references; c.curs = currents; c.T_init = hypotheses;
+  c.k = k; c.screen_level = screen_level; c.min_ratio = min_constraint_ratio;
+  c.prior = prior_information; c.ab_init = photometric_init;
+  c.results = results; c.ab_out = photometric; c.screen_ab = screen_photometric;
+  c.best = best; c.scores = scores; c.screen_results = screen_results;
+  c.iter_stats = iteration_stats; c.max_log = max_iteration_stats; c.maps = maps;
+  c.device_outputs = true;
+  return tracker_match(ctx, c);
 }
 
 int dvo_b200_residual_image_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* reference,

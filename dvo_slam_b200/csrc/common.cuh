@@ -12,6 +12,7 @@
 
 #include "../../include/dvo_b200.h"
 #include "create_args.h"
+#include "modes_args.h"
 #include "se3.cuh"
 
 namespace dvo_b200 {
@@ -298,18 +299,22 @@ struct MatchCall {
   double min_ratio = 0.0;                // k >= 1: hypothesis_score's minimum ratio of constraints to valid pixels
   const double* prior = nullptr;         // a motion prior: row-major 6 x 6 informations (host) in place of cfg->mu I (then 0)
   const double* ab_init = nullptr;       // photometric mode: the starting (alpha, beta) (host, 2 doubles each), NULL = (1, 0)
-  dvo_b200_result* results = nullptr;    // host, n; or
-  void* d_results = nullptr;             // device, n: the call enqueues its work and returns (k = 0, no other output)
-  double* ab_out = nullptr;              // != NULL: the photometric mode (pose, gain, bias); final (alpha, beta) (host, 2n)
-  double* screen_ab = nullptr;           // k >= 1, photometric: (alpha, beta) where each screening run ended (host, 2nk)
-  int32_t* best = nullptr;               // k >= 1: the chosen hypothesis of each pair (host, n)
-  double* scores = nullptr;              // k >= 1: the score of each hypothesis (host, nk)
-  dvo_b200_result* screen_results = nullptr;   // k >= 1: the result of each screening run (host, nk)
-  dvo_b200_iteration_stats* iter_stats = nullptr;   // iteration logs (host, max_log per pair)
+  dvo_b200_result* results = nullptr;    // n
+  double* ab_out = nullptr;              // != NULL: the photometric mode (pose, gain, bias); final (alpha, beta) (2n)
+  double* screen_ab = nullptr;           // k >= 1, photometric: (alpha, beta) where each screening run ended (2nk)
+  int32_t* best = nullptr;               // k >= 1: the chosen hypothesis of each pair (n)
+  double* scores = nullptr;              // k >= 1: the score of each hypothesis (nk)
+  dvo_b200_result* screen_results = nullptr;   // k >= 1: the result of each screening run (nk)
+  dvo_b200_iteration_stats* iter_stats = nullptr;   // iteration logs (max_log per pair)
   int max_log = 0;                       // entries per pair of iter_stats (ignored without it)
   const dvo_b200_weight_maps* maps = nullptr;   // also the weight maps (weight_maps.cu) of the returned alignments
+  // false: every output above is host memory, and the call returns once they hold the results.  true: every output is
+  // device memory of the context's device (maps: DVO_B200_MAPS_DEVICE); the call enqueues its work and returns, and its
+  // level flags surface at dvo_b200_synchronize.
+  bool device_outputs = false;
 };
 int tracker_match(dvo_b200_ctx* ctx, const MatchCall& c);
+PyramidView pyramid_view(const dvo_b200_pyramid* p, int level);   // what modes_args.h reads of a pyramid
 int check_level_flags(dvo_b200_ctx* ctx);   // after a stream synchronisation: did a level kernel report a timeout?
 // The test hooks: one iteration at T (staged as the leg's initial estimate and placed into the state by k_set_state).
 int tracker_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_pyramid* ref, dvo_b200_pyramid* cur,

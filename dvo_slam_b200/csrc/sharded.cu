@@ -8,7 +8,9 @@
 // multi-process form of the same sharding (one rank per GPU, NCCL all-gather of the result records) is
 // dvo_slam_b200/distributed.py on top of dvo_b200_match_batch_device.
 //
-// Written against the public C ABI only (include/dvo_b200.h): a caller could do the same with its own threads.
+// Written against the public C ABI only (include/dvo_b200.h): a caller could do the same with its own threads.  The checks
+// and the slicing of dvo_b200_match_batch_modes_sharded are those of modes_args.h, which reads nothing but what the ABI
+// exposes.
 #include <cuda_runtime.h>
 
 #include <string>
@@ -16,6 +18,7 @@
 #include <vector>
 
 #include "../../include/dvo_b200.h"
+#include "modes_args.h"
 
 struct dvo_b200_sharded {
   std::vector<int> devices;
@@ -55,6 +58,44 @@ int for_each_shard(dvo_b200_sharded* s, int64_t total, F&& body) {
       return fail(s, rc[size_t(k)], "shard " + std::to_string(k) + " (device " + std::to_string(s->devices[size_t(k)]) + "): " +
                                         dvo_b200_last_error(s->ctx[size_t(k)]));
   return 0;
+}
+
+// What modes_args.h reads of a pyramid and of a pointer, through the public ABI and the CUDA runtime
+dvo_b200::PyramidView public_view(const dvo_b200_pyramid* p, int level) {
+  dvo_b200::PyramidView v{dvo_b200_pyramid_num_levels(p), dvo_b200_pyramid_device(p), 0, 0, 0, 0};
+  dvo_b200_pyramid_level_info(p, 0, &v.w0, &v.h0, nullptr);
+  dvo_b200_pyramid_level_info(p, level, &v.w, &v.h, nullptr);   // leaves 0 x 0 for a level the pyramid does not have
+  return v;
+}
+
+dvo_b200::PtrWhere public_where(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return {dvo_b200::kPtrHost, -1}; }
+  if (a.type == cudaMemoryTypeDevice) return {dvo_b200::kPtrDevice, a.device};
+  if (a.type == cudaMemoryTypeManaged) return {dvo_b200::kPtrManaged, a.device};
+  return {dvo_b200::kPtrHost, -1};
+}
+
+// E of a shard's slice (modes_args.h: modes_entry) on the shard's context
+int call_entry(dvo_b200_ctx* ctx, const dvo_b200::ModesArgs& a) {
+  switch (dvo_b200::modes_entry(a)) {
+    case dvo_b200::kEntryMatch:
+      return dvo_b200_match_batch(ctx, a.cfg, a.n, a.refs, a.curs, a.hypotheses, a.results, a.iter_stats, a.max_log);
+    case dvo_b200::kEntryPhotometric:
+      return dvo_b200_match_batch_photometric(ctx, a.cfg, a.n, a.refs, a.curs, a.hypotheses, a.ab_init, a.results, a.ab, a.iter_stats,
+                                              a.max_log);
+    case dvo_b200::kEntryPrior:
+      return dvo_b200_match_batch_prior(ctx, a.cfg, a.n, a.refs, a.curs, a.hypotheses, a.prior, a.ab_init, a.ab, a.results, a.iter_stats,
+                                        a.max_log);
+    case dvo_b200::kEntryMaps:
+      return dvo_b200_match_batch_maps(ctx, a.cfg, a.n, a.refs, a.curs, a.hypotheses, a.prior, a.ab_init, a.ab, a.results, a.iter_stats,
+                                       a.max_log, a.maps);
+    case dvo_b200::kEntryHypotheses:
+      break;
+  }
+  return dvo_b200_match_batch_hypotheses_modes(ctx, a.cfg, a.n, a.refs, a.curs, a.k, a.hypotheses, a.screen_level, a.min_ratio, a.prior,
+                                               a.ab_init, a.ab, a.screen_ab, a.results, a.best, a.scores, a.screen_results, a.iter_stats,
+                                               a.max_log, a.maps);
 }
 
 }  // namespace
@@ -146,6 +187,29 @@ int dvo_b200_match_batch_sharded(dvo_b200_sharded* s, const dvo_b200_config* cfg
   return for_each_shard(s, n, [&](int k, int64_t b, int64_t e) {
     return dvo_b200_match_batch(s->ctx[size_t(k)], cfg, int32_t(e - b), references + b, currents + b, T_init ? T_init + 16 * b : nullptr, results + b,
                                 iteration_stats ? iteration_stats + size_t(b) * size_t(max_iteration_stats) : nullptr, max_iteration_stats);
+  });
+}
+
+int dvo_b200_match_batch_modes_sharded(dvo_b200_sharded* s, const dvo_b200_config* cfg, int32_t n, dvo_b200_pyramid* const* references,
+                                       dvo_b200_pyramid* const* currents, int32_t k, const double* hypotheses, int32_t screen_level,
+                                       double min_constraint_ratio, const double* prior_information, const double* photometric_init,
+                                       double* photometric, double* screen_photometric, dvo_b200_result* results, int32_t* best,
+                                       double* scores, dvo_b200_result* screen_results, dvo_b200_iteration_stats* iteration_stats,
+                                       int32_t max_iteration_stats, const dvo_b200_weight_maps* maps) {
+  if (!s) return DVO_B200_ERR_INVALID_ARGUMENT;
+  dvo_b200::ModesArgs a;
+  a.cfg = cfg; a.n = n; a.refs = references; a.curs = currents; a.k = k; a.hypotheses = hypotheses; a.screen_level = screen_level;
+  a.min_ratio = min_constraint_ratio; a.prior = prior_information; a.ab_init = photometric_init; a.ab = photometric;
+  a.screen_ab = screen_photometric; a.results = results; a.best = best; a.scores = scores; a.screen_results = screen_results;
+  a.iter_stats = iteration_stats; a.max_log = max_iteration_stats; a.maps = maps;
+  // the whole batch is checked before any shard starts, so a refusal leaves every shard's context untouched
+  int code = 0;
+  const std::string why = dvo_b200::modes_args_error(a, dvo_b200::kFormSharded, int(s->ctx.size()), s->devices.data(), public_view,
+                                                     public_where, &code);
+  if (!why.empty()) return fail(s, code, why);
+  return for_each_shard(s, n, [&](int shard, int64_t b, int64_t e) {
+    dvo_b200_weight_maps m;
+    return call_entry(s->ctx[size_t(shard)], dvo_b200::shard_slice(a, b, e, &m));
   });
 }
 

@@ -20,6 +20,7 @@
 #include "stages.cuh"
 #include "launch_plan.h"
 #include "hypotheses_args.h"
+#include "modes_args.h"
 
 #include <cstdio>
 #include <cstring>
@@ -1117,18 +1118,9 @@ std::vector<const dvo_b200_pyramid*> distinct_slabs(int n, dvo_b200_pyramid* con
 
 int check_batch(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int n, dvo_b200_pyramid* const* refs,
                 dvo_b200_pyramid* const* curs) {
-  if (!cfg || n <= 0 || !refs || !curs) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match: null argument");
-  if (cfg->first_level < cfg->last_level || cfg->last_level < 0 || cfg->first_level >= kMaxLevels)
-    return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match: config not sane (FirstLevel >= LastLevel >= 0 required)");
-  if (cfg->max_iterations_per_level < 0) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match: max iterations < 0");
-  for (int i = 0; i < n; ++i) {
-    if (!refs[i] || !curs[i]) return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match: null pyramid");
-    if (refs[i]->levels <= cfg->first_level || curs[i]->levels <= cfg->first_level)
-      return set_error(ctx, DVO_B200_ERR_INVALID_ARGUMENT, "match: pyramid has fewer levels than FirstLevel+1");
-    if (refs[i]->L[0].w != refs[0]->L[0].w || refs[i]->L[0].h != refs[0]->L[0].h ||
-        curs[i]->L[0].w != refs[0]->L[0].w || curs[i]->L[0].h != refs[0]->L[0].h)
-      return set_error(ctx, DVO_B200_ERR_SHAPE_MISMATCH, "match: all pyramids of a batch must share width/height");
-  }
+  int code = 0;
+  const std::string why = batch_args_error(cfg, n, refs, curs, pyramid_view, &code);
+  if (!why.empty()) return set_error(ctx, code, why);
   // order this stream after the builds (possibly on another ctx's stream, possibly still running) of every pyramid
   for (const dvo_b200_pyramid* p : distinct_slabs(n, refs, curs)) wait_for_pyramid(ctx, p);
   return 0;
@@ -1353,13 +1345,19 @@ int ensure_pinned_results(dvo_b200_ctx* ctx, size_t bytes) {
 }
 
 // Enqueue the copy of (alpha, beta) of the n brightness states at src to dst, 2 n doubles of the pinned results buffer
-int copy_back_photometric(dvo_b200_ctx* ctx, void* dst, const AffineState* src, size_t n) {
-  DVO_CUDA(ctx, cudaMemcpy2DAsync(dst, 2 * sizeof(double), src->ab, sizeof(AffineState), 2 * sizeof(double), n,
-                                  cudaMemcpyDeviceToHost, ctx->stream));
+// (kind: device to host) or of the caller's device memory (device to device)
+int copy_back_photometric(dvo_b200_ctx* ctx, void* dst, const AffineState* src, size_t n, cudaMemcpyKind kind) {
+  DVO_CUDA(ctx, cudaMemcpy2DAsync(dst, 2 * sizeof(double), src->ab, sizeof(AffineState), 2 * sizeof(double), n, kind, ctx->stream));
   return 0;
 }
 
 }  // namespace
+
+// What modes_args.h reads of a pyramid, from its fields
+PyramidView pyramid_view(const dvo_b200_pyramid* p, int level) {
+  const bool has = level >= 0 && level < p->levels;
+  return PyramidView{p->levels, p->device, p->L[0].w, p->L[0].h, has ? p->L[level].w : 0, has ? p->L[level].h : 0};
+}
 
 // A match (k = 0) is one leg over levels first .. last of the n pairs.  A multi-hypothesis match (include/dvo_b200.h) is two:
 // the screening leg runs n k virtual pairs, pair p k + j being (refs[p], curs[p]) from H[p][j] (and Lambda[p][j],
@@ -1371,7 +1369,9 @@ int copy_back_photometric(dvo_b200_ctx* ctx, void* dst, const AffineState* src, 
 // and AffineStates of the last leg whichever the call.  The device stage holds the results (n), screen results (n k, if
 // requested), scores (n k) and best (n; none of the three with k = 0), copied back through the pinned results buffer in
 // that layout, followed there at the next 16-byte boundary by (alpha, beta) of the n pairs and of the n k screening runs
-// (if requested).  A device-results call writes its results to d_results and uses neither.
+// (if requested).  A device-output call (MatchCall::device_outputs) has k_finalize and k_pick_hypotheses write the
+// caller's buffers, copies (alpha, beta) and the iteration logs device to device, and uses neither buffer; without a scores
+// output its scores go to the device stage.
 int tracker_match(dvo_b200_ctx* ctx, const MatchCall& c) {
   const dvo_b200_config* const cfg = c.cfg;
   dvo_b200_pyramid* const* const refs = c.refs;
@@ -1404,26 +1404,31 @@ int tracker_match(dvo_b200_ctx* ctx, const MatchCall& c) {
   const size_t out_bytes = best_at + (k ? sizeof(int32_t) * (size_t)n : 0);
   const size_t ab_at = (out_bytes + 15) / 16 * 16, ab_bytes = v.affine ? sizeof(double) * 2 * (size_t)n : 0;
   const size_t screen_ab_bytes = c.screen_ab ? sizeof(double) * 2 * (size_t)nk : 0;
-  if (!c.d_results) {
+  const bool dev = c.device_outputs;
+  if (!dev) {
     if ((rc = ensure_stage(ctx, out_bytes, 0))) return rc;
     if ((rc = ensure_pinned_results(ctx, ab_at + ab_bytes + screen_ab_bytes))) return rc;
+  } else if (k && !c.scores && (rc = ensure_stage(ctx, score_bytes, 0))) {   // the scores k_pick_hypotheses ranks
+    return rc;
   }
   const double* const tinit = cfg->use_initial_estimate ? c.T_init : nullptr;
   if ((rc = stage_inputs(ctx, legs, nlegs, tinit, c.ab_init, c.prior, max_log, v))) return rc;
   for (int i = 0; i < legs[0].plan.nlaunch; ++i)
     if ((rc = launch_segments(ctx, cfg, legs[0], i, tinit ? ws.d_tinit : nullptr, max_log, nullptr, 0, v))) return rc;
+  // where k_finalize and k_pick_hypotheses write: the caller's buffers, or the device stage that is copied back
   char* const d_out = (char*)ctx->d_stage;
-  dvo_b200_result* const d_res = c.d_results ? (dvo_b200_result*)c.d_results : (dvo_b200_result*)d_out;
+  dvo_b200_result* const d_res = dev ? c.results : (dvo_b200_result*)d_out;
   if (k) {
     const Leg &screen = legs[0], &chosen = legs[1];
-    if (c.screen_results) finalize(ctx, ws.d_state, (dvo_b200_result*)(d_out + res_bytes), nk);
+    if (c.screen_results) finalize(ctx, ws.d_state, dev ? c.screen_results : (dvo_b200_result*)(d_out + res_bytes), nk);
     {
       ProfScope prof(ctx, 2);
       auto pick = v.affine ? (v.prior ? k_pick_hypotheses<true, true> : k_pick_hypotheses<true, false>)
                            : (v.prior ? k_pick_hypotheses<false, true> : k_pick_hypotheses<false, false>);
       pick<<<(n + 3) / 4, 128, 0, st>>>(ws.d_state, ws.d_iter_log, ws.d_state + chosen.pair0, ws.d_iter_log + chosen.pair0 * max_log,
-                                        max_log, n, k, screen.first - screen.last, c.min_ratio, (double*)(d_out + scores_at),
-                                        (int*)(d_out + best_at), v.affine ? ws.d_affine : nullptr,
+                                        max_log, n, k, screen.first - screen.last, c.min_ratio,
+                                        dev && c.scores ? c.scores : (double*)(d_out + (dev ? 0 : scores_at)),
+                                        dev ? c.best : (int*)(d_out + best_at), v.affine ? ws.d_affine : nullptr,
                                         v.affine ? ws.d_affine + chosen.pair0 : nullptr, v.prior ? ws.d_prior : nullptr,
                                         v.prior ? ws.d_prior + 36 * chosen.pair0 : nullptr);
       ctx->launches++;
@@ -1435,14 +1440,20 @@ int tracker_match(dvo_b200_ctx* ctx, const MatchCall& c) {
   if (c.maps)
     weight_maps_launch(ctx, *c.maps, n, refs[0], last, ws.d_state + z.pair0, ws.d_pair_level + z.desc0 + z.ndesc - n,
                        v.affine ? ws.d_affine + z.pair0 : nullptr);
+  const size_t log_bytes = sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log;
+  if (dev) {   // the rest of the outputs, device to device; nothing crosses to the host and nothing waits
+    if (ab_bytes && (rc = copy_back_photometric(ctx, c.ab_out, ws.d_affine + z.pair0, (size_t)n, cudaMemcpyDeviceToDevice))) return rc;
+    if (screen_ab_bytes && (rc = copy_back_photometric(ctx, c.screen_ab, ws.d_affine, (size_t)nk, cudaMemcpyDeviceToDevice))) return rc;
+    if (log_bytes)
+      DVO_CUDA(ctx, cudaMemcpyAsync(c.iter_stats, ws.d_iter_log + z.pair0 * max_log, log_bytes, cudaMemcpyDeviceToDevice, st));
+  }
   if ((rc = end_call(ctx, n, refs, curs, z.flag0 + z.plan.nlaunch))) return rc;
-  if (c.d_results) return 0;   // a device-results call leaves its level flags to dvo_b200_synchronize
+  if (dev) return 0;   // a device-output call leaves its level flags to dvo_b200_synchronize
 
   char* const hr = (char*)ctx->h_results;
-  const size_t log_bytes = sizeof(dvo_b200_iteration_stats) * (size_t)n * max_log;
   DVO_CUDA(ctx, cudaMemcpyAsync(hr, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
-  if (ab_bytes && (rc = copy_back_photometric(ctx, hr + ab_at, ws.d_affine + z.pair0, (size_t)n))) return rc;
-  if (screen_ab_bytes && (rc = copy_back_photometric(ctx, hr + ab_at + ab_bytes, ws.d_affine, (size_t)nk))) return rc;
+  if (ab_bytes && (rc = copy_back_photometric(ctx, hr + ab_at, ws.d_affine + z.pair0, (size_t)n, cudaMemcpyDeviceToHost))) return rc;
+  if (screen_ab_bytes && (rc = copy_back_photometric(ctx, hr + ab_at + ab_bytes, ws.d_affine, (size_t)nk, cudaMemcpyDeviceToHost))) return rc;
   if (c.maps && (rc = weight_maps_copy_back(ctx, *c.maps, n, refs[0], last))) return rc;
   if (log_bytes)
     DVO_CUDA(ctx, cudaMemcpyAsync(c.iter_stats, ws.d_iter_log + z.pair0 * max_log, log_bytes, cudaMemcpyDeviceToHost, st));

@@ -42,7 +42,10 @@ def tensor_to_results(t: torch.Tensor):
 
 
 def all_gather_results(local: torch.Tensor, total: int) -> torch.Tensor:
-    """All-gather per-rank result records [n_r, RESULT_BYTES] into [total, RESULT_BYTES] in pair order."""
+    """All-gather per-rank rows [n_r, m] into [total, m] in pair order, rank r holding the rows of shard_range(total, ws, r):
+    any dtype and any m, padded to the largest shard.  The result records [n_r, RESULT_BYTES] uint8, and the other per-pair
+    outputs of Engine.match_batch_modes_device as rows: (alpha, beta) [n_r, 2] float64, best as [n_r, 1] int32 and the
+    scores [n_r, k] float64."""
     if not dist.is_initialized() or dist.get_world_size() == 1:
         return local
     ws = dist.get_world_size()

@@ -39,7 +39,8 @@ ABI_SYMBOLS = [
     "dvo_b200_pyramid_create_rectified_device_batch", "dvo_b200_depth_rays", "dvo_b200_depth_registration_create",
     "dvo_b200_depth_registration_release", "dvo_b200_pyramid_create_registered_batch",
     "dvo_b200_pyramid_create_registered_device_batch", "dvo_b200_match_batch_prior", "dvo_b200_match_batch_maps",
-    "dvo_b200_match_batch_hypotheses", "dvo_b200_match_batch_hypotheses_modes",
+    "dvo_b200_match_batch_hypotheses", "dvo_b200_match_batch_hypotheses_modes", "dvo_b200_match_batch_modes_device",
+    "dvo_b200_match_batch_modes_sharded",
 ]
 
 # dvo_b200_estimator
@@ -219,6 +220,79 @@ def _iteration_log(cfg, n, with_iterations):
     return (IterationStats * (n * max_log))(), max_log
 
 
+def _modes_inputs(n, T_init, hypotheses, prior_information, photometric_init, photometric):
+    """The inputs of a modes call (dvo_b200_match_batch_modes_device / _sharded) as C rows: (k, T_init or hypotheses, Lambda,
+    (alpha, beta)_0).  hypotheses None: k = 0, T_init [n, 4, 4] or None, prior_information [n, 6, 6], photometric_init [n, 2];
+    else hypotheses [n, k, 4, 4] and the per-hypothesis layouts [n, k, 6, 6] and [n, k, 2]."""
+    if hypotheses is None:
+        return (0, _rows(T_init, "T_init", (n, 4, 4), 16), _rows(prior_information, "prior_information", (n, 6, 6), 36),
+                _photometric_init(photometric, photometric_init, (n, 2)))
+    if T_init is not None:
+        raise ValueError("T_init with hypotheses: the hypotheses are the initial estimates")
+    H = np.asarray(hypotheses, dtype=np.float64)
+    if H.ndim != 4 or H.shape[0] != n or H.shape[2:] != (4, 4):
+        raise ValueError(f"hypotheses {H.shape}: want [{n}, k, 4, 4]")
+    k = H.shape[1]
+    return (k, _rows(H, "hypotheses", H.shape, 16), _rows(prior_information, "prior_information", (n, k, 6, 6), 36),
+            _photometric_init(photometric, photometric_init, (n, k, 2)))
+
+
+def _maps_shapes(level_size, refs, cfg, mask_weight):
+    """{name: (shape, dtype name)} of the weight maps of n references; level_size(ref, level) -> (w, h).  The references of
+    one call share their size (ValueError otherwise)."""
+    L = cfg.last_level
+    sizes = {tuple(level_size(r, L)) + tuple(level_size(r, 0)) for r in refs}
+    if len(sizes) != 1:
+        raise ValueError(f"references of {len(sizes)} different sizes: the maps take one size per call")
+    w, h, w0, h0 = sizes.pop()
+    n = len(refs)
+    out = {k: ((n, h, w), "float32") for k in ("weight", "residual_i", "residual_z")}
+    out["estimate"] = ((n, 4, 4), "float64")
+    out["precision"] = ((n, 2, 2), "float32")
+    if mask_weight is not None:
+        out["mask"] = ((n, h0, w0), "uint8")
+    return out
+
+
+def _address(a) -> int:
+    """the address of a torch tensor or a numpy array"""
+    return a.data_ptr() if hasattr(a, "data_ptr") else a.ctypes.data
+
+
+def _weight_maps(maps, memory, mask_weight) -> "WeightMaps":
+    """The dvo_b200_weight_maps of a dict of maps (_maps_shapes' names; torch tensors or numpy arrays) in memory "device" or
+    "host"; the mask's plane with mask_weight only."""
+    wm = WeightMaps()
+    wm.memory = MAPS_MEMORY[memory]
+    for k in ("weight", "residual_i", "residual_z"):
+        _, h, w = maps[k].shape
+        setattr(wm, k, MapPlane(_address(maps[k]), 4 * w, 4 * w * h))
+    if "mask" in maps:
+        _, h0, w0 = maps["mask"].shape
+        wm.mask = MapPlane(_address(maps["mask"]), w0, w0 * h0)
+        wm.mask_weight = float(mask_weight)
+    wm.estimate = C.cast(_address(maps["estimate"]), C.POINTER(C.c_double))
+    wm.precision = C.cast(_address(maps["precision"]), C.POINTER(C.c_float))
+    return wm
+
+
+def _modes_outputs(n, k, max_log, screen_results, photometric):
+    """{name: (shape, dtype name)} of the outputs of a modes call other than the maps, keyed by their argument's name"""
+    out = {"results": ((n, C.sizeof(CResult)), "uint8")}
+    if k:
+        out["best"] = ((n,), "int32")
+        out["scores"] = ((n, k), "float64")
+        if screen_results:
+            out["screen_results"] = ((n, k, C.sizeof(CResult)), "uint8")
+    if photometric:
+        out["photometric"] = ((n, 2), "float64")
+        if k and screen_results:
+            out["screen_photometric"] = ((n, k, 2), "float64")
+    if max_log:
+        out["iterations"] = ((n, max_log, C.sizeof(IterationStats)), "uint8")
+    return out
+
+
 class IterationStats(C.Structure):
     _fields_ = [("level", C.c_int32), ("id", C.c_int32), ("valid_constraints", C.c_int64),
                 ("tdist_log_likelihood", C.c_double), ("tdist_precision", C.c_double * 4),
@@ -383,6 +457,11 @@ def load_library():
     L.dvo_b200_match_batch_hypotheses_modes.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), i32, dp, i32, C.c_double,
                                                          dp, dp, dp, dp, C.POINTER(CResult), C.POINTER(i32), dp, C.POINTER(CResult),
                                                          C.POINTER(IterationStats), i32, C.POINTER(WeightMaps)]
+    L.dvo_b200_match_batch_modes_device.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), i32, dp, i32, C.c_double,
+                                                     dp, dp, vp, vp, vp, vp, vp, vp, vp, i32, C.POINTER(WeightMaps)]
+    L.dvo_b200_match_batch_modes_sharded.argtypes = [vp, C.POINTER(Config), i32, C.POINTER(vp), C.POINTER(vp), i32, dp, i32, C.c_double,
+                                                      dp, dp, dp, dp, C.POINTER(CResult), C.POINTER(i32), dp, C.POINTER(CResult),
+                                                      C.POINTER(IterationStats), i32, C.POINTER(WeightMaps)]
     L.dvo_b200_residual_image_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, fp, C.POINTER(i64)]
     L.dvo_b200_linearize_photometric.argtypes = [vp, C.POINTER(Config), vp, vp, i32, dp, dp, i32, fp, C.POINTER(i64), fp, fp, dp, dp]
     L.dvo_b200_set_estimator.argtypes = [vp, i32]
@@ -799,29 +878,86 @@ class Engine:
         """The torch CUDA tensors of match_batch_maps and the WeightMaps that points at them, with the engine's stream ordered
         after torch's current stream (the engine's stream writes memory that stream allocated; the call synchronises)."""
         import torch
-        n = len(refs)
-        L = cfg.last_level
-        sizes = {tuple(r.level_info(L)[:2]) + tuple(r.level_info(0)[:2]) for r in refs}
-        if len(sizes) != 1:
-            raise ValueError(f"references of {len(sizes)} different sizes: match_batch_maps takes one size per call")
-        w, h, w0, h0 = sizes.pop()
         dev = torch.device("cuda", self.device)
-        maps = {k: torch.empty((n, h, w), dtype=torch.float32, device=dev) for k in ("weight", "residual_i", "residual_z")}
-        maps["estimate"] = torch.empty((n, 4, 4), dtype=torch.float64, device=dev)
-        maps["precision"] = torch.empty((n, 2, 2), dtype=torch.float32, device=dev)
-        wm = WeightMaps()
-        wm.memory = MAPS_MEMORY["device"]
-        for k in ("weight", "residual_i", "residual_z"):
-            setattr(wm, k, MapPlane(maps[k].data_ptr(), 4 * w, 4 * w * h))
-        if mask_weight is not None:
-            maps["mask"] = torch.empty((n, h0, w0), dtype=torch.uint8, device=dev)
-            wm.mask = MapPlane(maps["mask"].data_ptr(), w0, w0 * h0)
-            wm.mask_weight = float(mask_weight)
-        wm.estimate = C.cast(maps["estimate"].data_ptr(), C.POINTER(C.c_double))
-        wm.precision = C.cast(maps["precision"].data_ptr(), C.POINTER(C.c_float))
+        maps = {k: torch.empty(shape, dtype=getattr(torch, dt), device=dev)
+                for k, (shape, dt) in _maps_shapes(lambda r, l: r.level_info(l)[:2], refs, cfg, mask_weight).items()}
         current = torch.cuda.current_stream(dev)
         torch.cuda.ExternalStream(self.stream, device=dev).wait_stream(current)
-        return maps, wm
+        return maps, _weight_maps(maps, "device", mask_weight)
+
+    def device_outputs(self, refs, cfg: Config, k: int = 0, screen_results: bool = False, photometric: bool = False,
+                       with_iterations: bool = False, maps: bool = False, mask_weight=None) -> dict:
+        """The outputs of match_batch_modes_device for n = len(refs) pairs, as torch CUDA tensors on the engine's device, each
+        under the name of its argument: "results" [n, sizeof(dvo_b200_result)] uint8 (distributed.tensor_to_results reads
+        them), with k >= 1 "best" [n] int32 and "scores" [n, k] float64, with screen_results also "screen_results"
+        [n, k, sizeof(dvo_b200_result)] uint8; photometric: "photometric" [n, 2] float64, and with k >= 1 and screen_results
+        "screen_photometric" [n, k, 2]; with_iterations: "iterations" [n, max_log, sizeof(dvo_b200_iteration_stats)] uint8,
+        room for every iteration of cfg's levels; maps or mask_weight: "maps", the dict of match_batch_maps, and
+        "mask_weight"."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        n = len(refs)
+        max_log = _iteration_log(cfg, 0, with_iterations)[1]
+        out = {name: torch.empty(shape, dtype=getattr(torch, dt), device=dev)
+               for name, (shape, dt) in _modes_outputs(n, k, max_log, screen_results, photometric).items()}
+        if maps or mask_weight is not None:
+            out["maps"] = {name: torch.empty(shape, dtype=getattr(torch, dt), device=dev)
+                           for name, (shape, dt) in _maps_shapes(lambda r, l: r.level_info(l)[:2], refs, cfg, mask_weight).items()}
+            if mask_weight is not None:
+                out["mask_weight"] = float(mask_weight)
+        return out
+
+    def _ordered_with_torch(self, tensors, call):
+        """call() with the engine's stream ordered after torch's current stream, which allocated the tensors, and that stream
+        ordered after the engine's work when call() returns: torch work on the current stream, and the caching allocator's
+        reuse of the tensors' memory, then follow the writes.  Every tensor must be a contiguous CUDA tensor on the engine's
+        device.  Returns call()'s status."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        for t in tensors:
+            if not (t.is_cuda and t.device == dev and t.is_contiguous()):
+                raise ValueError(f"an output on {t.device} (contiguous: {t.is_contiguous()}): want contiguous tensors on {dev}")
+        current = torch.cuda.current_stream(dev)
+        ext = torch.cuda.ExternalStream(self.stream, device=dev)
+        ext.wait_stream(current)
+        rc = call()
+        current.wait_stream(ext)
+        return rc
+
+    def match_batch_modes_device(self, refs, curs, cfg: Config, out: dict, T_init=None, hypotheses=None, screen_level=None,
+                                 min_constraint_ratio: float = 0.0, prior_information=None, photometric_init=None):
+        """Every alignment mode with its outputs left in device memory (dvo_b200_match_batch_modes_device): out is a dict
+        made by device_outputs, and which of its outputs are present selects the mode (photometric, maps) and what is
+        written (screen results, iteration logs).  hypotheses None: one alignment per pair from T_init ([n, 4, 4] or None),
+        prior_information [n, 6, 6]; else the multi-hypothesis alignment of match_batch_hypotheses, hypotheses [n, k, 4, 4],
+        prior_information [n, k, 6, 6] and photometric_init [n, k, 2], with screen_level required.  The bytes written are
+        those of match_batch, match_batch_photometric, match_batch_maps or match_batch_hypotheses with the same arguments.
+        The inputs are staged before the call returns; the work is enqueued on engine.stream after torch's current stream,
+        and the call returns without waiting for it.  Torch's current stream is then ordered after that work, so torch work
+        queued on it (an all-gather of the outputs) reads them complete; anything else must wait on engine.stream before it
+        reads out (torch.cuda.ExternalStream(engine.stream), or engine.synchronize(), which also reports a level-kernel
+        timeout)."""
+        n = len(refs)
+        assert n == len(curs) and n > 0
+        k, H, lam, ab0 = _modes_inputs(n, T_init, hypotheses, prior_information, photometric_init, "photometric" in out)
+        if k and screen_level is None:
+            raise ValueError("hypotheses without screen_level")
+        max_log = int(out["iterations"].shape[1]) if "iterations" in out else 0
+        want = _modes_outputs(n, k, max_log, "screen_results" in out, "photometric" in out)
+        for name, t in out.items():
+            if name in ("maps", "mask_weight"):
+                continue
+            if name not in want or tuple(t.shape) != want[name][0] or str(t.dtype) != "torch." + want[name][1]:
+                raise ValueError(f"out[{name!r}]: {getattr(t, 'dtype', None)} {tuple(getattr(t, 'shape', ()))}, want "
+                                 + (f"{want[name][1]} {want[name][0]}" if name in want else f"no such output with k = {k}"))
+        maps = out.get("maps")
+        tensors = [t for name, t in out.items() if name not in ("maps", "mask_weight")] + list((maps or {}).values())
+        wm = _weight_maps(maps, "device", out.get("mask_weight")) if maps is not None else None
+        p = lambda name: C.c_void_p(_address(out[name])) if name in out else None
+        self._check(self._ordered_with_torch(tensors, lambda: self.lib.dvo_b200_match_batch_modes_device(
+            self.ctx, C.byref(cfg), n, _handles(refs), _handles(curs), k, _ptr(H), int(screen_level or 0), float(min_constraint_ratio),
+            _ptr(lam), _ptr(ab0), p("photometric"), p("screen_photometric"), p("results"), p("best"), p("scores"), p("screen_results"),
+            p("iterations"), max_log, C.byref(wm) if wm is not None else None)))
 
     def match_batch_maps(self, refs, curs, cfg: Config, T_init=None, prior_information=None, photometric_init=None,
                          photometric: bool = False, mask_weight=None, with_iterations: bool = False):
@@ -1037,6 +1173,58 @@ class ShardedEngine:
     def release(self, handles):
         for p in handles:
             self.lib.dvo_b200_pyramid_release(p)
+
+    def match_batch_modes(self, refs, curs, cfg: Config | None = None, T_init=None, hypotheses=None, screen_level=None,
+                          min_constraint_ratio: float = 0.0, with_iterations: bool = False, screen_results: bool = False,
+                          prior_information=None, photometric_init=None, photometric: bool = False, maps: bool = False,
+                          mask_weight=None):
+        """Every alignment mode over the shards (dvo_b200_match_batch_modes_sharded); refs / curs: Pyramid objects or the
+        handles pyramid_batch returns, pair i on the device of the shard that owns it.  hypotheses None: one alignment per
+        pair, returning what Engine.match_batch_maps (maps or mask_weight), match_batch_photometric (photometric) or
+        match_batch returns; else the multi-hypothesis alignment, returning what Engine.match_batch_hypotheses returns
+        (cfg defaults to Config(use_initial_estimate=1)).  The maps are host numpy arrays."""
+        n = len(refs)
+        assert n == len(curs) and n > 0
+        if cfg is None:
+            cfg = Config(use_initial_estimate=1) if hypotheses is not None else Config()
+        k, H, lam, ab0 = _modes_inputs(n, T_init, hypotheses, prior_information, photometric_init, photometric)
+        if k and screen_level is None:
+            raise ValueError("hypotheses without screen_level")
+        handle = lambda p: p.handle if isinstance(p, Pyramid) else p.value
+        rh, ch = (C.c_void_p * n)(*map(handle, refs)), (C.c_void_p * n)(*map(handle, curs))
+        res = (CResult * n)()
+        log, max_log = _iteration_log(cfg, n, with_iterations)
+        best = np.zeros(n, dtype=np.int32) if k else None
+        scores = np.zeros((n, k), dtype=np.float64) if k else None
+        screen = (CResult * (n * k))() if k and screen_results else None
+        ab = np.zeros((n, 2), dtype=np.float64) if photometric else None
+        screen_ab = np.zeros((n, k, 2), dtype=np.float64) if k and photometric and screen_results else None
+        hmaps = wm = None
+        if maps or mask_weight is not None:
+            def level_size(h, level):
+                w, ht = C.c_int32(), C.c_int32()
+                self._check(self.lib.dvo_b200_pyramid_level_info(h, level, C.byref(w), C.byref(ht), None))
+                return w.value, ht.value
+            hmaps = {name: np.zeros(shape, dtype=dt) for name, (shape, dt) in _maps_shapes(level_size, list(rh), cfg, mask_weight).items()}
+            wm = _weight_maps(hmaps, "host", mask_weight)
+        self._check(self.lib.dvo_b200_match_batch_modes_sharded(
+            self.h, C.byref(cfg), n, rh, ch, k, _ptr(H), int(screen_level or 0), float(min_constraint_ratio), _ptr(lam), _ptr(ab0), _ptr(ab),
+            _ptr(screen_ab), res, _ptr(best, C.POINTER(C.c_int32)), _ptr(scores), screen, log, max_log,
+            C.byref(wm) if wm is not None else None))
+        results = _results(res, n, log, max_log)
+        if not k:
+            if hmaps is not None:
+                return (results, hmaps, ab) if photometric else (results, hmaps)
+            return (results, ab) if photometric else results
+        out = (results, best, scores)
+        if screen_results:
+            flat = [Result(screen[i]) for i in range(n * k)]
+            out += ([flat[i * k:(i + 1) * k] for i in range(n)],)
+        if photometric:
+            out += (ab,) + ((screen_ab,) if screen_results else ())
+        if hmaps is not None:
+            out += (hmaps,)
+        return out
 
     def match_batch(self, refs, curs, cfg: Config, T_init=None):
         n = len(refs)

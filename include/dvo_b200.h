@@ -509,7 +509,7 @@ int dvo_b200_linearize(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, dvo_b200_p
  *   outputs    transformation and log_likelihood keep their meaning.  information is the Schur complement of the 8 x 8
  *              (prior included) onto the pose, A_xx - A_xp A_pp^-1 A_px, times 0.008^2 as by default; iteration stats carry
  *              the pose part of the increment and the same Schur complement; level stats are unchanged.
- * Not provided in this mode: match_batch_device and the sharded forms. */
+ * Outputs in device memory and several GPUs: dvo_b200_match_batch_modes_device and _modes_sharded below. */
 
 /* dvo_b200_match_batch in the photometric mode.  photometric_init: 2n doubles (alpha, beta) per pair, or NULL = (1, 0) each;
  * photometric: 2n doubles out, the final (alpha, beta) of each pair.  A NULL photometric or a non-finite photometric_init is
@@ -555,7 +555,7 @@ int dvo_b200_linearize_photometric(dvo_b200_ctx* ctx, const dvo_b200_config* cfg
  * Arithmetic: b_i + sum_j Lambda_ij li_j is an in-order FMA chain over j and A_ij + Lambda_ij one addition, so Lambda = mu I
  * returns the bits of dvo_b200_match_batch[_photometric] with cfg->mu = mu in everything but the prior log-likelihood (and
  * with it log_likelihood), which may differ in the last bits; Lambda = 0 returns the bits of mu = 0 in everything.
- * Not provided in this mode: match_batch_device and the sharded forms. */
+ * Outputs in device memory and several GPUs: dvo_b200_match_batch_modes_device and _modes_sharded below. */
 
 /* dvo_b200_match_batch with a prior information per pair.  prior_information: n * 36 doubles, pair p's Lambda at p * 36.
  * photometric NULL: the default 6-unknown mode; non-NULL: the photometric mode, photometric_init and photometric as in
@@ -659,7 +659,7 @@ int dvo_b200_match_batch_maps(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int
  * quarter of the pixels of the next finer one.  Reference-role and both-role masks, cfg->mu and mixed intrinsics are
  * supported as by dvo_b200_match_batch; the photometric mode, motion priors and weight maps through
  * dvo_b200_match_batch_hypotheses_modes below.
- * Not provided in this mode: match_batch_device and the sharded forms. */
+ * Outputs in device memory and several GPUs: dvo_b200_match_batch_modes_device and _modes_sharded below. */
 #define DVO_B200_MAX_HYPOTHESES 64
 
 /* hypotheses: n * k * 16 doubles, H[p][j] at (p * k + j) * 16.  results, best: n each.  scores: n * k or NULL.
@@ -711,6 +711,51 @@ int dvo_b200_match_batch_hypotheses_modes(dvo_b200_ctx* ctx, const dvo_b200_conf
                                           double* screen_photometric, dvo_b200_result* results, int32_t* best, double* scores,
                                           dvo_b200_result* screen_results, dvo_b200_iteration_stats* iteration_stats,
                                           int32_t max_iteration_stats, const dvo_b200_weight_maps* maps);
+
+/* ---- every mode with its outputs in device memory, and over several GPUs --------------------------------------------------
+ * The arguments of dvo_b200_match_batch_hypotheses_modes, with k = 0 allowed.  k = 0: one plain alignment per pair;
+ * hypotheses is then T_init (n * 16 doubles or NULL), prior_information n * 36 doubles and photometric_init 2n; screen_level
+ * and min_constraint_ratio are ignored; best, scores, screen_results and screen_photometric must be NULL.  Let E be the
+ * call the arguments stand for: for k >= 1 dvo_b200_match_batch_hypotheses_modes; for k = 0 by what is non-NULL, maps ->
+ * dvo_b200_match_batch_maps, else prior_information -> _prior, else photometric -> _photometric, else dvo_b200_match_batch.
+ * Every output is, byte for byte, what E returns on one context with the same arguments, for both estimators, every mask
+ * role set, mixed intrinsics, every batch size and every launch plan.
+ * Refused with DVO_B200_ERR_INVALID_ARGUMENT (DVO_B200_ERR_SHAPE_MISMATCH where E returns it), the last error set, before
+ * anything is staged or launched: everything E refuses, first and in E's order (E's batch checks over the whole batch
+ * included); for k = 0 an output only k >= 1 writes, and photometric_init without photometric; then the form's own
+ * checks below.  The messages name the pair, and the hypothesis when there is one. */
+
+/* The outputs in device memory: every output pointer is device or managed memory of the context's device, maps included,
+ * which must be DVO_B200_MAPS_DEVICE.  The inputs (hypotheses / T_init, priors, photometric_init) are host memory and
+ * staged as by E; the caller may free them when the call returns.  The call may wait for the context's earlier work before
+ * staging; it enqueues its own work and returns without waiting for it, and copies nothing to the host
+ * (dvo_b200_d2h_bytes does not move; dvo_b200_h2d_bytes and dvo_b200_kernel_launches move as for E).  A level-kernel
+ * timeout surfaces at dvo_b200_synchronize.  Its own refusals, after E's: maps in DVO_B200_MAPS_HOST; then, per output in
+ * argument order, a pointer not aligned to its element, and a first or last byte that cudaPointerGetAttributes does not
+ * report as device or managed memory of the context's device.  dvo_b200_match_batch_device is this call with k = 0, every
+ * mode argument NULL and only results. */
+int dvo_b200_match_batch_modes_device(dvo_b200_ctx* ctx, const dvo_b200_config* cfg, int32_t n,
+                                      dvo_b200_pyramid* const* references, dvo_b200_pyramid* const* currents, int32_t k,
+                                      const double* hypotheses, int32_t screen_level, double min_constraint_ratio,
+                                      const double* prior_information, const double* photometric_init, double* photometric,
+                                      double* screen_photometric, dvo_b200_result* results, int32_t* best, double* scores,
+                                      dvo_b200_result* screen_results, dvo_b200_iteration_stats* iteration_stats,
+                                      int32_t max_iteration_stats, const dvo_b200_weight_maps* maps);
+/* Over the shards of s (one context and host thread per device), outputs in host memory; maps, if given, must be
+ * DVO_B200_MAPS_HOST.  Pairs are split by dvo_b200_shard_range, and pair p takes onto its shard its k hypotheses, priors
+ * and photometric_init rows, its slice of every output (results, best, scores, screen_results, photometric,
+ * screen_photometric, iteration_stats at p * max_iteration_stats) and its maps (planes at data + p * image_bytes, estimate,
+ * precision).  Each shard runs E on its own context, with that context's estimator; a pair's bits do not depend on its
+ * batch, so with the same estimator everywhere the outputs are E's on one context.  The whole batch is checked before any
+ * shard starts, so a refusal leaves every shard's context untouched: after E's checks, a pair whose pyramids do not live on
+ * the device of the shard that owns it, then maps in DVO_B200_MAPS_DEVICE.  Returns once every shard is done. */
+int dvo_b200_match_batch_modes_sharded(dvo_b200_sharded* s, const dvo_b200_config* cfg, int32_t n,
+                                       dvo_b200_pyramid* const* references, dvo_b200_pyramid* const* currents, int32_t k,
+                                       const double* hypotheses, int32_t screen_level, double min_constraint_ratio,
+                                       const double* prior_information, const double* photometric_init, double* photometric,
+                                       double* screen_photometric, dvo_b200_result* results, int32_t* best, double* scores,
+                                       dvo_b200_result* screen_results, dvo_b200_iteration_stats* iteration_stats,
+                                       int32_t max_iteration_stats, const dvo_b200_weight_maps* maps);
 
 /* ---- profiling hooks (bench.py roofline): per-kernel-class accumulated device time measured with
  *      CUDA events on the ctx stream.  classes: 0 residual/scale stage, 1 normal-equation stage,
